@@ -60,18 +60,38 @@ def measured_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
-def recorded_traffic():
-    """DRAM bytes per launch of the walk kernel from the committed ncu capture (not measured in this
-    run: dram__bytes needs ncu), with the capture it comes from; or None."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        return {"dram_bytes_per_launch": t["dram_bytes_per_launch"],
-                "source": "profiles/traffic.json (%s)" % t.get("source", "ncu capture")}
-    except Exception:
-        return None
+# --dump-outputs: an output with more rows than this is written as a fixed seeded sample of its rows
+# (plus the sampled row indices), which keeps a dump of any config under 64 MB
+DUMP_ROWS = 1 << 20
+
+
+def dump_outputs(eng, dirname, write):
+    """Writes what a caller of the timed path receives after its last step, as float64 .npy files:
+    flux per element, and the parent element and position of every particle of this rank's stripe
+    (with several ranks, the dump is rank 0's: the summed flux and rank 0's particles).  Every rank
+    reads (reading the flux may gather the shares of a reduce-scatter exchange); only `write` saves."""
+    import numpy as np
+
+    def sample(n):  # None: all rows
+        return None if n <= DUMP_ROWS else np.sort(np.random.default_rng(0x5EED).choice(n, DUMP_ROWS, replace=False))
+
+    flux, fi = eng.flux, sample(eng.num_elements)
+    pi = sample(eng.num_particles)
+    out = {"flux": flux if fi is None else flux[fi],
+           "elem_ids": eng.elem_ids if pi is None else eng.elem_ids[pi],
+           "positions": eng.positions if pi is None else eng.positions[pi]}
+    if fi is not None:
+        out["flux_index"] = fi
+    if pi is not None:
+        out["particle_index"] = pi
+    if not write:
+        return
+    os.makedirs(dirname, exist_ok=True)
+    for name, arr in out.items():
+        np.save(os.path.join(dirname, f"{name}.npy"), np.ascontiguousarray(arr, dtype=np.float64))
 
 
 def bind_to_gpu_node(torch, index):
@@ -261,8 +281,10 @@ class GpuArm:
             self.dist.all_reduce(t, op=getattr(self.dist.ReduceOp, op))
         return [float(x) for x in t]
 
-    def measure(self, cfg_name, n, steps, warmup, e2e=True, e2e_modes=False, clocks=False, scaling="weak"):
-        """Device-resident and end-to-end throughput of `cfg_name` with n particles on this rank."""
+    def measure(self, cfg_name, n, steps, warmup, e2e=True, e2e_modes=False, clocks=False, scaling="weak",
+                dump_dir=None):
+        """Device-resident and end-to-end throughput of `cfg_name` with n particles on this rank;
+        dump_dir: write the device-resident arm's outputs there after its timed steps."""
         from pumiumtally_b200.tally import PumiTally
         from pumiumtally_b200.workload import CONFIGS, SyntheticWorkload
 
@@ -376,6 +398,8 @@ class GpuArm:
                 out["variant"], " incl. binning pass" if out["variant"] in (15, 16, 17, 21, 24, 25, 26) else "", steps,
                 kernel_ms / max(steps, 1)),
             "algorithmic_bytes_per_launch": alg_bytes / max(steps, 1), "peak_source": peak_src}
+        if dump_dir:
+            dump_outputs(eng, dump_dir, write=rank == 0)
         del eng
 
         # ---------------- end-to-end arm through the host-pointer C ABI: `e2e` ------
@@ -506,7 +530,7 @@ def run_gpu(args, rank, local_rank, world):
     if world == 1 and cfg.get("gpus", 1) > 1 and not args.particles:
         n = cfg["particles"] // cfg["gpus"] if args.per_gpu_share else cfg["particles"]
     main = arm.measure(args.config, n, args.steps, args.warmup, e2e=not args.no_e2e,
-                       e2e_modes=not args.no_e2e_modes, clocks=True)
+                       e2e_modes=not args.no_e2e_modes, clocks=True, dump_dir=args.dump_outputs)
 
     # ---- the multi-GPU configurations BASELINE.json names, measured beside the headline ----------
     # c4 on 4 GPUs (1 M particles / 4), c5 on 8 GPUs (100 M particles / 8), and c5 strong scaling
@@ -531,10 +555,7 @@ def run_gpu(args, rank, local_rank, world):
         arm.dist.destroy_process_group()
     if rank != 0:
         return
-    traffic = recorded_traffic() if (args.config == "c2" and not args.particles) else None
     roof = dict(main["roofline"])
-    roof["traffic"] = traffic["dram_bytes_per_launch"] if traffic else None
-    roof["traffic_source"] = traffic["source"] if traffic else None
     line = {
         "metric": METRIC, "value": main["value"], "unit": UNIT, "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": main["ms_per_step"], "higher_is_better": True,
@@ -590,8 +611,14 @@ def main():
                     help="skip the extra blocks when the headline measurement has already taken this long")
     ap.add_argument("--no-extra", action="store_true",
                     help="N>1: skip the extra blocks (c4 on 4 GPUs, c5 on 8 GPUs, c5 strong scaling)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the device-resident arm's flux, parent elements and "
+                         "positions to DIR/<name>.npy (float64; arrays over 2^20 rows as a fixed seeded sample; "
+                         "with several ranks: the summed flux and rank 0's particles)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
+    if args.steps < 1:
+        raise SystemExit("bench.py: --steps must be at least 1")
     rank, local_rank, world = env_int("RANK", 0), env_int("LOCAL_RANK", 0), env_int("WORLD_SIZE", 1)
     if args.impl == "reference":
         run_reference(args, rank)

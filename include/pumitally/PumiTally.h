@@ -1,4 +1,4 @@
-// pumitally::PumiTally -- drop-in facade of the B200 track-length tally engine.
+// pumitally::PumiTally -- drop-in facade of the H100 track-length tally engine.
 //
 // This header declares the same class, in the same namespace, with the same
 // member functions, argument types, const-ness and data layout (one
@@ -7,7 +7,7 @@
 // against either header links against either library: the Itanium-mangled
 // symbols are identical (checked by tests/test_abi_symbols.py).
 //
-// Everything behind the pointer is new: CUDA kernels for sm_100a reached through
+// Everything behind the pointer is new: CUDA kernels for sm_90a reached through
 // the extern "C" layer in include/pumitally_c.h.
 #ifndef PUMITALLY_PUMITALLY_H
 #define PUMITALLY_PUMITALLY_H

@@ -1,5 +1,5 @@
 /*
- * pumitally_c.h -- C ABI of libpumitally.so (B200 track-length tally engine).
+ * pumitally_c.h -- C ABI of libpumitally.so (H100 track-length tally engine).
  *
  * Plain pointers and sizes only.  The first five entry points are one-to-one
  * with the reference's public interface, which is what any FFI for this path
@@ -169,7 +169,7 @@ int pumitally_allreduce_tally(pumitally_engine *e);
  * the whole array, i.e. normally once, at the end of the run. */
 int pumitally_reduce_tally_to_owners(pumitally_engine *e);
 /* Which of the two is quicker depends on the size of the flux array and on the algorithm NCCL picks for
- * it (8 B200s: 8 MB -- all-reduce 0.10 ms, reduce-scatter 4.3 ms; 79 MB -- 0.9 ms and 0.43 ms), so
+ * it (either can be the quicker by a large factor), so
  * pumitally_comm_init times both on the engine's own mesh, agrees on the result across the ranks, and
  * this call -- the one a driver should make at batch end -- runs the quicker one.  Read the decision
  * with pumitally_get_option("exchange_choice") (0 all-reduce, 1 reduce-scatter) and the two times with

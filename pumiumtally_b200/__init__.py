@@ -1,6 +1,6 @@
-"""B200-native unstructured-mesh track-length tally engine.
+"""H100-native unstructured-mesh track-length tally engine.
 
-The product is ``lib/libpumitally.so`` (CUDA kernels for sm_100a + C++ host side,
+The product is ``lib/libpumitally.so`` (CUDA kernels for sm_90a + C++ host side,
 C ABI in ``include/pumitally_c.h``, C++ facade ``pumitally::PumiTally``).  This
 package holds its sources (``csrc/``), the in-tree build, a ctypes mirror of the
 reference interface (``tally.PumiTally``) and the synthetic mesh / particle

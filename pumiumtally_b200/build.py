@@ -1,6 +1,6 @@
 """In-tree build of libpumitally.so (CUDA kernels + C++ host side + C ABI).
 
-``nvcc`` cross-compiles for sm_100a without a GPU, so this runs in the CPU
+``nvcc`` cross-compiles for sm_90a without a GPU, so this runs in the CPU
 container; the resulting ``pumiumtally_b200/lib/libpumitally.so`` travels to
 the GPU box with the repo snapshot (it is git-ignored, not gpurun-ignored).
 """
@@ -35,7 +35,7 @@ SOURCES = [
 ]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fopenmp,-pthread,-Wall,-fvisibility=default",
     "-I", os.path.join(ROOT, "include"),
@@ -69,7 +69,8 @@ def build_library(force: bool = False, verbose: bool = False, experiments: bool 
     nvcc = _nvcc()
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".hpp", ".cuh", ".h"))]
     headers += [os.path.join(ROOT, "include", "pumitally_c.h"),
-                os.path.join(ROOT, "include", "pumitally", "PumiTally.h")]
+                os.path.join(ROOT, "include", "pumitally", "PumiTally.h"),
+                os.path.abspath(__file__)]  # NVCC_FLAGS live here: a change of flags or target rebuilds everything
     newest_header = max(os.path.getmtime(h) for h in headers)
     objs, relink = [], force or not os.path.exists(lib)
     for src in sources:
@@ -84,7 +85,7 @@ def build_library(force: bool = False, verbose: bool = False, experiments: bool 
             relink = True
     if relink:
         cmd = [nvcc, "-shared", "-o", lib, *objs, "-Xcompiler", "-fopenmp,-pthread", "-lgomp", "-ldl", "-lz",
-               "-gencode", "arch=compute_100a,code=sm_100a"]
+               "-gencode", "arch=compute_90a,code=sm_90a"]
         if verbose:
             print(" ".join(cmd), file=sys.stderr)
         subprocess.check_call(cmd)

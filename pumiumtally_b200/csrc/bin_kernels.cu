@@ -32,7 +32,7 @@ __device__ __forceinline__ int32_t cell_of(const SeedGrid &g, double x, double y
 // re-sourced particles beforehand); the key is then the stored position
 // mid != nullptr: the key is the cell of the track's midpoint (origin + dest) / 2 instead of its start:
 // the tets a track touches then lie within half a track length of the key cell, which shrinks the halo of
-// the in-flight window (the working set that has to stay in L2) -- profiles/r02/README.md, c5.
+// the in-flight window (the working set that has to stay in L2).
 __global__ void bin_count_kernel(SeedGrid g, const double *__restrict__ origin, const ParticleState *__restrict__ state,
                                  const double *__restrict__ mid, const int8_t *__restrict__ flying, int32_t begin,
                                  int32_t end, int32_t *__restrict__ pcell, unsigned int *__restrict__ count) {
@@ -146,11 +146,15 @@ __global__ void bin_pack_kernel(const int32_t *__restrict__ pcell, int32_t begin
   const unsigned long long tail = (unsigned long long)(uint32_t)i |
                                   ((unsigned long long)(((uint32_t)s.elem & kIdMask) | (moved ? 0x80000000u : 0u)) << 32);
   PackedRow *row = rows + atomicAdd(cursor + c, 1u);
-  asm volatile("st.global.L1::no_allocate.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(row),
+  asm volatile(
+      "st.global.L1::no_allocate.v2.b64 [%0], {%1,%2};\n\t"
+      "st.global.L1::no_allocate.v2.b64 [%0+16], {%3,%4};" ::"l"(row),
                "l"(__double_as_longlong(ox)), "l"(__double_as_longlong(oy)), "l"(__double_as_longlong(oz)),
                "l"(__double_as_longlong(dx))
                : "memory");
-  asm volatile("st.global.L1::no_allocate.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(reinterpret_cast<char *>(row) + 32),
+  asm volatile(
+      "st.global.L1::no_allocate.v2.b64 [%0], {%1,%2};\n\t"
+      "st.global.L1::no_allocate.v2.b64 [%0+16], {%3,%4};" ::"l"(reinterpret_cast<char *>(row) + 32),
                "l"(__double_as_longlong(dy)), "l"(__double_as_longlong(dz)), "l"(__double_as_longlong(w)), "l"(tail)
                : "memory");
 }

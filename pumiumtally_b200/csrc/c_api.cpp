@@ -272,6 +272,6 @@ int64_t pumitally_debug_stage(const double *origin, const double *dest, int8_t *
   }
 }
 
-const char *pumitally_version(void) { return "pumitally-b200 0.2 (sm_100a)"; }
+const char *pumitally_version(void) { return "pumitally-b200 0.2 (sm_90a)"; }
 
 }  // extern "C"

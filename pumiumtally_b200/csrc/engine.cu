@@ -320,8 +320,8 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   // is walked once per bin with the flying flags masked down to that bin's particles and the tally pointed
   // at that bin's flux array -- the walk kernels themselves are the unfiltered ones.  One more pass (array
   // nbins_, never reported) flies the particles whose bin is outside [0, nbins_): they move, unscored.
-  // The streaming kernel pays for every particle of the range in every pass, flying or not (measured on c2:
-  // 2.7 ms unfiltered, 5.5 ms with 4 bins, 10.3 ms with 8); the packed kernel's sort pass keeps only the flying
+  // The streaming kernel pays for every particle of the range in every pass, flying or not; the packed kernel's
+  // sort pass keeps only the flying
   // ones, so its passes cost what their members cost.  Unless the caller has fixed the kernel, binned moves use it.
   const int saved_variant = move_variant_, saved_tag = move_tag_;
   if (auto_variant_ && d_weights) {
@@ -657,12 +657,10 @@ int Engine::move_to_next_location(const double *origin, const double *dest, int8
   PTB_CUDA_OK(cudaSetDevice(device_));
   begin_move();
   // Pipeline stage size, unless the caller set it: 512 Ki particles for the streaming kernel (shortest tail); the
-  // sorted kernels pay a fixed price per launch (a scan over all seed-grid cells), so their stages are 2 Mi
-  // (c5 share, 50 M particles per GPU from pageable arrays: 58.6 ms per move with 1 Mi stages, 86.5 ms with 512 Ki).
+  // sorted kernels pay a fixed price per launch (a scan over all seed-grid cells), so their stages are 2 Mi.
   const int32_t chunk = chunk_;
   // The auto-tuner compares kernel times; in a host move the sorted kernel it may prefer would also need the
-  // larger stages, whose longer tail costs more than the kernel wins (c2 from pageable arrays: 11.1 ms against
-  // 9.4 ms per move).  So a host move of more than one stage keeps the engine's base kernel and does not take
+  // larger stages, whose longer tail can cost more than the kernel wins.  So a host move of more than one stage keeps the engine's base kernel and does not take
   // part in the exploration; the tuner works for device-pointer moves and single-stage host moves (c4's 1 M tracks).
   if (auto_variant_ && variant_is_packed(move_variant_) && !variant_is_packed(variant_) && n_ > chunk_) {
     move_variant_ = variant_;
@@ -1287,11 +1285,11 @@ int Engine::get_stats(EngineStats *out) {
   return 0;
 }
 
-// The tet table of config c2 (128 MB) still half-fits the L2, and streaming the particles in
-// storage order through the TMA stages is fastest.  Once the table is several times the L2
-// (config c5: 1.26 GB) nearly every record fetch is a random 32-byte DRAM access; processing the
-// particles in spatial order (binning pass + gather staging) then pays for itself twice over
-// (profiles/r01/README.md, section q).
+// While the tet table still half-fits the L2, streaming the particles in storage order through the TMA
+// stages is fastest.  Once the table is more than twice the L2, most record fetches are random 32-byte
+// DRAM accesses and processing the particles in spatial order (binning pass + gather staging) pays for
+// itself: on an H100 (50 MB of L2) that is already config c2 (128 MB of records; 6.3 ms per move against
+// 18.2 ms streaming, 400 W card) and config c5 (1.26 GB).
 int Engine::choose_variant() const {
   int l2 = 0;
   cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, device_);
@@ -1372,7 +1370,7 @@ int Engine::set_option(const std::string &name, int64_t v) {
     chunk_ = int32_t(std::min<int64_t>(v, INT_MAX)) & ~1023;  // keeps every range 16-byte aligned
     chunk_user_set_ = true;
   } else if (name == "die_split") {
-    // Experiment, off by default (measured: c4 5 % slower, c5 1.6 % faster, c2 unchanged -- profiles/r02/README.md):
+    // Experiment, off by default:
     // the SMs of each L2 partition take the sorted particles from their own end of the sequence.
     die_split_ = v != 0;
     if (die_split_) {
@@ -1478,14 +1476,14 @@ int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
   PTB_CUDA_OK(cudaEventCreate(&ev_ar1_));
   PTB_CUDA_OK(cudaMemsetAsync(d_scratch_, 0, size_t(mesh_.ntets) * sizeof(double), compute_));
   if (nccl_allreduce_sum_f64(nccl_comm_, d_scratch_, d_flux_global_, size_t(mesh_.ntets), compute_)) return 1;
-  // ... and so does every other collective the first time it is used (measured: 0.86 s for the first
-  // ncclReduceScatter on 8 GPUs): warm up the reduce-scatter / all-gather pair of reduce_tally_to_owners too.
+  // ... and so does every other collective the first time it is used (the first ncclReduceScatter can take
+  // most of a second): warm up the reduce-scatter / all-gather pair of reduce_tally_to_owners too.
   // d_flux_ is all zeros here or holds this rank's tally, which the exchange does not modify.
   if (nccl_reduce_scatter_sum_f64(nccl_comm_, d_flux_, d_flux_global_ + size_t(rank_) * share_, share_, compute_)) return 1;
   if (nccl_all_gather_f64(nccl_comm_, d_flux_global_ + size_t(rank_) * share_, d_flux_global_, share_, compute_)) return 1;
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   // Which of the two batch-end exchanges is quicker depends on the array size and on what NCCL picks for it
-  // (measured on 8 B200s: 8 MB of flux -- all-reduce 0.10 ms, reduce-scatter 4.3 ms; 79 MB -- 0.9 ms and 0.43 ms):
+  // (either can be the quicker by a large factor):
   // time both on this mesh and let exchange_tally() use the quicker one.  The times are summed over the ranks
   // so that every rank takes the same decision.
   double t[2] = {1e30, 1e30};

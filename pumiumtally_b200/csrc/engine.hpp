@@ -142,7 +142,7 @@ class Engine {
   void begin_move();
   int block_ = 128;
   bool chunk_user_set_ = false;
-  int32_t chunk_ = 1 << 19;  // particles per H2D/compute pipeline stage (c2 from pageable arrays: 9.28 ms per move; 2^18: 10.0, 2^20: 9.5, 2^21: 10.9)
+  int32_t chunk_ = 1 << 19;  // particles per H2D/compute pipeline stage
   // Seed grid for relocation / localisation.  The reference walks straight from the particle's old
   // position to the new one and stops at the hull if that segment leaves the mesh -- on a mesh with
   // concavities or voids even when the new position is inside.  Starting from a seed cell instead
@@ -229,8 +229,8 @@ class Engine {
   int ensure_patch_buffers(int nchunks);
   int move_direct(const double *origin, const double *dest, int8_t *flying, const double *weights, int nchunks);
   // Page-locked caller arrays (pinned by the caller, or by option register_host): see move_pinned().
-  // Off by default: on the measured box the positions travelling back (24 B per particle, device->host)
-  // slow the uploads down more than the saved host work buys (profiles/r02/README.md).
+  // Off by default: the positions travelling back (24 B per particle, device->host) can slow the uploads
+  // down more than the saved host work buys.
   bool pinned_path_ = false;
   double *h_pos_ = nullptr;            // pinned mirror of the device's particle positions [3N]
   bool pos_mirror_valid_ = false;

@@ -1,4 +1,4 @@
-// Measured alternatives to the product walk kernels (DESIGN.md section 4, profiles/r01/README.md):
+// Measured alternatives to the product walk kernels (DESIGN.md section 4):
 // thread-per-particle TMA fetch (1), four lanes per particle (2), persistent kernel without /
 // with other L2 policies (3-7, 13), binned gather without L1 (15, 17), compact layout +
 // edge-function walk (20-23), packed rows with L1-allocating loads (25, 26).  All share the

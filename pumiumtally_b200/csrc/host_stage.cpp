@@ -88,9 +88,8 @@ void HostPool::begin(const std::function<void(int)> &fn) {
 }
 
 // The caller must not spin for the length of a job: a spinning thread on the sibling hyperthread of a
-// worker halves that worker's speed, and the slowest worker sets the pace (measured: 2x on the whole
-// pass).  A short spin catches jobs that are about to finish, then it sleeps until the last worker
-// signals.
+// worker slows that worker down, and the slowest worker sets the pace of the whole pass.  A short spin
+// catches jobs that are about to finish, then it sleeps until the last worker signals.
 void HostPool::end() {
   if (!in_flight_) return;
   for (int spins = 0; spins < 200 && done_.load(std::memory_order_acquire) != n_; ++spins) _mm_pause();

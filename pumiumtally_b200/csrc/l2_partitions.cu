@@ -1,8 +1,8 @@
-// Which SMs share an L2 partition?  (B200: two dies, one partition each; every partition keeps its own copy of
-// what its SMs read -- scripts/l2_probe3.cu, profiles/r02/z_l2_probe_die_map.txt.)  One SM reads a set of
+// Which SMs share an L2 partition?  (On a GPU whose L2 partitions each cache what their own SMs read, a line held
+// only by the far partition costs a longer trip; on an H100 this probe finds no two groups.)  One SM reads a set of
 // disjoint regions; then every SM chases a pointer chain through "its" region for the first time: SMs of the
-// warming SM's partition see L2-hit latency (~290 cycles), the others pay the trip to the other partition
-// (~470).  The engine uses the map to give each partition its own end of a sorted particle sequence
+// warming SM's partition see L2-hit latency, the others pay the trip to the other partition.  The engine
+// uses the map to give each partition its own end of a sorted particle sequence
 // (walk_persist.cuh, "die split"); when the result is not clearly two groups the split stays off.
 #include <algorithm>
 #include <cstdint>

@@ -43,7 +43,7 @@ __device__ __forceinline__ void tally_add(double *ptr, double v) {
 // Experiment (north_star: "warp-aggregated atomicAdd to cut contention"): lanes of the warp that tally
 // into the same tet in this step are found with match.any, their contributions are summed with
 // shuffles and one lane issues the reduction.  Called by every converged lane; `on` = this lane has
-// something to add.  Measured in profiles/r02 (variants 28, 29); not used by the product kernels.
+// something to add.  Experiment variants 28, 29; not used by the product kernels.
 __device__ __forceinline__ void tally_add_aggregated(double *flux, int32_t e, double v, bool on) {
   const unsigned act = __activemask();
   const int lane = threadIdx.x & 31;
@@ -193,9 +193,10 @@ struct VertexRec;
 struct TetStart;
 
 // Persistent per-particle state: position + parent element in one 32-byte, 32-byte aligned
-// record = one DRAM/L2 sector.  A particle is read with one 256-bit load and written back with
-// one full-sector 256-bit store (no read-modify-write fill), in whatever order particles are
-// processed.  (Reference: DPS members origin + the tracer's elem_ids, PumiTallyImpl.h:39-41.)
+// record = one DRAM/L2 sector.  A particle is read with two 128-bit loads of the same sector and
+// written back with two 128-bit stores that cover the whole sector (no read-modify-write fill), in
+// whatever order particles are processed.  (Reference: DPS members origin + the tracer's elem_ids,
+// PumiTallyImpl.h:39-41.)
 struct alignas(32) ParticleState {
   double x, y, z;
   int32_t elem;
@@ -206,7 +207,10 @@ static_assert(sizeof(ParticleState) == 32, "ParticleState must be one sector");
 PTB_HD ParticleState load_state(const ParticleState *p) {
 #if defined(__CUDA_ARCH__)
   unsigned long long a, b, c, d;
-  asm volatile("ld.global.L1::no_allocate.v4.b64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+  asm volatile(
+      "ld.global.L1::no_allocate.v2.b64 {%0,%1}, [%4];\n\t"
+      "ld.global.L1::no_allocate.v2.b64 {%2,%3}, [%4+16];"
+      : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
   ParticleState s;
   s.x = __longlong_as_double((long long)a);
   s.y = __longlong_as_double((long long)b);
@@ -220,7 +224,9 @@ PTB_HD ParticleState load_state(const ParticleState *p) {
 }
 PTB_HD void store_state(ParticleState *p, double x, double y, double z, int32_t elem) {
 #if defined(__CUDA_ARCH__)
-  asm volatile("st.global.L1::no_allocate.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(p),
+  asm volatile(
+      "st.global.L1::no_allocate.v2.b64 [%0], {%1,%2};\n\t"
+      "st.global.L1::no_allocate.v2.b64 [%0+16], {%3,%4};" ::"l"(p),
                "l"((unsigned long long)__double_as_longlong(x)), "l"((unsigned long long)__double_as_longlong(y)),
                "l"((unsigned long long)__double_as_longlong(z)), "l"((unsigned long long)(uint32_t)elem)
                : "memory");

@@ -1,4 +1,4 @@
-// sm_100a kernels of the track-length tally engine: the kernels the engine chooses between.
+// sm_90a kernels of the track-length tally engine: the kernels the engine chooses between.
 //
 // One fused kernel per particle range does what the reference spreads over
 // K1..K12 of SURVEY.md section 2b: the "set dest" kernels
@@ -22,8 +22,8 @@ namespace ptb {
 namespace {
 
 // ---------------------------------------------------------------- variant 0
-// Thread per particle; the 128-byte record arrives as four 256-bit loads
-// (LDG.E.ENL2.256), one per face.
+// Thread per particle; the 128-byte record arrives as four 32-byte sectors
+// (two 128-bit loads each), one per face.
 
 __global__ void __launch_bounds__(256) walk_ldg_kernel(const WalkParams P) {
   const int i = P.begin + blockIdx.x * blockDim.x + threadIdx.x;
@@ -320,7 +320,11 @@ cudaError_t launch_sum_flying_weights(const int8_t *flying, const double *weight
                                       double *total, cudaStream_t stream) {
   if (end <= begin) return cudaSuccess;
   const int n = end - begin;
-  sum_flying_weights_kernel<<<std::min((n + 255) / 256, 1184), 256, 0, stream>>>(flying, weights, begin, end, total);
+  // grid-stride sum: at most 8 blocks of 256 per SM of the current device
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 1;
+  sum_flying_weights_kernel<<<std::min((n + 255) / 256, 8 * sms), 256, 0, stream>>>(flying, weights, begin, end, total);
   return cudaGetLastError();
 }
 

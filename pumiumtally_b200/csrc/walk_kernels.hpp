@@ -1,4 +1,4 @@
-// Launch interface of the sm_100a walk/tally kernels (walk_kernels.cu).
+// Launch interface of the sm_90a walk/tally kernels (walk_kernels.cu).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -8,13 +8,13 @@
 
 namespace ptb {
 
-// Values are stable (profiles/ refer to them); the gaps are experiments that were measured,
+// Values are stable (options and tests refer to them); the gaps are experiments that were measured,
 // lost and removed (9/10 other refill thresholds, 11/12/14 cooperative transposed fetch, 18).
 // libpumitally.so contains the four kernels the engine chooses between -- 0, 8, 16, 24; the other
 // numbers are measured alternatives compiled only into libpumitally_exp.so
 // (experiments/walk_experiments.cu, build flag PTB_EXPERIMENTS).
 enum WalkVariant : int {
-  kVariantLdg = 0,    // thread per particle, 4 x 256-bit loads of the tet record (first correct path)
+  kVariantLdg = 0,    // thread per particle, the tet record as 4 sectors of two 128-bit loads (first correct path)
   kVariantBulk = 1,   // thread per particle, record staged in smem by cp.async.bulk + mbarrier
   kVariantQuad = 2,   // 4 lanes per particle (lane per face), coalesced 32 B loads
   kVariantPersist = 3,               // persistent warps, TMA-staged particle chunks, per-lane refill

@@ -29,9 +29,13 @@ __device__ __forceinline__ void flush_counters(const WalkParams &P, const Counte
   }
 }
 
+// One 32-byte face sector as two 128-bit loads (the widest global access on sm_90), issued back to back.
 __device__ __forceinline__ void load_face_256(const double *p, double &a, double &b, double &c,
                                               double &d) {
-  asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(p));
+  asm volatile(
+      "ld.global.nc.v2.f64 {%0,%1}, [%4];\n\t"
+      "ld.global.nc.v2.f64 {%2,%3}, [%4+16];"
+      : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(p));
 }
 
 constexpr int kRowBytes = 144;
@@ -71,8 +75,7 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
 // ---------------------------------------------------------------- variant 3
 // Persistent warps with per-lane refill.  Track lengths are roughly geometric
 // and relocation walks are ~10x longer than tally walks, so with one particle
-// per thread a warp idles most of its lanes (measured: 3.9 of 32 lanes active
-// per instruction).  Here every warp owns two shared-memory stages of 32
+// per thread a warp idles most of its lanes.  Here every warp owns two shared-memory stages of 32
 // particles each, filled asynchronously by the TMA unit (cp.async.bulk of the
 // SoA/AoS slices, completion on an mbarrier); a lane that finishes its particle
 // takes the next slot of the current stage in the same loop iteration, and
@@ -174,13 +177,12 @@ __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedR
 }
 
 // Fetch modes of the persistent kernel (how a lane gets its 128-byte tet record):
-//   0  four plain 256-bit loads
+//   0  four plain 32-byte sector loads (two 128-bit loads each)
 //   1  as 0, tet loads carry an L2 evict_last policy and skip L1; the particle stream
 //      (staging copies, state stores) is evict_first -- keeps the tet table L2-resident
 //   2  as 1, plus the L2::128B prefetch size (first sector miss pulls the whole line)
 //   3  one cp.async.bulk of 128 B per lane into a shared-memory row (policies as 1)
-//   (4 was a cooperative quad-load + shared-memory transpose; measured 4.9 ms vs 3.0 ms on c2,
-//      profiles/r01/README.md section c/d, and removed)
+//   (4 was a cooperative quad-load + shared-memory transpose: slower, removed)
 //   5  as 1 but the tet loads allocate in L1 (worth it once particles are processed in
 //      spatial order and neighbouring lanes/warps revisit the same records)
 //   6  compact layout + edge-function exit test (walk_compact.cuh): one 32-byte TetLinks sector and
@@ -220,13 +222,16 @@ template <int FETCH>
 __device__ __forceinline__ void load_face(const double *p, uint64_t pol, double &a, double &b,
                                           double &c, double &d) {
   if constexpr (FETCH == kFetchPolicy || FETCH == kFetchPolicyAgg)
-    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f64 {%0,%1,%2,%3}, [%4], %5;"
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%4], %5;\n\t"
+                 "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%2,%3}, [%4+16], %5;"
         : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(p), "l"(pol));
   else if constexpr (FETCH == kFetchPolicyL1 || FETCH == kFetchPolicyL1Agg)
-    asm volatile("ld.global.nc.L2::cache_hint.v4.f64 {%0,%1,%2,%3}, [%4], %5;"
+    asm volatile("ld.global.nc.L2::cache_hint.v2.f64 {%0,%1}, [%4], %5;\n\t"
+                 "ld.global.nc.L2::cache_hint.v2.f64 {%2,%3}, [%4+16], %5;"
         : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(p), "l"(pol));
   else if constexpr (FETCH == kFetchPolicy128)
-    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.L2::128B.v4.f64 {%0,%1,%2,%3}, [%4], %5;"
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.L2::128B.v2.f64 {%0,%1}, [%4], %5;\n\t"
+                 "ld.global.nc.L1::no_allocate.L2::cache_hint.L2::128B.v2.f64 {%2,%3}, [%4+16], %5;"
         : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(p), "l"(pol));
   else
     load_face_256(p, a, b, c, d);
@@ -323,9 +328,8 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r
   advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back, c, true);
 }
 
-// Lean crossing step.  ncu's source view of plane_step() (profiles/r02/README.md, section kernel) shows the
-// compiler sinking the third record load below the arithmetic on the first two -- its latency is then
-// paid a second time (14 % of all stall samples) -- and ~330 warp instructions per warp step.  Here the
+// Lean crossing step.  The compiler can sink the third record load of plane_step() below the arithmetic on
+// the first two, so its latency is paid a second time.  Here the
 // three loads are one asm block (issued back to back, before any use), the neighbour is decoded once,
 // the parallel-face tolerance is computed once per step, and the ray target is not carried in registers
 // (end_ray<true> re-reads it from the caller's array), which makes room for the loads in flight.
@@ -334,17 +338,23 @@ __device__ __forceinline__ void load_faces3(const double *p0, const double *p1, 
                                             double (&q)[3][4]) {
   if constexpr (L1ALLOC)
     asm volatile(
-        "ld.global.nc.L2::cache_hint.v4.f64 {%0,%1,%2,%3}, [%12], %15;\n\t"
-        "ld.global.nc.L2::cache_hint.v4.f64 {%4,%5,%6,%7}, [%13], %15;\n\t"
-        "ld.global.nc.L2::cache_hint.v4.f64 {%8,%9,%10,%11}, [%14], %15;"
+        "ld.global.nc.L2::cache_hint.v2.f64 {%0,%1}, [%12], %15;\n\t"
+        "ld.global.nc.L2::cache_hint.v2.f64 {%2,%3}, [%12+16], %15;\n\t"
+        "ld.global.nc.L2::cache_hint.v2.f64 {%4,%5}, [%13], %15;\n\t"
+        "ld.global.nc.L2::cache_hint.v2.f64 {%6,%7}, [%13+16], %15;\n\t"
+        "ld.global.nc.L2::cache_hint.v2.f64 {%8,%9}, [%14], %15;\n\t"
+        "ld.global.nc.L2::cache_hint.v2.f64 {%10,%11}, [%14+16], %15;"
         : "=d"(q[0][0]), "=d"(q[0][1]), "=d"(q[0][2]), "=d"(q[0][3]), "=d"(q[1][0]), "=d"(q[1][1]), "=d"(q[1][2]),
           "=d"(q[1][3]), "=d"(q[2][0]), "=d"(q[2][1]), "=d"(q[2][2]), "=d"(q[2][3])
         : "l"(p0), "l"(p1), "l"(p2), "l"(pol));
   else
     asm volatile(
-        "ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f64 {%0,%1,%2,%3}, [%12], %15;\n\t"
-        "ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f64 {%4,%5,%6,%7}, [%13], %15;\n\t"
-        "ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f64 {%8,%9,%10,%11}, [%14], %15;"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%12], %15;\n\t"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%2,%3}, [%12+16], %15;\n\t"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%4,%5}, [%13], %15;\n\t"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%6,%7}, [%13+16], %15;\n\t"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%8,%9}, [%14], %15;\n\t"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%10,%11}, [%14+16], %15;"
         : "=d"(q[0][0]), "=d"(q[0][1]), "=d"(q[0][2]), "=d"(q[0][3]), "=d"(q[1][0]), "=d"(q[1][1]), "=d"(q[1][2]),
           "=d"(q[1][3]), "=d"(q[2][0]), "=d"(q[2][1]), "=d"(q[2][2]), "=d"(q[2][3])
         : "l"(p0), "l"(p1), "l"(p2), "l"(pol));
@@ -369,9 +379,8 @@ __device__ __forceinline__ void plane_step_lean(const WalkParams &P, int my_i, R
   int32_t nb, bk;
   decode_lean(sc, r.e, nb, bk);
   // The next tet is known here, ~80 instructions (a division, the tally, the loop overhead) before its
-  // record is asked for: start the line on its way from DRAM to L2 now.  Half of the record fetches miss
-  // in L2 on config c2 and a warp issues only one instruction every ~14 cycles, so the prefetch has
-  // roughly a DRAM latency of head start.
+  // record is asked for: start the line on its way from DRAM to L2 now.  Once the tet table is larger
+  // than the L2 many record fetches miss there, and the prefetch gives such a miss a head start.
   if (nb >= 0 && sc.bnum < sc.bden)
     asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(P.tets + nb));
   advance<true>(P, my_i, r, exit_parameter(sc), nb, bk, c, true);
@@ -382,7 +391,8 @@ constexpr int kPlaneMode = -2;  // EdgeRay::dv of a ray that is finishing on the
 
 __device__ __forceinline__ void ld256_b64(const void *p, uint64_t pol, unsigned long long &a,
                                           unsigned long long &b, unsigned long long &c, unsigned long long &d) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.b64 {%0,%1,%2,%3}, [%4], %5;"
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%4], %5;\n\t"
+               "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%2,%3}, [%4+16], %5;"
                : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p), "l"(pol));
 }
 
@@ -545,9 +555,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const WalkPar
   const int claim_run = GATHER ? min(max(P.claim_run, 1), kClaimRun) : 1;
   int run_base = 0, run_next = 0, run_end = 0, ids0 = 0, ids1 = 0;
   int pend_base = -1, pend0 = 0, pend1 = 0;
-  // Die split (sorted modes only).  A B200's L2 is two partitions, one per die, and each keeps its own copy of
-  // every line its SMs touch (profiles/r02/z_l2_probe_die_map.txt: a line only the other die has read costs 467
-  // cycles instead of 290, and a table read by all SMs stays resident only up to half the L2).  When all SMs
+  // Die split (sorted modes only).  On a GPU whose L2 is two partitions that each cache the lines their own SMs
+  // touch, a line only the other partition holds costs a longer trip.  When all SMs
   // work through the sorted particles front to back, both partitions hold the same window of the mesh.  Here
   // the SMs of partition 0 take chunks from the front of the sequence and those of partition 1 from its own
   // start further back (the sequence is cut in proportion to the SM counts), so each partition caches only its

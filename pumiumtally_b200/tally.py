@@ -106,7 +106,7 @@ def _host_f64(a, what):
 
 
 class PumiTally:
-    """Track-length tally engine on one B200.
+    """Track-length tally engine on one H100.
 
     ``PumiTally(mesh_filename, num_particles)`` follows the reference constructor;
     ``PumiTally.from_arrays(coords, tet2vert, num_particles)`` takes the mesh in memory.

@@ -34,5 +34,5 @@ for run in runs:
     segs = st1["segments"] - st0["segments"]
     ms = e0.elapsed_time(e1)
     print(json.dumps({"mode": mode, "variant": variant, "ms": round(ms, 3), "gseg_s": round(segs / ms / 1e6, 2),
-                      "frac": round((128 * segs + 89 * (st1["tracks"] - st0["tracks"])) / (ms * 1e-3) / 6574.1e9, 3)}), flush=True)
+                      "frac": round((128 * segs + 89 * (st1["tracks"] - st0["tracks"])) / (ms * 1e-3) / 3350e9, 3)}), flush=True)
     del eng

@@ -1,8 +1,9 @@
 """Regenerates the committed golden fixtures.
 
 t1_known_answers.json is transcribed from the reference's own known-answer test
-(/root/reference/test/test_pumi_tally_impl_methods.cpp; line numbers inside the file) -- it is not
-generated.  c1_oracle.npz is produced here by the CPU oracle (oracle/umtally_oracle.c), which is
+(test/test_pumi_tally_impl_methods.cpp of the reference; line numbers inside the file) -- it is not
+generated, and neither is reference_facade_symbols.json: the undefined symbols of the
+tests/test_abi_symbols.py translation unit compiled against the reference's PumiTally.h.  c1_oracle.npz is produced here by the CPU oracle (oracle/umtally_oracle.c), which is
 pinned against t1_known_answers.json and the brute-force integrator by tests/test_oracle_golden.py.
 
     python tests/golden/make_golden.py

@@ -1081,9 +1081,23 @@ def _full_size_oracle_parity(cfg_name, n, steps=2, engine_opts=None):
 
 
 def test_config_c2_full_size_oracle_parity():
-    """BASELINE configs[1]: 998,250 tets, 10 M particles, element for element against the oracle."""
+    """BASELINE configs[1]: 998,250 tets, 10 M particles, element for element against the oracle.  The engine's
+    own kernel: the binned one once the 128 MB tet table exceeds twice the L2 (an H100's 50 MB), else the
+    streaming kernel or the packed one the auto-tuner may prefer."""
+    import torch
+
     eng, _ = _full_size_oracle_parity("c2", CONFIGS["c2"]["particles"])
-    assert eng.get_option("variant") in (8, 24)
+    table = eng.num_elements * 128  # one 128-byte record per tet
+    l2 = torch.cuda.get_device_properties(0).L2_cache_size
+    assert eng.get_option("variant") in ((16,) if table > 2 * l2 else (8, 24))
+
+
+def test_config_c2_full_size_oracle_parity_streaming_kernel():
+    """The same with the streaming kernel pinned (variant 8).  The engine picks it for tet tables up to twice
+    the L2; where c2's 128 MB table is larger than that (an H100) this keeps it checked at full size against
+    a table that does not fit the L2."""
+    eng, _ = _full_size_oracle_parity("c2", CONFIGS["c2"]["particles"], engine_opts={"variant": 8})
+    assert eng.get_option("variant") == 8
 
 
 def test_config_c4_full_size_oracle_parity():
@@ -1145,12 +1159,19 @@ def test_walks_cut_short_by_the_crossing_limit_are_reported_and_recoverable(vari
 def test_die_split_of_the_sorted_kernels_keeps_results(variant):
     """Option die_split=1: the SMs of each L2 partition take the sorted particles from their own end of the
     sequence (two ticket counters + work stealing); every particle is still walked exactly once."""
+    import torch
+
     coords, t2v, wl = box_case((8, 8, 8), 60_000)
     e = gpu_engine(variant, chunk=16384)(coords, t2v, wl.n)
     e.set_option("die_split", 1)
     assert e.get_option("die_split") == 1
     n0 = e.get_option("l2_partition0_sms")
-    assert n0 == 0 or 40 <= n0 <= 108  # a B200: 76 of 148; 0 = no two groups found (the split then stays off)
+    nsms = torch.cuda.get_device_properties(0).multi_processor_count
+    # A map is only kept when SM 0's partition holds 40-60 % of the SMs; 0 = no two groups found and the split
+    # stays off.  On an H100 the latency probe finds no two groups (n0 == 0 of 132 SMs), so there this test only
+    # checks that switching the option on leaves the results right; the split itself is exercised only on a GPU
+    # whose probe returns a map.
+    assert n0 == 0 or 2 * nsms <= 5 * n0 <= 3 * nsms
     run_workload(e, OraclePumiTally(coords, t2v, wl.n), wl, steps=3, label=f"die split v{variant}")
     st = e.stats()
     assert st["lost"] == 0 and st["tracks"] > 0
