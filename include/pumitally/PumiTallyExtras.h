@@ -36,6 +36,17 @@ inline int MoveToNextLocationBinned(const PumiTally &tally, double *particle_ori
                                                 weights, bins, size);
 }
 
+// Scores: `nscores` responses per particle, tallied in one walk; MoveToNextLocationScored adds
+// length * weights[i] * responses[i*nscores + k] to score k (see pumitally_set_scores in pumitally_c.h).
+// bins may be nullptr (no score filter).
+inline int SetScores(const PumiTally &tally, int32_t nscores) { return pumitally_set_scores(engine_of(tally), nscores); }
+inline int MoveToNextLocationScored(const PumiTally &tally, double *particle_origin, double *particle_destinations,
+                                    int8_t *flying, double *weights, const double *responses, const int32_t *bins,
+                                    int32_t size) {
+  return pumitally_move_to_next_location_scored(engine_of(tally), particle_origin, particle_destinations, flying,
+                                                weights, responses, bins, size);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

@@ -122,7 +122,8 @@ int pumitally_set_output_name(pumitally_engine *e, const char *filename);
  * (crossing limit per walk; 0 = number of elements + 16, the default), "l2_fetch", "autotune"
  * (1 = default: while "variant" is automatic the engine times the streaming and the sorted/packed
  * kernel on moves 1-4 of every 64 and keeps the faster one).  Read-only: "launches", "staged",
- * "stage_host_us", "stage_sent_bytes". */
+ * "stage_host_us", "stage_sent_bytes", "scores", "walk_blocks_per_sm" (blocks per SM of the last
+ * persistent walk kernel launched). */
 int pumitally_set_option(pumitally_engine *e, const char *name, int64_t value);
 int64_t pumitally_get_option(const pumitally_engine *e, const char *name);
 
@@ -146,10 +147,12 @@ int pumitally_set_state_device(pumitally_engine *e, const double *d_xyz, const i
                                int32_t first, int32_t count, void *stream);
 int pumitally_get_state_device(pumitally_engine *e, double *d_xyz, int32_t *d_elem, int32_t first,
                                int32_t count, void *stream);
-/* raw flux in the caller's element numbering into device memory d_out[num_elements] */
+/* raw flux in the caller's element numbering into device memory d_out[num_elements] (with score bins
+ * and scores: every bin and score, [bin][score][element]) */
 int pumitally_get_flux_device(pumitally_engine *e, double *d_out, void *stream);
 /* device address of the raw flux array (double[num_elements]); NOTE: in the engine's internal
- * (spatially sorted) element order -- use pumitally_get_flux for the caller's numbering */
+ * (spatially sorted) element order -- use pumitally_get_flux for the caller's numbering.  With score
+ * bins and scores the array is [bin][element][stride], see pumitally_set_scores */
 double *pumitally_flux_device_ptr(pumitally_engine *e);
 int pumitally_synchronize(pumitally_engine *e);
 
@@ -200,6 +203,46 @@ int pumitally_move_to_next_location_device_binned(pumitally_engine *e, const dou
                                                   const double *d_destinations, const int8_t *d_flying,
                                                   const double *d_weights, const int32_t *d_bins,
                                                   int32_t size, void *stream);
+
+/* ---- additive: scores (several responses per track, one walk) --------------
+ * An OpenMC tally on a mesh filter usually carries several scores (flux, fission, heating, absorption,
+ * ...).  The track-length estimate of score x in element e is the sum of l * w * Sigma_x(E) over the
+ * segments in e, and within one move a particle keeps its material and energy, so Sigma_x is one number
+ * per particle and move: a response.  pumitally_set_scores(e, nscores), 1 <= nscores <= 8, gives every
+ * score bin nscores flux arrays (any other value returns non-zero and changes nothing); it resets the
+ * tally, combines with pumitally_set_score_bins in either order and is refused after
+ * pumitally_comm_init.  Read it back with pumitally_get_scores or the option "scores".
+ * The scored moves take responses double[nscores * num_particles], particle-major (r[i*nscores + k],
+ * never NULL), and bins int32[num_particles] or NULL with the score filter's meaning.  Each segment of
+ * length l of particle i in element e adds l * w[i] * r[i*nscores + k] to score k of the particle's
+ * bin, for every k; a bin outside [0, nbins) flies and scores nothing.  Everything else is the plain
+ * move: relocation, clipping at the hull, flying[] zeroed by the host version, the same statistics, and
+ * parent elements and positions identical to a plain move with the same origin, dest, flying and
+ * weights.  A non-finite w * r is treated like a non-finite weight: zero-length flight, counted as
+ * lost, nothing tallied.  With nscores = 1 a scored move equals a plain move with weights w * r.
+ * One walk serves all scores (the record fetches, relocation and positions are shared; every further
+ * score adds one reduction per crossing), where nscores engines would walk nscores times.
+ * With nscores > 1 the plain and binned moves (and PumiTally::MoveToNextLocation) print an error,
+ * return non-zero and touch nothing, flying[] included.
+ * Results are [bin][score][element] in the caller's element numbering: pumitally_get_flux and
+ * pumitally_get_normalized_flux accept n = num_elements (bin 0, score 0) or n = nbins * nscores *
+ * num_elements (everything); pumitally_get_flux_device writes everything.  Volume and source
+ * normalisation apply to every score alike (mode 3 still sums the weights, not the responses);
+ * pumitally_reset_tally zeroes every score and the batch-end exchange moves all of them.
+ * WriteTallyResults writes score 0 as "flux" / "flux_bin<b>", exactly as without scores, and every
+ * score k >= 1 as "score<k>" (sum over the bins) and, with several bins, "score<k>_bin<b>".
+ * The internal array behind pumitally_flux_device_ptr is [bin][element][stride] with stride = nscores
+ * padded to 1, 2, 4 or 8 (internal element order). */
+int pumitally_set_scores(pumitally_engine *e, int32_t nscores);
+int32_t pumitally_get_scores(const pumitally_engine *e);
+int pumitally_move_to_next_location_scored(pumitally_engine *e, const double *particle_origin,
+                                           const double *particle_destinations, int8_t *flying,
+                                           const double *weights, const double *responses,
+                                           const int32_t *bins, int32_t size);
+int pumitally_move_to_next_location_device_scored(pumitally_engine *e, const double *d_origin,
+                                                  const double *d_destinations, const int8_t *d_flying,
+                                                  const double *d_weights, const double *d_responses,
+                                                  const int32_t *d_bins, int32_t size, void *stream);
 
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */

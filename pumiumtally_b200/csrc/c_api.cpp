@@ -161,6 +161,33 @@ int pumitally_move_to_next_location_device_binned(pumitally_engine *e, const dou
   });
 }
 
+int pumitally_set_scores(pumitally_engine *e, int32_t nscores) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_scores(nscores); });
+}
+int32_t pumitally_get_scores(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "scores")) : 0;
+}
+int pumitally_move_to_next_location_scored(pumitally_engine *e, const double *origin, const double *dest, int8_t *flying,
+                                           const double *weights, const double *responses, const int32_t *bins,
+                                           int32_t size) {
+  if (size > 0 && (!origin || !dest || !flying || !weights)) {
+    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: null input array\n");
+    return 1;
+  }
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.move_to_next_location_scored(origin, dest, flying, weights, responses, bins, size);
+  });
+}
+int pumitally_move_to_next_location_device_scored(pumitally_engine *e, const double *d_origin, const double *d_dest,
+                                                  const int8_t *d_flying, const double *d_weights,
+                                                  const double *d_responses, const int32_t *d_bins, int32_t size,
+                                                  void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.move_to_next_location_device_scored(d_origin, d_dest, d_flying, d_weights, d_responses, d_bins, size,
+                                                 static_cast<cudaStream_t>(stream));
+  });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

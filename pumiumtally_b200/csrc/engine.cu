@@ -146,6 +146,9 @@ Engine::~Engine() {
   if (ev_bins_free_) cudaEventDestroy(ev_bins_free_);
   cudaFree(d_mask_);
   cudaFree(d_bins_);
+  cudaFree(d_resp_);
+  if (h_resp_) cudaFreeHost(h_resp_);
+  if (ev_resp_) cudaEventDestroy(ev_resp_);
   if (h_bins_) cudaFreeHost(h_bins_);
   if (ev_copy0_) cudaEventDestroy(ev_copy0_);
   if (ev_copy1_) cudaEventDestroy(ev_copy1_);
@@ -257,9 +260,15 @@ void Engine::begin_move() {
   // sorting costs per particle, walking per crossing: with thousands of particles per tet (config c3) the
   // sorted variant cannot win and two exploration moves would cost more than an epoch can pay back
   if (int64_t(n_) > 16 * mesh_.ntets) return;
+  // a scored move runs the kernel a plain move would run outside the exploration, and is never timed for it
+  // (its walk costs more per crossing): the tuner's clock counts plain moves only
+  if (cur_resp_) {
+    move_variant_ = tuned_variant_;
+    return;
+  }
   // exploration moves 1..4 of every epoch in the order streaming, packed, packed, streaming (move 0 of a
   // run is atypical: nothing has been re-sourced yet); decision when all four have been timed
-  const uint64_t k = moves_ % kTuneEpoch;
+  const uint64_t k = (moves_ - scored_moves_) % kTuneEpoch;
   if (k >= 1 && k <= 4) {
     if (k == 1) { explore_ms_[0] = explore_ms_[1] = 0.0; explore_complete_ = false; }
     move_tag_ = (k == 2 || k == 3) ? 1 : 0;
@@ -332,7 +341,7 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   for (int32_t b = 0; b <= nbins_ && !rc; ++b) {
     if (launch_bin_mask(d_flying, cur_bins_, b, nbins_, d_mask_, begin, end, stream) != cudaSuccess) { rc = 1; break; }
     ++launches_;
-    rc = launch_range_into(d_flux_ + size_t(b) * size_t(mesh_.ntets), d_origin, d_dest, d_mask_, d_weights, begin, end, stream, timed);
+    rc = launch_range_into(d_flux_ + size_t(b) * bin_len(), d_origin, d_dest, d_mask_, d_weights, begin, end, stream, timed);
   }
   move_variant_ = saved_variant;
   move_tag_ = saved_tag;
@@ -343,7 +352,10 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
                               const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, bool timed) {
   if (d_dest && d_weights && initial_weight_pending_)  // first tracks of the batch: their total weight
     PTB_CUDA_OK(launch_sum_flying_weights(d_flying, d_weights, begin, end, d_initial_weight_, stream));
-  WalkParams p{};
+  ScoredWalkParams sp{};
+  WalkParams &p = sp;
+  const bool scored = cur_resp_ && d_dest;
+  if (scored) sp.sc = ScoreParams{cur_resp_, nscores_, stride_};
   p.tets = d_tets_;
   p.links = d_links_;
   p.verts = d_verts_;
@@ -430,7 +442,14 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
     launches_ += 5;  // count, 3-kernel scan, scatter
     p.flying = nullptr;  // order[] holds flying particles only
   }
-  PTB_CUDA_OK(launch_walk(p, variant, block_, stream));
+  if (scored) {
+    if (!walk_variant_available(variant) || launch_walk_scored(sp, variant, block_, stream) != cudaSuccess) {
+      fprintf(stderr, "[pumitally] ERROR: scored moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n", variant);
+      return 1;
+    }
+  } else {
+    PTB_CUDA_OK(launch_walk(p, variant, block_, stream));
+  }
   ++launches_;
   if (timed) {
     PTB_CUDA_OK(cudaEventRecord(t.b, stream));
@@ -644,8 +663,20 @@ int Engine::ensure_patch_buffers(int nchunks) {
 //
 // Direct path (option host_path=0, or no pinned memory to be had): plain cudaMemcpyAsync of all
 // four arrays from the caller's memory, optionally page-locked first (option register_host).
+bool Engine::refuse_unscored(const char *what) const {
+  if (nscores_ == 1) return false;
+  fprintf(stderr, "[pumitally] ERROR: %s: the engine has %d scores; use the scored move\n", what, nscores_);
+  return true;
+}
+
 int Engine::move_to_next_location(const double *origin, const double *dest, int8_t *flying,
                                   const double *weights, int32_t size) {
+  if (refuse_unscored("MoveToNextLocation")) return 1;
+  return move_host_entry(origin, dest, flying, weights, size);
+}
+
+int Engine::move_host_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                            int32_t size) {
   if (int64_t(size) != 3 * int64_t(n_)) {
     fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation size %d != 3 * num_particles (%d)\n", size, n_);
     return 1;
@@ -1020,6 +1051,12 @@ int Engine::move_direct(const double *origin, const double *dest, int8_t *flying
 int Engine::move_to_next_location_device(const double *d_origin, const double *d_dest,
                                          const int8_t *d_flying, const double *d_weights,
                                          int32_t size, cudaStream_t stream) {
+  if (refuse_unscored("MoveToNextLocation(device)")) return 1;
+  return move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
+}
+
+int Engine::move_device_entry(const double *d_origin, const double *d_dest, const int8_t *d_flying,
+                              const double *d_weights, int32_t size, cudaStream_t stream) {
   if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
     fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation(device): bad size or not initialised\n");
     return 1;
@@ -1044,14 +1081,31 @@ int Engine::set_score_bins(int32_t nbins) {
     fprintf(stderr, "[pumitally] ERROR: set_score_bins after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
+  return resize_flux(nbins, nscores_);
+}
+
+// Scores (walk_core.cuh, ScoreParams): the flux array becomes [bin][element][score_stride(nscores)].
+int Engine::set_scores(int32_t nscores) {
+  if (nscores < 1 || nscores > kMaxScores) return 1;
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_scores after comm_init (the exchange buffers are sized by then)\n");
+    return 1;
+  }
+  return resize_flux(nbins_, nscores);
+}
+
+int Engine::resize_flux(int32_t nbins, int32_t nscores) {
   if (synchronize()) return 1;
-  const size_t E = size_t(mesh_.ntets), len = size_t(nbins > 1 ? nbins + 1 : 1) * E + kFluxPad;
+  const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores));
+  const size_t len = size_t(nbins > 1 ? nbins + 1 : 1) * E * stride + kFluxPad;
   double *nf = nullptr;
   PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&nf), len * sizeof(double)));
   cudaFree(d_flux_);
   d_flux_ = nf;
   flux_alloc_ = len;
   nbins_ = nbins;
+  nscores_ = nscores;
+  stride_ = int32_t(stride);
   if (nbins > 1 && !d_mask_) {
     PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
     PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_bins_), std::max<size_t>(size_t(n_), 4) * sizeof(int32_t)));
@@ -1064,8 +1118,14 @@ int Engine::set_score_bins(int32_t nbins) {
 // ordinary host path (the pinned-caller variant excepted, whose relocation pass knows nothing of bins).
 int Engine::move_to_next_location_binned(const double *origin, const double *dest, int8_t *flying, const double *weights,
                                          const int32_t *bins, int32_t size) {
-  if (!bins || nbins_ == 1) return move_to_next_location(origin, dest, flying, weights, size);
-  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) return move_to_next_location(origin, dest, flying, weights, size);  // prints the error
+  if (refuse_unscored("MoveToNextLocationBinned")) return 1;
+  return move_binned_entry(origin, dest, flying, weights, bins, size);
+}
+
+int Engine::move_binned_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                              const int32_t *bins, int32_t size) {
+  if (!bins || nbins_ == 1) return move_host_entry(origin, dest, flying, weights, size);
+  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) return move_host_entry(origin, dest, flying, weights, size);  // prints the error
   PTB_CUDA_OK(cudaSetDevice(device_));
   if (!ev_bins_) {
     PTB_CUDA_OK(cudaEventCreateWithFlags(&ev_bins_, cudaEventDisableTiming));
@@ -1109,7 +1169,7 @@ int Engine::move_to_next_location_binned(const double *origin, const double *des
   // two stage passes: unless the caller chose the stage size, binned moves use stages of 2 Mi particles
   const int32_t chunk = chunk_;
   if (!chunk_user_set_) chunk_ = std::max(chunk_, int32_t(1) << 21);
-  const int rc = move_to_next_location(origin, dest, flying, weights, size);
+  const int rc = move_host_entry(origin, dest, flying, weights, size);
   chunk_ = chunk;
   pinned_path_ = pinned_path;
   cur_bins_ = nullptr;
@@ -1120,9 +1180,92 @@ int Engine::move_to_next_location_binned(const double *origin, const double *des
 int Engine::move_to_next_location_device_binned(const double *d_origin, const double *d_dest, const int8_t *d_flying,
                                                 const double *d_weights, const int32_t *d_bins, int32_t size,
                                                 cudaStream_t stream) {
+  if (refuse_unscored("MoveToNextLocationBinned(device)")) return 1;
   cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
-  const int rc = move_to_next_location_device(d_origin, d_dest, d_flying, d_weights, size, stream);
+  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
   cur_bins_ = nullptr;
+  return rc;
+}
+
+// MoveToNextLocation with nscores_ responses per particle (host pointers); bins as for the binned move.  The
+// responses travel as the bins do: one copy ahead of the particle data, through a pinned copy the worker pool
+// makes when the caller's array is pageable; everything else is the ordinary host path (the pinned-caller
+// variant excepted, whose relocation pass knows nothing of scores).
+int Engine::move_to_next_location_scored(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                                         const double *responses, const int32_t *bins, int32_t size) {
+  if (!responses) {
+    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: null responses array\n");
+    return 1;
+  }
+  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
+    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: bad size or not initialised\n");
+    return 1;
+  }
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const size_t cnt = size_t(n_) * size_t(nscores_);
+  if (resp_cap_ < cnt) {
+    PTB_CUDA_OK(cudaDeviceSynchronize());
+    cudaFree(d_resp_);
+    if (h_resp_) cudaFreeHost(h_resp_);
+    d_resp_ = h_resp_ = nullptr;
+    resp_cap_ = 0;
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_resp_), std::max<size_t>(cnt, 1) * sizeof(double)));
+    resp_cap_ = cnt;
+  }
+  if (!ev_resp_) PTB_CUDA_OK(cudaEventCreateWithFlags(&ev_resp_, cudaEventDisableTiming));
+  // d_resp_ is read by the previous scored move's kernels until they are done
+  PTB_CUDA_OK(cudaEventRecord(ev_resp_, compute_));
+  PTB_CUDA_OK(cudaStreamWaitEvent(copy_, ev_resp_, 0));
+  const double *src = responses;
+  if (!host_is_pinned(responses)) {
+    if (!h_resp_ && cudaHostAlloc(reinterpret_cast<void **>(&h_resp_), std::max<size_t>(resp_cap_, 1) * sizeof(double),
+                                  cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      h_resp_ = nullptr;
+    }
+    if (h_resp_) {  // the previous move's DMA out of it was waited for before that move returned
+      double *dst = h_resp_;
+      if (stager_) {
+        HostPool &pool = stager_->pool();
+        const int T = pool.size();
+        pool.run([&](int t) {
+          const size_t lo = cnt * size_t(t) / size_t(T), hi = cnt * size_t(t + 1) / size_t(T);
+          std::memcpy(dst + lo, responses + lo, (hi - lo) * sizeof(double));
+        });
+      } else {
+        std::memcpy(dst, responses, cnt * sizeof(double));
+      }
+      src = h_resp_;
+    }
+  }
+  PTB_CUDA_OK(cudaMemcpyAsync(d_resp_, src, cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
+  PTB_CUDA_OK(cudaEventRecord(ev_resp_, copy_));
+  h2d_bytes_ += 8.0 * double(cnt);
+  cur_resp_ = d_resp_;
+  const bool pinned_path = pinned_path_;
+  pinned_path_ = false;
+  const int rc = (bins && nbins_ > 1) ? move_binned_entry(origin, dest, flying, weights, bins, size)
+                                      : move_host_entry(origin, dest, flying, weights, size);
+  pinned_path_ = pinned_path;
+  cur_resp_ = nullptr;
+  if (rc == 0) ++scored_moves_;
+  PTB_CUDA_OK(cudaEventSynchronize(ev_resp_));  // the caller gets `responses` back with the other arrays
+  return rc;
+}
+
+int Engine::move_to_next_location_device_scored(const double *d_origin, const double *d_dest, const int8_t *d_flying,
+                                                const double *d_weights, const double *d_responses,
+                                                const int32_t *d_bins, int32_t size, cudaStream_t stream) {
+  if (!d_responses) {
+    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored(device): null responses array\n");
+    return 1;
+  }
+  cur_resp_ = d_responses;
+  cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
+  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
+  cur_bins_ = nullptr;
+  cur_resp_ = nullptr;
+  if (rc == 0) ++scored_moves_;
   return rc;
 }
 
@@ -1164,19 +1307,69 @@ int Engine::get_state_device(double *d_xyz, int32_t *d_elem, int32_t first, int3
   return 0;
 }
 
-// (all score bins, bin-major: nbins * E values)
+// (all score bins and scores: nbins * nscores * E values, [bin][score][element])
 int Engine::get_flux_device(double *d_out, cudaStream_t stream) {
   PTB_CUDA_OK(cudaSetDevice(device_));
   if (ensure_element_maps() || gather_shares()) return 1;
   const size_t E = size_t(mesh_.ntets);
+  if (nscores_ > 1) {
+    for (int32_t b = 0; b < nbins_; ++b)
+      PTB_CUDA_OK(launch_scores_to_caller_order(flux_view() + size_t(b) * bin_len(), d_orig_of_internal_,
+                                                d_out + size_t(b) * size_t(nscores_) * E, mesh_.ntets, nscores_, stride_, stream));
+    return 0;
+  }
   for (int32_t b = 0; b < nbins_; ++b)
     PTB_CUDA_OK(launch_flux_to_caller_order(flux_view() + size_t(b) * E, d_orig_of_internal_, d_out + size_t(b) * E, mesh_.ntets, stream));
   return 0;
 }
 
-// n == E: the first (or only) score bin; n == nbins * E: every bin, bin-major
+// Every bin and score of the scored tally, [bin][score][element] in the caller's numbering: raw, or normalised
+// as get_normalized_flux does it.
+int Engine::copy_results(std::vector<double> &out, bool normalized) {
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_);
+  double per_source = 1.0;
+  if (normalized) {
+    per_source = source_normalization();
+    if (!(per_source > 0.0)) {
+      fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
+      return 1;
+    }
+  }
+  if (ensure_element_maps()) return 1;
+  double *d_tmp = nullptr;
+  PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_tmp), std::max<size_t>(S * E, 1) * sizeof(double)));
+  out.resize(B * S * E);
+  std::vector<double> tmp(S * E);
+  int rc = 0;
+  for (size_t b = 0; b < B && !rc; ++b) {
+    const double *f = flux_view() + b * bin_len();
+    cudaError_t e = normalized ? launch_normalize_scores(f, d_volume_, d_tmp, int64_t(E), nscores_, stride_, per_source, compute_)
+                               : launch_scores_to_caller_order(f, d_orig_of_internal_, d_tmp, int64_t(E), nscores_, stride_, compute_);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+    if (e == cudaSuccess) e = cudaMemcpy(normalized ? tmp.data() : out.data() + b * S * E, d_tmp, S * E * sizeof(double), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) {
+      fprintf(stderr, "[pumitally] CUDA error %s reading the scores\n", cudaGetErrorString(e));
+      rc = 1;
+    } else if (normalized) {
+      for (size_t k = 0; k < S; ++k)
+        for (size_t i = 0; i < E; ++i) out[(b * S + k) * E + size_t(mesh_.orig_of_internal[i])] = tmp[k * E + i];
+    }
+  }
+  cudaFree(d_tmp);
+  return rc;
+}
+
+// n == E: the first (or only) score bin (score 0); n == nbins * nscores * E: everything, [bin][score][element]
 int Engine::get_flux(double *out, int64_t n) {
   const int64_t E = mesh_.ntets;
+  if (nscores_ > 1) {
+    if (n != E && n != int64_t(nbins_) * nscores_ * E) return 1;
+    if (synchronize() || gather_shares()) return 1;
+    std::vector<double> all;
+    if (copy_results(all, false)) return 1;
+    std::memcpy(out, all.data(), size_t(n) * sizeof(double));
+    return 0;
+  }
   if (n != E && n != int64_t(nbins_) * E) return 1;
   if (synchronize() || gather_shares()) return 1;
   std::vector<double> tmp(static_cast<size_t>(n));
@@ -1189,6 +1382,18 @@ int Engine::get_flux(double *out, int64_t n) {
 // NormalizeFlux (PumiTallyImpl.cpp:382-409); n as for get_flux (the volumes are always E values)
 int Engine::get_normalized_flux(double *out_flux, double *out_volume, int64_t n) {
   const int64_t E = mesh_.ntets;
+  if (nscores_ > 1) {
+    if (n != E && n != int64_t(nbins_) * nscores_ * E) return 1;
+    if (synchronize() || gather_shares()) return 1;
+    if (out_flux) {
+      std::vector<double> all;
+      if (copy_results(all, true)) return 1;
+      std::memcpy(out_flux, all.data(), size_t(n) * sizeof(double));
+    }
+    if (out_volume)
+      for (int64_t i = 0; i < E; ++i) out_volume[mesh_.orig_of_internal[i]] = mesh_.volume[i];
+    return 0;
+  }
   if (n != E && n != int64_t(nbins_) * E) return 1;
   if (synchronize() || gather_shares()) return 1;
   if (out_flux) {
@@ -1259,6 +1464,7 @@ int Engine::reset_tally() {
   PTB_CUDA_OK(cudaMemset(d_initial_weight_, 0, sizeof(double)));
   initial_weight_pending_ = true;
   PTB_CUDA_OK(cudaMemset(d_flux_, 0, flux_alloc_ * sizeof(double)));
+  scored_moves_ = 0;
   PTB_CUDA_OK(cudaMemset(d_stats_, 0, sizeof(DeviceStats)));
   flux_global_valid_ = flux_owned_only_ = false;
   kernel_ms_ = 0.0;
@@ -1315,6 +1521,8 @@ int64_t Engine::get_option(const std::string &name) const {
   }
   if (name == "allreduce_us") return int64_t(allreduce_ms_ * 1e3);  // device time of the last batch-end exchange
   if (name == "score_bins") return nbins_;
+  if (name == "scores") return nscores_;
+  if (name == "walk_blocks_per_sm") return walk_blocks_per_sm();  // occupancy of the last persistent walk kernel launched
   if (name == "die_split") return die_split_ ? 1 : 0;
   if (name == "l2_partition0_sms") return die0_sms_;  // SMs in the L2 partition of SM 0 (0: no map found)
   if (name == "exchange_choice") return exchange_choice_;  // what exchange_tally() does: 0 all-reduce, 1 reduce-scatter
@@ -1437,6 +1645,7 @@ int64_t Engine::debug_order(int32_t *out, int64_t n) {
 
 // FinalizeTallies (PumiTallyImpl.cpp:411-416)
 int Engine::write_tally_results() {
+  if (nscores_ > 1) return write_scored_results();
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
   if (get_normalized_flux(nf.data(), vol.data(), int64_t(nf.size()))) return 1;  // caller's element order
@@ -1453,6 +1662,35 @@ int Engine::write_tally_results() {
   }
   std::string err;
   if (!write_vtk_dataset(output_name_, mesh_, nf, vol, rank_, nranks_, &err, extra)) {
+    fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
+    return 1;
+  }
+  return 0;
+}
+
+// Scored tally: "flux" and "flux_bin<b>" are score 0, exactly as a one-score engine writes them; every score
+// k >= 1 adds "score<k>" (the sum over the bins) and, with several bins, "score<k>_bin<b>".
+int Engine::write_scored_results() {
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_);
+  std::vector<double> all(B * S * E), vol(E);
+  if (get_normalized_flux(all.data(), vol.data(), int64_t(all.size()))) return 1;
+  std::vector<std::vector<double>> sums(S);
+  for (size_t k = 0; k < S; ++k) {
+    sums[k].assign(all.begin() + k * E, all.begin() + (k + 1) * E);
+    for (size_t b = 1; b < B; ++b)
+      for (size_t i = 0; i < E; ++i) sums[k][i] += all[(b * S + k) * E + i];
+  }
+  std::vector<std::pair<std::string, const double *>> extra;
+  if (B > 1)
+    for (size_t b = 0; b < B; ++b) extra.emplace_back("flux_bin" + std::to_string(b), all.data() + b * S * E);
+  for (size_t k = 1; k < S; ++k) {
+    extra.emplace_back("score" + std::to_string(k), sums[k].data());
+    if (B > 1)
+      for (size_t b = 0; b < B; ++b)
+        extra.emplace_back("score" + std::to_string(k) + "_bin" + std::to_string(b), all.data() + (b * S + k) * E);
+  }
+  std::string err;
+  if (!write_vtk_dataset(output_name_, mesh_, sums[0], vol, rank_, nranks_, &err, extra)) {
     fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
     return 1;
   }

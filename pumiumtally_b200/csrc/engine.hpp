@@ -56,6 +56,17 @@ class Engine {
                                    const int32_t *bins, int32_t size);
   int move_to_next_location_device_binned(const double *d_origin, const double *d_dest, const int8_t *d_flying,
                                           const double *d_weights, const int32_t *d_bins, int32_t size, cudaStream_t stream);
+  // Scores: nscores responses per particle and move, tallied in one walk (walk_core.cuh, ScoreParams).  A scored
+  // move adds l * w[i] * r[i*nscores + k] to score k of the particle's bin for every segment of length l.
+  // Resets the tally; before comm_init.  With nscores > 1 only the scored moves are accepted.
+  int set_scores(int32_t nscores);
+  int32_t scores() const { return nscores_; }
+  int move_to_next_location_scored(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                                   const double *responses, const int32_t *bins, int32_t size);
+  int move_to_next_location_device_scored(const double *d_origin, const double *d_dest, const int8_t *d_flying,
+                                          const double *d_weights, const double *d_responses, const int32_t *d_bins,
+                                          int32_t size, cudaStream_t stream);
+  // n == E: bin 0, score 0; n == nbins * nscores * E: everything, [bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
   int set_state_device(const double *d_xyz, const int32_t *d_elem, int32_t first, int32_t count, cudaStream_t stream);
@@ -103,8 +114,26 @@ class Engine {
   int die0_sms_ = 0, nsms_ = 0;
   bool die_split_ = false;
   int32_t nbins_ = 1;
+  int32_t nscores_ = 1, stride_ = 1;  // scores, and doubles per element of d_flux_ (score_stride(nscores_))
   size_t flux_alloc_ = 0;             // doubles allocated at d_flux_
-  size_t flux_len() const { return size_t(nbins_) * size_t(mesh_.ntets); }  // reported part of d_flux_
+  // reported part of d_flux_: [bin][element][stride_]
+  size_t flux_len() const { return size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
+  size_t bin_len() const { return size_t(mesh_.ntets) * size_t(stride_); }
+  int resize_flux(int32_t nbins, int32_t nscores);
+  bool refuse_unscored(const char *what) const;
+  int move_host_entry(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size);
+  int move_device_entry(const double *d_origin, const double *d_dest, const int8_t *d_flying, const double *d_weights,
+                        int32_t size, cudaStream_t stream);
+  int move_binned_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                        const int32_t *bins, int32_t size);
+  int copy_results(std::vector<double> &out, bool normalized);
+  int write_scored_results();  // everything, [bin][score][element], caller's order
+  const double *cur_resp_ = nullptr;  // device responses of the scored move being launched
+  double *d_resp_ = nullptr;          // [N * nscores_] responses of a host-pointer scored move
+  double *h_resp_ = nullptr;          // pinned copy of the caller's responses on their way to the device
+  size_t resp_cap_ = 0;               // doubles allocated at d_resp_ / h_resp_
+  cudaEvent_t ev_resp_ = nullptr;
+  uint64_t scored_moves_ = 0;         // scored moves since the last reset (they are not the auto-tuner's samples)
   const int32_t *cur_bins_ = nullptr; // device array of the move being launched (binned moves only)
   int8_t *d_mask_ = nullptr;          // [N] flying flags of one bin
   int32_t *d_bins_ = nullptr;         // [N] bins of a host-pointer move

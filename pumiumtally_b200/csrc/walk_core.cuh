@@ -314,6 +314,38 @@ struct WalkParams {
   unsigned int *work_counter2;
 };
 
+// ---- scored walk: several responses per track ------------------------------------------------------
+// Within one move a particle keeps its material and energy, so every cross section is constant along
+// the track: the caller passes one response r[i,k] per particle and score (e.g. the macroscopic cross
+// sections) and a segment of length l in element e adds l * w[i] * r[i,k] to score k of e.  One walk
+// serves all scores: the record fetches, the relocation and the positions are shared, each score costs
+// one more reduction per crossing.
+constexpr int kMaxScores = 8;
+
+// Doubles per element of the internal flux array ([bin][element][score]): nscores padded to 1, 2, 4 or 8,
+// so that the scores of one element share one 32-byte sector (nscores <= 4) or one 64-byte half line and
+// the reductions of a crossing all land in one L2 line.
+PTB_HD int score_stride(int nscores) { return nscores <= 1 ? 1 : nscores <= 2 ? 2 : nscores <= 4 ? 4 : 8; }
+
+struct ScoreParams {
+  const double *responses;  // [N * nscores], particle-major: r[i * nscores + k]
+  int32_t nscores;          // 1..kMaxScores
+  int32_t stride;           // score_stride(nscores)
+};
+
+// Parameters of a scored launch: the plain ones, unchanged, followed by the scores.
+struct ScoredWalkParams : WalkParams {
+  ScoreParams sc;
+};
+
+// One lane's scores.  wl[k * step] = w * r[i,k] * |u| of the lane's current track: written when the tally
+// phase starts, read at every crossing (on the device a per-lane shared-memory slot, lane-contiguous per k).
+struct ScoreLane {
+  const double *responses;
+  double *wl;
+  int32_t n, stride, step;
+};
+
 constexpr int kStageReloc = 0;  // phase 1: move to caller's origin, tally off
 constexpr int kStageTally = 1;  // phase 2: fly to destination, tally on
 constexpr int kStageDone = 2;
@@ -353,24 +385,52 @@ PTB_HD bool all_finite(double a, double b, double c) { return (a * 0.0 + b * 0.0
 
 // Tally phase towards (tx,ty,tz) with weight w.  A non-finite destination or weight turns the flight
 // into a zero-length one (the particle stays where it is, nothing is tallied) and counts as lost.
+// NS > 0: scored walk of up to NS scores (sl->n of them); particle i's responses are read here, once per
+// track, and w * r[i,k] follows the rule for the weight.  w * r is exactly the weight a plain move with
+// weights w * r[:,k] carries, so every score is that move's tally.
+template <int NS = 0>
 PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, double z, double tx, double ty,
-                           double tz, double w, Counters &c, bool writer) {
-  if (!all_finite(tx, ty, tz) || !all_finite(w, 0.0, 0.0)) {
-    tx = x; ty = y; tz = z;
-    w = 0.0;
-    if (writer) c.lost++;
+                           double tz, double w, Counters &c, bool writer, int i = 0,
+                           const ScoreLane *sl = nullptr) {
+  if constexpr (NS == 0) {
+    if (!all_finite(tx, ty, tz) || !all_finite(w, 0.0, 0.0)) {
+      tx = x; ty = y; tz = z;
+      w = 0.0;
+      if (writer) c.lost++;
+    }
+    set_ray(P, r, x, y, z, tx, ty, tz);
+    const double len = sqrt(r.ux * r.ux + r.uy * r.uy + r.uz * r.uz);
+    r.wl = w * len;
+  } else {
+    bool bad = !all_finite(tx, ty, tz) || !all_finite(w, 0.0, 0.0);
+    const double *rp = sl->responses + (size_t)i * sl->n;
+PTB_UNROLL
+    for (int k = 0; k < NS; ++k)
+      if (k < sl->n) {
+        const double wr = w * PTB_LDG(rp + k);
+        bad = bad || !all_finite(wr, 0.0, 0.0);
+        sl->wl[k * sl->step] = wr;
+      }
+    if (bad) {
+      tx = x; ty = y; tz = z;
+      if (writer) c.lost++;
+    }
+    set_ray(P, r, x, y, z, tx, ty, tz);
+    const double len = sqrt(r.ux * r.ux + r.uy * r.uy + r.uz * r.uz);
+    r.wl = 0.0;  // (unused: the scores carry the weights)
+PTB_UNROLL
+    for (int k = 0; k < NS; ++k)
+      if (k < sl->n) sl->wl[k * sl->step] = bad ? 0.0 : sl->wl[k * sl->step] * len;
   }
-  set_ray(P, r, x, y, z, tx, ty, tz);
-  const double len = sqrt(r.ux * r.ux + r.uy * r.uy + r.uz * r.uz);
-  r.wl = w * len;
   r.stage = kStageTally;
   if (writer) c.tracks++;
 }
 
+template <int NS = 0>
 PTB_HD void start_tally(const WalkParams &P, int i, Ray &r, double x, double y, double z,
-                        Counters &c, bool writer) {
-  start_tally_to(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
-                 PTB_LDG(P.dest + 3 * (size_t)i + 2), PTB_LDG(P.weights + i), c, writer);
+                        Counters &c, bool writer, const ScoreLane *sl = nullptr) {
+  start_tally_to<NS>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
+                     PTB_LDG(P.dest + 3 * (size_t)i + 2), PTB_LDG(P.weights + i), c, writer, i, sl);
 }
 
 // Phase 1 for a particle at (x,y,z) in tet r.e whose caller-side origin is (tx,ty,tz).
@@ -400,7 +460,9 @@ PTB_HD void start_reloc(const WalkParams &P, Ray &r, double x, double y, double 
 }
 
 // K1/K2/K3 of the reference folded into the prologue: pick the walk target.
-PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool writer) {
+template <int NS = 0>
+PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool writer,
+                           const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
   const bool fly = P.flying ? (P.flying[i] == 1) : true;  // only the value 1 flies (Impl.cpp:95)
   if (!fly) return;  // dest := own origin => zero-length walk, nothing changes (Impl.cpp:100-102)
@@ -419,16 +481,16 @@ PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool
       return;
     }
   }
-  if (P.dest) start_tally(P, i, r, x, y, z, c, writer);
+  if (P.dest) start_tally<NS>(P, i, r, x, y, z, c, writer, sl);
 }
 
 // The current ray ended (target reached, hull hit, or iteration limit).
 // kReloadTarget: the caller does not keep Ray::tx,ty,tz alive in registers (the compact-layout
 // kernel); the target is read back from the caller's array, where it came from: dest[] in the
 // tally phase, origin[] in phase 1.  Same values, six registers fewer in the crossing loop.
-template <bool kReloadTarget = false>
+template <bool kReloadTarget = false, int NS = 0>
 PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tnew, Counters &c,
-                    bool writer) {
+                    bool writer, const ScoreLane *sl = nullptr) {
   // crossings of the ray that just ended: tally contributions in the tally phase, relocation crossings
   // otherwise (counted here, once per ray, instead of once per crossing)
   if (writer) {
@@ -456,7 +518,7 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
     x = fma(tnew, r.ux, r.ox) + P.cx; y = fma(tnew, r.uy, r.oy) + P.cy; z = fma(tnew, r.uz, r.oz) + P.cz;
   }
   if (r.stage != kStageTally && P.dest) {
-    start_tally(P, i, r, x, y, z, c, writer);  // phase 2 starts where phase 1 ended
+    start_tally<NS>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
   } else {
     if (writer) {
       store_state(P.state + i, x, y, z, r.e);
@@ -466,11 +528,21 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
 }
 
 // Functor body for one crossing, given the tracer's answer (texit, next).
-template <bool kReloadTarget = false, bool kAggregateTally = false>
+// NS > 0: scored walk (start_tally_to); one reduction per score into the element's scores.
+template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0>
 PTB_HD void advance(const WalkParams &P, int i, Ray &r, double texit, int32_t next, int32_t back,
-                    Counters &c, bool writer) {
+                    Counters &c, bool writer, const ScoreLane *sl = nullptr) {
   const bool reached = !(texit < 1.0);  // last_exit == -1: destination inside this tet
   const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
+  if constexpr (NS > 0) {
+    if (r.stage == kStageTally && writer) {
+      const double dt = tnew - r.tcur;
+      double *f = P.flux + (size_t)r.e * sl->stride;
+PTB_UNROLL
+      for (int k = 0; k < NS; ++k)
+        if (k < sl->n) PTB_TALLY_ADD(f + k, dt * sl->wl[k * sl->step]);
+    }
+  } else {
 #if defined(__CUDA_ARCH__)
   if constexpr (kAggregateTally) {
     tally_add_aggregated(P.flux, r.e, (tnew - r.tcur) * r.wl, r.stage == kStageTally && writer);
@@ -478,12 +550,13 @@ PTB_HD void advance(const WalkParams &P, int i, Ray &r, double texit, int32_t ne
 #endif
   if (r.stage == kStageTally && writer)  // EvaluateFlux (Impl.cpp:362-379)
     PTB_TALLY_ADD(P.flux + r.e, (tnew - r.tcur) * r.wl);
+  }
   const bool hull = !reached && next < 0;  // next_elems == -1 (Impl.cpp:270-271)
   r.iters++;
   const bool over = r.iters >= P.max_iters;
   if (reached || hull || over) {
     if (over && !reached && !hull && writer && r.stage != kStageSeed) c.lost++;
-    end_ray<kReloadTarget>(P, i, r, reached, tnew, c, writer);
+    end_ray<kReloadTarget, NS>(P, i, r, reached, tnew, c, writer, sl);
   } else {
     r.e = next;  // UpdateCurrentElement (Impl.cpp:247-253)
     r.entry = back;

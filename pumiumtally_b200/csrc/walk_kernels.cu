@@ -25,12 +25,16 @@ namespace {
 // Thread per particle; the 128-byte record arrives as four 32-byte sectors
 // (two 128-bit loads each), one per face.
 
-__global__ void __launch_bounds__(256) walk_ldg_kernel(const WalkParams P) {
+// NS > 0: scored walk (walk_persist.cuh); the lanes' score slots are sized for the largest block.
+template <int NS = 0>
+__global__ void __launch_bounds__(256) walk_ldg_kernel(const KernelParams<NS> P) {
   const int i = P.begin + blockIdx.x * blockDim.x + threadIdx.x;
+  __shared__ double score_wl[NS > 0 ? NS : 1][NS > 0 ? 256 : 1];
+  const ScoreLane sl = score_lane<NS, 256>(P, &score_wl[0][0]);
   Counters c;
   Ray r;
   r.stage = kStageDone;
-  if (i < P.end) begin_particle(P, i, r, c, true);
+  if (i < P.end) begin_particle<NS>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
   while (r.stage != kStageDone) {
     const double *rec = P.tets[r.e].d;
     double raw[16];
@@ -39,7 +43,7 @@ __global__ void __launch_bounds__(256) walk_ldg_kernel(const WalkParams P) {
       load_face_256(rec + 4 * f, raw[4 * f], raw[4 * f + 1], raw[4 * f + 2], raw[4 * f + 3]);
     ExitScan sc;
     scan_record(raw, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
-    advance(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true);
+    advance<false, false, NS>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
   }
   flush_counters(P, c);
 }
@@ -170,6 +174,24 @@ __global__ void normalize_kernel(const double *flux, const double *volume, doubl
   if (e < n) out[e] = flux[e] / volume[e] / per_source;  // per_source == 1: bit-identical to flux / volume
 }
 
+// Scored flux ([element][stride], internal order) -> out[k * n + caller's element id] for k < nscores
+__global__ void scores_to_caller_order_kernel(const double *flux, const int32_t *orig_of_internal, double *out, int64_t n,
+                                              int32_t nscores, int32_t stride) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const int32_t o = orig_of_internal[e];
+  for (int k = 0; k < nscores; ++k) out[k * n + o] = flux[e * stride + k];
+}
+
+// Scored flux -> out[k * n + e] = flux[e * stride + k] / volume[e] / per_source (internal element order)
+__global__ void normalize_scores_kernel(const double *flux, const double *volume, double *out, int64_t n, int32_t nscores,
+                                        int32_t stride, double per_source) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const double v = volume[e];
+  for (int k = 0; k < nscores; ++k) out[k * n + e] = flux[e * stride + k] / v / per_source;
+}
+
 // Score filter (engine.cu, launch_range): the flying flags of the particles whose score bin is `bin`
 // (bin == nbins: of those whose bin is outside [0, nbins) -- they fly, unscored)
 __global__ void bin_mask_kernel(const int8_t *flying, const int32_t *bins, int32_t bin, int32_t nbins, int8_t *mask,
@@ -223,6 +245,32 @@ cudaError_t launch_walk(const WalkParams &p, int variant, int block, cudaStream_
 #endif
   }
 }
+
+cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block, cudaStream_t stream) {
+  const long long n = (long long)p.end - p.begin;
+  if (n <= 0) return cudaSuccess;
+  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores || p.sc.stride != score_stride(p.sc.nscores) || !p.sc.responses)
+    return cudaErrorInvalidValue;
+  if (block != 64 && block != 128 && block != 256) block = 128;
+  switch (variant) {
+    case kVariantLdg: {
+      const unsigned grid = (unsigned)((n + block - 1) / block);
+      walk_ldg_kernel<kMaxScores><<<grid, block, 0, stream>>>(p);
+      return cudaGetLastError();
+    }
+    case kVariantPersistRefill8:
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores>(p, n, stream);
+    case kVariantPersistGatherL1:
+      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores>(p, n, stream);
+    case kVariantPacked:
+      if (!p.rows) return cudaErrorInvalidValue;
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores>(p, n, stream);
+    default:
+      return cudaErrorInvalidValue;  // the experiments have no scored instantiation
+  }
+}
+
+int walk_blocks_per_sm() { return last_persist_occupancy(); }
 
 bool walk_variant_available(int variant) {
   switch (variant) {
@@ -306,6 +354,22 @@ cudaError_t launch_normalize(const double *flux, const double *volume, double *o
                              double per_source, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
   normalize_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(flux, volume, out, n, per_source);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_scores_to_caller_order(const double *flux, const int32_t *orig_of_internal, double *out, int64_t n,
+                                          int32_t nscores, int32_t stride, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  scores_to_caller_order_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(flux, orig_of_internal, out, n, nscores,
+                                                                                  stride);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_normalize_scores(const double *flux, const double *volume, double *out, int64_t n, int32_t nscores,
+                                    int32_t stride, double per_source, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  normalize_scores_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(flux, volume, out, n, nscores, stride,
+                                                                            per_source);
   return cudaGetLastError();
 }
 

@@ -56,6 +56,11 @@ inline bool variant_is_packed(int v) {
 
 cudaError_t launch_walk(const WalkParams &p, int variant, int block, cudaStream_t stream);
 bool walk_variant_available(int variant);  // compiled into this library?
+// Scored walk (walk_core.cuh, ScoreParams): same kernels, instantiated for up to kMaxScores scores; product
+// variants 0, 8, 16, 24 only.  p.flux is [element][p.sc.stride].
+cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block, cudaStream_t stream);
+// blocks per SM the occupancy calculator gave the last persistent walk kernel launched (0: none yet)
+int walk_blocks_per_sm();
 // origin == nullptr: the binning key is the stored position (state)
 // mid != nullptr: the key is the midpoint of (start, mid[i]) -- pass the dest array
 cudaError_t launch_bin_particles(const SeedGrid &g, const double *origin, const ParticleState *state,
@@ -90,6 +95,12 @@ cudaError_t launch_get_state(const ParticleState *state, double *xyz, int32_t *e
                              int32_t begin, int32_t end, cudaStream_t stream);
 cudaError_t launch_flux_to_caller_order(const double *flux, const int32_t *orig_of_internal, double *out, int64_t n,
                                         cudaStream_t stream);
+// scored flux [n][stride] (internal order) -> out[k * n + caller's id], k < nscores
+cudaError_t launch_scores_to_caller_order(const double *flux, const int32_t *orig_of_internal, double *out, int64_t n,
+                                          int32_t nscores, int32_t stride, cudaStream_t stream);
+// scored flux [n][stride] -> out[k * n + e] = flux / volume / per_source (internal order)
+cudaError_t launch_normalize_scores(const double *flux, const double *volume, double *out, int64_t n, int32_t nscores,
+                                    int32_t stride, double per_source, cudaStream_t stream);
 // xyz[3i..3i+2] = position of particle i for i in [begin, end)
 cudaError_t launch_export_positions(const ParticleState *state, double *xyz, int32_t begin, int32_t end,
                                     cudaStream_t stream);

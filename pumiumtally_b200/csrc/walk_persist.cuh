@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <cstddef>
 #include <cstdint>
+#include <type_traits>
 
 #include "walk_compact.cuh"
 #include "walk_core.cuh"
@@ -134,9 +135,10 @@ __device__ __forceinline__ void stage_load(const WalkParams &P, int chunk, Parti
   }
 }
 
-// begin_particle() reading the staged copy instead of global memory
+// begin_particle() reading the staged copy instead of global memory (i: the slot's particle index)
+template <int NS = 0>
 __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const ParticleStage *st, int s,
-                                                 Ray &r, Counters &c) {
+                                                 Ray &r, Counters &c, int i = 0, const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
   const bool fly = P.flying ? (st->fly[s] == 1) : true;
   if (!fly) return;
@@ -153,11 +155,14 @@ __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const Part
       return;
     }
   }
-  if (P.dest) start_tally_to(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true);
+  if (P.dest)
+    start_tally_to<NS>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true, i, sl);
 }
 
 // begin_particle() for a packed row (only flying particles have rows).  Returns the particle id.
-__device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedRow *row, Ray &r, Counters &c) {
+template <int NS = 0>
+__device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedRow *row, Ray &r, Counters &c,
+                                              const ScoreLane *sl = nullptr) {
   const int id = row->id;
   const uint32_t el = row->elem;
   const double ox = row->ox, oy = row->oy, oz = row->oz;
@@ -172,7 +177,7 @@ __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedR
     return id;
   }
   r.e = (int32_t)(el & kIdMask);
-  start_tally_to(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true);
+  start_tally_to<NS>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
   return id;
 }
 
@@ -301,8 +306,9 @@ __device__ __forceinline__ void stage_gather(const WalkParams &P, int id, int co
 // One crossing on the plane records.  Entry-face elision: after a crossing the face the ray came
 // in through is known (r.entry) and can never be the exit, so only the other three 32-byte
 // sectors of the record are fetched; the first tet of a ray needs all four.
-template <int FETCH>
-__device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r, Counters &c, uint64_t pol) {
+template <int FETCH, int NS = 0>
+__device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r, Counters &c, uint64_t pol,
+                                           const ScoreLane *sl = nullptr) {
   ExitScan sc;
   const double *rec = P.tets[r.e].d;
   const int en = r.entry;
@@ -325,7 +331,8 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r
     face_payload(q3[0], q3[1], q3[2], q3[3], r.e, 3, nb, bk);
     scan_face(sc, q3[0], q3[1], q3[2], q3[3], nb, bk, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
   }
-  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back, c, true);
+  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back, c,
+                                                                              true, sl);
 }
 
 // Lean crossing step.  The compiler can sink the third record load of plane_step() below the arithmetic on
@@ -520,8 +527,24 @@ constexpr int kClaimRun = 4;  // gather mode: a warp takes up to this many conse
 // iteration, at the price of a few idle lanes in the walk step.
 // STAGING: 0 = particle arrays streamed in storage order (TMA bulk copies of the SoA/AoS slices),
 // 1 = gather through order[] (binned), 2 = packed rows written by the binning pass (binned, streamed).
-template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING>
-__global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const WalkParams P) {
+// NS: 0 = the plain tally; > 0 = scored walk of up to NS scores (plane-record fetch modes only).  Where the
+// scores of a lane live: a shared-memory slot per lane and score (NS * BLOCK doubles per block), written
+// once per track, read once per crossing and score -- registers would cost 2 * NS of them, beyond the
+// budget of __launch_bounds__(BLOCK, MINB), and re-reading the caller's array per crossing would add NS
+// loads to the memory pipe the walk is bound by.
+template <int NS>
+using KernelParams = std::conditional_t<NS == 0, WalkParams, ScoredWalkParams>;
+
+// The lane's ScoreLane, built where it is used from the parameters and the thread index, so that nothing of
+// it stays live in registers across the crossing loop.  wl0: slot 0 of lane 0; STEP lanes per score.
+template <int NS, int STEP>
+__device__ __forceinline__ ScoreLane score_lane(const KernelParams<NS> &P, double *wl0) {
+  if constexpr (NS > 0) return ScoreLane{P.sc.responses, wl0 + threadIdx.x, P.sc.nscores, P.sc.stride, STEP};
+  else return ScoreLane{};
+}
+
+template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING, int NS = 0>
+__global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelParams<NS> P) {
   constexpr bool GATHER = STAGING == 1;
   constexpr bool PACKED = STAGING == 2;
   constexpr int WARPS = BLOCK / 32;
@@ -532,6 +555,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const WalkPar
   __shared__ __align__(128) unsigned char rows[kRows ? WARPS : 1][kRows ? 32 * kRowBytes : 16];
   constexpr bool kEdge = FETCH == kFetchEdge;
   __shared__ double targets[kEdge ? BLOCK : 1][3];  // compact layout: each lane's ray target
+  static_assert(NS == 0 || (!kEdge && !kRows), "scored walks run on the plane records");
+  __shared__ double score_wl[NS > 0 ? NS : 1][NS > 0 ? BLOCK : 1];  // scored walk: ScoreLane::wl of each lane
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t bar0 = smem_u32(&bars[warp][0]);
   const uint32_t bar_row = bar0 + 16;
@@ -670,10 +695,13 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const WalkPar
       const int slot = cursor + __popc(idle & ((1u << lane) - 1u));
       if (r.stage == kStageDone && slot < cur_count) {
         if constexpr (PACKED) {
-          my_i = begin_from_row(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c);
+          const ScoreLane sl = score_lane<NS, BLOCK>(P, &score_wl[0][0]);
+          my_i = begin_from_row<NS>(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c,
+                                    NS > 0 ? &sl : nullptr);
         } else {
           my_i = GATHER ? stages[warp][cur].id[slot] : P.begin + chunk_cur * kChunk + slot;
-          begin_from_stage(P, &stages[warp][cur], slot, r, c);
+          const ScoreLane sl = score_lane<NS, BLOCK>(P, &score_wl[0][0]);
+          begin_from_stage<NS>(P, &stages[warp][cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
         }
         if constexpr (FETCH == kFetchEdge) {
           g.dv = 0;
@@ -729,27 +757,46 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const WalkPar
       } else if constexpr (FETCH == kFetchLean || FETCH == kFetchLeanL1) {
         plane_step_lean<FETCH>(P, my_i, r, c, keep);
       } else {
-        plane_step<FETCH>(P, my_i, r, c, keep);
+        const ScoreLane sl = score_lane<NS, BLOCK>(P, &score_wl[0][0]);
+        plane_step<FETCH, NS>(P, my_i, r, c, keep, NS > 0 ? &sl : nullptr);
       }
     }
   }
   flush_counters(P, c);
 }
 
-template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1>
-cudaError_t launch_persist(const WalkParams &p, long long n, cudaStream_t stream) {
+// Blocks per SM of the last persistent launch (diagnostics: engine option "walk_blocks_per_sm").
+inline int &last_persist_occupancy() {
+  static int occ = 0;
+  return occ;
+}
+
+template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1, int NS = 0>
+cudaError_t launch_persist(const KernelParams<NS> &p, long long n, cudaStream_t stream) {
   static int sms = 0, occ = 0;
   if (!sms) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int carve = CARVE < 0 ? (int)cudaSharedmemCarveoutMaxShared : CARVE;
+    if (NS > 0 && CARVE >= 0) {
+      // the scores' slots must not cost resident blocks: widen the carveout to what MINB blocks need
+      cudaFuncAttributes fa{};
+      int per_sm = 0, reserved = 0;
+      cudaFuncGetAttributes(&fa, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS>);
+      cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+      cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+      if (per_sm > 0)
+        carve = std::max(carve, (int)((100LL * MINB * ((long long)fa.sharedSizeBytes + reserved) + per_sm - 1) / per_sm));
+      carve = std::min(carve, 100);
+    }
     // leave as much of the unified L1/smem array to shared memory as the kernel can use
-    cudaFuncSetAttribute(walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER>,
-                         cudaFuncAttributePreferredSharedMemoryCarveout,
-                         CARVE < 0 ? (int)cudaSharedmemCarveoutMaxShared : CARVE);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER>, BLOCK, 0);
+    cudaFuncSetAttribute(walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS>,
+                         cudaFuncAttributePreferredSharedMemoryCarveout, carve);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS>, BLOCK, 0);
     if (occ < 1) occ = 1;
   }
+  last_persist_occupancy() = occ;
   const long long nchunks = (n + kChunk - 1) / kChunk;
   const long long want = (nchunks + BLOCK / 32 - 1) / (BLOCK / 32);
   const unsigned grid = (unsigned)std::min<long long>(want, (long long)sms * occ);
@@ -759,7 +806,7 @@ cudaError_t launch_persist(const WalkParams &p, long long n, cudaStream_t stream
     e = cudaMemsetAsync(p.work_counter2, 0, sizeof(unsigned int), stream);
     if (e != cudaSuccess) return e;
   }
-  walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER><<<grid, BLOCK, 0, stream>>>(p);
+  walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS><<<grid, BLOCK, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -44,6 +44,12 @@ C_API = {
         C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "pumitally_set_score_bins": (C.c_int, [C.c_void_p, C.c_int32]),
     "pumitally_get_score_bins": (C.c_int32, [C.c_void_p]),
+    "pumitally_set_scores": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_get_scores": (C.c_int32, [C.c_void_p]),
+    "pumitally_move_to_next_location_scored": (C.c_int, [C.c_void_p, _dp, _dp, _bp, _dp, _dp, _ip, C.c_int32]),
+    "pumitally_move_to_next_location_device_scored": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                  C.c_void_p]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -218,6 +224,58 @@ class PumiTally:
 
     def normalized_flux_bins(self):
         f, v = np.empty((self.score_bins, self.num_elements)), np.empty(self.num_elements)
+        if self._L.pumitally_get_normalized_flux(self._h, f.ctypes.data_as(_dp), v.ctypes.data_as(_dp), f.size):
+            raise RuntimeError("get_normalized_flux failed")
+        return f, v
+
+    # ---- scores ------------------------------------------------------------------
+    def set_scores(self, nscores: int):
+        """nscores responses per particle, tallied in one walk (resets the tally); 1 <= nscores <= 8."""
+        if self._L.pumitally_set_scores(self._h, int(nscores)):
+            raise ValueError(f"set_scores({nscores}) failed")
+
+    @property
+    def scores(self) -> int:
+        return int(self._L.pumitally_get_scores(self._h))
+
+    def MoveToNextLocationScored(self, particle_origin, particle_destinations, flying, weights, responses, bins=None,
+                                 size=None):
+        """Score k of every segment gets length * weights[i] * responses[i, k]; responses: [num_particles, nscores]."""
+        o = _host_f64(particle_origin, "particle_origin")
+        d = _host_f64(particle_destinations, "particle_destinations")
+        w = _host_f64(weights, "weights")
+        r = _host_f64(responses, "responses")
+        if not (isinstance(flying, np.ndarray) and flying.dtype == np.int8 and flying.flags.c_contiguous):
+            raise TypeError("flying must be a contiguous int8 numpy array (the engine zeroes it)")
+        if r.size != w.size * self.scores:
+            raise TypeError(f"responses must hold num_particles * {self.scores} values")
+        bp = None
+        if bins is not None:
+            if not (isinstance(bins, np.ndarray) and bins.dtype == np.int32 and bins.flags.c_contiguous and bins.size == w.size):
+                raise TypeError("bins must be a contiguous int32 numpy array, one entry per particle")
+            bp = bins.ctypes.data_as(_ip)
+        size = o.size if size is None else int(size)
+        if self._L.pumitally_move_to_next_location_scored(self._h, o.ctypes.data_as(_dp), d.ctypes.data_as(_dp),
+                                                          flying.ctypes.data_as(_bp), w.ctypes.data_as(_dp),
+                                                          r.ctypes.data_as(_dp), bp, size):
+            raise RuntimeError("MoveToNextLocationScored failed")
+
+    def move_device_scored(self, d_origin, d_dest, d_flying, d_weights, d_responses, d_bins=None, stream=None):
+        """Scored move on device addresses (responses particle-major); enqueues on ``stream`` and returns."""
+        if self._L.pumitally_move_to_next_location_device_scored(self._h, d_origin, d_dest, d_flying, d_weights,
+                                                                 d_responses, d_bins, 3 * self.num_particles, stream):
+            raise RuntimeError("MoveToNextLocationScored(device) failed")
+
+    @property
+    def flux_scores(self):
+        """Raw flux of every score bin and score: array [nbins, nscores, num_elements]."""
+        out = np.empty((self.score_bins, self.scores, self.num_elements))
+        if self._L.pumitally_get_flux(self._h, out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError("get_flux failed")
+        return out
+
+    def normalized_flux_scores(self):
+        f, v = np.empty((self.score_bins, self.scores, self.num_elements)), np.empty(self.num_elements)
         if self._L.pumitally_get_normalized_flux(self._h, f.ctypes.data_as(_dp), v.ctypes.data_as(_dp), f.size):
             raise RuntimeError("get_normalized_flux failed")
         return f, v
