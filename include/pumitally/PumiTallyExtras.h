@@ -47,6 +47,19 @@ inline int MoveToNextLocationScored(const PumiTally &tally, double *particle_ori
                                                 weights, responses, bins, size);
 }
 
+// Time filter: track-length scores split between the time bins [edges[j], edges[j+1]) each flight spans
+// (see pumitally_set_time_bins in pumitally_c.h).  times[i] is particle i's time at its origin, speeds[i]
+// its speed; responses may be nullptr with one score, bins may be nullptr (no score filter).
+inline int SetTimeBins(const PumiTally &tally, const double *edges, int32_t nedges) {
+  return pumitally_set_time_bins(engine_of(tally), edges, nedges);
+}
+inline int MoveToNextLocationTimed(const PumiTally &tally, double *particle_origin, double *particle_destinations,
+                                   int8_t *flying, double *weights, const double *times, const double *speeds,
+                                   const double *responses, const int32_t *bins, int32_t size) {
+  return pumitally_move_to_next_location_timed(engine_of(tally), particle_origin, particle_destinations, flying,
+                                               weights, times, speeds, responses, bins, size);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

@@ -122,8 +122,8 @@ int pumitally_set_output_name(pumitally_engine *e, const char *filename);
  * (crossing limit per walk; 0 = number of elements + 16, the default), "l2_fetch", "autotune"
  * (1 = default: while "variant" is automatic the engine times the streaming and the sorted/packed
  * kernel on moves 1-4 of every 64 and keeps the faster one).  Read-only: "launches", "staged",
- * "stage_host_us", "stage_sent_bytes", "scores", "walk_blocks_per_sm" (blocks per SM of the last
- * persistent walk kernel launched). */
+ * "stage_host_us", "stage_sent_bytes", "scores", "time_bins", "walk_blocks_per_sm" (blocks per SM of
+ * the last persistent walk kernel launched). */
 int pumitally_set_option(pumitally_engine *e, const char *name, int64_t value);
 int64_t pumitally_get_option(const pumitally_engine *e, const char *name);
 
@@ -243,6 +243,49 @@ int pumitally_move_to_next_location_device_scored(pumitally_engine *e, const dou
                                                   const double *d_destinations, const int8_t *d_flying,
                                                   const double *d_weights, const double *d_responses,
                                                   const int32_t *d_bins, int32_t size, void *stream);
+
+/* ---- additive: time filter (track-length scores split between time bins) ----
+ * Time advances along a flight, so one flight can span several bins of a pulsed-source or time-of-flight
+ * tally.  pumitally_set_time_bins(e, edges, nedges) sets the edges T_0 < T_1 < ... < T_n, n = nedges - 1,
+ * 1 <= n <= 1024; bin j is [T_j, T_{j+1}).  The edges must be finite and strictly increasing; anything else,
+ * or a flux array that cannot be allocated (nelements * nbins * padded nscores * n doubles), returns
+ * non-zero and changes nothing.  edges == NULL with nedges == 0 removes the filter.  The call resets the
+ * tally, combines with pumitally_set_score_bins and pumitally_set_scores in any order and is refused after
+ * pumitally_comm_init.  pumitally_get_time_bins (or the option "time_bins") returns n, 0 without a filter.
+ * The timed moves take, besides the scored move's arguments, times double[num_particles] (particle i's
+ * time at its origin) and speeds double[num_particles] (mesh length units per time unit), never NULL;
+ * responses may be NULL only with one score (every response 1), bins may be NULL (no score filter).  A
+ * segment of particle i in element e covers track distance [s_a, s_b], i.e. the times
+ * [times[i] + s_a/speeds[i], times[i] + s_b/speeds[i]]; for every time bin j it overlaps it adds
+ * w[i] * r[i,k] * speeds[i] * overlap_j (the track length spent in bin j) to score k of bin bins[i] in time
+ * bin j.  A track starting exactly on an edge starts in the bin above it; a flight ending exactly on an
+ * edge adds nothing to the next bin.  What lies before T_0 or at or after T_n is not tallied: the particle
+ * flies, unscored there.  Relocation carries no time.  A non-finite time, or a speed that is not finite and
+ * > 0, is treated like a non-finite weight: zero-length flight, counted as lost, nothing tallied.
+ * Everything else is the plain move: parent elements, positions, clipping at the hull, flying[] zeroed by
+ * the host version, and the statistics (segments are counted once per crossing, not once per piece).
+ * While time bins are set the plain, binned and scored moves (and PumiTally::MoveToNextLocation) print an
+ * error, return non-zero and touch nothing, flying[] included; a timed move without time bins is refused
+ * the same way.
+ * Results are [time][bin][score][element] in the caller's element numbering: pumitally_get_flux and
+ * pumitally_get_normalized_flux accept n = num_elements (time bin 0, bin 0, score 0) or n = ntime * nbins
+ * * nscores * num_elements; pumitally_get_flux_device writes everything.  Volume and source normalisation
+ * are unchanged (nothing is divided by the bin width); pumitally_reset_tally and the batch-end exchange
+ * cover every time bin.  WriteTallyResults writes every array it writes without time bins as the sum over
+ * the time bins, under the same name, and for every time bin j the same arrays with "_t<j>" after the
+ * score name: "flux_t<j>", "flux_t<j>_bin<b>", "score<k>_t<j>", "score<k>_t<j>_bin<b>".
+ * The internal array behind pumitally_flux_device_ptr is [time][bin][element][stride]. */
+int pumitally_set_time_bins(pumitally_engine *e, const double *edges, int32_t nedges);
+int32_t pumitally_get_time_bins(const pumitally_engine *e);
+int pumitally_move_to_next_location_timed(pumitally_engine *e, const double *particle_origin,
+                                          const double *particle_destinations, int8_t *flying,
+                                          const double *weights, const double *times, const double *speeds,
+                                          const double *responses, const int32_t *bins, int32_t size);
+int pumitally_move_to_next_location_device_timed(pumitally_engine *e, const double *d_origin,
+                                                 const double *d_destinations, const int8_t *d_flying,
+                                                 const double *d_weights, const double *d_times,
+                                                 const double *d_speeds, const double *d_responses,
+                                                 const int32_t *d_bins, int32_t size, void *stream);
 
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */

@@ -188,6 +188,33 @@ int pumitally_move_to_next_location_device_scored(pumitally_engine *e, const dou
   });
 }
 
+int pumitally_set_time_bins(pumitally_engine *e, const double *edges, int32_t nedges) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_time_bins(edges, nedges); });
+}
+int32_t pumitally_get_time_bins(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "time_bins")) : 0;
+}
+int pumitally_move_to_next_location_timed(pumitally_engine *e, const double *origin, const double *dest, int8_t *flying,
+                                          const double *weights, const double *times, const double *speeds,
+                                          const double *responses, const int32_t *bins, int32_t size) {
+  if (size > 0 && (!origin || !dest || !flying || !weights)) {
+    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationTimed: null input array\n");
+    return 1;
+  }
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.move_to_next_location_timed(origin, dest, flying, weights, times, speeds, responses, bins, size);
+  });
+}
+int pumitally_move_to_next_location_device_timed(pumitally_engine *e, const double *d_origin, const double *d_dest,
+                                                 const int8_t *d_flying, const double *d_weights, const double *d_times,
+                                                 const double *d_speeds, const double *d_responses,
+                                                 const int32_t *d_bins, int32_t size, void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.move_to_next_location_device_timed(d_origin, d_dest, d_flying, d_weights, d_times, d_speeds, d_responses,
+                                                d_bins, size, static_cast<cudaStream_t>(stream));
+  });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

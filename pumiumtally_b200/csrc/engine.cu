@@ -146,9 +146,12 @@ Engine::~Engine() {
   if (ev_bins_free_) cudaEventDestroy(ev_bins_free_);
   cudaFree(d_mask_);
   cudaFree(d_bins_);
-  cudaFree(d_resp_);
-  if (h_resp_) cudaFreeHost(h_resp_);
-  if (ev_resp_) cudaEventDestroy(ev_resp_);
+  for (AuxUpload *u : {&resp_up_, &time_up_}) {
+    cudaFree(u->d);
+    if (u->h) cudaFreeHost(u->h);
+    if (u->ev) cudaEventDestroy(u->ev);
+  }
+  cudaFree(d_edges_);
   if (h_bins_) cudaFreeHost(h_bins_);
   if (ev_copy0_) cudaEventDestroy(ev_copy0_);
   if (ev_copy1_) cudaEventDestroy(ev_copy1_);
@@ -260,9 +263,9 @@ void Engine::begin_move() {
   // sorting costs per particle, walking per crossing: with thousands of particles per tet (config c3) the
   // sorted variant cannot win and two exploration moves would cost more than an epoch can pay back
   if (int64_t(n_) > 16 * mesh_.ntets) return;
-  // a scored move runs the kernel a plain move would run outside the exploration, and is never timed for it
-  // (its walk costs more per crossing): the tuner's clock counts plain moves only
-  if (cur_resp_) {
+  // a scored or timed move runs the kernel a plain move would run outside the exploration, and is never timed
+  // for it (its walk costs more per crossing): the tuner's clock counts plain moves only
+  if (cur_resp_ || cur_times_) {
     move_variant_ = tuned_variant_;
     return;
   }
@@ -324,6 +327,7 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   last_stream_ = stream;
   last_stream_set_ = true;
   if (d_dest) flux_global_valid_ = flux_owned_only_ = false;  // the local tally moves on; the last exchange no longer describes it
+  cur_slice_ = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
   if (!(cur_bins_ && d_dest)) return launch_range_into(d_flux_, d_origin, d_dest, d_flying, d_weights, begin, end, stream, timed);
   // Score filter: particles are independent and a particle that does not fly is not touched, so the range
   // is walked once per bin with the flying flags masked down to that bin's particles and the tally pointed
@@ -341,7 +345,10 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   for (int32_t b = 0; b <= nbins_ && !rc; ++b) {
     if (launch_bin_mask(d_flying, cur_bins_, b, nbins_, d_mask_, begin, end, stream) != cudaSuccess) { rc = 1; break; }
     ++launches_;
-    rc = launch_range_into(d_flux_ + size_t(b) * bin_len(), d_origin, d_dest, d_mask_, d_weights, begin, end, stream, timed);
+    // the unreported array follows every reported one (with a time filter, all time bins of a bin-b pass go to it)
+    cur_slice_ = b < nbins_ ? int64_t(nbins_) * int64_t(bin_len()) : 0;
+    rc = launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : flux_len()), d_origin, d_dest, d_mask_, d_weights,
+                           begin, end, stream, timed);
   }
   move_variant_ = saved_variant;
   move_tag_ = saved_tag;
@@ -352,10 +359,13 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
                               const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, bool timed) {
   if (d_dest && d_weights && initial_weight_pending_)  // first tracks of the batch: their total weight
     PTB_CUDA_OK(launch_sum_flying_weights(d_flying, d_weights, begin, end, d_initial_weight_, stream));
-  ScoredWalkParams sp{};
-  WalkParams &p = sp;
-  const bool scored = cur_resp_ && d_dest;
+  TimedWalkParams tp{};
+  ScoredWalkParams &sp = tp;
+  WalkParams &p = tp;
+  const bool timed_walk = cur_times_ && d_dest;
+  const bool scored = (cur_resp_ || timed_walk) && d_dest;
   if (scored) sp.sc = ScoreParams{cur_resp_, nscores_, stride_};
+  if (timed_walk) tp.tm = TimeParams{d_edges_, cur_times_, cur_speeds_, ntime_, cur_slice_};
   p.tets = d_tets_;
   p.links = d_links_;
   p.verts = d_verts_;
@@ -442,7 +452,12 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
     launches_ += 5;  // count, 3-kernel scan, scatter
     p.flying = nullptr;  // order[] holds flying particles only
   }
-  if (scored) {
+  if (timed_walk) {
+    if (!walk_variant_available(variant) || launch_walk_timed(tp, variant, block_, stream) != cudaSuccess) {
+      fprintf(stderr, "[pumitally] ERROR: timed moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n", variant);
+      return 1;
+    }
+  } else if (scored) {
     if (!walk_variant_available(variant) || launch_walk_scored(sp, variant, block_, stream) != cudaSuccess) {
       fprintf(stderr, "[pumitally] ERROR: scored moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n", variant);
       return 1;
@@ -664,8 +679,15 @@ int Engine::ensure_patch_buffers(int nchunks) {
 // Direct path (option host_path=0, or no pinned memory to be had): plain cudaMemcpyAsync of all
 // four arrays from the caller's memory, optionally page-locked first (option register_host).
 bool Engine::refuse_unscored(const char *what) const {
+  if (refuse_untimed(what)) return true;
   if (nscores_ == 1) return false;
   fprintf(stderr, "[pumitally] ERROR: %s: the engine has %d scores; use the scored move\n", what, nscores_);
+  return true;
+}
+
+bool Engine::refuse_untimed(const char *what) const {
+  if (ntime_ == 0) return false;
+  fprintf(stderr, "[pumitally] ERROR: %s: the engine has %d time bins; use the timed move\n", what, ntime_);
   return true;
 }
 
@@ -1081,7 +1103,7 @@ int Engine::set_score_bins(int32_t nbins) {
     fprintf(stderr, "[pumitally] ERROR: set_score_bins after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins, nscores_);
+  return resize_flux(nbins, nscores_, ntime_);
 }
 
 // Scores (walk_core.cuh, ScoreParams): the flux array becomes [bin][element][score_stride(nscores)].
@@ -1091,21 +1113,62 @@ int Engine::set_scores(int32_t nscores) {
     fprintf(stderr, "[pumitally] ERROR: set_scores after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores);
+  return resize_flux(nbins_, nscores, ntime_);
 }
 
-int Engine::resize_flux(int32_t nbins, int32_t nscores) {
+// Time filter (walk_core.cuh, TimeParams): the flux array becomes [time][bin][element][stride], the edges live on
+// the device.  Nothing changes unless the edges are valid and the new array can be allocated.
+int Engine::set_time_bins(const double *edges, int32_t nedges) {
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_time_bins after comm_init (the exchange buffers are sized by then)\n");
+    return 1;
+  }
+  if (!edges && nedges == 0) {  // no time filter
+    if (resize_flux(nbins_, nscores_, 0)) return 1;
+    cudaFree(d_edges_);
+    d_edges_ = nullptr;
+    return 0;
+  }
+  if (!edges || nedges < 2 || nedges - 1 > kMaxTimeBins) return 1;
+  for (int32_t j = 0; j < nedges; ++j)
+    if (!std::isfinite(edges[j]) || (j > 0 && !(edges[j] > edges[j - 1]))) return 1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  double *ne = nullptr;
+  if (cudaMalloc(reinterpret_cast<void **>(&ne), size_t(nedges) * sizeof(double)) != cudaSuccess) {
+    cudaGetLastError();
+    return 1;
+  }
+  if (cudaMemcpy(ne, edges, size_t(nedges) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
+      resize_flux(nbins_, nscores_, nedges - 1)) {
+    cudaGetLastError();
+    cudaFree(ne);
+    return 1;
+  }
+  cudaFree(d_edges_);
+  d_edges_ = ne;
+  return 0;
+}
+
+int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime) {
   if (synchronize()) return 1;
   const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores));
-  const size_t len = size_t(nbins > 1 ? nbins + 1 : 1) * E * stride + kFluxPad;
+  // [time][bin][element][stride], then the unreported array of the particles no bin matches
+  const size_t len = (size_t(ntime > 0 ? ntime : 1) * size_t(nbins) + (nbins > 1 ? 1 : 0)) * E * stride + kFluxPad;
   double *nf = nullptr;
-  PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&nf), len * sizeof(double)));
+  const cudaError_t err = cudaMalloc(reinterpret_cast<void **>(&nf), len * sizeof(double));
+  if (err != cudaSuccess) {
+    cudaGetLastError();
+    fprintf(stderr, "[pumitally] ERROR: no device memory for a flux array of %zu doubles (%s)\n", len,
+            cudaGetErrorString(err));
+    return 1;
+  }
   cudaFree(d_flux_);
   d_flux_ = nf;
   flux_alloc_ = len;
   nbins_ = nbins;
   nscores_ = nscores;
   stride_ = int32_t(stride);
+  ntime_ = ntime;
   if (nbins > 1 && !d_mask_) {
     PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
     PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_bins_), std::max<size_t>(size_t(n_), 4) * sizeof(int32_t)));
@@ -1187,61 +1250,86 @@ int Engine::move_to_next_location_device_binned(const double *d_origin, const do
   return rc;
 }
 
+// Per-particle doubles of a host-pointer move that travel as the bins do: one copy ahead of the particle data on
+// the copy stream, through a pinned copy the worker pool makes when a caller's array is pageable.  a and, if not
+// null, b (cnt doubles each) land back to back in u.d; u.ev is recorded after the copy.
+int Engine::upload_doubles(AuxUpload &u, const double *a, const double *b, size_t cnt) {
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const size_t total = cnt * (b ? 2 : 1);
+  if (u.cap < total) {
+    PTB_CUDA_OK(cudaDeviceSynchronize());
+    cudaFree(u.d);
+    if (u.h) cudaFreeHost(u.h);
+    u.d = u.h = nullptr;
+    u.cap = 0;
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&u.d), std::max<size_t>(total, 1) * sizeof(double)));
+    u.cap = total;
+  }
+  if (!u.ev) PTB_CUDA_OK(cudaEventCreateWithFlags(&u.ev, cudaEventDisableTiming));
+  // u.d is read by the previous move's kernels until they are done
+  PTB_CUDA_OK(cudaEventRecord(u.ev, compute_));
+  PTB_CUDA_OK(cudaStreamWaitEvent(copy_, u.ev, 0));
+  const double *src[2] = {a, b};
+  const int narr = b ? 2 : 1;
+  bool staged = false;
+  if (!host_is_pinned(a) || (b && !host_is_pinned(b))) {
+    if (!u.h && cudaHostAlloc(reinterpret_cast<void **>(&u.h), std::max<size_t>(u.cap, 1) * sizeof(double),
+                              cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      u.h = nullptr;
+    }
+    if (u.h) {  // the previous move's DMA out of it was waited for before that move returned
+      double *dst = u.h;
+      for (int k = 0; k < narr; ++k) {
+        const double *from = src[k];
+        double *to = dst + size_t(k) * cnt;
+        if (stager_) {
+          HostPool &pool = stager_->pool();
+          const int T = pool.size();
+          pool.run([&](int t) {
+            const size_t lo = cnt * size_t(t) / size_t(T), hi = cnt * size_t(t + 1) / size_t(T);
+            std::memcpy(to + lo, from + lo, (hi - lo) * sizeof(double));
+          });
+        } else {
+          std::memcpy(to, from, cnt * sizeof(double));
+        }
+      }
+      PTB_CUDA_OK(cudaMemcpyAsync(u.d, u.h, total * sizeof(double), cudaMemcpyHostToDevice, copy_));
+      staged = true;
+    }
+  }
+  if (!staged)
+    for (int k = 0; k < narr; ++k)
+      PTB_CUDA_OK(cudaMemcpyAsync(u.d + size_t(k) * cnt, src[k], cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
+  PTB_CUDA_OK(cudaEventRecord(u.ev, copy_));
+  h2d_bytes_ += 8.0 * double(total);
+  return 0;
+}
+
 // MoveToNextLocation with nscores_ responses per particle (host pointers); bins as for the binned move.  The
-// responses travel as the bins do: one copy ahead of the particle data, through a pinned copy the worker pool
-// makes when the caller's array is pageable; everything else is the ordinary host path (the pinned-caller
+// responses travel as the bins do (upload_doubles); everything else is the ordinary host path (the pinned-caller
 // variant excepted, whose relocation pass knows nothing of scores).
 int Engine::move_to_next_location_scored(const double *origin, const double *dest, int8_t *flying, const double *weights,
                                          const double *responses, const int32_t *bins, int32_t size) {
+  if (refuse_untimed("MoveToNextLocationScored")) return 1;
   if (!responses) {
     fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: null responses array\n");
     return 1;
   }
+  return move_scored_entry(origin, dest, flying, weights, responses, bins, size);
+}
+
+// (responses == nullptr: a timed move with one score, every response 1)
+int Engine::move_scored_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                              const double *responses, const int32_t *bins, int32_t size) {
   if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
     fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: bad size or not initialised\n");
     return 1;
   }
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const size_t cnt = size_t(n_) * size_t(nscores_);
-  if (resp_cap_ < cnt) {
-    PTB_CUDA_OK(cudaDeviceSynchronize());
-    cudaFree(d_resp_);
-    if (h_resp_) cudaFreeHost(h_resp_);
-    d_resp_ = h_resp_ = nullptr;
-    resp_cap_ = 0;
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_resp_), std::max<size_t>(cnt, 1) * sizeof(double)));
-    resp_cap_ = cnt;
+  if (responses) {
+    if (upload_doubles(resp_up_, responses, nullptr, size_t(n_) * size_t(nscores_))) return 1;
+    cur_resp_ = resp_up_.d;
   }
-  if (!ev_resp_) PTB_CUDA_OK(cudaEventCreateWithFlags(&ev_resp_, cudaEventDisableTiming));
-  // d_resp_ is read by the previous scored move's kernels until they are done
-  PTB_CUDA_OK(cudaEventRecord(ev_resp_, compute_));
-  PTB_CUDA_OK(cudaStreamWaitEvent(copy_, ev_resp_, 0));
-  const double *src = responses;
-  if (!host_is_pinned(responses)) {
-    if (!h_resp_ && cudaHostAlloc(reinterpret_cast<void **>(&h_resp_), std::max<size_t>(resp_cap_, 1) * sizeof(double),
-                                  cudaHostAllocDefault) != cudaSuccess) {
-      cudaGetLastError();
-      h_resp_ = nullptr;
-    }
-    if (h_resp_) {  // the previous move's DMA out of it was waited for before that move returned
-      double *dst = h_resp_;
-      if (stager_) {
-        HostPool &pool = stager_->pool();
-        const int T = pool.size();
-        pool.run([&](int t) {
-          const size_t lo = cnt * size_t(t) / size_t(T), hi = cnt * size_t(t + 1) / size_t(T);
-          std::memcpy(dst + lo, responses + lo, (hi - lo) * sizeof(double));
-        });
-      } else {
-        std::memcpy(dst, responses, cnt * sizeof(double));
-      }
-      src = h_resp_;
-    }
-  }
-  PTB_CUDA_OK(cudaMemcpyAsync(d_resp_, src, cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
-  PTB_CUDA_OK(cudaEventRecord(ev_resp_, copy_));
-  h2d_bytes_ += 8.0 * double(cnt);
-  cur_resp_ = d_resp_;
   const bool pinned_path = pinned_path_;
   pinned_path_ = false;
   const int rc = (bins && nbins_ > 1) ? move_binned_entry(origin, dest, flying, weights, bins, size)
@@ -1249,13 +1337,14 @@ int Engine::move_to_next_location_scored(const double *origin, const double *des
   pinned_path_ = pinned_path;
   cur_resp_ = nullptr;
   if (rc == 0) ++scored_moves_;
-  PTB_CUDA_OK(cudaEventSynchronize(ev_resp_));  // the caller gets `responses` back with the other arrays
+  if (responses) PTB_CUDA_OK(cudaEventSynchronize(resp_up_.ev));  // the caller gets `responses` back with the other arrays
   return rc;
 }
 
 int Engine::move_to_next_location_device_scored(const double *d_origin, const double *d_dest, const int8_t *d_flying,
                                                 const double *d_weights, const double *d_responses,
                                                 const int32_t *d_bins, int32_t size, cudaStream_t stream) {
+  if (refuse_untimed("MoveToNextLocationScored(device)")) return 1;
   if (!d_responses) {
     fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored(device): null responses array\n");
     return 1;
@@ -1265,6 +1354,59 @@ int Engine::move_to_next_location_device_scored(const double *d_origin, const do
   const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
   cur_bins_ = nullptr;
   cur_resp_ = nullptr;
+  if (rc == 0) ++scored_moves_;
+  return rc;
+}
+
+// The arguments every timed move needs, checked before anything is touched.
+bool Engine::timed_args_ok(const char *what, const void *times, const void *speeds, const void *responses) const {
+  if (ntime_ == 0) {
+    fprintf(stderr, "[pumitally] ERROR: %s: the engine has no time bins (set_time_bins)\n", what);
+    return false;
+  }
+  if (!times || !speeds) {
+    fprintf(stderr, "[pumitally] ERROR: %s: null times or speeds array\n", what);
+    return false;
+  }
+  if (!responses && nscores_ != 1) {
+    fprintf(stderr, "[pumitally] ERROR: %s: null responses array with %d scores\n", what, nscores_);
+    return false;
+  }
+  return true;
+}
+
+// Timed move (host pointers): the scored move plus each particle's time at its origin and speed.  Times and
+// speeds travel together, one copy ahead of the responses and the particle data (16 bytes per particle).
+int Engine::move_to_next_location_timed(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                                        const double *times, const double *speeds, const double *responses,
+                                        const int32_t *bins, int32_t size) {
+  if (!timed_args_ok("MoveToNextLocationTimed", times, speeds, responses)) return 1;
+  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
+    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationTimed: bad size or not initialised\n");
+    return 1;
+  }
+  if (upload_doubles(time_up_, times, speeds, size_t(n_))) return 1;
+  cur_times_ = time_up_.d;
+  cur_speeds_ = time_up_.d + n_;
+  const int rc = move_scored_entry(origin, dest, flying, weights, responses, bins, size);
+  cur_times_ = cur_speeds_ = nullptr;
+  PTB_CUDA_OK(cudaEventSynchronize(time_up_.ev));
+  return rc;
+}
+
+int Engine::move_to_next_location_device_timed(const double *d_origin, const double *d_dest, const int8_t *d_flying,
+                                               const double *d_weights, const double *d_times, const double *d_speeds,
+                                               const double *d_responses, const int32_t *d_bins, int32_t size,
+                                               cudaStream_t stream) {
+  if (!timed_args_ok("MoveToNextLocationTimed(device)", d_times, d_speeds, d_responses)) return 1;
+  cur_times_ = d_times;
+  cur_speeds_ = d_speeds;
+  cur_resp_ = d_responses;
+  cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
+  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
+  cur_bins_ = nullptr;
+  cur_resp_ = nullptr;
+  cur_times_ = cur_speeds_ = nullptr;
   if (rc == 0) ++scored_moves_;
   return rc;
 }
@@ -1307,13 +1449,13 @@ int Engine::get_state_device(double *d_xyz, int32_t *d_elem, int32_t first, int3
   return 0;
 }
 
-// (all score bins and scores: nbins * nscores * E values, [bin][score][element])
+// (all time bins, score bins and scores: ntime * nbins * nscores * E values, [time][bin][score][element])
 int Engine::get_flux_device(double *d_out, cudaStream_t stream) {
   PTB_CUDA_OK(cudaSetDevice(device_));
   if (ensure_element_maps() || gather_shares()) return 1;
   const size_t E = size_t(mesh_.ntets);
-  if (nscores_ > 1) {
-    for (int32_t b = 0; b < nbins_; ++b)
+  if (multi_results()) {
+    for (int32_t b = 0; b < result_arrays(); ++b)
       PTB_CUDA_OK(launch_scores_to_caller_order(flux_view() + size_t(b) * bin_len(), d_orig_of_internal_,
                                                 d_out + size_t(b) * size_t(nscores_) * E, mesh_.ntets, nscores_, stride_, stream));
     return 0;
@@ -1323,10 +1465,10 @@ int Engine::get_flux_device(double *d_out, cudaStream_t stream) {
   return 0;
 }
 
-// Every bin and score of the scored tally, [bin][score][element] in the caller's numbering: raw, or normalised
-// as get_normalized_flux does it.
+// Every time bin, bin and score of the tally, [time][bin][score][element] in the caller's numbering: raw, or
+// normalised as get_normalized_flux does it.  (Time bin t of bin b is internal array t * nbins + b.)
 int Engine::copy_results(std::vector<double> &out, bool normalized) {
-  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_);
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
   double per_source = 1.0;
   if (normalized) {
     per_source = source_normalization();
@@ -1359,11 +1501,12 @@ int Engine::copy_results(std::vector<double> &out, bool normalized) {
   return rc;
 }
 
-// n == E: the first (or only) score bin (score 0); n == nbins * nscores * E: everything, [bin][score][element]
+// n == E: the first (or only) score bin (score 0, time bin 0); n == ntime * nbins * nscores * E: everything,
+// [time][bin][score][element]
 int Engine::get_flux(double *out, int64_t n) {
   const int64_t E = mesh_.ntets;
-  if (nscores_ > 1) {
-    if (n != E && n != int64_t(nbins_) * nscores_ * E) return 1;
+  if (multi_results()) {
+    if (n != E && n != int64_t(result_arrays()) * nscores_ * E) return 1;
     if (synchronize() || gather_shares()) return 1;
     std::vector<double> all;
     if (copy_results(all, false)) return 1;
@@ -1382,8 +1525,8 @@ int Engine::get_flux(double *out, int64_t n) {
 // NormalizeFlux (PumiTallyImpl.cpp:382-409); n as for get_flux (the volumes are always E values)
 int Engine::get_normalized_flux(double *out_flux, double *out_volume, int64_t n) {
   const int64_t E = mesh_.ntets;
-  if (nscores_ > 1) {
-    if (n != E && n != int64_t(nbins_) * nscores_ * E) return 1;
+  if (multi_results()) {
+    if (n != E && n != int64_t(result_arrays()) * nscores_ * E) return 1;
     if (synchronize() || gather_shares()) return 1;
     if (out_flux) {
       std::vector<double> all;
@@ -1522,6 +1665,7 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "allreduce_us") return int64_t(allreduce_ms_ * 1e3);  // device time of the last batch-end exchange
   if (name == "score_bins") return nbins_;
   if (name == "scores") return nscores_;
+  if (name == "time_bins") return ntime_;
   if (name == "walk_blocks_per_sm") return walk_blocks_per_sm();  // occupancy of the last persistent walk kernel launched
   if (name == "die_split") return die_split_ ? 1 : 0;
   if (name == "l2_partition0_sms") return die0_sms_;  // SMs in the L2 partition of SM 0 (0: no map found)
@@ -1645,7 +1789,7 @@ int64_t Engine::debug_order(int32_t *out, int64_t n) {
 
 // FinalizeTallies (PumiTallyImpl.cpp:411-416)
 int Engine::write_tally_results() {
-  if (nscores_ > 1) return write_scored_results();
+  if (multi_results()) return write_scored_results();
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
   if (get_normalized_flux(nf.data(), vol.data(), int64_t(nf.size()))) return 1;  // caller's element order
@@ -1668,26 +1812,39 @@ int Engine::write_tally_results() {
   return 0;
 }
 
-// Scored tally: "flux" and "flux_bin<b>" are score 0, exactly as a one-score engine writes them; every score
-// k >= 1 adds "score<k>" (the sum over the bins) and, with several bins, "score<k>_bin<b>".
+// Scored or timed tally: "flux" and "flux_bin<b>" are score 0, exactly as a one-score engine writes them; every
+// score k >= 1 adds "score<k>" (the sum over the bins) and, with several bins, "score<k>_bin<b>".  With time bins
+// these are sums over the time bins, and every time bin j adds the same arrays with "_t<j>" after the score name:
+// "flux_t<j>", "flux_t<j>_bin<b>", "score<k>_t<j>", "score<k>_t<j>_bin<b>".
 int Engine::write_scored_results() {
-  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_);
-  std::vector<double> all(B * S * E), vol(E);
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_), T = nslices();
+  std::vector<double> all(T * B * S * E), vol(E);
   if (get_normalized_flux(all.data(), vol.data(), int64_t(all.size()))) return 1;
-  std::vector<std::vector<double>> sums(S);
-  for (size_t k = 0; k < S; ++k) {
-    sums[k].assign(all.begin() + k * E, all.begin() + (k + 1) * E);
-    for (size_t b = 1; b < B; ++b)
-      for (size_t i = 0; i < E; ++i) sums[k][i] += all[(b * S + k) * E + i];
-  }
+  // sets[0]: the sum over the time bins; sets[1 + j]: time bin j (only with a time filter).  [bin][score][element]
+  std::vector<std::vector<double>> sets;
+  sets.emplace_back(all.begin(), all.begin() + B * S * E);
+  for (size_t t = 1; t < T; ++t)
+    for (size_t i = 0; i < B * S * E; ++i) sets[0][i] += all[t * B * S * E + i];
+  if (ntime_ > 0)
+    for (size_t t = 0; t < T; ++t) sets.emplace_back(all.begin() + t * B * S * E, all.begin() + (t + 1) * B * S * E);
+  // per set and score: the sum over the bins
+  std::vector<std::vector<double>> sums(sets.size() * S);
+  for (size_t q = 0; q < sets.size(); ++q)
+    for (size_t k = 0; k < S; ++k) {
+      std::vector<double> &sum = sums[q * S + k];
+      sum.assign(sets[q].begin() + k * E, sets[q].begin() + (k + 1) * E);
+      for (size_t b = 1; b < B; ++b)
+        for (size_t i = 0; i < E; ++i) sum[i] += sets[q][(b * S + k) * E + i];
+    }
   std::vector<std::pair<std::string, const double *>> extra;
-  if (B > 1)
-    for (size_t b = 0; b < B; ++b) extra.emplace_back("flux_bin" + std::to_string(b), all.data() + b * S * E);
-  for (size_t k = 1; k < S; ++k) {
-    extra.emplace_back("score" + std::to_string(k), sums[k].data());
-    if (B > 1)
-      for (size_t b = 0; b < B; ++b)
-        extra.emplace_back("score" + std::to_string(k) + "_bin" + std::to_string(b), all.data() + (b * S + k) * E);
+  for (size_t q = 0; q < sets.size(); ++q) {
+    const std::string t = q == 0 ? "" : "_t" + std::to_string(q - 1);
+    for (size_t k = 0; k < S; ++k) {
+      const std::string name = k == 0 ? "flux" + t : "score" + std::to_string(k) + t;
+      if (q > 0 || k > 0) extra.emplace_back(name, sums[q * S + k].data());  // (set 0, score 0 is the main array)
+      if (B > 1)
+        for (size_t b = 0; b < B; ++b) extra.emplace_back(name + "_bin" + std::to_string(b), sets[q].data() + (b * S + k) * E);
+    }
   }
   std::string err;
   if (!write_vtk_dataset(output_name_, mesh_, sums[0], vol, rank_, nranks_, &err, extra)) {

@@ -66,7 +66,20 @@ class Engine {
   int move_to_next_location_device_scored(const double *d_origin, const double *d_dest, const int8_t *d_flying,
                                           const double *d_weights, const double *d_responses, const int32_t *d_bins,
                                           int32_t size, cudaStream_t stream);
-  // n == E: bin 0, score 0; n == nbins * nscores * E: everything, [bin][score][element]
+  // Time filter: edges T_0 < ... < T_nt (nt = nedges - 1, 1..kMaxTimeBins); a timed move splits every segment
+  // between the time bins [T_j, T_j+1) it spans, by the time spent in each (walk_core.cuh, TimeParams).  edges ==
+  // nullptr with nedges == 0 removes the filter.  Resets the tally; before comm_init.  While time bins are set only
+  // the timed moves are accepted.
+  int set_time_bins(const double *edges, int32_t nedges);
+  int32_t time_bins() const { return ntime_; }
+  int move_to_next_location_timed(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                                  const double *times, const double *speeds, const double *responses,
+                                  const int32_t *bins, int32_t size);
+  int move_to_next_location_device_timed(const double *d_origin, const double *d_dest, const int8_t *d_flying,
+                                         const double *d_weights, const double *d_times, const double *d_speeds,
+                                         const double *d_responses, const int32_t *d_bins, int32_t size,
+                                         cudaStream_t stream);
+  // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
   int set_state_device(const double *d_xyz, const int32_t *d_elem, int32_t first, int32_t count, cudaStream_t stream);
@@ -115,25 +128,42 @@ class Engine {
   bool die_split_ = false;
   int32_t nbins_ = 1;
   int32_t nscores_ = 1, stride_ = 1;  // scores, and doubles per element of d_flux_ (score_stride(nscores_))
+  int32_t ntime_ = 0;                 // time bins (0: no time filter)
   size_t flux_alloc_ = 0;             // doubles allocated at d_flux_
-  // reported part of d_flux_: [bin][element][stride_]
-  size_t flux_len() const { return size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
+  // reported part of d_flux_: [time][bin][element][stride_]
+  size_t nslices() const { return ntime_ > 0 ? size_t(ntime_) : 1; }
+  size_t flux_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
   size_t bin_len() const { return size_t(mesh_.ntets) * size_t(stride_); }
-  int resize_flux(int32_t nbins, int32_t nscores);
+  int32_t result_arrays() const { return int32_t(nslices()) * nbins_; }  // (time, bin) arrays of bin_len() doubles
+  bool multi_results() const { return nscores_ > 1 || ntime_ > 0; }      // results laid out [time][bin][score][element]
+  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime);
   bool refuse_unscored(const char *what) const;
+  bool refuse_untimed(const char *what) const;
+  bool timed_args_ok(const char *what, const void *times, const void *speeds, const void *responses) const;
   int move_host_entry(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size);
   int move_device_entry(const double *d_origin, const double *d_dest, const int8_t *d_flying, const double *d_weights,
                         int32_t size, cudaStream_t stream);
   int move_binned_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
                         const int32_t *bins, int32_t size);
+  int move_scored_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
+                        const double *responses, const int32_t *bins, int32_t size);
   int copy_results(std::vector<double> &out, bool normalized);
-  int write_scored_results();  // everything, [bin][score][element], caller's order
+  int write_scored_results();  // everything, [time][bin][score][element], caller's order
+  // per-particle doubles of a host-pointer move on their way to the device (upload_doubles)
+  struct AuxUpload {
+    double *d = nullptr;  // device copy
+    double *h = nullptr;  // pinned copy of pageable caller arrays
+    size_t cap = 0;       // doubles allocated at d / h
+    cudaEvent_t ev = nullptr;
+  };
+  int upload_doubles(AuxUpload &u, const double *a, const double *b, size_t cnt);
   const double *cur_resp_ = nullptr;  // device responses of the scored move being launched
-  double *d_resp_ = nullptr;          // [N * nscores_] responses of a host-pointer scored move
-  double *h_resp_ = nullptr;          // pinned copy of the caller's responses on their way to the device
-  size_t resp_cap_ = 0;               // doubles allocated at d_resp_ / h_resp_
-  cudaEvent_t ev_resp_ = nullptr;
-  uint64_t scored_moves_ = 0;         // scored moves since the last reset (they are not the auto-tuner's samples)
+  AuxUpload resp_up_;                 // [N * nscores_] responses of a host-pointer scored move
+  const double *cur_times_ = nullptr, *cur_speeds_ = nullptr;  // device arrays of the timed move being launched
+  AuxUpload time_up_;                 // [2N] times, then speeds, of a host-pointer timed move
+  double *d_edges_ = nullptr;         // [ntime_ + 1] time bin edges
+  int64_t cur_slice_ = 0;             // doubles between time bins of the array the launch tallies into
+  uint64_t scored_moves_ = 0;         // scored and timed moves since the last reset (not the auto-tuner's samples)
   const int32_t *cur_bins_ = nullptr; // device array of the move being launched (binned moves only)
   int8_t *d_mask_ = nullptr;          // [N] flying flags of one bin
   int32_t *d_bins_ = nullptr;         // [N] bins of a host-pointer move

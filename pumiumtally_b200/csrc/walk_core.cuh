@@ -346,6 +346,35 @@ struct ScoreLane {
   int32_t n, stride, step;
 };
 
+// ---- timed walk: a time filter that splits every segment between time bins ------------------------
+// Time advances along a flight (t = times[i] + s / speeds[i] at track distance s), so one segment can span
+// several bins [T_j, T_j+1) of a time filter.  The timed walk is the scored one plus time: a segment adds
+// w * r[i,k] * |u| * (ray-parameter overlap with bin j) to score k of time bin j, which is the track length
+// spent in the bin.  Only the walk knows where a segment lies along the flight, so the split happens here:
+// the common crossing (exit before the bin's upper edge) costs one comparison and issues exactly the scored
+// step's reductions; each edge crossed costs one division.
+constexpr int kMaxTimeBins = 1024;
+
+struct TimeParams {
+  const double *edges;   // [nt + 1], finite, strictly increasing
+  const double *times;   // [N] time of particle i at its origin
+  const double *speeds;  // [N] mesh length units per time unit, finite and > 0
+  int32_t nt;            // time bins, 1..kMaxTimeBins
+  int64_t slice;         // doubles from time bin j to j + 1 of the same array (0: every bin into one array)
+};
+
+// Parameters of a timed launch: the scored ones, unchanged, followed by the time filter.
+struct TimedWalkParams : ScoredWalkParams {
+  TimeParams tm;
+};
+
+// One lane's scores and time state.  Next to the score slots, at wl[(NS + m) * step]: m = 0 the time at ray
+// parameter 0, m = 1 the time per unit ray parameter (|u| / v), m = 2 the upper edge of the current bin;
+// *bin is the current bin (-1: before T_0, nt: at or after T_nt; neither is tallied).
+struct TimeLane : ScoreLane {
+  int32_t *bin;
+};
+
 constexpr int kStageReloc = 0;  // phase 1: move to caller's origin, tally off
 constexpr int kStageTally = 1;  // phase 2: fly to destination, tally on
 constexpr int kStageDone = 2;
@@ -385,10 +414,65 @@ PTB_HD bool all_finite(double a, double b, double c) { return (a * 0.0 + b * 0.0
 
 // Tally phase towards (tx,ty,tz) with weight w.  A non-finite destination or weight turns the flight
 // into a zero-length one (the particle stays where it is, nothing is tallied) and counts as lost.
+// Timed walk, start of a track: the lane's time state for a flight that is at time t0 at ray parameter 0 and
+// spends tpp time units per unit ray parameter.  The starting bin is found by binary search over the edges
+// (a start exactly on an edge belongs to the bin above it); a bad track gets bin nt, which tallies nothing.
+template <int NS>
+PTB_HD void time_start(const TimedWalkParams &T, const TimeLane *tl, double t0, double tpp, bool bad) {
+  const double *ed = T.tm.edges;
+  const int nt = T.tm.nt;
+  int lo = 0, hi = nt + 1;  // lo: number of edges <= t0
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (PTB_LDG(ed + mid) <= t0) lo = mid + 1;
+    else hi = mid;
+  }
+  const int j = bad ? nt : lo - 1;
+  double *wl = tl->wl;
+  wl[NS * tl->step] = bad ? 0.0 : t0;
+  wl[(NS + 1) * tl->step] = bad ? 0.0 : tpp;
+  wl[(NS + 2) * tl->step] = j < nt ? PTB_LDG(ed + j + 1) : __builtin_huge_val();
+  *tl->bin = j;
+}
+
+// Timed walk, one crossing: the segment [tcur, tnew] (ray parameters) of element e.  While the exit time lies
+// beyond the current bin's upper edge, the segment is cut at the edge's ray parameter and the bins are walked
+// forward (time only increases along a ray).  A flight that ends exactly on an edge stays in the bin below.
+template <int NS>
+PTB_HD void time_tally(const TimedWalkParams &T, int32_t e, double tcur, double tnew, const TimeLane *tl) {
+  const int step = tl->step;
+  double *wl = tl->wl;
+  const double t0 = wl[NS * step], tpp = wl[(NS + 1) * step];
+  double tup = wl[(NS + 2) * step];
+  int j = *tl->bin;
+  double *f = T.flux + (size_t)e * tl->stride;
+  double p = tcur;
+  for (;;) {
+    const bool split = fma(tnew, tpp, t0) > tup;
+    const double pe = split ? fmin(fmax((tup - t0) / tpp, p), tnew) : tnew;
+    if (j >= 0 && j < T.tm.nt) {
+      const double dt = pe - p;
+      double *fj = f + (size_t)j * (size_t)T.tm.slice;
+PTB_UNROLL
+      for (int k = 0; k < NS; ++k)
+        if (k < tl->n) PTB_TALLY_ADD(fj + k, dt * wl[k * step]);
+    }
+    if (!split) return;
+    p = pe;
+    ++j;
+    tup = j < T.tm.nt ? PTB_LDG(T.tm.edges + j + 1) : __builtin_huge_val();
+    wl[(NS + 2) * step] = tup;
+    *tl->bin = j;
+  }
+}
+
 // NS > 0: scored walk of up to NS scores (sl->n of them); particle i's responses are read here, once per
 // track, and w * r[i,k] follows the rule for the weight.  w * r is exactly the weight a plain move with
 // weights w * r[:,k] carries, so every score is that move's tally.
-template <int NS = 0>
+// TM: timed walk (NS > 0, sl is a TimeLane): particle i's time and speed are read here too; a non-finite time
+// or a speed that is not finite and > 0 is a bad track like a non-finite weight.  No responses (nullptr):
+// every r[i,k] is 1.
+template <int NS = 0, bool TM = false>
 PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, double z, double tx, double ty,
                            double tz, double w, Counters &c, bool writer, int i = 0,
                            const ScoreLane *sl = nullptr) {
@@ -403,11 +487,18 @@ PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, doub
     r.wl = w * len;
   } else {
     bool bad = !all_finite(tx, ty, tz) || !all_finite(w, 0.0, 0.0);
+    double t0 = 0.0, v = 1.0;
+    if constexpr (TM) {
+      const TimedWalkParams &T = static_cast<const TimedWalkParams &>(P);
+      t0 = PTB_LDG(T.tm.times + i);
+      v = PTB_LDG(T.tm.speeds + i);
+      bad = bad || !all_finite(t0, v, 0.0) || !(v > 0.0);
+    }
     const double *rp = sl->responses + (size_t)i * sl->n;
 PTB_UNROLL
     for (int k = 0; k < NS; ++k)
       if (k < sl->n) {
-        const double wr = w * PTB_LDG(rp + k);
+        const double wr = w * ((!TM || sl->responses) ? PTB_LDG(rp + k) : 1.0);
         bad = bad || !all_finite(wr, 0.0, 0.0);
         sl->wl[k * sl->step] = wr;
       }
@@ -421,15 +512,17 @@ PTB_UNROLL
 PTB_UNROLL
     for (int k = 0; k < NS; ++k)
       if (k < sl->n) sl->wl[k * sl->step] = bad ? 0.0 : sl->wl[k * sl->step] * len;
+    if constexpr (TM)
+      time_start<NS>(static_cast<const TimedWalkParams &>(P), static_cast<const TimeLane *>(sl), t0, len / v, bad);
   }
   r.stage = kStageTally;
   if (writer) c.tracks++;
 }
 
-template <int NS = 0>
+template <int NS = 0, bool TM = false>
 PTB_HD void start_tally(const WalkParams &P, int i, Ray &r, double x, double y, double z,
                         Counters &c, bool writer, const ScoreLane *sl = nullptr) {
-  start_tally_to<NS>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
+  start_tally_to<NS, TM>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
                      PTB_LDG(P.dest + 3 * (size_t)i + 2), PTB_LDG(P.weights + i), c, writer, i, sl);
 }
 
@@ -460,7 +553,7 @@ PTB_HD void start_reloc(const WalkParams &P, Ray &r, double x, double y, double 
 }
 
 // K1/K2/K3 of the reference folded into the prologue: pick the walk target.
-template <int NS = 0>
+template <int NS = 0, bool TM = false>
 PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool writer,
                            const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -481,14 +574,14 @@ PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool
       return;
     }
   }
-  if (P.dest) start_tally<NS>(P, i, r, x, y, z, c, writer, sl);
+  if (P.dest) start_tally<NS, TM>(P, i, r, x, y, z, c, writer, sl);
 }
 
 // The current ray ended (target reached, hull hit, or iteration limit).
 // kReloadTarget: the caller does not keep Ray::tx,ty,tz alive in registers (the compact-layout
 // kernel); the target is read back from the caller's array, where it came from: dest[] in the
 // tally phase, origin[] in phase 1.  Same values, six registers fewer in the crossing loop.
-template <bool kReloadTarget = false, int NS = 0>
+template <bool kReloadTarget = false, int NS = 0, bool TM = false>
 PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tnew, Counters &c,
                     bool writer, const ScoreLane *sl = nullptr) {
   // crossings of the ray that just ended: tally contributions in the tally phase, relocation crossings
@@ -518,7 +611,7 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
     x = fma(tnew, r.ux, r.ox) + P.cx; y = fma(tnew, r.uy, r.oy) + P.cy; z = fma(tnew, r.uz, r.oz) + P.cz;
   }
   if (r.stage != kStageTally && P.dest) {
-    start_tally<NS>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
+    start_tally<NS, TM>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
   } else {
     if (writer) {
       store_state(P.state + i, x, y, z, r.e);
@@ -529,12 +622,16 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
 
 // Functor body for one crossing, given the tracer's answer (texit, next).
 // NS > 0: scored walk (start_tally_to); one reduction per score into the element's scores.
-template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0>
+// TM: timed walk (time_tally); the same reductions, into the time bins the segment spans.
+template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0, bool TM = false>
 PTB_HD void advance(const WalkParams &P, int i, Ray &r, double texit, int32_t next, int32_t back,
                     Counters &c, bool writer, const ScoreLane *sl = nullptr) {
   const bool reached = !(texit < 1.0);  // last_exit == -1: destination inside this tet
   const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
-  if constexpr (NS > 0) {
+  if constexpr (TM) {
+    if (r.stage == kStageTally && writer)
+      time_tally<NS>(static_cast<const TimedWalkParams &>(P), r.e, r.tcur, tnew, static_cast<const TimeLane *>(sl));
+  } else if constexpr (NS > 0) {
     if (r.stage == kStageTally && writer) {
       const double dt = tnew - r.tcur;
       double *f = P.flux + (size_t)r.e * sl->stride;
@@ -556,7 +653,7 @@ PTB_UNROLL
   const bool over = r.iters >= P.max_iters;
   if (reached || hull || over) {
     if (over && !reached && !hull && writer && r.stage != kStageSeed) c.lost++;
-    end_ray<kReloadTarget, NS>(P, i, r, reached, tnew, c, writer, sl);
+    end_ray<kReloadTarget, NS, TM>(P, i, r, reached, tnew, c, writer, sl);
   } else {
     r.e = next;  // UpdateCurrentElement (Impl.cpp:247-253)
     r.entry = back;

@@ -26,15 +26,17 @@ namespace {
 // (two 128-bit loads each), one per face.
 
 // NS > 0: scored walk (walk_persist.cuh); the lanes' score slots are sized for the largest block.
-template <int NS = 0>
-__global__ void __launch_bounds__(256) walk_ldg_kernel(const KernelParams<NS> P) {
+// TM: timed walk (NS > 0); the lanes' time slots sit next to the scores.
+template <int NS, bool TM>
+__device__ __forceinline__ void ldg_walk(const KernelParams<NS, TM> &P) {
   const int i = P.begin + blockIdx.x * blockDim.x + threadIdx.x;
-  __shared__ double score_wl[NS > 0 ? NS : 1][NS > 0 ? 256 : 1];
-  const ScoreLane sl = score_lane<NS, 256>(P, &score_wl[0][0]);
+  __shared__ double score_wl[kLaneSlots<NS, TM>][NS > 0 ? 256 : 1];
+  __shared__ int32_t time_bin[TM ? 256 : 1];
+  const auto sl = walk_lane<NS, 256, TM>(P, &score_wl[0][0], &time_bin[0]);
   Counters c;
   Ray r;
   r.stage = kStageDone;
-  if (i < P.end) begin_particle<NS>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
+  if (i < P.end) begin_particle<NS, TM>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
   while (r.stage != kStageDone) {
     const double *rec = P.tets[r.e].d;
     double raw[16];
@@ -43,10 +45,17 @@ __global__ void __launch_bounds__(256) walk_ldg_kernel(const KernelParams<NS> P)
       load_face_256(rec + 4 * f, raw[4 * f], raw[4 * f + 1], raw[4 * f + 2], raw[4 * f + 3]);
     ExitScan sc;
     scan_record(raw, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
-    advance<false, false, NS>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
+    advance<false, false, NS, TM>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
   }
   flush_counters(P, c);
 }
+
+template <int NS = 0>
+__global__ void __launch_bounds__(256) walk_ldg_kernel(const KernelParams<NS> P) { ldg_walk<NS, false>(P); }
+
+// The timed walk's arithmetic would take the kernel past 64 registers, from four resident blocks of 256 lanes
+// to three: it is held to the four its plain twin has.
+__global__ void __launch_bounds__(256, 4) walk_ldg_timed_kernel(const TimedWalkParams P) { ldg_walk<kMaxScores, true>(P); }
 
 // ------------------------------------------------------------ small kernels
 
@@ -267,6 +276,33 @@ cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block
       return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores>(p, n, stream);
     default:
       return cudaErrorInvalidValue;  // the experiments have no scored instantiation
+  }
+}
+
+cudaError_t launch_walk_timed(const TimedWalkParams &p, int variant, int block, cudaStream_t stream) {
+  const long long n = (long long)p.end - p.begin;
+  if (n <= 0) return cudaSuccess;
+  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores || p.sc.stride != score_stride(p.sc.nscores) ||
+      (!p.sc.responses && p.sc.nscores != 1))
+    return cudaErrorInvalidValue;
+  if (p.tm.nt < 1 || p.tm.nt > kMaxTimeBins || p.tm.slice < 0 || !p.tm.edges || !p.tm.times || !p.tm.speeds)
+    return cudaErrorInvalidValue;
+  if (block != 64 && block != 128 && block != 256) block = 128;
+  switch (variant) {
+    case kVariantLdg: {
+      const unsigned grid = (unsigned)((n + block - 1) / block);
+      walk_ldg_timed_kernel<<<grid, block, 0, stream>>>(p);
+      return cudaGetLastError();
+    }
+    case kVariantPersistRefill8:
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores, true>(p, n, stream);
+    case kVariantPersistGatherL1:
+      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores, true>(p, n, stream);
+    case kVariantPacked:
+      if (!p.rows) return cudaErrorInvalidValue;
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores, true>(p, n, stream);
+    default:
+      return cudaErrorInvalidValue;  // the experiments have no timed instantiation
   }
 }
 

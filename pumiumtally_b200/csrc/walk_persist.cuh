@@ -136,7 +136,7 @@ __device__ __forceinline__ void stage_load(const WalkParams &P, int chunk, Parti
 }
 
 // begin_particle() reading the staged copy instead of global memory (i: the slot's particle index)
-template <int NS = 0>
+template <int NS = 0, bool TM = false>
 __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const ParticleStage *st, int s,
                                                  Ray &r, Counters &c, int i = 0, const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -156,11 +156,11 @@ __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const Part
     }
   }
   if (P.dest)
-    start_tally_to<NS>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true, i, sl);
+    start_tally_to<NS, TM>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true, i, sl);
 }
 
 // begin_particle() for a packed row (only flying particles have rows).  Returns the particle id.
-template <int NS = 0>
+template <int NS = 0, bool TM = false>
 __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedRow *row, Ray &r, Counters &c,
                                               const ScoreLane *sl = nullptr) {
   const int id = row->id;
@@ -177,7 +177,7 @@ __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedR
     return id;
   }
   r.e = (int32_t)(el & kIdMask);
-  start_tally_to<NS>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
+  start_tally_to<NS, TM>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
   return id;
 }
 
@@ -306,7 +306,7 @@ __device__ __forceinline__ void stage_gather(const WalkParams &P, int id, int co
 // One crossing on the plane records.  Entry-face elision: after a crossing the face the ray came
 // in through is known (r.entry) and can never be the exit, so only the other three 32-byte
 // sectors of the record are fetched; the first tet of a ray needs all four.
-template <int FETCH, int NS = 0>
+template <int FETCH, int NS = 0, bool TM = false>
 __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r, Counters &c, uint64_t pol,
                                            const ScoreLane *sl = nullptr) {
   ExitScan sc;
@@ -331,8 +331,8 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r
     face_payload(q3[0], q3[1], q3[2], q3[3], r.e, 3, nb, bk);
     scan_face(sc, q3[0], q3[1], q3[2], q3[3], nb, bk, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
   }
-  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back, c,
-                                                                              true, sl);
+  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back,
+                                                                                  c, true, sl);
 }
 
 // Lean crossing step.  The compiler can sink the third record load of plane_step() below the arithmetic on
@@ -532,8 +532,14 @@ constexpr int kClaimRun = 4;  // gather mode: a warp takes up to this many conse
 // once per track, read once per crossing and score -- registers would cost 2 * NS of them, beyond the
 // budget of __launch_bounds__(BLOCK, MINB), and re-reading the caller's array per crossing would add NS
 // loads to the memory pipe the walk is bound by.
-template <int NS>
-using KernelParams = std::conditional_t<NS == 0, WalkParams, ScoredWalkParams>;
+// TM: timed walk (NS > 0): the lane's time state sits in three more slots next to its scores (TimeLane) and its
+// current bin in a per-lane int: 3.5 KB more per block of 128 lanes, no register held across the crossing loop.
+template <int NS, bool TM = false>
+using KernelParams = std::conditional_t<TM, TimedWalkParams, std::conditional_t<NS == 0, WalkParams, ScoredWalkParams>>;
+
+// Shared-memory rows of score_wl: the scores, and for the timed walk its three time slots.
+template <int NS, bool TM>
+constexpr int kLaneSlots = NS > 0 ? NS + (TM ? 3 : 0) : 1;
 
 // The lane's ScoreLane, built where it is used from the parameters and the thread index, so that nothing of
 // it stays live in registers across the crossing loop.  wl0: slot 0 of lane 0; STEP lanes per score.
@@ -543,8 +549,26 @@ __device__ __forceinline__ ScoreLane score_lane(const KernelParams<NS> &P, doubl
   else return ScoreLane{};
 }
 
-template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING, int NS = 0>
-__global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelParams<NS> P) {
+// score_lane() of the timed walk, plus the lane's bin slot (bin0: lane 0's); for TM == false exactly score_lane().
+template <int NS, int STEP, bool TM>
+__device__ __forceinline__ std::conditional_t<TM, TimeLane, ScoreLane> walk_lane(const KernelParams<NS, TM> &P, double *wl0,
+                                                                                 int32_t *bin0) {
+  if constexpr (TM) {
+    TimeLane tl;
+    tl.responses = P.sc.responses;
+    tl.wl = wl0 + threadIdx.x;
+    tl.n = P.sc.nscores;
+    tl.stride = P.sc.stride;
+    tl.step = STEP;
+    tl.bin = bin0 + threadIdx.x;
+    return tl;
+  } else {
+    return score_lane<NS, STEP>(P, wl0);
+  }
+}
+
+template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING, int NS = 0, bool TM = false>
+__global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelParams<NS, TM> P) {
   constexpr bool GATHER = STAGING == 1;
   constexpr bool PACKED = STAGING == 2;
   constexpr int WARPS = BLOCK / 32;
@@ -556,7 +580,9 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
   constexpr bool kEdge = FETCH == kFetchEdge;
   __shared__ double targets[kEdge ? BLOCK : 1][3];  // compact layout: each lane's ray target
   static_assert(NS == 0 || (!kEdge && !kRows), "scored walks run on the plane records");
-  __shared__ double score_wl[NS > 0 ? NS : 1][NS > 0 ? BLOCK : 1];  // scored walk: ScoreLane::wl of each lane
+  static_assert(!TM || NS > 0, "the timed walk is a scored walk");
+  __shared__ double score_wl[kLaneSlots<NS, TM>][NS > 0 ? BLOCK : 1];  // scored walk: ScoreLane::wl of each lane
+  __shared__ int32_t time_bin[TM ? BLOCK : 1];                          // timed walk: TimeLane::bin of each lane
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t bar0 = smem_u32(&bars[warp][0]);
   const uint32_t bar_row = bar0 + 16;
@@ -695,13 +721,13 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
       const int slot = cursor + __popc(idle & ((1u << lane) - 1u));
       if (r.stage == kStageDone && slot < cur_count) {
         if constexpr (PACKED) {
-          const ScoreLane sl = score_lane<NS, BLOCK>(P, &score_wl[0][0]);
-          my_i = begin_from_row<NS>(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c,
+          const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
+          my_i = begin_from_row<NS, TM>(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c,
                                     NS > 0 ? &sl : nullptr);
         } else {
           my_i = GATHER ? stages[warp][cur].id[slot] : P.begin + chunk_cur * kChunk + slot;
-          const ScoreLane sl = score_lane<NS, BLOCK>(P, &score_wl[0][0]);
-          begin_from_stage<NS>(P, &stages[warp][cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
+          const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
+          begin_from_stage<NS, TM>(P, &stages[warp][cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
         }
         if constexpr (FETCH == kFetchEdge) {
           g.dv = 0;
@@ -757,8 +783,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
       } else if constexpr (FETCH == kFetchLean || FETCH == kFetchLeanL1) {
         plane_step_lean<FETCH>(P, my_i, r, c, keep);
       } else {
-        const ScoreLane sl = score_lane<NS, BLOCK>(P, &score_wl[0][0]);
-        plane_step<FETCH, NS>(P, my_i, r, c, keep, NS > 0 ? &sl : nullptr);
+        const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
+        plane_step<FETCH, NS, TM>(P, my_i, r, c, keep, NS > 0 ? &sl : nullptr);
       }
     }
   }
@@ -771,8 +797,8 @@ inline int &last_persist_occupancy() {
   return occ;
 }
 
-template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1, int NS = 0>
-cudaError_t launch_persist(const KernelParams<NS> &p, long long n, cudaStream_t stream) {
+template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1, int NS = 0, bool TM = false>
+cudaError_t launch_persist(const KernelParams<NS, TM> &p, long long n, cudaStream_t stream) {
   static int sms = 0, occ = 0;
   if (!sms) {
     int dev = 0;
@@ -783,7 +809,7 @@ cudaError_t launch_persist(const KernelParams<NS> &p, long long n, cudaStream_t 
       // the scores' slots must not cost resident blocks: widen the carveout to what MINB blocks need
       cudaFuncAttributes fa{};
       int per_sm = 0, reserved = 0;
-      cudaFuncGetAttributes(&fa, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS>);
+      cudaFuncGetAttributes(&fa, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM>);
       cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
       cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
       if (per_sm > 0)
@@ -791,9 +817,9 @@ cudaError_t launch_persist(const KernelParams<NS> &p, long long n, cudaStream_t 
       carve = std::min(carve, 100);
     }
     // leave as much of the unified L1/smem array to shared memory as the kernel can use
-    cudaFuncSetAttribute(walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS>,
+    cudaFuncSetAttribute(walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM>,
                          cudaFuncAttributePreferredSharedMemoryCarveout, carve);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS>, BLOCK, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM>, BLOCK, 0);
     if (occ < 1) occ = 1;
   }
   last_persist_occupancy() = occ;
@@ -806,7 +832,7 @@ cudaError_t launch_persist(const KernelParams<NS> &p, long long n, cudaStream_t 
     e = cudaMemsetAsync(p.work_counter2, 0, sizeof(unsigned int), stream);
     if (e != cudaSuccess) return e;
   }
-  walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS><<<grid, BLOCK, 0, stream>>>(p);
+  walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM><<<grid, BLOCK, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -50,6 +50,12 @@ C_API = {
     "pumitally_move_to_next_location_device_scored": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                   C.c_void_p]),
+    "pumitally_set_time_bins": (C.c_int, [C.c_void_p, _dp, C.c_int32]),
+    "pumitally_get_time_bins": (C.c_int32, [C.c_void_p]),
+    "pumitally_move_to_next_location_timed": (C.c_int, [C.c_void_p, _dp, _dp, _bp, _dp, _dp, _dp, _dp, _ip, C.c_int32]),
+    "pumitally_move_to_next_location_device_timed": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                  C.c_void_p, C.c_int32, C.c_void_p]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -276,6 +282,76 @@ class PumiTally:
 
     def normalized_flux_scores(self):
         f, v = np.empty((self.score_bins, self.scores, self.num_elements)), np.empty(self.num_elements)
+        if self._L.pumitally_get_normalized_flux(self._h, f.ctypes.data_as(_dp), v.ctypes.data_as(_dp), f.size):
+            raise RuntimeError("get_normalized_flux failed")
+        return f, v
+
+    # ---- time filter -------------------------------------------------------------
+    def set_time_bins(self, edges):
+        """Time bins [edges[j], edges[j+1]) (finite, strictly increasing, 2..1025 edges; resets the tally).
+        ``None`` removes the filter."""
+        if edges is None:
+            rc = self._L.pumitally_set_time_bins(self._h, None, 0)
+        else:
+            e = np.ascontiguousarray(edges, dtype=np.float64).reshape(-1)
+            rc = self._L.pumitally_set_time_bins(self._h, e.ctypes.data_as(_dp), int(e.size))
+        if rc:
+            raise ValueError("set_time_bins failed")
+
+    @property
+    def time_bins(self) -> int:
+        """Number of time bins, 0 without a time filter."""
+        return int(self._L.pumitally_get_time_bins(self._h))
+
+    def MoveToNextLocationTimed(self, particle_origin, particle_destinations, flying, weights, times, speeds,
+                                responses=None, bins=None, size=None):
+        """Scored move whose segments are split between the time bins they span: times[i] is particle i's time at
+        its origin, speeds[i] its speed (mesh length units per time unit).  responses may be None with one score."""
+        o = _host_f64(particle_origin, "particle_origin")
+        d = _host_f64(particle_destinations, "particle_destinations")
+        w = _host_f64(weights, "weights")
+        t = _host_f64(times, "times")
+        v = _host_f64(speeds, "speeds")
+        if not (isinstance(flying, np.ndarray) and flying.dtype == np.int8 and flying.flags.c_contiguous):
+            raise TypeError("flying must be a contiguous int8 numpy array (the engine zeroes it)")
+        if t.size != w.size or v.size != w.size:
+            raise TypeError("times and speeds must hold one value per particle")
+        rp = None
+        if responses is not None:
+            r = _host_f64(responses, "responses")
+            if r.size != w.size * self.scores:
+                raise TypeError(f"responses must hold num_particles * {self.scores} values")
+            rp = r.ctypes.data_as(_dp)
+        bp = None
+        if bins is not None:
+            if not (isinstance(bins, np.ndarray) and bins.dtype == np.int32 and bins.flags.c_contiguous and bins.size == w.size):
+                raise TypeError("bins must be a contiguous int32 numpy array, one entry per particle")
+            bp = bins.ctypes.data_as(_ip)
+        size = o.size if size is None else int(size)
+        if self._L.pumitally_move_to_next_location_timed(self._h, o.ctypes.data_as(_dp), d.ctypes.data_as(_dp),
+                                                         flying.ctypes.data_as(_bp), w.ctypes.data_as(_dp),
+                                                         t.ctypes.data_as(_dp), v.ctypes.data_as(_dp), rp, bp, size):
+            raise RuntimeError("MoveToNextLocationTimed failed")
+
+    def move_device_timed(self, d_origin, d_dest, d_flying, d_weights, d_times, d_speeds, d_responses=None, d_bins=None,
+                          stream=None):
+        """Timed move on device addresses; enqueues on ``stream`` and returns."""
+        if self._L.pumitally_move_to_next_location_device_timed(self._h, d_origin, d_dest, d_flying, d_weights, d_times,
+                                                                d_speeds, d_responses, d_bins, 3 * self.num_particles,
+                                                                stream):
+            raise RuntimeError("MoveToNextLocationTimed(device) failed")
+
+    @property
+    def flux_time(self):
+        """Raw flux of every time bin, score bin and score: array [ntime, nbins, nscores, num_elements]."""
+        out = np.empty((max(self.time_bins, 1), self.score_bins, self.scores, self.num_elements))
+        if self._L.pumitally_get_flux(self._h, out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError("get_flux failed")
+        return out
+
+    def normalized_flux_time(self):
+        f = np.empty((max(self.time_bins, 1), self.score_bins, self.scores, self.num_elements))
+        v = np.empty(self.num_elements)
         if self._L.pumitally_get_normalized_flux(self._h, f.ctypes.data_as(_dp), v.ctypes.data_as(_dp), f.size):
             raise RuntimeError("get_normalized_flux failed")
         return f, v
