@@ -60,6 +60,11 @@ inline int MoveToNextLocationTimed(const PumiTally &tally, double *particle_orig
                                                weights, times, speeds, responses, bins, size);
 }
 
+// Linear flux moments (see pumitally_set_moments in pumitally_c.h): with order 1 every move, MoveToNextLocation
+// included, also tallies the first spatial moment of the flux in each element; pumitally_get_flux_gradient then
+// gives the gradient of the flux's linear projection.
+inline int SetMoments(const PumiTally &tally, int32_t order) { return pumitally_set_moments(engine_of(tally), order); }
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

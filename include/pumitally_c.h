@@ -122,8 +122,8 @@ int pumitally_set_output_name(pumitally_engine *e, const char *filename);
  * (crossing limit per walk; 0 = number of elements + 16, the default), "l2_fetch", "autotune"
  * (1 = default: while "variant" is automatic the engine times the streaming and the sorted/packed
  * kernel on moves 1-4 of every 64 and keeps the faster one).  Read-only: "launches", "staged",
- * "stage_host_us", "stage_sent_bytes", "scores", "time_bins", "walk_blocks_per_sm" (blocks per SM of
- * the last persistent walk kernel launched). */
+ * "stage_host_us", "stage_sent_bytes", "scores", "time_bins", "moments", "walk_blocks_per_sm" (blocks
+ * per SM of the last persistent walk kernel launched). */
 int pumitally_set_option(pumitally_engine *e, const char *name, int64_t value);
 int64_t pumitally_get_option(const pumitally_engine *e, const char *name);
 
@@ -286,6 +286,39 @@ int pumitally_move_to_next_location_device_timed(pumitally_engine *e, const doub
                                                  const double *d_weights, const double *d_times,
                                                  const double *d_speeds, const double *d_responses,
                                                  const int32_t *d_bins, int32_t size, void *stream);
+
+/* ---- additive: linear flux moments (first spatial moments of every track-length score) ----
+ * pumitally_set_moments(e, order): order 1 makes every move also tally, per element e, score, bin and
+ * time bin, the first moment of the track-length estimate about the element's centroid c_e: a segment of
+ * length l with midpoint x_mid adds w * r * l * (x_mid - c_e), an unbiased estimate of the integral of
+ * (x - c_e) * phi over the element.  Order 0 (the default) stops it; any other order, or a flux array that
+ * cannot be allocated (4 times the array without moments), returns non-zero and changes nothing.  The call
+ * resets the tally, combines with pumitally_set_score_bins, pumitally_set_scores and
+ * pumitally_set_time_bins in any order and is refused after pumitally_comm_init.
+ * pumitally_get_moments (or the read-only option "moments") returns the order.
+ * Every move tallies moments while they are set: the plain, binned, scored and timed moves, host and device,
+ * and PumiTally::MoveToNextLocation (the plain and binned moves as one score with every response 1; the
+ * rules that refuse a move with several scores or with time bins are unchanged).  Apart from the moments a
+ * move does exactly what it does without them: parent elements, positions, clipping, flying[] and the
+ * statistics are the same, and so is the flux (pumitally_get_flux, pumitally_get_normalized_flux,
+ * pumitally_get_flux_device and the VTK arrays return what they return without moments, up to the order of
+ * the reductions).
+ * pumitally_get_flux_moments(e, out, n) writes the raw first moments m1; pumitally_get_flux_gradient(e,
+ * out, n) writes g = M_e^-1 m1, M_e = integral over the element of (x - c_e)(x - c_e)^T, divided by the
+ * source-normalisation divisor of pumitally_get_normalized_flux: normalized_flux + g . (x - c_e) is then
+ * the L2 projection of the flux onto linear functions on the element (exact for a flux linear in it).
+ * Both are [time][bin][score][element][3] in the caller's element numbering, n = 3 * num_elements (time
+ * bin 0, bin 0, score 0) or 3 * ntime * nbins * nscores * num_elements; both follow the batch-end exchange
+ * as pumitally_get_flux does, and both return non-zero without moments.  WriteTallyResults writes, after
+ * every array it writes without moments, "<name>_grad": the normalised gradient, a 3-component cell array
+ * (the gradient of a sum over bins or time bins is the sum of the gradients).
+ * Behind pumitally_flux_device_ptr an element's record is [m0 of the S scores][Rx][Ry][Rz], S slots each
+ * (S = nscores padded to 1, 2, 4 or 8; stride 4 S), [time][bin][element][4 S] overall; R is the first
+ * moment about the mesh centre C (the middle of the bounding box), m1 = R - (c_e - C) * m0. */
+int pumitally_set_moments(pumitally_engine *e, int32_t order);
+int32_t pumitally_get_moments(const pumitally_engine *e);
+int pumitally_get_flux_moments(pumitally_engine *e, double *out, int64_t n);
+int pumitally_get_flux_gradient(pumitally_engine *e, double *out, int64_t n);
 
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */

@@ -215,6 +215,19 @@ int pumitally_move_to_next_location_device_timed(pumitally_engine *e, const doub
   });
 }
 
+int pumitally_set_moments(pumitally_engine *e, int32_t order) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_moments(order); });
+}
+int32_t pumitally_get_moments(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "moments")) : 0;
+}
+int pumitally_get_flux_moments(pumitally_engine *e, double *out, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_flux_moments(out, n); });
+}
+int pumitally_get_flux_gradient(pumitally_engine *e, double *out, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_flux_gradient(out, n); });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

@@ -263,9 +263,9 @@ void Engine::begin_move() {
   // sorting costs per particle, walking per crossing: with thousands of particles per tet (config c3) the
   // sorted variant cannot win and two exploration moves would cost more than an epoch can pay back
   if (int64_t(n_) > 16 * mesh_.ntets) return;
-  // a scored or timed move runs the kernel a plain move would run outside the exploration, and is never timed
-  // for it (its walk costs more per crossing): the tuner's clock counts plain moves only
-  if (cur_resp_ || cur_times_) {
+  // a scored, timed or moment move runs the kernel a plain move would run outside the exploration, and is never
+  // timed for it (its walk costs more per crossing): the tuner's clock counts plain moves only
+  if (cur_resp_ || cur_times_ || moments_) {
     move_variant_ = tuned_variant_;
     return;
   }
@@ -363,7 +363,8 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
   ScoredWalkParams &sp = tp;
   WalkParams &p = tp;
   const bool timed_walk = cur_times_ && d_dest;
-  const bool scored = (cur_resp_ || timed_walk) && d_dest;
+  // with moments every tallying move is a scored one; the plain and binned moves have one score and no responses
+  const bool scored = (cur_resp_ || timed_walk || moments_) && d_dest;
   if (scored) sp.sc = ScoreParams{cur_resp_, nscores_, stride_};
   if (timed_walk) tp.tm = TimeParams{d_edges_, cur_times_, cur_speeds_, ntime_, cur_slice_};
   p.tets = d_tets_;
@@ -453,13 +454,14 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
     p.flying = nullptr;  // order[] holds flying particles only
   }
   if (timed_walk) {
-    if (!walk_variant_available(variant) || launch_walk_timed(tp, variant, block_, stream) != cudaSuccess) {
+    if (!walk_variant_available(variant) || launch_walk_timed(tp, variant, block_, stream, moments_ > 0) != cudaSuccess) {
       fprintf(stderr, "[pumitally] ERROR: timed moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n", variant);
       return 1;
     }
   } else if (scored) {
-    if (!walk_variant_available(variant) || launch_walk_scored(sp, variant, block_, stream) != cudaSuccess) {
-      fprintf(stderr, "[pumitally] ERROR: scored moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n", variant);
+    if (!walk_variant_available(variant) || launch_walk_scored(sp, variant, block_, stream, moments_ > 0) != cudaSuccess) {
+      fprintf(stderr, "[pumitally] ERROR: scored and moment moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n",
+              variant);
       return 1;
     }
   } else {
@@ -694,7 +696,9 @@ bool Engine::refuse_untimed(const char *what) const {
 int Engine::move_to_next_location(const double *origin, const double *dest, int8_t *flying,
                                   const double *weights, int32_t size) {
   if (refuse_unscored("MoveToNextLocation")) return 1;
-  return move_host_entry(origin, dest, flying, weights, size);
+  const int rc = move_host_entry(origin, dest, flying, weights, size);
+  if (rc == 0 && moments_) ++scored_moves_;
+  return rc;
 }
 
 int Engine::move_host_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
@@ -1074,7 +1078,9 @@ int Engine::move_to_next_location_device(const double *d_origin, const double *d
                                          const int8_t *d_flying, const double *d_weights,
                                          int32_t size, cudaStream_t stream) {
   if (refuse_unscored("MoveToNextLocation(device)")) return 1;
-  return move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
+  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
+  if (rc == 0 && moments_) ++scored_moves_;
+  return rc;
 }
 
 int Engine::move_device_entry(const double *d_origin, const double *d_dest, const int8_t *d_flying,
@@ -1103,7 +1109,7 @@ int Engine::set_score_bins(int32_t nbins) {
     fprintf(stderr, "[pumitally] ERROR: set_score_bins after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins, nscores_, ntime_);
+  return resize_flux(nbins, nscores_, ntime_, moments_);
 }
 
 // Scores (walk_core.cuh, ScoreParams): the flux array becomes [bin][element][score_stride(nscores)].
@@ -1113,7 +1119,7 @@ int Engine::set_scores(int32_t nscores) {
     fprintf(stderr, "[pumitally] ERROR: set_scores after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores, ntime_);
+  return resize_flux(nbins_, nscores, ntime_, moments_);
 }
 
 // Time filter (walk_core.cuh, TimeParams): the flux array becomes [time][bin][element][stride], the edges live on
@@ -1124,7 +1130,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (!edges && nedges == 0) {  // no time filter
-    if (resize_flux(nbins_, nscores_, 0)) return 1;
+    if (resize_flux(nbins_, nscores_, 0, moments_)) return 1;
     cudaFree(d_edges_);
     d_edges_ = nullptr;
     return 0;
@@ -1139,7 +1145,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (cudaMemcpy(ne, edges, size_t(nedges) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
-      resize_flux(nbins_, nscores_, nedges - 1)) {
+      resize_flux(nbins_, nscores_, nedges - 1, moments_)) {
     cudaGetLastError();
     cudaFree(ne);
     return 1;
@@ -1149,9 +1155,19 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
   return 0;
 }
 
-int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime) {
+// Linear moments (walk_core.cuh, moment_tally): the element's record grows from S to kMomentSlots * S doubles.
+int Engine::set_moments(int32_t order) {
+  if (order != 0 && order != 1) return 1;
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_moments after comm_init (the exchange buffers are sized by then)\n");
+    return 1;
+  }
+  return resize_flux(nbins_, nscores_, ntime_, order);
+}
+
+int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments) {
   if (synchronize()) return 1;
-  const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores));
+  const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores)) * (moments ? kMomentSlots : 1);
   // [time][bin][element][stride], then the unreported array of the particles no bin matches
   const size_t len = (size_t(ntime > 0 ? ntime : 1) * size_t(nbins) + (nbins > 1 ? 1 : 0)) * E * stride + kFluxPad;
   double *nf = nullptr;
@@ -1169,6 +1185,7 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime) {
   nscores_ = nscores;
   stride_ = int32_t(stride);
   ntime_ = ntime;
+  moments_ = moments;
   if (nbins > 1 && !d_mask_) {
     PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
     PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_bins_), std::max<size_t>(size_t(n_), 4) * sizeof(int32_t)));
@@ -1182,7 +1199,9 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime) {
 int Engine::move_to_next_location_binned(const double *origin, const double *dest, int8_t *flying, const double *weights,
                                          const int32_t *bins, int32_t size) {
   if (refuse_unscored("MoveToNextLocationBinned")) return 1;
-  return move_binned_entry(origin, dest, flying, weights, bins, size);
+  const int rc = move_binned_entry(origin, dest, flying, weights, bins, size);
+  if (rc == 0 && moments_) ++scored_moves_;
+  return rc;
 }
 
 int Engine::move_binned_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
@@ -1247,6 +1266,7 @@ int Engine::move_to_next_location_device_binned(const double *d_origin, const do
   cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
   const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
   cur_bins_ = nullptr;
+  if (rc == 0 && moments_) ++scored_moves_;
   return rc;
 }
 
@@ -1522,6 +1542,58 @@ int Engine::get_flux(double *out, int64_t n) {
   return 0;
 }
 
+// The linear moments of every result array, [time][bin][score][element][3] in the caller's numbering: m1 about each
+// element's centroid, or the gradient g = M^-1 m1 divided by the source normalisation (linear_moments()).
+int Engine::copy_moments(std::vector<double> &out, bool gradient) {
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
+  const int slot = stride_ / kMomentSlots;
+  double per_source = 1.0;
+  if (gradient) {
+    per_source = source_normalization();
+    if (!(per_source > 0.0)) {
+      fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
+      return 1;
+    }
+  }
+  std::vector<double> raw(B * bin_len());
+  PTB_CUDA_OK(cudaMemcpy(raw.data(), flux_view(), raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  out.resize(B * S * E * 3);
+  const double *xyz = mesh_.coords.data();
+#pragma omp parallel for schedule(static)
+  for (int64_t i = 0; i < int64_t(E); ++i) {
+    double v[12];
+    for (int q = 0; q < 4; ++q)
+      for (int a = 0; a < 3; ++a) v[3 * q + a] = xyz[3 * size_t(mesh_.t2v[4 * i + q]) + a];
+    const size_t o = size_t(mesh_.orig_of_internal[i]);
+    for (size_t b = 0; b < B; ++b)
+      for (size_t k = 0; k < S; ++k) {
+        double m1[3], g[3];
+        linear_moments(v, mesh_.center, raw.data() + b * bin_len() + size_t(i) * size_t(stride_), slot, int(k), m1, g);
+        double *dst = out.data() + ((b * S + k) * E + o) * 3;
+        for (int a = 0; a < 3; ++a) dst[a] = gradient ? g[a] / per_source : m1[a];
+      }
+  }
+  return 0;
+}
+
+// n == 3E: time bin 0, bin 0, score 0; n == 3 * ntime * nbins * nscores * E: everything
+int Engine::get_moments_entry(double *out, int64_t n, bool gradient) {
+  const int64_t E = mesh_.ntets;
+  if (!moments_) {
+    fprintf(stderr, "[pumitally] ERROR: the engine tallies no moments (set_moments)\n");
+    return 1;
+  }
+  if (n != 3 * E && n != 3 * int64_t(result_arrays()) * nscores_ * E) return 1;
+  if (synchronize() || gather_shares()) return 1;
+  std::vector<double> all;
+  if (copy_moments(all, gradient)) return 1;
+  std::memcpy(out, all.data(), size_t(n) * sizeof(double));
+  return 0;
+}
+
+int Engine::get_flux_moments(double *out, int64_t n) { return get_moments_entry(out, n, false); }
+int Engine::get_flux_gradient(double *out, int64_t n) { return get_moments_entry(out, n, true); }
+
 // NormalizeFlux (PumiTallyImpl.cpp:382-409); n as for get_flux (the volumes are always E values)
 int Engine::get_normalized_flux(double *out_flux, double *out_volume, int64_t n) {
   const int64_t E = mesh_.ntets;
@@ -1666,6 +1738,7 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "score_bins") return nbins_;
   if (name == "scores") return nscores_;
   if (name == "time_bins") return ntime_;
+  if (name == "moments") return moments_;
   if (name == "walk_blocks_per_sm") return walk_blocks_per_sm();  // occupancy of the last persistent walk kernel launched
   if (name == "die_split") return die_split_ ? 1 : 0;
   if (name == "l2_partition0_sms") return die0_sms_;  // SMs in the L2 partition of SM 0 (0: no map found)
@@ -1815,11 +1888,30 @@ int Engine::write_tally_results() {
 // Scored or timed tally: "flux" and "flux_bin<b>" are score 0, exactly as a one-score engine writes them; every
 // score k >= 1 adds "score<k>" (the sum over the bins) and, with several bins, "score<k>_bin<b>".  With time bins
 // these are sums over the time bins, and every time bin j adds the same arrays with "_t<j>" after the score name:
-// "flux_t<j>", "flux_t<j>_bin<b>", "score<k>_t<j>", "score<k>_t<j>_bin<b>".
+// "flux_t<j>", "flux_t<j>_bin<b>", "score<k>_t<j>", "score<k>_t<j>_bin<b>".  With moments every one of these arrays
+// is followed by "<name>_grad", its normalised gradient (3 components; a sum's gradient is the sum of the gradients).
 int Engine::write_scored_results() {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_), T = nslices();
-  std::vector<double> all(T * B * S * E), vol(E);
+  std::vector<double> all(T * B * S * E), vol(E), grad;
   if (get_normalized_flux(all.data(), vol.data(), int64_t(all.size()))) return 1;
+  if (moments_ && copy_moments(grad, true)) return 1;
+  // the same sums for the gradients, 3 values per element: gsets[q] [bin][score][element][3], gsums[q * S + k]
+  std::vector<std::vector<double>> gsets, gsums;
+  if (moments_) {
+    gsets.emplace_back(grad.begin(), grad.begin() + B * S * E * 3);
+    for (size_t t = 1; t < T; ++t)
+      for (size_t i = 0; i < B * S * E * 3; ++i) gsets[0][i] += grad[t * B * S * E * 3 + i];
+    if (ntime_ > 0)
+      for (size_t t = 0; t < T; ++t)
+        gsets.emplace_back(grad.begin() + t * B * S * E * 3, grad.begin() + (t + 1) * B * S * E * 3);
+    for (size_t q = 0; q < gsets.size(); ++q)
+      for (size_t k = 0; k < S; ++k) {
+        std::vector<double> sum(gsets[q].begin() + k * E * 3, gsets[q].begin() + (k + 1) * E * 3);
+        for (size_t b = 1; b < B; ++b)
+          for (size_t i = 0; i < E * 3; ++i) sum[i] += gsets[q][(b * S + k) * E * 3 + i];
+        gsums.push_back(std::move(sum));
+      }
+  }
   // sets[0]: the sum over the time bins; sets[1 + j]: time bin j (only with a time filter).  [bin][score][element]
   std::vector<std::vector<double>> sets;
   sets.emplace_back(all.begin(), all.begin() + B * S * E);
@@ -1837,17 +1929,31 @@ int Engine::write_scored_results() {
         for (size_t i = 0; i < E; ++i) sum[i] += sets[q][(b * S + k) * E + i];
     }
   std::vector<std::pair<std::string, const double *>> extra;
+  std::vector<int> ncomp;
+  auto add = [&](const std::string &name, const double *a, const double *g) {
+    if (a) {
+      extra.emplace_back(name, a);
+      ncomp.push_back(1);
+    }
+    if (moments_) {
+      extra.emplace_back(name + "_grad", g);
+      ncomp.push_back(3);
+    }
+  };
   for (size_t q = 0; q < sets.size(); ++q) {
     const std::string t = q == 0 ? "" : "_t" + std::to_string(q - 1);
     for (size_t k = 0; k < S; ++k) {
       const std::string name = k == 0 ? "flux" + t : "score" + std::to_string(k) + t;
-      if (q > 0 || k > 0) extra.emplace_back(name, sums[q * S + k].data());  // (set 0, score 0 is the main array)
+      // (set 0, score 0 is the main array)
+      add(name, (q > 0 || k > 0) ? sums[q * S + k].data() : nullptr, moments_ ? gsums[q * S + k].data() : nullptr);
       if (B > 1)
-        for (size_t b = 0; b < B; ++b) extra.emplace_back(name + "_bin" + std::to_string(b), sets[q].data() + (b * S + k) * E);
+        for (size_t b = 0; b < B; ++b)
+          add(name + "_bin" + std::to_string(b), sets[q].data() + (b * S + k) * E,
+              moments_ ? gsets[q].data() + (b * S + k) * E * 3 : nullptr);
     }
   }
   std::string err;
-  if (!write_vtk_dataset(output_name_, mesh_, sums[0], vol, rank_, nranks_, &err, extra)) {
+  if (!write_vtk_dataset(output_name_, mesh_, sums[0], vol, rank_, nranks_, &err, extra, ncomp)) {
     fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
     return 1;
   }

@@ -79,6 +79,14 @@ class Engine {
                                          const double *d_weights, const double *d_times, const double *d_speeds,
                                          const double *d_responses, const int32_t *d_bins, int32_t size,
                                          cudaStream_t stream);
+  // Linear flux moments (walk_core.cuh, moment_tally): order 1 makes every move also tally the first spatial moment
+  // of every score, order 0 stops it.  Resets the tally; before comm_init.  Combines with bins, scores and time bins.
+  int set_moments(int32_t order);
+  int32_t moments() const { return moments_; }
+  // n == 3E: time bin 0, bin 0, score 0; n == 3 * ntime * nbins * nscores * E: everything,
+  // [time][bin][score][element][3].  m1 about each element's centroid (raw), or g = M^-1 m1 (normalised).
+  int get_flux_moments(double *out, int64_t n);
+  int get_flux_gradient(double *out, int64_t n);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -127,16 +135,21 @@ class Engine {
   int die0_sms_ = 0, nsms_ = 0;
   bool die_split_ = false;
   int32_t nbins_ = 1;
-  int32_t nscores_ = 1, stride_ = 1;  // scores, and doubles per element of d_flux_ (score_stride(nscores_))
+  int32_t nscores_ = 1, stride_ = 1;  // scores, and doubles per element of d_flux_ (score_stride(nscores_), times
+                                      // kMomentSlots with moments)
   int32_t ntime_ = 0;                 // time bins (0: no time filter)
+  int32_t moments_ = 0;               // moment order (0: none, 1: linear; walk_core.cuh, moment_tally)
   size_t flux_alloc_ = 0;             // doubles allocated at d_flux_
   // reported part of d_flux_: [time][bin][element][stride_]
   size_t nslices() const { return ntime_ > 0 ? size_t(ntime_) : 1; }
   size_t flux_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
   size_t bin_len() const { return size_t(mesh_.ntets) * size_t(stride_); }
   int32_t result_arrays() const { return int32_t(nslices()) * nbins_; }  // (time, bin) arrays of bin_len() doubles
-  bool multi_results() const { return nscores_ > 1 || ntime_ > 0; }      // results laid out [time][bin][score][element]
-  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime);
+  // results laid out [time][bin][score][element] (and read through the score-stride kernels)
+  bool multi_results() const { return nscores_ > 1 || ntime_ > 0 || moments_ > 0; }
+  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments);
+  int copy_moments(std::vector<double> &out, bool gradient);  // every result array, [time][bin][score][element][3]
+  int get_moments_entry(double *out, int64_t n, bool gradient);
   bool refuse_unscored(const char *what) const;
   bool refuse_untimed(const char *what) const;
   bool timed_args_ok(const char *what, const void *times, const void *speeds, const void *responses) const;

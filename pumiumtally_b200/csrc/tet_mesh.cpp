@@ -509,4 +509,38 @@ bool HostMesh::build_compact(std::string *err) {
   return true;
 }
 
+void linear_moments(const double v[12], const double C[3], const double *rec, int S, int k, double m1[3], double g[3]) {
+  double c[3], d[4][3];
+  for (int a = 0; a < 3; ++a) c[a] = 0.25 * (v[a] + v[3 + a] + v[6 + a] + v[9 + a]);
+  for (int i = 0; i < 4; ++i)
+    for (int a = 0; a < 3; ++a) d[i][a] = v[3 * i + a] - c[a];
+  const double m0 = rec[k];
+  for (int a = 0; a < 3; ++a) m1[a] = rec[(1 + a) * S + k] - (c[a] - C[a]) * m0;
+  // V from the edge vectors (the d_i differ from them by the same translation)
+  const double e1[3] = {d[1][0] - d[0][0], d[1][1] - d[0][1], d[1][2] - d[0][2]};
+  const double e2[3] = {d[2][0] - d[0][0], d[2][1] - d[0][1], d[2][2] - d[0][2]};
+  const double e3[3] = {d[3][0] - d[0][0], d[3][1] - d[0][1], d[3][2] - d[0][2]};
+  const double vol = std::fabs(e1[0] * (e2[1] * e3[2] - e2[2] * e3[1]) - e1[1] * (e2[0] * e3[2] - e2[2] * e3[0]) +
+                               e1[2] * (e2[0] * e3[1] - e2[1] * e3[0])) / 6.0;
+  double M[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
+  for (int i = 0; i < 4; ++i)
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) M[a][b] += d[i][a] * d[i][b];
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) M[a][b] *= vol / 20.0;
+  // symmetric 3x3 solve by the adjugate
+  const double A00 = M[1][1] * M[2][2] - M[1][2] * M[2][1], A01 = M[0][2] * M[2][1] - M[0][1] * M[2][2],
+               A02 = M[0][1] * M[1][2] - M[0][2] * M[1][1], A11 = M[0][0] * M[2][2] - M[0][2] * M[2][0],
+               A12 = M[0][2] * M[1][0] - M[0][0] * M[1][2], A22 = M[0][0] * M[1][1] - M[0][1] * M[1][0];
+  const double det = M[0][0] * A00 + M[0][1] * (M[1][2] * M[2][0] - M[1][0] * M[2][2]) + M[0][2] * (M[1][0] * M[2][1] - M[1][1] * M[2][0]);
+  if (!(std::fabs(det) > 0.0) || !std::isfinite(det)) {
+    g[0] = g[1] = g[2] = 0.0;
+    return;
+  }
+  const double inv = 1.0 / det;
+  g[0] = (A00 * m1[0] + A01 * m1[1] + A02 * m1[2]) * inv;
+  g[1] = (A01 * m1[0] + A11 * m1[1] + A12 * m1[2]) * inv;
+  g[2] = (A02 * m1[0] + A12 * m1[1] + A22 * m1[2]) * inv;
+}
+
 }  // namespace ptb

@@ -121,6 +121,13 @@ struct HostMesh {
   bool build_compact(std::string *err);
 };
 
+// Linear flux moments of one element from the walk's raw record (walk_core.cuh, moment_tally).  v: the element's
+// four vertices (12 doubles, the caller's coordinates); C: the centre the walk accumulated about (HostMesh::center);
+// rec: the element's record, S slots per moment ([m0][Rx][Ry][Rz]); k: the score.  Returns m1 = R - (c - C) m0, the
+// first moment about the centroid c, and g = M^-1 m1 with M = (V/20) sum_i (v_i - c)(v_i - c)^T, the gradient of the
+// flux's L2 projection onto linear functions on the element.  fp64; a degenerate element (M singular) gets g = 0.
+void linear_moments(const double v[12], const double C[3], const double *rec, int S, int k, double m1[3], double g[3]);
+
 // Generators / readers (tet_mesh.cpp, osh_reader.cpp)
 void build_kuhn_box(int nx, int ny, int nz, double lx, double ly, double lz,
                     std::vector<double> *coords, std::vector<int32_t> *t2v);

@@ -26,7 +26,9 @@ struct Block {
 
 bool write_vtk_dataset(const std::string &path, const HostMesh &m, const std::vector<double> &flux,
                        const std::vector<double> &volume, int rank, int nranks, std::string *err,
-                       const std::vector<std::pair<std::string, const double *>> &extra) {
+                       const std::vector<std::pair<std::string, const double *>> &extra,
+                       const std::vector<int> &extra_ncomp) {
+  auto ncomp = [&](size_t i) { return i < extra_ncomp.size() ? uint64_t(extra_ncomp[i]) : uint64_t(1); };
   if (!make_dir(path, err) || !make_dir(path + "/pieces", err)) return false;
   const uint64_t V = uint64_t(m.nverts), Etot = uint64_t(m.ntets);
   // One piece per rank.  After the batch-end exchange every rank holds the same global tally, so
@@ -53,7 +55,8 @@ bool write_vtk_dataset(const std::string &path, const HostMesh &m, const std::ve
   std::vector<Block> blocks = {{m.coords.data(), V * 24}, {conn.data() + 4 * e0, E * 16},
                                {offsets.data(), E * 4},   {types.data(), E},
                                {flux.data() + e0, E * 8}, {volume.data() + e0, E * 8}};
-  for (const auto &x : extra) blocks.push_back({x.second + e0, E * 8});  // whole-mesh arrays, caller's element order
+  for (size_t i = 0; i < extra.size(); ++i)  // whole-mesh arrays, caller's element order
+    blocks.push_back({extra[i].second + e0 * ncomp(i), E * 8 * ncomp(i)});
   std::vector<uint64_t> off(blocks.size());
   uint64_t acc = 0;
   for (size_t i = 0; i < blocks.size(); ++i) { off[i] = acc; acc += 8 + blocks[i].bytes; }
@@ -75,7 +78,8 @@ bool write_vtk_dataset(const std::string &path, const HostMesh &m, const std::ve
     << "<DataArray type=\"Float64\" Name=\"flux\" NumberOfComponents=\"1\" format=\"appended\" offset=\"" << off[4] << "\"/>\n"
     << "<DataArray type=\"Float64\" Name=\"volume\" NumberOfComponents=\"1\" format=\"appended\" offset=\"" << off[5] << "\"/>\n";
   for (size_t i = 0; i < extra.size(); ++i)
-    f << "<DataArray type=\"Float64\" Name=\"" << extra[i].first << "\" NumberOfComponents=\"1\" format=\"appended\" offset=\"" << off[6 + i] << "\"/>\n";
+    f << "<DataArray type=\"Float64\" Name=\"" << extra[i].first << "\" NumberOfComponents=\"" << ncomp(i)
+      << "\" format=\"appended\" offset=\"" << off[6 + i] << "\"/>\n";
   f << "</CellData>\n"
     << "</Piece>\n</UnstructuredGrid>\n<AppendedData encoding=\"raw\">\n_";
   for (size_t i = 0; i < blocks.size(); ++i) {
@@ -96,7 +100,8 @@ bool write_vtk_dataset(const std::string &path, const HostMesh &m, const std::ve
       << "<PCellData>\n"
       << "<PDataArray type=\"Float64\" Name=\"flux\" NumberOfComponents=\"1\"/>\n"
       << "<PDataArray type=\"Float64\" Name=\"volume\" NumberOfComponents=\"1\"/>\n";
-    for (const auto &x : extra) p << "<PDataArray type=\"Float64\" Name=\"" << x.first << "\" NumberOfComponents=\"1\"/>\n";
+    for (size_t i = 0; i < extra.size(); ++i)
+      p << "<PDataArray type=\"Float64\" Name=\"" << extra[i].first << "\" NumberOfComponents=\"" << ncomp(i) << "\"/>\n";
     p << "</PCellData>\n";
     for (int r = 0; r < nranks; ++r) p << "<Piece Source=\"pieces/piece_" << r << ".vtu\"/>\n";
     p << "</PUnstructuredGrid>\n</VTKFile>\n";

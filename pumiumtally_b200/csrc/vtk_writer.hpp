@@ -16,9 +16,12 @@ namespace ptb {
 // whole-mesh arrays in the caller's element order; rank r of nranks writes the
 // r-th contiguous slice of the elements as its piece, rank 0 also the .pvtu.
 // `extra`: further named Float64 cell arrays of the same shape (the per-bin fluxes of a filtered tally).
+// `extra_ncomp[i]`: components per element of extra[i], interleaved (3 for the flux gradients); 1 where the vector
+// is shorter.
 bool write_vtk_dataset(const std::string &path, const HostMesh &mesh,
                        const std::vector<double> &flux, const std::vector<double> &volume,
                        int rank, int nranks, std::string *err,
-                       const std::vector<std::pair<std::string, const double *>> &extra = {});
+                       const std::vector<std::pair<std::string, const double *>> &extra = {},
+                       const std::vector<int> &extra_ncomp = {});
 
 }  // namespace ptb

@@ -375,6 +375,35 @@ struct TimeLane : ScoreLane {
   int32_t *bin;
 };
 
+// ---- linear flux moments: the first spatial moment of every score ---------------------------------
+// A segment of length l from ray parameter p to q adds w * r * l to score k and, with moments, w * r * l * (mid - C)
+// to its first moment, mid = o + (p + q) / 2 * u the segment midpoint: the integral of (x - C) along a straight
+// segment is exactly l * (mid - C).  The kernel accumulates about the mesh centre C (Ray::ox.., WalkParams::cx..),
+// where the midpoint is already in registers; the host centres each element's record on its centroid c_e once at
+// read time (m1 = R - (c_e - C) * m0, linear_moments() in tet_mesh.cpp).  An element's record is
+// [m0 of scores 0..S-1][Rx 0..S-1][Ry 0..S-1][Rz 0..S-1], S = score_stride(nscores): its stride is 4 S doubles and
+// m0 of score k stays at slot k, so with one score the four reductions of a crossing are one 32-byte sector.
+constexpr int kMomentSlots = 4;
+
+// The moments of one segment: a = (q - p) * wl[k] of every score is the tally step's own operand, unchanged.
+template <int NS>
+PTB_HD void moment_tally(double *f, const ScoreLane *sl, double p, double q, double ox, double oy, double oz, double ux,
+                         double uy, double uz) {
+  const double s = 0.5 * (p + q);
+  const double mx = fma(s, ux, ox), my = fma(s, uy, oy), mz = fma(s, uz, oz);
+  const int S = sl->stride / kMomentSlots;
+  const double dt = q - p;
+PTB_UNROLL
+  for (int k = 0; k < NS; ++k)
+    if (k < sl->n) {
+      const double a = dt * sl->wl[k * sl->step];
+      PTB_TALLY_ADD(f + k, a);
+      PTB_TALLY_ADD(f + S + k, a * mx);
+      PTB_TALLY_ADD(f + 2 * S + k, a * my);
+      PTB_TALLY_ADD(f + 3 * S + k, a * mz);
+    }
+}
+
 constexpr int kStageReloc = 0;  // phase 1: move to caller's origin, tally off
 constexpr int kStageTally = 1;  // phase 2: fly to destination, tally on
 constexpr int kStageDone = 2;
@@ -438,8 +467,10 @@ PTB_HD void time_start(const TimedWalkParams &T, const TimeLane *tl, double t0, 
 // Timed walk, one crossing: the segment [tcur, tnew] (ray parameters) of element e.  While the exit time lies
 // beyond the current bin's upper edge, the segment is cut at the edge's ray parameter and the bins are walked
 // forward (time only increases along a ray).  A flight that ends exactly on an edge stays in the bin below.
-template <int NS>
-PTB_HD void time_tally(const TimedWalkParams &T, int32_t e, double tcur, double tnew, const TimeLane *tl) {
+// MO: every piece [p, pe] also adds its first moment (moment_tally), with the ray's origin o and direction u.
+template <int NS, bool MO = false>
+PTB_HD void time_tally(const TimedWalkParams &T, int32_t e, double tcur, double tnew, const TimeLane *tl,
+                       const Ray *ray = nullptr) {
   const int step = tl->step;
   double *wl = tl->wl;
   const double t0 = wl[NS * step], tpp = wl[(NS + 1) * step];
@@ -453,9 +484,13 @@ PTB_HD void time_tally(const TimedWalkParams &T, int32_t e, double tcur, double 
     if (j >= 0 && j < T.tm.nt) {
       const double dt = pe - p;
       double *fj = f + (size_t)j * (size_t)T.tm.slice;
+      if constexpr (MO) {
+        moment_tally<NS>(fj, tl, p, pe, ray->ox, ray->oy, ray->oz, ray->ux, ray->uy, ray->uz);
+      } else {
 PTB_UNROLL
-      for (int k = 0; k < NS; ++k)
-        if (k < tl->n) PTB_TALLY_ADD(fj + k, dt * wl[k * step]);
+        for (int k = 0; k < NS; ++k)
+          if (k < tl->n) PTB_TALLY_ADD(fj + k, dt * wl[k * step]);
+      }
     }
     if (!split) return;
     p = pe;
@@ -472,7 +507,8 @@ PTB_UNROLL
 // TM: timed walk (NS > 0, sl is a TimeLane): particle i's time and speed are read here too; a non-finite time
 // or a speed that is not finite and > 0 is a bad track like a non-finite weight.  No responses (nullptr):
 // every r[i,k] is 1.
-template <int NS = 0, bool TM = false>
+// MO: moment walk (NS > 0); responses may be nullptr here too (every r[i,k] 1), for the plain and binned moves.
+template <int NS = 0, bool TM = false, bool MO = false>
 PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, double z, double tx, double ty,
                            double tz, double w, Counters &c, bool writer, int i = 0,
                            const ScoreLane *sl = nullptr) {
@@ -498,7 +534,7 @@ PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, doub
 PTB_UNROLL
     for (int k = 0; k < NS; ++k)
       if (k < sl->n) {
-        const double wr = w * ((!TM || sl->responses) ? PTB_LDG(rp + k) : 1.0);
+        const double wr = w * ((!(TM || MO) || sl->responses) ? PTB_LDG(rp + k) : 1.0);
         bad = bad || !all_finite(wr, 0.0, 0.0);
         sl->wl[k * sl->step] = wr;
       }
@@ -519,10 +555,10 @@ PTB_UNROLL
   if (writer) c.tracks++;
 }
 
-template <int NS = 0, bool TM = false>
+template <int NS = 0, bool TM = false, bool MO = false>
 PTB_HD void start_tally(const WalkParams &P, int i, Ray &r, double x, double y, double z,
                         Counters &c, bool writer, const ScoreLane *sl = nullptr) {
-  start_tally_to<NS, TM>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
+  start_tally_to<NS, TM, MO>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
                      PTB_LDG(P.dest + 3 * (size_t)i + 2), PTB_LDG(P.weights + i), c, writer, i, sl);
 }
 
@@ -553,7 +589,7 @@ PTB_HD void start_reloc(const WalkParams &P, Ray &r, double x, double y, double 
 }
 
 // K1/K2/K3 of the reference folded into the prologue: pick the walk target.
-template <int NS = 0, bool TM = false>
+template <int NS = 0, bool TM = false, bool MO = false>
 PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool writer,
                            const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -574,14 +610,14 @@ PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool
       return;
     }
   }
-  if (P.dest) start_tally<NS, TM>(P, i, r, x, y, z, c, writer, sl);
+  if (P.dest) start_tally<NS, TM, MO>(P, i, r, x, y, z, c, writer, sl);
 }
 
 // The current ray ended (target reached, hull hit, or iteration limit).
 // kReloadTarget: the caller does not keep Ray::tx,ty,tz alive in registers (the compact-layout
 // kernel); the target is read back from the caller's array, where it came from: dest[] in the
 // tally phase, origin[] in phase 1.  Same values, six registers fewer in the crossing loop.
-template <bool kReloadTarget = false, int NS = 0, bool TM = false>
+template <bool kReloadTarget = false, int NS = 0, bool TM = false, bool MO = false>
 PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tnew, Counters &c,
                     bool writer, const ScoreLane *sl = nullptr) {
   // crossings of the ray that just ended: tally contributions in the tally phase, relocation crossings
@@ -611,7 +647,7 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
     x = fma(tnew, r.ux, r.ox) + P.cx; y = fma(tnew, r.uy, r.oy) + P.cy; z = fma(tnew, r.uz, r.oz) + P.cz;
   }
   if (r.stage != kStageTally && P.dest) {
-    start_tally<NS, TM>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
+    start_tally<NS, TM, MO>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
   } else {
     if (writer) {
       store_state(P.state + i, x, y, z, r.e);
@@ -623,14 +659,18 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
 // Functor body for one crossing, given the tracer's answer (texit, next).
 // NS > 0: scored walk (start_tally_to); one reduction per score into the element's scores.
 // TM: timed walk (time_tally); the same reductions, into the time bins the segment spans.
-template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0, bool TM = false>
+// MO: moment walk (NS > 0): each of those reductions comes with the three of its first moment (moment_tally).
+template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0, bool TM = false, bool MO = false>
 PTB_HD void advance(const WalkParams &P, int i, Ray &r, double texit, int32_t next, int32_t back,
                     Counters &c, bool writer, const ScoreLane *sl = nullptr) {
   const bool reached = !(texit < 1.0);  // last_exit == -1: destination inside this tet
   const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
   if constexpr (TM) {
     if (r.stage == kStageTally && writer)
-      time_tally<NS>(static_cast<const TimedWalkParams &>(P), r.e, r.tcur, tnew, static_cast<const TimeLane *>(sl));
+      time_tally<NS, MO>(static_cast<const TimedWalkParams &>(P), r.e, r.tcur, tnew, static_cast<const TimeLane *>(sl), &r);
+  } else if constexpr (MO) {
+    if (r.stage == kStageTally && writer)
+      moment_tally<NS>(P.flux + (size_t)r.e * sl->stride, sl, r.tcur, tnew, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
   } else if constexpr (NS > 0) {
     if (r.stage == kStageTally && writer) {
       const double dt = tnew - r.tcur;
@@ -653,7 +693,7 @@ PTB_UNROLL
   const bool over = r.iters >= P.max_iters;
   if (reached || hull || over) {
     if (over && !reached && !hull && writer && r.stage != kStageSeed) c.lost++;
-    end_ray<kReloadTarget, NS, TM>(P, i, r, reached, tnew, c, writer, sl);
+    end_ray<kReloadTarget, NS, TM, MO>(P, i, r, reached, tnew, c, writer, sl);
   } else {
     r.e = next;  // UpdateCurrentElement (Impl.cpp:247-253)
     r.entry = back;

@@ -27,7 +27,8 @@ namespace {
 
 // NS > 0: scored walk (walk_persist.cuh); the lanes' score slots are sized for the largest block.
 // TM: timed walk (NS > 0); the lanes' time slots sit next to the scores.
-template <int NS, bool TM>
+// MO: moment walk (NS > 0; walk_core.cuh, moment_tally).
+template <int NS, bool TM, bool MO = false>
 __device__ __forceinline__ void ldg_walk(const KernelParams<NS, TM> &P) {
   const int i = P.begin + blockIdx.x * blockDim.x + threadIdx.x;
   __shared__ double score_wl[kLaneSlots<NS, TM>][NS > 0 ? 256 : 1];
@@ -36,7 +37,7 @@ __device__ __forceinline__ void ldg_walk(const KernelParams<NS, TM> &P) {
   Counters c;
   Ray r;
   r.stage = kStageDone;
-  if (i < P.end) begin_particle<NS, TM>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
+  if (i < P.end) begin_particle<NS, TM, MO>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
   while (r.stage != kStageDone) {
     const double *rec = P.tets[r.e].d;
     double raw[16];
@@ -45,7 +46,7 @@ __device__ __forceinline__ void ldg_walk(const KernelParams<NS, TM> &P) {
       load_face_256(rec + 4 * f, raw[4 * f], raw[4 * f + 1], raw[4 * f + 2], raw[4 * f + 3]);
     ExitScan sc;
     scan_record(raw, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
-    advance<false, false, NS, TM>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
+    advance<false, false, NS, TM, MO>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
   }
   flush_counters(P, c);
 }
@@ -56,6 +57,14 @@ __global__ void __launch_bounds__(256) walk_ldg_kernel(const KernelParams<NS> P)
 // The timed walk's arithmetic would take the kernel past 64 registers, from four resident blocks of 256 lanes
 // to three: it is held to the four its plain twin has.
 __global__ void __launch_bounds__(256, 4) walk_ldg_timed_kernel(const TimedWalkParams P) { ldg_walk<kMaxScores, true>(P); }
+
+// The moment walks' arithmetic is held to the same four blocks.
+__global__ void __launch_bounds__(256, 4) walk_ldg_moments_kernel(const ScoredWalkParams P) {
+  ldg_walk<kMaxScores, false, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_timed_moments_kernel(const TimedWalkParams P) {
+  ldg_walk<kMaxScores, true, true>(P);
+}
 
 // ------------------------------------------------------------ small kernels
 
@@ -255,12 +264,30 @@ cudaError_t launch_walk(const WalkParams &p, int variant, int block, cudaStream_
   }
 }
 
-cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block, cudaStream_t stream) {
+cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block, cudaStream_t stream, bool moments) {
   const long long n = (long long)p.end - p.begin;
   if (n <= 0) return cudaSuccess;
-  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores || p.sc.stride != score_stride(p.sc.nscores) || !p.sc.responses)
+  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores ||
+      p.sc.stride != score_stride(p.sc.nscores) * (moments ? kMomentSlots : 1) ||
+      (!p.sc.responses && !(moments && p.sc.nscores == 1)))
     return cudaErrorInvalidValue;
   if (block != 64 && block != 128 && block != 256) block = 128;
+  if (moments) switch (variant) {
+    case kVariantLdg: {
+      const unsigned grid = (unsigned)((n + block - 1) / block);
+      walk_ldg_moments_kernel<<<grid, block, 0, stream>>>(p);
+      return cudaGetLastError();
+    }
+    case kVariantPersistRefill8:
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores, false, true>(p, n, stream);
+    case kVariantPersistGatherL1:
+      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores, false, true>(p, n, stream);
+    case kVariantPacked:
+      if (!p.rows) return cudaErrorInvalidValue;
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores, false, true>(p, n, stream);
+    default:
+      return cudaErrorInvalidValue;  // the experiments have no moment instantiation
+  }
   switch (variant) {
     case kVariantLdg: {
       const unsigned grid = (unsigned)((n + block - 1) / block);
@@ -279,15 +306,32 @@ cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block
   }
 }
 
-cudaError_t launch_walk_timed(const TimedWalkParams &p, int variant, int block, cudaStream_t stream) {
+cudaError_t launch_walk_timed(const TimedWalkParams &p, int variant, int block, cudaStream_t stream, bool moments) {
   const long long n = (long long)p.end - p.begin;
   if (n <= 0) return cudaSuccess;
-  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores || p.sc.stride != score_stride(p.sc.nscores) ||
+  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores ||
+      p.sc.stride != score_stride(p.sc.nscores) * (moments ? kMomentSlots : 1) ||
       (!p.sc.responses && p.sc.nscores != 1))
     return cudaErrorInvalidValue;
   if (p.tm.nt < 1 || p.tm.nt > kMaxTimeBins || p.tm.slice < 0 || !p.tm.edges || !p.tm.times || !p.tm.speeds)
     return cudaErrorInvalidValue;
   if (block != 64 && block != 128 && block != 256) block = 128;
+  if (moments) switch (variant) {
+    case kVariantLdg: {
+      const unsigned grid = (unsigned)((n + block - 1) / block);
+      walk_ldg_timed_moments_kernel<<<grid, block, 0, stream>>>(p);
+      return cudaGetLastError();
+    }
+    case kVariantPersistRefill8:
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores, true, true>(p, n, stream);
+    case kVariantPersistGatherL1:
+      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores, true, true>(p, n, stream);
+    case kVariantPacked:
+      if (!p.rows) return cudaErrorInvalidValue;
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores, true, true>(p, n, stream);
+    default:
+      return cudaErrorInvalidValue;  // the experiments have no moment instantiation
+  }
   switch (variant) {
     case kVariantLdg: {
       const unsigned grid = (unsigned)((n + block - 1) / block);

@@ -136,7 +136,7 @@ __device__ __forceinline__ void stage_load(const WalkParams &P, int chunk, Parti
 }
 
 // begin_particle() reading the staged copy instead of global memory (i: the slot's particle index)
-template <int NS = 0, bool TM = false>
+template <int NS = 0, bool TM = false, bool MO = false>
 __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const ParticleStage *st, int s,
                                                  Ray &r, Counters &c, int i = 0, const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -156,11 +156,11 @@ __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const Part
     }
   }
   if (P.dest)
-    start_tally_to<NS, TM>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true, i, sl);
+    start_tally_to<NS, TM, MO>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true, i, sl);
 }
 
 // begin_particle() for a packed row (only flying particles have rows).  Returns the particle id.
-template <int NS = 0, bool TM = false>
+template <int NS = 0, bool TM = false, bool MO = false>
 __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedRow *row, Ray &r, Counters &c,
                                               const ScoreLane *sl = nullptr) {
   const int id = row->id;
@@ -177,7 +177,7 @@ __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedR
     return id;
   }
   r.e = (int32_t)(el & kIdMask);
-  start_tally_to<NS, TM>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
+  start_tally_to<NS, TM, MO>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
   return id;
 }
 
@@ -306,7 +306,7 @@ __device__ __forceinline__ void stage_gather(const WalkParams &P, int id, int co
 // One crossing on the plane records.  Entry-face elision: after a crossing the face the ray came
 // in through is known (r.entry) and can never be the exit, so only the other three 32-byte
 // sectors of the record are fetched; the first tet of a ray needs all four.
-template <int FETCH, int NS = 0, bool TM = false>
+template <int FETCH, int NS = 0, bool TM = false, bool MO = false>
 __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r, Counters &c, uint64_t pol,
                                            const ScoreLane *sl = nullptr) {
   ExitScan sc;
@@ -331,7 +331,7 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r
     face_payload(q3[0], q3[1], q3[2], q3[3], r.e, 3, nb, bk);
     scan_face(sc, q3[0], q3[1], q3[2], q3[3], nb, bk, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
   }
-  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back,
+  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM, MO>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back,
                                                                                   c, true, sl);
 }
 
@@ -567,7 +567,7 @@ __device__ __forceinline__ std::conditional_t<TM, TimeLane, ScoreLane> walk_lane
   }
 }
 
-template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING, int NS = 0, bool TM = false>
+template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING, int NS = 0, bool TM = false, bool MO = false>
 __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelParams<NS, TM> P) {
   constexpr bool GATHER = STAGING == 1;
   constexpr bool PACKED = STAGING == 2;
@@ -722,12 +722,12 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
       if (r.stage == kStageDone && slot < cur_count) {
         if constexpr (PACKED) {
           const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-          my_i = begin_from_row<NS, TM>(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c,
+          my_i = begin_from_row<NS, TM, MO>(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c,
                                     NS > 0 ? &sl : nullptr);
         } else {
           my_i = GATHER ? stages[warp][cur].id[slot] : P.begin + chunk_cur * kChunk + slot;
           const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-          begin_from_stage<NS, TM>(P, &stages[warp][cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
+          begin_from_stage<NS, TM, MO>(P, &stages[warp][cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
         }
         if constexpr (FETCH == kFetchEdge) {
           g.dv = 0;
@@ -784,7 +784,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
         plane_step_lean<FETCH>(P, my_i, r, c, keep);
       } else {
         const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-        plane_step<FETCH, NS, TM>(P, my_i, r, c, keep, NS > 0 ? &sl : nullptr);
+        plane_step<FETCH, NS, TM, MO>(P, my_i, r, c, keep, NS > 0 ? &sl : nullptr);
       }
     }
   }
@@ -797,7 +797,8 @@ inline int &last_persist_occupancy() {
   return occ;
 }
 
-template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1, int NS = 0, bool TM = false>
+template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1, int NS = 0, bool TM = false,
+          bool MO = false>
 cudaError_t launch_persist(const KernelParams<NS, TM> &p, long long n, cudaStream_t stream) {
   static int sms = 0, occ = 0;
   if (!sms) {
@@ -809,7 +810,7 @@ cudaError_t launch_persist(const KernelParams<NS, TM> &p, long long n, cudaStrea
       // the scores' slots must not cost resident blocks: widen the carveout to what MINB blocks need
       cudaFuncAttributes fa{};
       int per_sm = 0, reserved = 0;
-      cudaFuncGetAttributes(&fa, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM>);
+      cudaFuncGetAttributes(&fa, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>);
       cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
       cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
       if (per_sm > 0)
@@ -817,9 +818,9 @@ cudaError_t launch_persist(const KernelParams<NS, TM> &p, long long n, cudaStrea
       carve = std::min(carve, 100);
     }
     // leave as much of the unified L1/smem array to shared memory as the kernel can use
-    cudaFuncSetAttribute(walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM>,
+    cudaFuncSetAttribute(walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>,
                          cudaFuncAttributePreferredSharedMemoryCarveout, carve);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM>, BLOCK, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>, BLOCK, 0);
     if (occ < 1) occ = 1;
   }
   last_persist_occupancy() = occ;
@@ -832,7 +833,7 @@ cudaError_t launch_persist(const KernelParams<NS, TM> &p, long long n, cudaStrea
     e = cudaMemsetAsync(p.work_counter2, 0, sizeof(unsigned int), stream);
     if (e != cudaSuccess) return e;
   }
-  walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM><<<grid, BLOCK, 0, stream>>>(p);
+  walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO><<<grid, BLOCK, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -56,6 +56,10 @@ C_API = {
     "pumitally_move_to_next_location_device_timed": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                   C.c_void_p, C.c_int32, C.c_void_p]),
+    "pumitally_set_moments": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_get_moments": (C.c_int32, [C.c_void_p]),
+    "pumitally_get_flux_moments": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pumitally_get_flux_gradient": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -355,6 +359,32 @@ class PumiTally:
         if self._L.pumitally_get_normalized_flux(self._h, f.ctypes.data_as(_dp), v.ctypes.data_as(_dp), f.size):
             raise RuntimeError("get_normalized_flux failed")
         return f, v
+
+    # ---- linear flux moments -------------------------------------------------------
+    def set_moments(self, order: int):
+        """1: every move also tallies the first spatial moment of each score in each element; 0: no moments (the
+        default).  Resets the tally."""
+        if self._L.pumitally_set_moments(self._h, int(order)):
+            raise ValueError("set_moments failed")
+
+    @property
+    def moments(self) -> int:
+        """Moment order, 0 without moments."""
+        return int(self._L.pumitally_get_moments(self._h))
+
+    def _moment_array(self, fn, what):
+        out = np.empty((max(self.time_bins, 1), self.score_bins, self.scores, self.num_elements, 3))
+        if fn(self._h, out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError(f"{what} failed")
+        return out
+
+    def flux_moments(self):
+        """Raw first moments about each element's centroid: array [ntime, nbins, nscores, num_elements, 3]."""
+        return self._moment_array(self._L.pumitally_get_flux_moments, "get_flux_moments")
+
+    def flux_gradient(self):
+        """Normalised flux gradient of each element's linear flux, shaped as flux_moments()."""
+        return self._moment_array(self._L.pumitally_get_flux_gradient, "get_flux_gradient")
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
