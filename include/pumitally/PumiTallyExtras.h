@@ -65,6 +65,17 @@ inline int MoveToNextLocationTimed(const PumiTally &tally, double *particle_orig
 // gives the gradient of the flux's linear projection.
 inline int SetMoments(const PumiTally &tally, int32_t order) { return pumitally_set_moments(engine_of(tally), order); }
 
+// Point queries (see pumitally_locate_points in pumitally_c.h): the element containing each of npts points (AoS xyz),
+// -1 outside the mesh; and every normalised result at the points, [time][bin][score][point], n = npts or
+// ntime * nbins * nscores * npts (the linear reconstruction with moments, NaN outside).  out_elem may be nullptr.
+inline int LocatePoints(const PumiTally &tally, const double *xyz, int64_t npts, int32_t *out_elem) {
+  return pumitally_locate_points(engine_of(tally), xyz, npts, out_elem);
+}
+inline int EvaluatePoints(const PumiTally &tally, const double *xyz, int64_t npts, double *out, int64_t n,
+                          int32_t *out_elem = nullptr) {
+  return pumitally_evaluate_points(engine_of(tally), xyz, npts, out, n, out_elem);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

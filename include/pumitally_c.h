@@ -320,6 +320,31 @@ int32_t pumitally_get_moments(const pumitally_engine *e);
 int pumitally_get_flux_moments(pumitally_engine *e, double *out, int64_t n);
 int pumitally_get_flux_gradient(pumitally_engine *e, double *out, int64_t n);
 
+/* ---- additive: point queries (locate points in the mesh, evaluate the results there) ----
+ * For consumers whose points are not the tally's elements (a thermal or CFD solver's quadrature points or nodes, a
+ * collision estimator, a mesh source or weight-window lookup).  Points are npts AoS coordinates (x, y, z), caller's
+ * frame; npts may exceed 2^31.  A query may be made at any time after construction (before CopyInitialPosition too)
+ * and changes nothing: particle positions and elements, the tally, the statistics and the kernel auto-tuner are the
+ * same before and after it.
+ * pumitally_locate_points writes the element (caller's numbering) containing each point to out_elem[npts], -1 for a
+ * point outside the mesh or with a non-finite coordinate.  This holds on convex and non-convex meshes (notches,
+ * voids).  A point on a face, edge or vertex shared by several elements gets one of them.  A point within 1e-10 times
+ * the mesh extent (the longest edge of its bounding box) of the hull may get a hull element or -1.
+ * pumitally_locate_points_device does the same on device arrays, enqueued on `stream` (no synchronisation).
+ * Host-pointer calls work through device buffers of the option "chunk" points, whatever npts is.
+ * pumitally_evaluate_points writes the normalised result of every time bin, score bin and score at each point to
+ * out, [time][bin][score][point]: n = npts (time bin 0, bin 0, score 0) or ntime * nbins * nscores * npts, anything
+ * else returns non-zero.  The value is pumitally_get_normalized_flux's for the containing element e, plus, with
+ * moments, g_e . (x - c_e) (g_e as pumitally_get_flux_gradient returns it, c_e the average of e's four vertices);
+ * NaN outside the mesh.  It follows the batch-end exchange and the source normalisation as
+ * pumitally_get_normalized_flux does (after pumitally_reduce_tally_to_owners it gathers the shares: collective) and
+ * fails where it fails.  out_elem[npts] receives the elements as pumitally_locate_points does, or is NULL. */
+int pumitally_locate_points(pumitally_engine *e, const double *xyz, int64_t npts, int32_t *out_elem);
+int pumitally_locate_points_device(pumitally_engine *e, const double *d_xyz, int64_t npts, int32_t *d_elem,
+                                   void *stream);
+int pumitally_evaluate_points(pumitally_engine *e, const double *xyz, int64_t npts, double *out, int64_t n,
+                              int32_t *out_elem);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

@@ -228,6 +228,20 @@ int pumitally_get_flux_gradient(pumitally_engine *e, double *out, int64_t n) {
   return guarded(e, [&](ptb::Engine &g) { return g.get_flux_gradient(out, n); });
 }
 
+int pumitally_locate_points(pumitally_engine *e, const double *xyz, int64_t npts, int32_t *out_elem) {
+  return guarded(e, [&](ptb::Engine &g) { return g.locate_points(xyz, npts, out_elem); });
+}
+int pumitally_locate_points_device(pumitally_engine *e, const double *d_xyz, int64_t npts, int32_t *d_elem,
+                                   void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.locate_points_device(d_xyz, npts, d_elem, static_cast<cudaStream_t>(stream));
+  });
+}
+int pumitally_evaluate_points(pumitally_engine *e, const double *xyz, int64_t npts, double *out, int64_t n,
+                              int32_t *out_elem) {
+  return guarded(e, [&](ptb::Engine &g) { return g.evaluate_points(xyz, npts, out, n, out_elem); });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

@@ -185,6 +185,9 @@ Engine::~Engine() {
   cudaFree(d_cell_rank_);
   cudaFree(d_pcell_); cudaFree(d_order_); cudaFree(d_cell_count_); cudaFree(d_cell_sums_);
   cudaFree(d_work_count_);
+  cudaFree(d_cand_off_); cudaFree(d_cand_);
+  cudaFree(d_qxyz_); cudaFree(d_qout_); cudaFree(d_qint_); cudaFree(d_qelem_);
+  cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
   if (compute_) cudaStreamDestroy(compute_);
   if (copy_) cudaStreamDestroy(copy_);
 }
@@ -326,7 +329,7 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   }
   last_stream_ = stream;
   last_stream_set_ = true;
-  if (d_dest) flux_global_valid_ = flux_owned_only_ = false;  // the local tally moves on; the last exchange no longer describes it
+  if (d_dest) flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on; the last exchange no longer describes it
   cur_slice_ = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
   if (!(cur_bins_ && d_dest)) return launch_range_into(d_flux_, d_origin, d_dest, d_flying, d_weights, begin, end, stream, timed);
   // Score filter: particles are independent and a particle that does not fly is not touched, so the range
@@ -1656,6 +1659,7 @@ int Engine::set_source_normalization(int mode, double value) {
   if (mode < 0 || mode > 3 || (mode == 2 && !(value > 0.0))) return 1;
   norm_mode_ = mode;
   norm_value_ = value;
+  eval_valid_ = false;
   return 0;
 }
 
@@ -1681,7 +1685,7 @@ int Engine::reset_tally() {
   PTB_CUDA_OK(cudaMemset(d_flux_, 0, flux_alloc_ * sizeof(double)));
   scored_moves_ = 0;
   PTB_CUDA_OK(cudaMemset(d_stats_, 0, sizeof(DeviceStats)));
-  flux_global_valid_ = flux_owned_only_ = false;
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
   kernel_ms_ = 0.0;
   h2d_bytes_ = 0.0;
   moves_ = 0;
@@ -1739,6 +1743,7 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "scores") return nscores_;
   if (name == "time_bins") return ntime_;
   if (name == "moments") return moments_;
+  if (name == "locate_candidates") return int64_t(cand_entries_);  // entries of the point-location candidate lists
   if (name == "walk_blocks_per_sm") return walk_blocks_per_sm();  // occupancy of the last persistent walk kernel launched
   if (name == "die_split") return die_split_ ? 1 : 0;
   if (name == "l2_partition0_sms") return die0_sms_;  // SMs in the L2 partition of SM 0 (0: no map found)
@@ -1960,6 +1965,166 @@ int Engine::write_scored_results() {
   return 0;
 }
 
+// ------------------------------------------------------------------ point queries
+
+namespace {
+double mesh_extent(const HostMesh &m) {
+  return std::max({m.bbox_hi[0] - m.bbox_lo[0], m.bbox_hi[1] - m.bbox_lo[1], m.bbox_hi[2] - m.bbox_lo[2]});
+}
+}  // namespace
+
+LocateParams Engine::locate_params() const {
+  LocateParams p{};
+  p.tets = d_tets_;
+  p.grid = grid_;  // the seeds are used whatever the relocation walks do (option seed_grid)
+  p.max_iters = max_iters_ > 0 ? max_iters_ : int32_t(std::min<int64_t>(mesh_.ntets + 16, INT_MAX));
+  p.cx = mesh_.center[0]; p.cy = mesh_.center[1]; p.cz = mesh_.center[2];
+  p.sx = mesh_.centroid0[0]; p.sy = mesh_.centroid0[1]; p.sz = mesh_.centroid0[2];
+  p.start_elem = mesh_.start_elem;
+  p.convex = mesh_.hull_convex ? 1 : 0;
+  p.cand_off = d_cand_off_;
+  p.cand = d_cand_;
+  p.slack = kLocateSlack * mesh_extent(mesh_);
+  return p;
+}
+
+// A convex hull needs no candidate lists: a walk that meets it proves the point outside.
+int Engine::ensure_candidates() {
+  if (mesh_.hull_convex || candidates_ready_) return 0;
+  std::vector<int64_t> off;
+  std::vector<int32_t> tets;
+  cell_candidates(mesh_, grid_, kLocateBand * mesh_extent(mesh_), &off, &tets);
+  PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_cand_off_), off.size() * sizeof(int64_t)));
+  PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_cand_), std::max<size_t>(tets.size(), 1) * sizeof(int32_t)));
+  PTB_CUDA_OK(cudaMemcpy(d_cand_off_, off.data(), off.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
+  PTB_CUDA_OK(cudaMemcpy(d_cand_, tets.data(), tets.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+  cand_entries_ = tets.size();
+  candidates_ready_ = true;
+  return 0;
+}
+
+int Engine::ensure_query_buffers(size_t pts, size_t out_doubles) {
+  if (pts > q_cap_) {
+    cudaFree(d_qxyz_); cudaFree(d_qint_); cudaFree(d_qelem_);
+    d_qxyz_ = nullptr; d_qint_ = d_qelem_ = nullptr;
+    q_cap_ = 0;
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qxyz_), 3 * pts * sizeof(double)));
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qint_), pts * sizeof(int32_t)));
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qelem_), pts * sizeof(int32_t)));
+    q_cap_ = pts;
+  }
+  if (out_doubles > q_out_cap_) {
+    cudaFree(d_qout_);
+    d_qout_ = nullptr;
+    q_out_cap_ = 0;
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qout_), out_doubles * sizeof(double)));
+    q_out_cap_ = out_doubles;
+  }
+  return 0;
+}
+
+int Engine::locate_points(const double *xyz, int64_t npts, int32_t *out_elem) {
+  if (npts < 0 || (npts > 0 && (!xyz || !out_elem))) return 1;
+  if (npts == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const int64_t chunk = std::min<int64_t>(chunk_, npts);
+  if (ensure_element_maps() || ensure_candidates() || ensure_query_buffers(size_t(chunk), 0)) return 1;
+  const LocateParams p = locate_params();
+  for (int64_t b = 0; b < npts; b += chunk) {
+    const int64_t cnt = std::min(chunk, npts - b);
+    PTB_CUDA_OK(cudaMemcpyAsync(d_qxyz_, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
+    PTB_CUDA_OK(launch_locate(p, d_qxyz_, cnt, nullptr, d_qelem_, d_orig_of_internal_, compute_));
+    PTB_CUDA_OK(cudaMemcpyAsync(out_elem + b, d_qelem_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
+// The mesh tables a query reads never change after construction, so it needs no ordering against moves.
+int Engine::locate_points_device(const double *d_xyz, int64_t npts, int32_t *d_elem, cudaStream_t stream) {
+  if (npts < 0 || (npts > 0 && (!d_xyz || !d_elem))) return 1;
+  if (npts == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_element_maps() || ensure_candidates()) return 1;
+  const LocateParams p = locate_params();
+  const int64_t step = int64_t(1) << 30;  // points per launch
+  for (int64_t b = 0; b < npts; b += step)
+    PTB_CUDA_OK(launch_locate(p, d_xyz + 3 * b, std::min(step, npts - b), nullptr, d_elem + b,
+                              d_orig_of_internal_, stream));
+  return 0;
+}
+
+// The normalised results exactly as get_normalized_flux computes them (normalize_scores), and with moments the
+// gradient get_flux_gradient returns (copy_moments: linear_moments() in fp64 on the host), in internal element order.
+int Engine::build_eval_table() {
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
+  const double per_source = source_normalization();
+  if (!(per_source > 0.0)) {
+    fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
+    return 1;
+  }
+  cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
+  d_eval_vals_ = d_eval_grads_ = d_eval_cen_ = nullptr;
+  PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_eval_vals_), std::max<size_t>(B * S * E, 1) * sizeof(double)));
+  for (size_t b = 0; b < B; ++b)
+    PTB_CUDA_OK(launch_normalize_scores(flux_view() + b * bin_len(), d_volume_, d_eval_vals_ + b * S * E, int64_t(E),
+                                        nscores_, stride_, per_source, compute_));
+  if (moments_) {
+    std::vector<double> g;  // [time][bin][score][caller's element][3]
+    if (copy_moments(g, true)) return 1;
+    std::vector<double> gi(g.size()), cen(3 * E);
+    const double *xyz = mesh_.coords.data();
+#pragma omp parallel for schedule(static)
+    for (int64_t i = 0; i < int64_t(E); ++i) {
+      const size_t o = size_t(mesh_.orig_of_internal[i]);
+      for (size_t r = 0; r < B * S; ++r)
+        for (int a = 0; a < 3; ++a) gi[(r * E + size_t(i)) * 3 + a] = g[(r * E + o) * 3 + a];
+      for (int a = 0; a < 3; ++a) {  // the vertex average, as linear_moments() forms it
+        const int32_t *v = &mesh_.t2v[4 * size_t(i)];
+        cen[3 * size_t(i) + a] = 0.25 * (xyz[3 * size_t(v[0]) + a] + xyz[3 * size_t(v[1]) + a] + xyz[3 * size_t(v[2]) + a] +
+                                         xyz[3 * size_t(v[3]) + a]);
+      }
+    }
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_eval_grads_), std::max<size_t>(gi.size(), 1) * sizeof(double)));
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_eval_cen_), std::max<size_t>(cen.size(), 1) * sizeof(double)));
+    PTB_CUDA_OK(cudaMemcpy(d_eval_grads_, gi.data(), gi.size() * sizeof(double), cudaMemcpyHostToDevice));
+    PTB_CUDA_OK(cudaMemcpy(d_eval_cen_, cen.data(), cen.size() * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  eval_valid_ = true;
+  return 0;
+}
+
+int Engine::evaluate_points(const double *xyz, int64_t npts, double *out, int64_t n, int32_t *out_elem) {
+  const int64_t R = int64_t(result_arrays()) * nscores_;
+  if (npts < 0 || (npts > 0 && (!xyz || !out)) || (n != npts && n != R * npts)) {
+    fprintf(stderr, "[pumitally] ERROR: evaluate_points: n must be npts or ntime * nbins * nscores * npts (%lld)\n",
+            (long long)(R * npts));
+    return 1;
+  }
+  if (synchronize() || gather_shares()) return 1;
+  if (!eval_valid_ && build_eval_table()) return 1;
+  if (npts == 0) return 0;
+  const int64_t rows = n == npts ? 1 : R;
+  // the results of a chunk are at most 256 MB of device memory
+  const int64_t chunk = std::min<int64_t>(std::min<int64_t>(chunk_, std::max<int64_t>(1024, (int64_t(1) << 25) / rows)), npts);
+  if (ensure_element_maps() || ensure_candidates() || ensure_query_buffers(size_t(chunk), size_t(rows * chunk))) return 1;
+  const LocateParams p = locate_params();
+  for (int64_t b = 0; b < npts; b += chunk) {
+    const int64_t cnt = std::min(chunk, npts - b);
+    PTB_CUDA_OK(cudaMemcpyAsync(d_qxyz_, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
+    PTB_CUDA_OK(launch_locate(p, d_qxyz_, cnt, d_qint_, out_elem ? d_qelem_ : nullptr, d_orig_of_internal_, compute_));
+    PTB_CUDA_OK(launch_evaluate(d_qxyz_, d_qint_, cnt, d_eval_vals_, moments_ ? d_eval_grads_ : nullptr, d_eval_cen_,
+                                mesh_.ntets, int32_t(rows), d_qout_, cnt, compute_));
+    PTB_CUDA_OK(cudaMemcpy2DAsync(out + b, size_t(npts) * sizeof(double), d_qout_, size_t(cnt) * sizeof(double),
+                                  size_t(cnt) * sizeof(double), size_t(rows), cudaMemcpyDeviceToHost, compute_));
+    if (out_elem)
+      PTB_CUDA_OK(cudaMemcpyAsync(out_elem + b, d_qelem_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
 // ------------------------------------------------------------------ multi-GPU
 
 int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
@@ -2031,6 +2196,7 @@ int Engine::allreduce_tally() {
   if (cudaEventElapsedTime(&ms, ev_ar0_, ev_ar1_) == cudaSuccess) allreduce_ms_ = ms;
   flux_global_valid_ = true;
   flux_owned_only_ = false;
+  eval_valid_ = false;
   return 0;
 }
 
@@ -2046,6 +2212,7 @@ int Engine::reduce_tally_to_owners() {
   if (cudaEventElapsedTime(&ms, ev_ar0_, ev_ar1_) == cudaSuccess) allreduce_ms_ = ms;
   flux_global_valid_ = true;
   flux_owned_only_ = true;
+  eval_valid_ = false;
   return 0;
 }
 

@@ -87,6 +87,14 @@ class Engine {
   // [time][bin][score][element][3].  m1 about each element's centroid (raw), or g = M^-1 m1 (normalised).
   int get_flux_moments(double *out, int64_t n);
   int get_flux_gradient(double *out, int64_t n);
+  // Point queries (walk_core.cuh, locate_point).  locate: the element (caller's numbering) containing each of npts
+  // points (AoS xyz), -1 outside the mesh or for a non-finite coordinate.  evaluate: every normalised result at each
+  // point, [time][bin][score][point] (n == npts: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * npts:
+  // everything), get_normalized_flux's value of the element plus g . (x - c_e) with moments, NaN outside; out_elem may be
+  // nullptr.  Host calls work through chunk-sized device buffers.  A query changes no particle, tally or statistic.
+  int locate_points(const double *xyz, int64_t npts, int32_t *out_elem);
+  int locate_points_device(const double *d_xyz, int64_t npts, int32_t *d_elem, cudaStream_t stream);  // enqueue only
+  int evaluate_points(const double *xyz, int64_t npts, double *out, int64_t n, int32_t *out_elem);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -161,6 +169,24 @@ class Engine {
   int move_scored_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
                         const double *responses, const int32_t *bins, int32_t size);
   int copy_results(std::vector<double> &out, bool normalized);
+  // ---- point queries (locate_kernels.cu) ----
+  LocateParams locate_params() const;
+  int ensure_candidates();  // non-convex hull: the cells' candidate lists, built and uploaded at the first query
+  int64_t *d_cand_off_ = nullptr;
+  int32_t *d_cand_ = nullptr;
+  size_t cand_entries_ = 0;
+  bool candidates_ready_ = false;
+  // chunk-sized buffers of the host-pointer queries: points, internal and caller's element ids, results
+  size_t q_cap_ = 0, q_out_cap_ = 0;
+  double *d_qxyz_ = nullptr, *d_qout_ = nullptr;
+  int32_t *d_qint_ = nullptr, *d_qelem_ = nullptr;
+  int ensure_query_buffers(size_t pts, size_t out_doubles);
+  // evaluation table, internal element order: vals [R][E] normalised results, with moments grads [R][E][3] (the
+  // normalised gradient) and cen [E][3] (vertex-average centroids); valid until the next move, reset, exchange or change
+  // of the source normalisation or of the configuration
+  bool eval_valid_ = false;
+  double *d_eval_vals_ = nullptr, *d_eval_grads_ = nullptr, *d_eval_cen_ = nullptr;
+  int build_eval_table();
   int write_scored_results();  // everything, [time][bin][score][element], caller's order
   // per-particle doubles of a host-pointer move on their way to the device (upload_doubles)
   struct AuxUpload {

@@ -1,0 +1,79 @@
+// sm_90a kernels of the point queries: locate arbitrary points in the mesh (walk_core.cuh, locate_point) and evaluate
+// the normalised results there.  Thread per point; nothing here touches the particle state, the tally or the
+// statistics.
+#include <cmath>
+
+#include "walk_kernels.hpp"
+
+namespace ptb {
+namespace {
+
+// One tet record as four 32-byte sectors, two 128-bit read-only loads each.
+__device__ __forceinline__ void fetch_record(const TetRecord *tets, int32_t e, double (&r)[16]) {
+  const double *p = tets[e].d;
+#pragma unroll
+  for (int f = 0; f < 4; ++f)
+    asm volatile(
+        "ld.global.nc.v2.f64 {%0,%1}, [%4];\n\t"
+        "ld.global.nc.v2.f64 {%2,%3}, [%4+16];"
+        : "=d"(r[4 * f]), "=d"(r[4 * f + 1]), "=d"(r[4 * f + 2]), "=d"(r[4 * f + 3])
+        : "l"(p + 4 * f));
+}
+
+// internal[i]: the internal element id of point i (for the evaluation kernel), out[i]: the caller's element id; either
+// may be nullptr.
+__global__ void __launch_bounds__(256) locate_kernel(const LocateParams P, const double *__restrict__ xyz, int64_t n,
+                                                     int32_t *__restrict__ internal,
+                                                     int32_t *__restrict__ out, const int32_t *__restrict__ orig_of_internal) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double x = __ldg(xyz + 3 * i), y = __ldg(xyz + 3 * i + 1), z = __ldg(xyz + 3 * i + 2);
+  const int32_t e = locate_point(P, x, y, z, [&](int32_t t, double (&r)[16]) { fetch_record(P.tets, t, r); });
+  if (internal) internal[i] = e;
+  if (out) out[i] = e >= 0 ? __ldg(orig_of_internal + e) : -1;
+}
+
+// out[r * pitch + i] = vals[r * E + e] (+ grads[r * E + e] . (x - cen[e]) with moments) for the R results of the
+// element e = internal[i] that contains point i; NaN where e < 0.
+__global__ void __launch_bounds__(256) evaluate_kernel(const double *__restrict__ xyz, const int32_t *__restrict__ internal,
+                                                       int64_t n, const double *__restrict__ vals,
+                                                       const double *__restrict__ grads, const double *__restrict__ cen,
+                                                       int64_t E, int32_t R, double *__restrict__ out, int64_t pitch) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t e = internal[i];
+  if (e < 0) {
+    for (int32_t r = 0; r < R; ++r) out[r * pitch + i] = __longlong_as_double(0x7ff8000000000000ll);
+    return;
+  }
+  double dx = 0.0, dy = 0.0, dz = 0.0;
+  if (grads) {
+    dx = xyz[3 * i] - __ldg(cen + 3 * (int64_t)e);
+    dy = xyz[3 * i + 1] - __ldg(cen + 3 * (int64_t)e + 1);
+    dz = xyz[3 * i + 2] - __ldg(cen + 3 * (int64_t)e + 2);
+  }
+  for (int32_t r = 0; r < R; ++r) {
+    const int64_t j = r * E + e;
+    double v = __ldg(vals + j);
+    if (grads) v += __ldg(grads + 3 * j) * dx + __ldg(grads + 3 * j + 1) * dy + __ldg(grads + 3 * j + 2) * dz;
+    out[r * pitch + i] = v;
+  }
+}
+
+}  // namespace
+
+cudaError_t launch_locate(const LocateParams &p, const double *xyz, int64_t n, int32_t *internal, int32_t *out,
+                          const int32_t *orig_of_internal, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  locate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, xyz, n, internal, out, orig_of_internal);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_evaluate(const double *xyz, const int32_t *internal, int64_t n, const double *vals, const double *grads,
+                            const double *cen, int64_t E, int32_t R, double *out, int64_t pitch, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  evaluate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(xyz, internal, n, vals, grads, cen, E, R, out, pitch);
+  return cudaGetLastError();
+}
+
+}  // namespace ptb

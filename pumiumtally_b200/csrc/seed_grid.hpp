@@ -59,4 +59,49 @@ inline std::vector<int32_t> morton_cell_ranks(const SeedGrid &g) {
   return rank;
 }
 
+// Candidate tets of every grid cell for point location on a non-convex hull (locate_point in walk_core.cuh): CSR
+// lists, off[c] .. off[c + 1] of `tets` hold the internal ids of the tets whose bounding box, widened by `pad`,
+// overlaps cell c (closed intervals).  A tet that contains a point of the cell is therefore in the cell's list.
+inline void cell_candidates(const HostMesh &m, const SeedGrid &g, double pad, std::vector<int64_t> *off,
+                            std::vector<int32_t> *tets) {
+  const int64_t ncell = int64_t(g.nx) * g.ny * g.nz;
+  const int n[3] = {g.nx, g.ny, g.nz};
+  const double lo[3] = {g.x0, g.y0, g.z0};
+  auto range = [&](int64_t e, int lo_c[3], int hi_c[3]) {
+    for (int d = 0; d < 3; ++d) {
+      double a = m.coords[3 * size_t(m.t2v[4 * e]) + d], b = a;
+      for (int q = 1; q < 4; ++q) {
+        const double v = m.coords[3 * size_t(m.t2v[4 * e + q]) + d];
+        a = std::min(a, v);
+        b = std::max(b, v);
+      }
+      // cell k covers [lo + k h, lo + (k + 1) h]
+      const double fa = std::floor((a - pad - lo[d]) * g.inv_h) - 1.0, fb = std::floor((b + pad - lo[d]) * g.inv_h) + 1.0;
+      lo_c[d] = int(std::min(std::max(fa, 0.0), double(n[d] - 1)));
+      hi_c[d] = int(std::min(std::max(fb, 0.0), double(n[d] - 1)));
+      // trim the one-cell margin the floor above leaves for rounding, keeping every cell that overlaps
+      while (lo_c[d] < hi_c[d] && lo[d] + (lo_c[d] + 1) * g.h < a - pad) ++lo_c[d];
+      while (hi_c[d] > lo_c[d] && lo[d] + hi_c[d] * g.h > b + pad) --hi_c[d];
+    }
+  };
+  off->assign(size_t(ncell) + 1, 0);
+  for (int64_t e = 0; e < m.ntets; ++e) {
+    int a[3], b[3];
+    range(e, a, b);
+    for (int z = a[2]; z <= b[2]; ++z)
+      for (int y = a[1]; y <= b[1]; ++y)
+        for (int x = a[0]; x <= b[0]; ++x) ++(*off)[size_t((int64_t(z) * g.ny + y) * g.nx + x) + 1];
+  }
+  for (int64_t c = 0; c < ncell; ++c) (*off)[size_t(c) + 1] += (*off)[size_t(c)];
+  tets->resize(size_t((*off)[size_t(ncell)]));
+  std::vector<int64_t> cur(off->begin(), off->end() - 1);
+  for (int64_t e = 0; e < m.ntets; ++e) {
+    int a[3], b[3];
+    range(e, a, b);
+    for (int z = a[2]; z <= b[2]; ++z)
+      for (int y = a[1]; y <= b[1]; ++y)
+        for (int x = a[0]; x <= b[0]; ++x) (*tets)[size_t(cur[size_t((int64_t(z) * g.ny + y) * g.nx + x)]++)] = int32_t(e);
+  }
+}
+
 }  // namespace ptb

@@ -701,4 +701,91 @@ PTB_UNROLL
   }
 }
 
+// ---- point location: the element that contains an arbitrary point ---------------------------------
+// The walk of a relocation with tallying off, without a particle.  The point's seed-grid cell gives the start: the
+// cell's seed point and tet, or, for a cell without a seed on a convex hull, the centroid of the start element (where
+// localisation starts).  The walk runs over the plane records to the point and the tet it ends in contains it; on a
+// convex hull a walk that meets the hull proves the point outside.  On any other hull, a point whose walk meets the
+// hull, whose cell has no seed, or whose walk is stopped by the iteration limit is tested against the cell's candidate
+// tets instead (every tet whose bounding box overlaps the cell, a CSR list built on the host: cell_candidates() in
+// seed_grid.hpp) with the four face planes of each record.
+//
+// Hull band: a point closer than kLocateBand * extent to the hull (extent = the longest edge of the bounding box) may
+// get a hull tet or -1.  The walk decides such points on the hull planes, which are stored ~1e-13 * extent outwards
+// (tet_mesh.cpp); the candidate test accepts a point within kLocateSlack * extent of a tet when no tet contains it
+// strictly.  A point outside the bounding box, or with a non-finite coordinate, gets -1.
+constexpr double kLocateBand = 1e-10;
+constexpr double kLocateSlack = 1e-12;
+
+struct LocateParams : WalkParams {  // uses tets, grid (cell_tet), max_iters and the mesh centre cx, cy, cz
+  double sx, sy, sz;                // centroid of the start element (caller's coordinates)
+  int32_t start_elem;               // internal id of the start element
+  int32_t convex;                   // HostMesh::hull_convex
+  const int64_t *cand_off;          // [ncell + 1] candidate list of each cell; nullptr on a convex hull
+  const int32_t *cand;              // internal tet ids
+  double slack;                     // kLocateSlack * extent
+};
+
+// Face planes of record r against the mesh-centred point p: is n.p <= c + slack for all four?
+PTB_HD bool record_contains(const double (&r)[16], double px, double py, double pz, double slack) {
+  bool in = true;
+PTB_UNROLL
+  for (int f = 0; f < 4; ++f)
+    in = in && (r[4 * f + 3] - (r[4 * f] * px + r[4 * f + 1] * py + r[4 * f + 2] * pz) >= -slack);
+  return in;
+}
+
+// Exact fallback: the first of the cell's candidates that contains the point strictly, else the first within the
+// slack, else -1.  fetch(e, r) loads record e into r[16].
+template <class Fetch>
+PTB_HD int32_t locate_candidates(const LocateParams &P, int64_t cell, double px, double py, double pz, Fetch &&fetch) {
+  if (!P.cand_off) return -1;
+  const int64_t a = PTB_LDG(P.cand_off + cell), b = PTB_LDG(P.cand_off + cell + 1);
+  int32_t near = -1;
+  for (int64_t k = a; k < b; ++k) {
+    const int32_t t = PTB_LDG(P.cand + k);
+    double r[16];
+    fetch(t, r);
+    if (record_contains(r, px, py, pz, 0.0)) return t;
+    if (near < 0 && record_contains(r, px, py, pz, P.slack)) near = t;
+  }
+  return near;
+}
+
+// Internal id of the element containing (x, y, z) (caller's coordinates), -1 outside the mesh.  Touches no particle.
+template <class Fetch>
+PTB_HD int32_t locate_point(const LocateParams &P, double x, double y, double z, Fetch &&fetch) {
+  if (!all_finite(x, y, z)) return -1;
+  const SeedGrid &g = P.grid;
+  const double fx = (x - g.x0) * g.inv_h, fy = (y - g.y0) * g.inv_h, fz = (z - g.z0) * g.inv_h;
+  if (!(fx >= 0.0 && fy >= 0.0 && fz >= 0.0 && fx < (double)g.nx && fy < (double)g.ny && fz < (double)g.nz)) return -1;
+  const int cx = (int)fx, cy = (int)fy, cz = (int)fz;
+  const int64_t cell = ((int64_t)cz * g.ny + cy) * g.nx + cx;
+  const int32_t seed = PTB_LDG(g.cell_tet + cell);
+  Ray r;
+  if (seed >= 0) {
+    double sx, sy, sz;
+    seed_point(g, cx, cy, cz, sx, sy, sz);
+    set_ray(P, r, sx, sy, sz, x, y, z);
+    r.e = seed;
+  } else if (P.convex) {
+    set_ray(P, r, P.sx, P.sy, P.sz, x, y, z);
+    r.e = P.start_elem;
+  } else {
+    return locate_candidates(P, cell, x - P.cx, y - P.cy, z - P.cz, fetch);
+  }
+  for (;;) {
+    double rec[16];
+    fetch(r.e, rec);
+    ExitScan sc;
+    scan_record(rec, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
+    if (!(exit_parameter(sc) < 1.0)) return r.e;  // the point lies in this tet
+    const bool hull = sc.nbr < 0;
+    if (hull && P.convex) return -1;  // left a convex mesh on the way to the point: it is outside
+    if (hull || ++r.iters >= P.max_iters) break;
+    r.e = sc.nbr;
+  }
+  return locate_candidates(P, cell, x - P.cx, y - P.cy, z - P.cz, fetch);
+}
+
 }  // namespace ptb

@@ -126,4 +126,13 @@ cudaError_t launch_bin_mask(const int8_t *flying, const int32_t *bins, int32_t b
 cudaError_t launch_sum_flying_weights(const int8_t *flying, const double *weights, int32_t begin, int32_t end,
                                       double *total, cudaStream_t stream);
 
+// locate_kernels.cu.  Point location of n points (AoS xyz), thread per point (locate_point).  internal[i] <- internal
+// element id, out[i] <- caller's id (-1: outside); either may be nullptr.  n < 2^39.
+cudaError_t launch_locate(const LocateParams &p, const double *xyz, int64_t n, int32_t *internal, int32_t *out,
+                          const int32_t *orig_of_internal, cudaStream_t stream);
+// out[r * pitch + i] = vals[r * E + e] (+ grads[(r * E + e) * 3 ..] . (xyz_i - cen[3 e ..]) when grads != nullptr) for
+// r < R, e = internal[i]; NaN where e < 0.
+cudaError_t launch_evaluate(const double *xyz, const int32_t *internal, int64_t n, const double *vals, const double *grads,
+                            const double *cen, int64_t E, int32_t R, double *out, int64_t pitch, cudaStream_t stream);
+
 }  // namespace ptb

@@ -60,6 +60,9 @@ C_API = {
     "pumitally_get_moments": (C.c_int32, [C.c_void_p]),
     "pumitally_get_flux_moments": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pumitally_get_flux_gradient": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pumitally_locate_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _ip]),
+    "pumitally_locate_points_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "pumitally_evaluate_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, C.c_int64, _ip]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -385,6 +388,50 @@ class PumiTally:
     def flux_gradient(self):
         """Normalised flux gradient of each element's linear flux, shaped as flux_moments()."""
         return self._moment_array(self._L.pumitally_get_flux_gradient, "get_flux_gradient")
+
+    # ---- point queries -------------------------------------------------------------
+    @staticmethod
+    def _points(points):
+        p = _host_f64(points, "points")
+        if p.size % 3:
+            raise TypeError("points must hold x, y, z per point")
+        return p, p.size // 3
+
+    def locate(self, points):
+        """Element (caller's numbering) containing each point of ``points`` [npts, 3]; -1 outside the mesh."""
+        p, npts = self._points(points)
+        out = np.empty(npts, dtype=np.int32)
+        if self._L.pumitally_locate_points(self._h, p.ctypes.data_as(_dp), npts, out.ctypes.data_as(_ip)):
+            raise RuntimeError("locate_points failed")
+        return out
+
+    def locate_device(self, points, stream=None):
+        """locate() on a contiguous float64 CUDA tensor [npts, 3]: returns an int32 CUDA tensor, enqueued on ``stream``
+        (default: the current torch stream)."""
+        import torch
+
+        if not (points.is_cuda and points.dtype == torch.float64 and points.is_contiguous() and points.numel() % 3 == 0):
+            raise TypeError("points must be a contiguous float64 CUDA tensor of shape [npts, 3]")
+        npts = points.numel() // 3
+        out = torch.empty(npts, dtype=torch.int32, device=points.device)
+        if stream is None:
+            stream = torch.cuda.current_stream(points.device).cuda_stream
+        if self._L.pumitally_locate_points_device(self._h, points.data_ptr(), npts, out.data_ptr(), stream):
+            raise RuntimeError("locate_points_device failed")
+        return out
+
+    def evaluate(self, points, first_only=False):
+        """Normalised results at the points: (values [ntime, nbins, nscores, npts] -- the linear reconstruction with
+        moments, NaN outside the mesh -- and the elements as locate() gives them).  first_only: values [npts] of time
+        bin 0, bin 0, score 0."""
+        p, npts = self._points(points)
+        shape = (npts,) if first_only else (max(self.time_bins, 1), self.score_bins, self.scores, npts)
+        out = np.empty(shape)
+        elem = np.empty(npts, dtype=np.int32)
+        if self._L.pumitally_evaluate_points(self._h, p.ctypes.data_as(_dp), npts, out.ctypes.data_as(_dp), out.size,
+                                             elem.ctypes.data_as(_ip)):
+            raise RuntimeError("evaluate_points failed")
+        return out, elem
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
