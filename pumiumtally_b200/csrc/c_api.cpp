@@ -52,6 +52,24 @@ int guarded(pumitally_engine *e, F &&f) {
   }
 }
 
+// The particle data of a move; a device move never writes `flying`.
+ptb::Move move_of(const double *origin, const double *dest, const int8_t *flying, const double *weights, int32_t size,
+                  const ptb::MoveTally &tally = {}) {
+  return ptb::Move{origin, dest, const_cast<int8_t *>(flying), weights, size, tally};
+}
+
+int host_move(pumitally_engine *e, const char *what, const ptb::Move &m) {
+  if (m.size > 0 && (!m.origin || !m.dest || !m.flying || !m.weights)) {
+    fprintf(stderr, "[pumitally] ERROR: %s: null input array\n", what);
+    return 1;
+  }
+  return guarded(e, [&](ptb::Engine &g) { return g.move_to_next_location(m); });
+}
+
+int device_move(pumitally_engine *e, const ptb::Move &m, void *stream) {
+  return guarded(e, [&](ptb::Engine &g) { return g.move_to_next_location_device(m, static_cast<cudaStream_t>(stream)); });
+}
+
 }  // namespace
 
 extern "C" {
@@ -94,13 +112,7 @@ int pumitally_copy_initial_position(pumitally_engine *e, const double *xyz, int3
 
 int pumitally_move_to_next_location(pumitally_engine *e, const double *origin, const double *dest,
                                     int8_t *flying, const double *weights, int32_t size) {
-  if (size > 0 && (!origin || !dest || !flying || !weights)) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation: null input array\n");
-    return 1;
-  }
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location(origin, dest, flying, weights, size);
-  });
+  return host_move(e, "MoveToNextLocation", move_of(origin, dest, flying, weights, size));
 }
 
 int pumitally_write_tally_results(pumitally_engine *e) {
@@ -146,19 +158,12 @@ int32_t pumitally_get_score_bins(const pumitally_engine *e) {
 }
 int pumitally_move_to_next_location_binned(pumitally_engine *e, const double *origin, const double *dest,
                                            int8_t *flying, const double *weights, const int32_t *bins, int32_t size) {
-  if (size > 0 && (!origin || !dest || !flying || !weights)) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation: null input array\n");
-    return 1;
-  }
-  return guarded(e, [&](ptb::Engine &g) { return g.move_to_next_location_binned(origin, dest, flying, weights, bins, size); });
+  return host_move(e, "MoveToNextLocation", move_of(origin, dest, flying, weights, size, {ptb::MoveTally::kPlain, bins}));
 }
 int pumitally_move_to_next_location_device_binned(pumitally_engine *e, const double *d_origin, const double *d_dest,
                                                   const int8_t *d_flying, const double *d_weights, const int32_t *d_bins,
                                                   int32_t size, void *stream) {
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location_device_binned(d_origin, d_dest, d_flying, d_weights, d_bins, size,
-                                                 static_cast<cudaStream_t>(stream));
-  });
+  return device_move(e, move_of(d_origin, d_dest, d_flying, d_weights, size, {ptb::MoveTally::kPlain, d_bins}), stream);
 }
 
 int pumitally_set_scores(pumitally_engine *e, int32_t nscores) {
@@ -170,22 +175,15 @@ int32_t pumitally_get_scores(const pumitally_engine *e) {
 int pumitally_move_to_next_location_scored(pumitally_engine *e, const double *origin, const double *dest, int8_t *flying,
                                            const double *weights, const double *responses, const int32_t *bins,
                                            int32_t size) {
-  if (size > 0 && (!origin || !dest || !flying || !weights)) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: null input array\n");
-    return 1;
-  }
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location_scored(origin, dest, flying, weights, responses, bins, size);
-  });
+  return host_move(e, "MoveToNextLocationScored",
+                   move_of(origin, dest, flying, weights, size, {ptb::MoveTally::kScored, bins, responses}));
 }
 int pumitally_move_to_next_location_device_scored(pumitally_engine *e, const double *d_origin, const double *d_dest,
                                                   const int8_t *d_flying, const double *d_weights,
                                                   const double *d_responses, const int32_t *d_bins, int32_t size,
                                                   void *stream) {
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location_device_scored(d_origin, d_dest, d_flying, d_weights, d_responses, d_bins, size,
-                                                 static_cast<cudaStream_t>(stream));
-  });
+  return device_move(
+      e, move_of(d_origin, d_dest, d_flying, d_weights, size, {ptb::MoveTally::kScored, d_bins, d_responses}), stream);
 }
 
 int pumitally_set_time_bins(pumitally_engine *e, const double *edges, int32_t nedges) {
@@ -197,22 +195,15 @@ int32_t pumitally_get_time_bins(const pumitally_engine *e) {
 int pumitally_move_to_next_location_timed(pumitally_engine *e, const double *origin, const double *dest, int8_t *flying,
                                           const double *weights, const double *times, const double *speeds,
                                           const double *responses, const int32_t *bins, int32_t size) {
-  if (size > 0 && (!origin || !dest || !flying || !weights)) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationTimed: null input array\n");
-    return 1;
-  }
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location_timed(origin, dest, flying, weights, times, speeds, responses, bins, size);
-  });
+  return host_move(e, "MoveToNextLocationTimed",
+                   move_of(origin, dest, flying, weights, size, {ptb::MoveTally::kTimed, bins, responses, times, speeds}));
 }
 int pumitally_move_to_next_location_device_timed(pumitally_engine *e, const double *d_origin, const double *d_dest,
                                                  const int8_t *d_flying, const double *d_weights, const double *d_times,
                                                  const double *d_speeds, const double *d_responses,
                                                  const int32_t *d_bins, int32_t size, void *stream) {
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location_device_timed(d_origin, d_dest, d_flying, d_weights, d_times, d_speeds, d_responses,
-                                                d_bins, size, static_cast<cudaStream_t>(stream));
-  });
+  return device_move(e, move_of(d_origin, d_dest, d_flying, d_weights, size,
+                                {ptb::MoveTally::kTimed, d_bins, d_responses, d_times, d_speeds}), stream);
 }
 
 int pumitally_set_moments(pumitally_engine *e, int32_t order) {
@@ -292,10 +283,7 @@ int pumitally_copy_initial_position_device(pumitally_engine *e, const double *d_
 int pumitally_move_to_next_location_device(pumitally_engine *e, const double *d_origin,
                                            const double *d_dest, const int8_t *d_flying,
                                            const double *d_weights, int32_t size, void *stream) {
-  return guarded(e, [&](ptb::Engine &g) {
-    return g.move_to_next_location_device(d_origin, d_dest, d_flying, d_weights, size,
-                                          static_cast<cudaStream_t>(stream));
-  });
+  return device_move(e, move_of(d_origin, d_dest, d_flying, d_weights, size), stream);
 }
 int pumitally_set_state_device(pumitally_engine *e, const double *d_xyz, const int32_t *d_elem, int32_t first,
                                int32_t count, void *stream) {

@@ -142,17 +142,13 @@ Engine::~Engine() {
   cudaFree(d_flux_global_);
   if (ev_order_) cudaEventDestroy(ev_order_);
   if (ev_done_) cudaEventDestroy(ev_done_);
-  if (ev_bins_) cudaEventDestroy(ev_bins_);
-  if (ev_bins_free_) cudaEventDestroy(ev_bins_free_);
   cudaFree(d_mask_);
-  cudaFree(d_bins_);
-  for (AuxUpload *u : {&resp_up_, &time_up_}) {
+  for (AuxUpload *u : {&time_up_, &resp_up_, &bins_up_}) {
     cudaFree(u->d);
     if (u->h) cudaFreeHost(u->h);
     if (u->ev) cudaEventDestroy(u->ev);
   }
   cudaFree(d_edges_);
-  if (h_bins_) cudaFreeHost(h_bins_);
   if (ev_copy0_) cudaEventDestroy(ev_copy0_);
   if (ev_copy1_) cudaEventDestroy(ev_copy1_);
   if (ev_ar0_) cudaEventDestroy(ev_ar0_);
@@ -258,7 +254,7 @@ void Engine::collect_timers(bool wait) {
 }
 
 // Picks the kernel for the move that is about to be launched (see the auto-tuner note in engine.hpp).
-void Engine::begin_move() {
+void Engine::begin_move(bool scored) {
   collect_timers(false);
   move_variant_ = variant_;
   move_tag_ = -1;
@@ -268,7 +264,7 @@ void Engine::begin_move() {
   if (int64_t(n_) > 16 * mesh_.ntets) return;
   // a scored, timed or moment move runs the kernel a plain move would run outside the exploration, and is never
   // timed for it (its walk costs more per crossing): the tuner's clock counts plain moves only
-  if (cur_resp_ || cur_times_ || moments_) {
+  if (scored) {
     move_variant_ = tuned_variant_;
     return;
   }
@@ -317,7 +313,7 @@ int Engine::relocate_patches(const PatchEntry *d_list, int32_t count, cudaStream
 
 int Engine::launch_range(const double *d_origin, const double *d_dest, const int8_t *d_flying,
                          const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
-                         bool timed) {
+                         const MoveTally &t) {
   if (end <= begin) return 0;
   // Particle state, binning scratch and the ticket ring are shared by every launch: work enqueued on
   // another stream than the previous launch's (a device-pointer move on the caller's stream after a
@@ -330,46 +326,43 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   last_stream_ = stream;
   last_stream_set_ = true;
   if (d_dest) flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on; the last exchange no longer describes it
-  cur_slice_ = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
-  if (!(cur_bins_ && d_dest)) return launch_range_into(d_flux_, d_origin, d_dest, d_flying, d_weights, begin, end, stream, timed);
+  const int64_t slice = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
+  if (!(t.bins && d_dest))
+    return launch_range_into(d_flux_, d_origin, d_dest, d_flying, d_weights, begin, end, stream, t, slice, move_variant_,
+                             move_tag_);
   // Score filter: particles are independent and a particle that does not fly is not touched, so the range
   // is walked once per bin with the flying flags masked down to that bin's particles and the tally pointed
   // at that bin's flux array -- the walk kernels themselves are the unfiltered ones.  One more pass (array
   // nbins_, never reported) flies the particles whose bin is outside [0, nbins_): they move, unscored.
   // The streaming kernel pays for every particle of the range in every pass, flying or not; the packed kernel's
   // sort pass keeps only the flying
-  // ones, so its passes cost what their members cost.  Unless the caller has fixed the kernel, binned moves use it.
-  const int saved_variant = move_variant_, saved_tag = move_tag_;
-  if (auto_variant_ && d_weights) {
-    move_variant_ = kVariantPacked;
-    move_tag_ = -1;  // not one of the auto-tuner's exploration moves
-  }
-  int rc = 0;
-  for (int32_t b = 0; b <= nbins_ && !rc; ++b) {
-    if (launch_bin_mask(d_flying, cur_bins_, b, nbins_, d_mask_, begin, end, stream) != cudaSuccess) { rc = 1; break; }
+  // ones, so its passes cost what their members cost.  Unless the caller has fixed the kernel, binned moves use it,
+  // and are not one of the auto-tuner's exploration moves.
+  const bool packed = auto_variant_ && d_weights;
+  const int variant = packed ? int(kVariantPacked) : move_variant_, tag = packed ? -1 : move_tag_;
+  for (int32_t b = 0; b <= nbins_; ++b) {
+    if (launch_bin_mask(d_flying, t.bins, b, nbins_, d_mask_, begin, end, stream) != cudaSuccess) return 1;
     ++launches_;
     // the unreported array follows every reported one (with a time filter, all time bins of a bin-b pass go to it)
-    cur_slice_ = b < nbins_ ? int64_t(nbins_) * int64_t(bin_len()) : 0;
-    rc = launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : flux_len()), d_origin, d_dest, d_mask_, d_weights,
-                           begin, end, stream, timed);
+    if (launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : flux_len()), d_origin, d_dest, d_mask_,
+                          d_weights, begin, end, stream, t, b < nbins_ ? slice : 0, variant, tag))
+      return 1;
   }
-  move_variant_ = saved_variant;
-  move_tag_ = saved_tag;
-  return rc;
+  return 0;
 }
 
 int Engine::launch_range_into(double *d_flux, const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                              const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, bool timed) {
+                              const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
+                              const MoveTally &t, int64_t slice, int variant, int tag) {
   if (d_dest && d_weights && initial_weight_pending_)  // first tracks of the batch: their total weight
     PTB_CUDA_OK(launch_sum_flying_weights(d_flying, d_weights, begin, end, d_initial_weight_, stream));
   TimedWalkParams tp{};
-  ScoredWalkParams &sp = tp;
   WalkParams &p = tp;
-  const bool timed_walk = cur_times_ && d_dest;
+  const bool timed_walk = t.kind == MoveTally::kTimed && d_dest;
   // with moments every tallying move is a scored one; the plain and binned moves have one score and no responses
-  const bool scored = (cur_resp_ || timed_walk || moments_) && d_dest;
-  if (scored) sp.sc = ScoreParams{cur_resp_, nscores_, stride_};
-  if (timed_walk) tp.tm = TimeParams{d_edges_, cur_times_, cur_speeds_, ntime_, cur_slice_};
+  const bool scored = scored_move(t) && d_dest;
+  if (scored) tp.sc = ScoreParams{t.responses, nscores_, stride_};
+  if (timed_walk) tp.tm = TimeParams{d_edges_, t.times, t.speeds, ntime_, slice};
   p.tets = d_tets_;
   p.links = d_links_;
   p.verts = d_verts_;
@@ -397,24 +390,22 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
   auto aligned16 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
   p.bulk_ok = (begin % 16 == 0) && aligned16(d_origin) && aligned16(d_dest) && aligned16(d_flying) &&
               aligned16(d_weights);
-  TimerPair t{};
-  t.tag = -1;
-  if (timed) {
-    if (timers_free_.empty()) {
-      PTB_CUDA_OK(cudaEventCreate(&t.a));
-      PTB_CUDA_OK(cudaEventCreate(&t.b));
-    } else {
-      t = timers_free_.back();
-      timers_free_.pop_back();
-    }
-    t.tag = move_tag_;
-    if (t.tag >= 0) ++explore_pending_;
-    PTB_CUDA_OK(cudaEventRecord(t.a, stream));
+  TimerPair timer{};
+  if (timers_free_.empty()) {
+    PTB_CUDA_OK(cudaEventCreate(&timer.a));
+    PTB_CUDA_OK(cudaEventCreate(&timer.b));
+  } else {
+    timer = timers_free_.back();
+    timers_free_.pop_back();
   }
-  int variant = move_variant_;
-  const bool packed = variant_is_packed(variant);
-  if (packed && !(d_dest && d_weights)) variant = kVariantPersistRefill8;  // localisation
-  bool use_packed = packed && variant == move_variant_;
+  timer.tag = tag;
+  if (timer.tag >= 0) ++explore_pending_;
+  PTB_CUDA_OK(cudaEventRecord(timer.a, stream));
+  bool use_packed = variant_is_packed(variant);
+  if (use_packed && !(d_dest && d_weights)) {  // localisation
+    variant = kVariantPersistRefill8;
+    use_packed = false;
+  }
   if (use_packed && !d_rows_ &&
       cudaMalloc(reinterpret_cast<void **>(&d_rows_), std::max<size_t>(size_t(n_), 1) * sizeof(PackedRow)) != cudaSuccess) {
     cudaGetLastError();
@@ -456,25 +447,16 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
     launches_ += 5;  // count, 3-kernel scan, scatter
     p.flying = nullptr;  // order[] holds flying particles only
   }
-  if (timed_walk) {
-    if (!walk_variant_available(variant) || launch_walk_timed(tp, variant, block_, stream, moments_ > 0) != cudaSuccess) {
-      fprintf(stderr, "[pumitally] ERROR: timed moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n", variant);
-      return 1;
-    }
-  } else if (scored) {
-    if (!walk_variant_available(variant) || launch_walk_scored(sp, variant, block_, stream, moments_ > 0) != cudaSuccess) {
-      fprintf(stderr, "[pumitally] ERROR: scored and moment moves run on the kernels 0, 8, 16 and 24 only (variant %d)\n",
-              variant);
-      return 1;
-    }
-  } else {
-    PTB_CUDA_OK(launch_walk(p, variant, block_, stream));
+  const cudaError_t err = scored ? launch_walk_tallied(tp, timed_walk, moments_ > 0, variant, block_, stream)
+                                 : launch_walk(p, variant, block_, stream);
+  if (err != cudaSuccess) {
+    fprintf(stderr, "[pumitally] ERROR: walk kernel %d: %s (scored, timed and moment moves run on the kernels 0, 8, 16 "
+                    "and 24 only)\n", variant, cudaGetErrorString(err));
+    return 1;
   }
   ++launches_;
-  if (timed) {
-    PTB_CUDA_OK(cudaEventRecord(t.b, stream));
-    timers_busy_.push_back(t);
-  }
+  PTB_CUDA_OK(cudaEventRecord(timer.b, stream));
+  timers_busy_.push_back(timer);
   return 0;
 }
 
@@ -520,13 +502,7 @@ int Engine::copy_initial_position(const double *xyz, int32_t size) {
   const double *src = xyz;
   double *d_xyz = d_origin_;
   if (host_path_ != 0 && n_ > 0 && ensure_stage_buffers(xyz, size_t(size) * sizeof(double)) == 0) {
-    HostPool *pool_ = &stager_->pool();
-    const int T = pool_->size();
-    const int64_t total = int64_t(size);
-    pool_->run([&](int t) {
-      const int64_t lo = (total * t / T) & ~int64_t(7), hi = t == T - 1 ? total : (total * (t + 1) / T) & ~int64_t(7);
-      std::memcpy(h_dest_ + lo, xyz + lo, size_t(hi - lo) * sizeof(double));
-    });
+    pool_copy(h_dest_, xyz, size_t(size) * sizeof(double));
     src = h_dest_;
     d_xyz = d_dest_;
     mirror_valid_ = true;
@@ -535,7 +511,7 @@ int Engine::copy_initial_position(const double *xyz, int32_t size) {
   h2d_bytes_ += double(size) * sizeof(double);
   move_variant_ = variant_;
   move_tag_ = -1;
-  if (launch_range(d_xyz, nullptr, nullptr, nullptr, 0, n_, compute_, true)) return 1;
+  if (launch_range(d_xyz, nullptr, nullptr, nullptr, 0, n_, compute_)) return 1;
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   initialized_ = true;
   return 0;
@@ -549,7 +525,7 @@ int Engine::copy_initial_position_device(const double *d_xyz, int32_t size, cuda
   PTB_CUDA_OK(cudaSetDevice(device_));
   move_variant_ = variant_;
   move_tag_ = -1;
-  if (launch_range(d_xyz, nullptr, nullptr, nullptr, 0, n_, stream, true)) return 1;
+  if (launch_range(d_xyz, nullptr, nullptr, nullptr, 0, n_, stream)) return 1;
   initialized_ = true;
   return 0;
 }
@@ -650,8 +626,8 @@ int Engine::ensure_stage_buffers(const void *caller_mem, size_t caller_bytes) {
   return 0;
 }
 
-int Engine::ensure_patch_buffers(int nchunks) {
-  size_t cap = size_t(double(std::min<int64_t>(chunk_, n_)) * kPatchMaxFraction) + 64;
+int Engine::ensure_patch_buffers(int nchunks, int32_t chunk) {
+  size_t cap = size_t(double(std::min<int64_t>(chunk, n_)) * kPatchMaxFraction) + 64;
   if (h_patch_ && patch_cap_ >= cap && patch_chunks_ >= nchunks) return 0;
   // (grow only, in both dimensions: moves with different stage sizes -- binned and plain -- may alternate)
   cap = std::max(cap, patch_cap_);
@@ -683,58 +659,60 @@ int Engine::ensure_patch_buffers(int nchunks) {
 //
 // Direct path (option host_path=0, or no pinned memory to be had): plain cudaMemcpyAsync of all
 // four arrays from the caller's memory, optionally page-locked first (option register_host).
-bool Engine::refuse_unscored(const char *what) const {
-  if (refuse_untimed(what)) return true;
-  if (nscores_ == 1) return false;
-  fprintf(stderr, "[pumitally] ERROR: %s: the engine has %d scores; use the scored move\n", what, nscores_);
-  return true;
-}
-
-bool Engine::refuse_untimed(const char *what) const {
-  if (ntime_ == 0) return false;
-  fprintf(stderr, "[pumitally] ERROR: %s: the engine has %d time bins; use the timed move\n", what, ntime_);
-  return true;
-}
-
-int Engine::move_to_next_location(const double *origin, const double *dest, int8_t *flying,
-                                  const double *weights, int32_t size) {
-  if (refuse_unscored("MoveToNextLocation")) return 1;
-  const int rc = move_host_entry(origin, dest, flying, weights, size);
-  if (rc == 0 && moments_) ++scored_moves_;
-  return rc;
-}
-
-int Engine::move_host_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                            int32_t size) {
-  if (int64_t(size) != 3 * int64_t(n_)) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation size %d != 3 * num_particles (%d)\n", size, n_);
-    return 1;
-  }
-  if (!initialized_) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation before CopyInitialPosition\n");
-    return 1;
-  }
+//
+// Binned, scored and timed moves: the side arrays travel ahead of the particle data on the copy stream (times and
+// speeds, then responses, then bins), through a pinned copy made by the worker pool when a caller's array is pageable
+// (upload_aux), and are on the device before the call returns.  Everything else is the ordinary host path, except the
+// pinned-caller variant (move_pinned), whose relocation pass knows nothing of bins or scores.
+int Engine::move_to_next_location(const Move &m) {
+  if (move_refused(m, false)) return 1;
   PTB_CUDA_OK(cudaSetDevice(device_));
-  begin_move();
-  // Pipeline stage size, unless the caller set it: 512 Ki particles for the streaming kernel (shortest tail); the
-  // sorted kernels pay a fixed price per launch (a scan over all seed-grid cells), so their stages are 2 Mi.
-  const int32_t chunk = chunk_;
-  // The auto-tuner compares kernel times; in a host move the sorted kernel it may prefer would also need the
-  // larger stages, whose longer tail can cost more than the kernel wins.  So a host move of more than one stage keeps the engine's base kernel and does not take
-  // part in the exploration; the tuner works for device-pointer moves and single-stage host moves (c4's 1 M tracks).
-  if (auto_variant_ && variant_is_packed(move_variant_) && !variant_is_packed(variant_) && n_ > chunk_) {
-    move_variant_ = variant_;
-    move_tag_ = -1;
+  const MoveTally &t = m.tally;
+  const size_t N = size_t(n_);
+  MoveTally dev;  // t with the device copies of its arrays
+  dev.kind = t.kind;
+  cudaEvent_t sent[3];
+  int nsent = 0, rc = 0;
+  auto send = [&](AuxUpload &u, const void *a, const void *b, size_t bytes) {
+    if (rc == 0) rc = upload_aux(u, a, b, bytes);
+    if (rc == 0) sent[nsent++] = u.ev;
+    return rc == 0;
+  };
+  if (t.kind == MoveTally::kTimed && send(time_up_, t.times, t.speeds, N * sizeof(double))) {
+    dev.times = static_cast<const double *>(time_up_.d);
+    dev.speeds = dev.times + N;
   }
-  if (!chunk_user_set_ && (variant_is_gather(move_variant_) || variant_is_packed(move_variant_)))
-    chunk_ = std::max(chunk_, int32_t(1) << 21);
-  const int rc = move_host(origin, dest, flying, weights, size);
-  chunk_ = chunk;
+  if (t.responses && send(resp_up_, t.responses, nullptr, N * size_t(nscores_) * sizeof(double)))
+    dev.responses = static_cast<const double *>(resp_up_.d);
+  if (t.bins && nbins_ > 1 && send(bins_up_, t.bins, nullptr, N * sizeof(int32_t)))
+    dev.bins = static_cast<const int32_t *>(bins_up_.d);
+  if (rc == 0) {
+    begin_move(scored_move(t));
+    // Pipeline stage size, unless the caller set it: 512 Ki particles for the streaming kernel (shortest tail); the
+    // sorted kernels pay a fixed price per launch (a scan over all seed-grid cells), so their stages are 2 Mi.  A
+    // binned move walks every stage nbins + 1 times, seven small launches each, all enqueued by this thread between
+    // two stage passes: its stages are 2 Mi too.
+    int32_t chunk = chunk_;
+    if (!chunk_user_set_ && dev.bins) chunk = std::max(chunk, int32_t(1) << 21);
+    // The auto-tuner compares kernel times; in a host move the sorted kernel it may prefer would also need the
+    // larger stages, whose longer tail can cost more than the kernel wins.  So a host move of more than one stage keeps the engine's base kernel and does not take
+    // part in the exploration; the tuner works for device-pointer moves and single-stage host moves (c4's 1 M tracks).
+    if (auto_variant_ && variant_is_packed(move_variant_) && !variant_is_packed(variant_) && n_ > chunk) {
+      move_variant_ = variant_;
+      move_tag_ = -1;
+    }
+    if (!chunk_user_set_ && (variant_is_gather(move_variant_) || variant_is_packed(move_variant_)))
+      chunk = std::max(chunk, int32_t(1) << 21);
+    rc = move_host(m.origin, m.dest, m.flying, m.weights, m.size, dev, chunk);
+  }
+  while (nsent > 0) PTB_CUDA_OK(cudaEventSynchronize(sent[--nsent]));  // the caller gets them back with the others
+  if (rc == 0 && scored_move(t)) ++scored_moves_;
   return rc;
 }
 
-int Engine::move_host(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size) {
-  const int nchunks = n_ ? (n_ + chunk_ - 1) / chunk_ : 0;
+int Engine::move_host(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size,
+                      const MoveTally &dev, int32_t chunk) {
+  const int nchunks = n_ ? (n_ + chunk - 1) / chunk : 0;
   while (int(chunk_events_.size()) < nchunks + 2) {
     cudaEvent_t e;
     PTB_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -777,20 +755,21 @@ int Engine::move_host(const double *origin, const double *dest, int8_t *flying, 
   ++host_moves_;
   span_tag_ = probe;
   const bool staged = want_staged && n_ > 0 && ensure_stage_buffers(dest, size_t(size) * sizeof(double)) == 0 &&
-                      ensure_patch_buffers(nchunks) == 0;
-  if (!staged) return move_direct(origin, dest, flying, weights, nchunks);
+                      ensure_patch_buffers(nchunks, chunk) == 0;
+  if (!staged) return move_direct(origin, dest, flying, weights, nchunks, dev, chunk);
   follow_caller_memory(dest, size_t(size) * sizeof(double));
   // Caller arrays that are page-locked (by the caller, or just above) need no copy into the staging
   // slots: dest and weights go to the device straight from them, and the origins are compared with
-  // the device's own particle positions, which each move sends back (move_pinned).
-  if (pinned_path_ && host_is_pinned(origin) && host_is_pinned(dest) && host_is_pinned(weights) &&
+  // the device's own particle positions, which each move sends back (move_pinned).  Plain moves only.
+  const bool plain = dev.kind == MoveTally::kPlain && !dev.bins;
+  if (pinned_path_ && plain && host_is_pinned(origin) && host_is_pinned(dest) && host_is_pinned(weights) &&
       ensure_position_mirror(nchunks) == 0)
-    return move_pinned(origin, dest, flying, weights, nchunks);
+    return move_pinned(origin, dest, flying, weights, nchunks, chunk);
   pos_mirror_valid_ = false;  // the move below does not send positions back
 
   // a chunk's staging slots may be refilled once the previous move's copies out of them are done;
   // with an unchanged chunking that is chunk_events_[k], otherwise wait for the whole copy stream
-  if (staged_chunk_ != chunk_ || staged_chunks_ != nchunks) {
+  if (staged_chunk_ != chunk || staged_chunks_ != nchunks) {
     PTB_CUDA_OK(cudaStreamSynchronize(copy_));
     staged_chunks_ = 0;
   }
@@ -807,8 +786,8 @@ int Engine::move_host(const double *origin, const double *dest, int8_t *flying, 
   bool caller_memory_on_the_wire = false;
   const auto t_begin = std::chrono::steady_clock::now();
   auto range_of = [&](int k, int32_t &b, int32_t &e) {
-    b = int32_t(int64_t(k) * chunk_);
-    e = int32_t(std::min<int64_t>(n_, int64_t(b) + chunk_));
+    b = int32_t(int64_t(k) * chunk);
+    e = int32_t(std::min<int64_t>(n_, int64_t(b) + chunk));
   };
   // the staging slots of chunk k may be refilled once the previous move's copies out of them are done,
   // its pinned patch slot once the copies of chunk k - kPatchSlots of this move are done
@@ -852,7 +831,7 @@ int Engine::move_host(const double *origin, const double *dest, int8_t *flying, 
       PTB_CUDA_OK(launch_patch_origins(d_origin_, dp, int32_t(npatch), compute_));
       ++launches_;
     }
-    if (launch_range(d_origin_, d_dest_, d_flying_, d_weights_, b, e, compute_, true)) return 1;
+    if (launch_range(d_origin_, d_dest_, d_flying_, d_weights_, b, e, compute_, dev)) return 1;
   }
   PTB_CUDA_OK(cudaEventRecord(ev_copy1_, copy_));
   if (mark_move_done()) return 1;
@@ -862,7 +841,7 @@ int Engine::move_host(const double *origin, const double *dest, int8_t *flying, 
   stage_host_s_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
   stage_sent_bytes_ = sent;
   h2d_bytes_ += sent;
-  staged_chunk_ = chunk_;
+  staged_chunk_ = chunk;
   staged_chunks_ = nchunks;
   mirror_valid_ = true;
   initial_weight_pending_ = false;
@@ -919,13 +898,13 @@ int Engine::ensure_position_mirror(int nchunks) {
 // device->host direction of the link.  Host memory traffic per particle: 24 B origin + 24 B mirror
 // read by the pool, 33 B read and 24 B written by the DMA engines -- half of the staged path's.
 int Engine::move_pinned(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                        int nchunks) {
+                        int nchunks, int32_t chunk) {
   mirror_valid_ = false;  // the staged path's mirror does not see this move
   if (!ev_copy0_) {
     PTB_CUDA_OK(cudaEventCreate(&ev_copy0_));
     PTB_CUDA_OK(cudaEventCreate(&ev_copy1_));
   }
-  if (staged_chunk_ != chunk_ || staged_chunks_ != nchunks || !pos_mirror_valid_) {
+  if (staged_chunk_ != chunk || staged_chunks_ != nchunks || !pos_mirror_valid_) {
     PTB_CUDA_OK(cudaStreamSynchronize(copy_));
     PTB_CUDA_OK(cudaStreamSynchronize(d2h_));
     staged_chunks_ = 0;
@@ -944,8 +923,8 @@ int Engine::move_pinned(const double *origin, const double *dest, int8_t *flying
   double sent = 0.0;
   const auto t_begin = std::chrono::steady_clock::now();
   auto range_of = [&](int k, int32_t &b, int32_t &e) {
-    b = int32_t(int64_t(k) * chunk_);
-    e = int32_t(std::min<int64_t>(n_, int64_t(b) + chunk_));
+    b = int32_t(int64_t(k) * chunk);
+    e = int32_t(std::min<int64_t>(n_, int64_t(b) + chunk));
   };
   auto start_stage = [&](int k) -> int {
     if (k < staged_chunks_) {
@@ -984,7 +963,7 @@ int Engine::move_pinned(const double *origin, const double *dest, int8_t *flying
     // the export below reuses d_origin_: the previous move's device->host copy out of it must be done
     PTB_CUDA_OK(cudaStreamWaitEvent(compute_, pos_events_[k], 0));
     if (npatch > 0 && relocate_patches(dp, int32_t(npatch), compute_)) return 1;
-    if (launch_range(npatch < 0 ? d_origin_ : nullptr, d_dest_, d_flying_, d_weights_, b, e, compute_, true)) return 1;
+    if (launch_range(npatch < 0 ? d_origin_ : nullptr, d_dest_, d_flying_, d_weights_, b, e, compute_)) return 1;
     PTB_CUDA_OK(launch_export_positions(d_state_, d_origin_, b, e, compute_));
     ++launches_;
     PTB_CUDA_OK(cudaEventRecord(walk_events_[k], compute_));
@@ -1003,7 +982,7 @@ int Engine::move_pinned(const double *origin, const double *dest, int8_t *flying
   stage_sent_bytes_ = sent;
   h2d_bytes_ += sent;
   d2h_bytes_ += 24.0 * double(n_);
-  staged_chunk_ = chunk_;
+  staged_chunk_ = chunk;
   staged_chunks_ = nchunks;
   pos_mirror_valid_ = true;
   initial_weight_pending_ = false;
@@ -1038,7 +1017,7 @@ int Engine::mark_move_done() {
 
 // Direct path: every array is copied from the caller's memory as it is.
 int Engine::move_direct(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                        int nchunks) {
+                        int nchunks, const MoveTally &dev, int32_t chunk) {
   mirror_valid_ = false;  // the staging slots do not see this move
   pos_mirror_valid_ = false;
   cudaEvent_t ev_prev_done = chunk_events_[nchunks], ev_fly = chunk_events_[nchunks + 1];
@@ -1054,14 +1033,14 @@ int Engine::move_direct(const double *origin, const double *dest, int8_t *flying
   PTB_CUDA_OK(cudaMemcpyAsync(d_flying_, flying, size_t(n_), cudaMemcpyHostToDevice, copy_));
   PTB_CUDA_OK(cudaEventRecord(ev_fly, copy_));
   for (int k = 0; k < nchunks; ++k) {
-    const int32_t b = int32_t(int64_t(k) * chunk_), e = int32_t(std::min<int64_t>(n_, int64_t(b) + chunk_));
+    const int32_t b = int32_t(int64_t(k) * chunk), e = int32_t(std::min<int64_t>(n_, int64_t(b) + chunk));
     const size_t cnt = size_t(e - b);
     PTB_CUDA_OK(cudaMemcpyAsync(d_origin_ + 3 * size_t(b), origin + 3 * size_t(b), 3 * cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
     PTB_CUDA_OK(cudaMemcpyAsync(d_dest_ + 3 * size_t(b), dest + 3 * size_t(b), 3 * cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
     PTB_CUDA_OK(cudaMemcpyAsync(d_weights_ + b, weights + b, cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
     PTB_CUDA_OK(cudaEventRecord(chunk_events_[k], copy_));
     PTB_CUDA_OK(cudaStreamWaitEvent(compute_, chunk_events_[k], 0));
-    if (launch_range(d_origin_, d_dest_, d_flying_, d_weights_, b, e, compute_, true)) return 1;
+    if (launch_range(d_origin_, d_dest_, d_flying_, d_weights_, b, e, compute_, dev)) return 1;
   }
   PTB_CUDA_OK(cudaEventRecord(ev_copy1_, copy_));
   if (mark_move_done()) return 1;
@@ -1077,30 +1056,43 @@ int Engine::move_direct(const double *origin, const double *dest, int8_t *flying
   return 0;
 }
 
-int Engine::move_to_next_location_device(const double *d_origin, const double *d_dest,
-                                         const int8_t *d_flying, const double *d_weights,
-                                         int32_t size, cudaStream_t stream) {
-  if (refuse_unscored("MoveToNextLocation(device)")) return 1;
-  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
-  if (rc == 0 && moments_) ++scored_moves_;
-  return rc;
+// The refusals every move kind shares; `device`: the device-pointer entry point's name in the message.
+bool Engine::move_refused(const Move &m, bool device) const {
+  static const char *const names[] = {"MoveToNextLocation", "MoveToNextLocationScored", "MoveToNextLocationTimed"};
+  const MoveTally &t = m.tally;
+  const char *why = nullptr;
+  if (t.kind == MoveTally::kTimed) {
+    if (ntime_ == 0) why = "the engine has no time bins (set_time_bins)";
+    else if (!t.times || !t.speeds) why = "null times or speeds array";
+    else if (!t.responses && nscores_ != 1) why = "null responses array with several scores";
+  } else if (ntime_ > 0) {
+    why = "the engine has time bins; use the timed move";
+  } else if (t.kind == MoveTally::kScored && !t.responses) {
+    why = "null responses array";
+  } else if (t.kind == MoveTally::kPlain && nscores_ != 1) {
+    why = "the engine has several scores; use the scored move";
+  }
+  if (!why && int64_t(m.size) != 3 * int64_t(n_)) why = "size != 3 * num_particles";
+  if (!why && !initialized_) why = "called before CopyInitialPosition";
+  if (why) fprintf(stderr, "[pumitally] ERROR: %s%s: %s\n", names[t.kind], device ? "(device)" : "", why);
+  return why != nullptr;
 }
 
-int Engine::move_device_entry(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                              const double *d_weights, int32_t size, cudaStream_t stream) {
-  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocation(device): bad size or not initialised\n");
-    return 1;
-  }
+int Engine::move_to_next_location_device(const Move &m, cudaStream_t stream) {
+  if (move_refused(m, true)) return 1;
   PTB_CUDA_OK(cudaSetDevice(device_));
-  begin_move();
+  const bool scored = scored_move(m.tally);
+  begin_move(scored);
   // (the staging arrays are not touched: "pinned dest slots == device dest array" keeps holding, and the
   // next host move's origins are compared against them and patched exactly as after a host move;
   // the position mirror of the pinned-caller path, however, is out of date after this move)
   pos_mirror_valid_ = false;
-  if (launch_range(d_origin, d_dest, d_flying, d_weights, 0, n_, stream, true)) return 1;
+  MoveTally dev = m.tally;
+  if (nbins_ == 1) dev.bins = nullptr;
+  if (launch_range(m.origin, m.dest, m.flying, m.weights, 0, n_, stream, dev)) return 1;
   initial_weight_pending_ = false;
   ++moves_;
+  if (scored) ++scored_moves_;
   return 0;
 }
 
@@ -1189,249 +1181,63 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
   stride_ = int32_t(stride);
   ntime_ = ntime;
   moments_ = moments;
-  if (nbins > 1 && !d_mask_) {
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_bins_), std::max<size_t>(size_t(n_), 4) * sizeof(int32_t)));
-  }
+  if (nbins > 1 && !d_mask_) PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
   return reset_tally();  // a new set of arrays starts from zero
 }
 
-// MoveToNextLocation with a score bin per particle for this move (host pointers).  bins == nullptr or one
-// bin: the plain move.  The bins travel in one copy ahead of the particle data; everything else is the
-// ordinary host path (the pinned-caller variant excepted, whose relocation pass knows nothing of bins).
-int Engine::move_to_next_location_binned(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                                         const int32_t *bins, int32_t size) {
-  if (refuse_unscored("MoveToNextLocationBinned")) return 1;
-  const int rc = move_binned_entry(origin, dest, flying, weights, bins, size);
-  if (rc == 0 && moments_) ++scored_moves_;
-  return rc;
-}
-
-int Engine::move_binned_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                              const int32_t *bins, int32_t size) {
-  if (!bins || nbins_ == 1) return move_host_entry(origin, dest, flying, weights, size);
-  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) return move_host_entry(origin, dest, flying, weights, size);  // prints the error
+// A side array of a host-pointer move, a and, if not null, b (bytes each) back to back in u.d: one copy ahead of the
+// particle data on the copy stream, through a pinned copy the worker pool makes when a caller's array is pageable (a
+// pageable cudaMemcpyAsync of 40 MB blocks this thread for milliseconds before the staging of the particle data can
+// even start).  u.ev is recorded after the copy.
+int Engine::upload_aux(AuxUpload &u, const void *a, const void *b, size_t bytes) {
   PTB_CUDA_OK(cudaSetDevice(device_));
-  if (!ev_bins_) {
-    PTB_CUDA_OK(cudaEventCreateWithFlags(&ev_bins_, cudaEventDisableTiming));
-    PTB_CUDA_OK(cudaEventCreateWithFlags(&ev_bins_free_, cudaEventDisableTiming));
-  }
-  // d_bins_ is read by the mask kernels of the previous move until they are done
-  PTB_CUDA_OK(cudaEventRecord(ev_bins_free_, compute_));
-  PTB_CUDA_OK(cudaStreamWaitEvent(copy_, ev_bins_free_, 0));
-  // through a pinned copy made by the worker pool (a pageable cudaMemcpyAsync of 40 MB blocks this thread for
-  // milliseconds before the staging of the particle data can even start); the previous move's DMA out of it
-  // was waited for before that move returned
-  const int32_t *src = bins;
-  if (!host_is_pinned(bins)) {
-    if (!h_bins_ && cudaHostAlloc(reinterpret_cast<void **>(&h_bins_), std::max<size_t>(size_t(n_), 1) * sizeof(int32_t), cudaHostAllocDefault) != cudaSuccess) {
-      cudaGetLastError();
-      h_bins_ = nullptr;
-    }
-    if (h_bins_) {
-      int32_t *dst = h_bins_;
-      const size_t n = size_t(n_);
-      if (stager_) {  // (the pool exists from the first staged move on)
-        HostPool &pool = stager_->pool();
-        const int T = pool.size();
-        pool.run([&](int t) {
-          const size_t lo = n * size_t(t) / size_t(T), hi = n * size_t(t + 1) / size_t(T);
-          std::memcpy(dst + lo, bins + lo, (hi - lo) * sizeof(int32_t));
-        });
-      } else {
-        std::memcpy(dst, bins, n * sizeof(int32_t));
-      }
-      src = h_bins_;
-    }
-  }
-  PTB_CUDA_OK(cudaMemcpyAsync(d_bins_, src, size_t(n_) * sizeof(int32_t), cudaMemcpyHostToDevice, copy_));
-  PTB_CUDA_OK(cudaEventRecord(ev_bins_, copy_));
-  h2d_bytes_ += 4.0 * double(n_);
-  cur_bins_ = d_bins_;
-  const bool pinned_path = pinned_path_;
-  pinned_path_ = false;
-  // every pipeline stage is walked nbins + 1 times, seven small launches each, all enqueued by this thread between
-  // two stage passes: unless the caller chose the stage size, binned moves use stages of 2 Mi particles
-  const int32_t chunk = chunk_;
-  if (!chunk_user_set_) chunk_ = std::max(chunk_, int32_t(1) << 21);
-  const int rc = move_host_entry(origin, dest, flying, weights, size);
-  chunk_ = chunk;
-  pinned_path_ = pinned_path;
-  cur_bins_ = nullptr;
-  PTB_CUDA_OK(cudaEventSynchronize(ev_bins_));  // the caller gets `bins` back with the other arrays
-  return rc;
-}
-
-int Engine::move_to_next_location_device_binned(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                                                const double *d_weights, const int32_t *d_bins, int32_t size,
-                                                cudaStream_t stream) {
-  if (refuse_unscored("MoveToNextLocationBinned(device)")) return 1;
-  cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
-  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
-  cur_bins_ = nullptr;
-  if (rc == 0 && moments_) ++scored_moves_;
-  return rc;
-}
-
-// Per-particle doubles of a host-pointer move that travel as the bins do: one copy ahead of the particle data on
-// the copy stream, through a pinned copy the worker pool makes when a caller's array is pageable.  a and, if not
-// null, b (cnt doubles each) land back to back in u.d; u.ev is recorded after the copy.
-int Engine::upload_doubles(AuxUpload &u, const double *a, const double *b, size_t cnt) {
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const size_t total = cnt * (b ? 2 : 1);
+  const size_t total = bytes * (b ? 2 : 1);
   if (u.cap < total) {
     PTB_CUDA_OK(cudaDeviceSynchronize());
     cudaFree(u.d);
     if (u.h) cudaFreeHost(u.h);
     u.d = u.h = nullptr;
     u.cap = 0;
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&u.d), std::max<size_t>(total, 1) * sizeof(double)));
+    PTB_CUDA_OK(cudaMalloc(&u.d, std::max<size_t>(total, 1)));
     u.cap = total;
   }
   if (!u.ev) PTB_CUDA_OK(cudaEventCreateWithFlags(&u.ev, cudaEventDisableTiming));
   // u.d is read by the previous move's kernels until they are done
   PTB_CUDA_OK(cudaEventRecord(u.ev, compute_));
   PTB_CUDA_OK(cudaStreamWaitEvent(copy_, u.ev, 0));
-  const double *src[2] = {a, b};
+  const void *src[2] = {a, b};
   const int narr = b ? 2 : 1;
   bool staged = false;
   if (!host_is_pinned(a) || (b && !host_is_pinned(b))) {
-    if (!u.h && cudaHostAlloc(reinterpret_cast<void **>(&u.h), std::max<size_t>(u.cap, 1) * sizeof(double),
-                              cudaHostAllocDefault) != cudaSuccess) {
+    if (!u.h && cudaHostAlloc(&u.h, std::max<size_t>(u.cap, 1), cudaHostAllocDefault) != cudaSuccess) {
       cudaGetLastError();
       u.h = nullptr;
     }
     if (u.h) {  // the previous move's DMA out of it was waited for before that move returned
-      double *dst = u.h;
-      for (int k = 0; k < narr; ++k) {
-        const double *from = src[k];
-        double *to = dst + size_t(k) * cnt;
-        if (stager_) {
-          HostPool &pool = stager_->pool();
-          const int T = pool.size();
-          pool.run([&](int t) {
-            const size_t lo = cnt * size_t(t) / size_t(T), hi = cnt * size_t(t + 1) / size_t(T);
-            std::memcpy(to + lo, from + lo, (hi - lo) * sizeof(double));
-          });
-        } else {
-          std::memcpy(to, from, cnt * sizeof(double));
-        }
-      }
-      PTB_CUDA_OK(cudaMemcpyAsync(u.d, u.h, total * sizeof(double), cudaMemcpyHostToDevice, copy_));
+      for (int k = 0; k < narr; ++k) pool_copy(static_cast<char *>(u.h) + size_t(k) * bytes, src[k], bytes);
+      PTB_CUDA_OK(cudaMemcpyAsync(u.d, u.h, total, cudaMemcpyHostToDevice, copy_));
       staged = true;
     }
   }
   if (!staged)
     for (int k = 0; k < narr; ++k)
-      PTB_CUDA_OK(cudaMemcpyAsync(u.d + size_t(k) * cnt, src[k], cnt * sizeof(double), cudaMemcpyHostToDevice, copy_));
+      PTB_CUDA_OK(cudaMemcpyAsync(static_cast<char *>(u.d) + size_t(k) * bytes, src[k], bytes, cudaMemcpyHostToDevice, copy_));
   PTB_CUDA_OK(cudaEventRecord(u.ev, copy_));
-  h2d_bytes_ += 8.0 * double(total);
+  h2d_bytes_ += double(total);
   return 0;
 }
 
-// MoveToNextLocation with nscores_ responses per particle (host pointers); bins as for the binned move.  The
-// responses travel as the bins do (upload_doubles); everything else is the ordinary host path (the pinned-caller
-// variant excepted, whose relocation pass knows nothing of scores).
-int Engine::move_to_next_location_scored(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                                         const double *responses, const int32_t *bins, int32_t size) {
-  if (refuse_untimed("MoveToNextLocationScored")) return 1;
-  if (!responses) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: null responses array\n");
-    return 1;
+void Engine::pool_copy(void *dst, const void *src, size_t bytes) {
+  if (!stager_) {  // (the pool exists from the first staged move on)
+    std::memcpy(dst, src, bytes);
+    return;
   }
-  return move_scored_entry(origin, dest, flying, weights, responses, bins, size);
-}
-
-// (responses == nullptr: a timed move with one score, every response 1)
-int Engine::move_scored_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                              const double *responses, const int32_t *bins, int32_t size) {
-  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored: bad size or not initialised\n");
-    return 1;
-  }
-  if (responses) {
-    if (upload_doubles(resp_up_, responses, nullptr, size_t(n_) * size_t(nscores_))) return 1;
-    cur_resp_ = resp_up_.d;
-  }
-  const bool pinned_path = pinned_path_;
-  pinned_path_ = false;
-  const int rc = (bins && nbins_ > 1) ? move_binned_entry(origin, dest, flying, weights, bins, size)
-                                      : move_host_entry(origin, dest, flying, weights, size);
-  pinned_path_ = pinned_path;
-  cur_resp_ = nullptr;
-  if (rc == 0) ++scored_moves_;
-  if (responses) PTB_CUDA_OK(cudaEventSynchronize(resp_up_.ev));  // the caller gets `responses` back with the other arrays
-  return rc;
-}
-
-int Engine::move_to_next_location_device_scored(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                                                const double *d_weights, const double *d_responses,
-                                                const int32_t *d_bins, int32_t size, cudaStream_t stream) {
-  if (refuse_untimed("MoveToNextLocationScored(device)")) return 1;
-  if (!d_responses) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationScored(device): null responses array\n");
-    return 1;
-  }
-  cur_resp_ = d_responses;
-  cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
-  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
-  cur_bins_ = nullptr;
-  cur_resp_ = nullptr;
-  if (rc == 0) ++scored_moves_;
-  return rc;
-}
-
-// The arguments every timed move needs, checked before anything is touched.
-bool Engine::timed_args_ok(const char *what, const void *times, const void *speeds, const void *responses) const {
-  if (ntime_ == 0) {
-    fprintf(stderr, "[pumitally] ERROR: %s: the engine has no time bins (set_time_bins)\n", what);
-    return false;
-  }
-  if (!times || !speeds) {
-    fprintf(stderr, "[pumitally] ERROR: %s: null times or speeds array\n", what);
-    return false;
-  }
-  if (!responses && nscores_ != 1) {
-    fprintf(stderr, "[pumitally] ERROR: %s: null responses array with %d scores\n", what, nscores_);
-    return false;
-  }
-  return true;
-}
-
-// Timed move (host pointers): the scored move plus each particle's time at its origin and speed.  Times and
-// speeds travel together, one copy ahead of the responses and the particle data (16 bytes per particle).
-int Engine::move_to_next_location_timed(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                                        const double *times, const double *speeds, const double *responses,
-                                        const int32_t *bins, int32_t size) {
-  if (!timed_args_ok("MoveToNextLocationTimed", times, speeds, responses)) return 1;
-  if (int64_t(size) != 3 * int64_t(n_) || !initialized_) {
-    fprintf(stderr, "[pumitally] ERROR: MoveToNextLocationTimed: bad size or not initialised\n");
-    return 1;
-  }
-  if (upload_doubles(time_up_, times, speeds, size_t(n_))) return 1;
-  cur_times_ = time_up_.d;
-  cur_speeds_ = time_up_.d + n_;
-  const int rc = move_scored_entry(origin, dest, flying, weights, responses, bins, size);
-  cur_times_ = cur_speeds_ = nullptr;
-  PTB_CUDA_OK(cudaEventSynchronize(time_up_.ev));
-  return rc;
-}
-
-int Engine::move_to_next_location_device_timed(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                                               const double *d_weights, const double *d_times, const double *d_speeds,
-                                               const double *d_responses, const int32_t *d_bins, int32_t size,
-                                               cudaStream_t stream) {
-  if (!timed_args_ok("MoveToNextLocationTimed(device)", d_times, d_speeds, d_responses)) return 1;
-  cur_times_ = d_times;
-  cur_speeds_ = d_speeds;
-  cur_resp_ = d_responses;
-  cur_bins_ = (d_bins && nbins_ > 1) ? d_bins : nullptr;
-  const int rc = move_device_entry(d_origin, d_dest, d_flying, d_weights, size, stream);
-  cur_bins_ = nullptr;
-  cur_resp_ = nullptr;
-  cur_times_ = cur_speeds_ = nullptr;
-  if (rc == 0) ++scored_moves_;
-  return rc;
+  HostPool &pool = stager_->pool();
+  const size_t T = size_t(pool.size());
+  pool.run([&](int t) {  // 64-byte pieces
+    const size_t lo = (bytes * size_t(t) / T) & ~size_t(63), hi = size_t(t) == T - 1 ? bytes : (bytes * size_t(t + 1) / T) & ~size_t(63);
+    std::memcpy(static_cast<char *>(dst) + lo, static_cast<const char *>(src) + lo, hi - lo);
+  });
 }
 
 int Engine::synchronize() {
@@ -1493,13 +1299,7 @@ int Engine::get_flux_device(double *d_out, cudaStream_t stream) {
 int Engine::copy_results(std::vector<double> &out, bool normalized) {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
   double per_source = 1.0;
-  if (normalized) {
-    per_source = source_normalization();
-    if (!(per_source > 0.0)) {
-      fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
-      return 1;
-    }
-  }
+  if (normalized && !per_source_divisor(&per_source)) return 1;
   if (ensure_element_maps()) return 1;
   double *d_tmp = nullptr;
   PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_tmp), std::max<size_t>(S * E, 1) * sizeof(double)));
@@ -1551,13 +1351,7 @@ int Engine::copy_moments(std::vector<double> &out, bool gradient) {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
   const int slot = stride_ / kMomentSlots;
   double per_source = 1.0;
-  if (gradient) {
-    per_source = source_normalization();
-    if (!(per_source > 0.0)) {
-      fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
-      return 1;
-    }
-  }
+  if (gradient && !per_source_divisor(&per_source)) return 1;
   std::vector<double> raw(B * bin_len());
   PTB_CUDA_OK(cudaMemcpy(raw.data(), flux_view(), raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
   out.resize(B * S * E * 3);
@@ -1615,11 +1409,8 @@ int Engine::get_normalized_flux(double *out_flux, double *out_volume, int64_t n)
   if (n != E && n != int64_t(nbins_) * E) return 1;
   if (synchronize() || gather_shares()) return 1;
   if (out_flux) {
-    const double per_source = source_normalization();
-    if (!(per_source > 0.0)) {
-      fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
-      return 1;
-    }
+    double per_source = 1.0;
+    if (!per_source_divisor(&per_source)) return 1;
     std::vector<double> tmp(static_cast<size_t>(E));
     for (int64_t b = 0; b * E < n; ++b) {
       PTB_CUDA_OK(launch_normalize(flux_view() + size_t(b * E), d_volume_, d_scratch_, E, per_source, compute_));
@@ -1675,6 +1466,13 @@ double Engine::source_normalization() {
     }
     default: return 1.0;
   }
+}
+
+bool Engine::per_source_divisor(double *out) {
+  *out = source_normalization();
+  if (*out > 0.0) return true;
+  fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", *out);
+  return false;
 }
 
 int Engine::reset_tally() {
@@ -2058,11 +1856,8 @@ int Engine::locate_points_device(const double *d_xyz, int64_t npts, int32_t *d_e
 // gradient get_flux_gradient returns (copy_moments: linear_moments() in fp64 on the host), in internal element order.
 int Engine::build_eval_table() {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
-  const double per_source = source_normalization();
-  if (!(per_source > 0.0)) {
-    fprintf(stderr, "[pumitally] ERROR: source normalisation divisor is %g (no source weight seen yet?)\n", per_source);
-    return 1;
-  }
+  double per_source = 1.0;
+  if (!per_source_divisor(&per_source)) return 1;
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
   d_eval_vals_ = d_eval_grads_ = d_eval_cen_ = nullptr;
   PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_eval_vals_), std::max<size_t>(B * S * E, 1) * sizeof(double)));

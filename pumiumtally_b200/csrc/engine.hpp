@@ -26,6 +26,25 @@ struct EngineStats {
   uint64_t plane_fallbacks = 0;
 };
 
+// What a move tallies besides the track length, and the per-particle arrays that takes (nullptr: absent).
+struct MoveTally {
+  enum Kind { kPlain, kScored, kTimed };
+  Kind kind = kPlain;                  // kPlain includes the binned moves
+  const int32_t *bins = nullptr;       // [N] score bin per particle; counts only while the engine has several
+  const double *responses = nullptr;   // [N * nscores] (scored; timed with one score: optional, every response 1)
+  const double *times = nullptr;       // [N] time at the origin (timed)
+  const double *speeds = nullptr;      // [N] (timed)
+};
+
+// One call of a move entry point: host or device pointers, as the entry point taking it says.
+struct Move {
+  const double *origin = nullptr, *dest = nullptr;
+  int8_t *flying = nullptr;  // zeroed by a host move once consumed; a device move never writes it
+  const double *weights = nullptr;
+  int32_t size = 0;          // 3 * num_particles
+  MoveTally tally;
+};
+
 class Engine {
  public:
   // Throws std::runtime_error when no CUDA device is usable: there is no CPU path.
@@ -40,45 +59,26 @@ class Engine {
 
   // Host-pointer entry points (reference semantics; block until inputs are consumed).
   int copy_initial_position(const double *xyz, int32_t size);
-  int move_to_next_location(const double *origin, const double *dest, int8_t *flying,
-                            const double *weights, int32_t size);
+  int move_to_next_location(const Move &m);
   // Device-pointer entry points (enqueue only).
   int copy_initial_position_device(const double *d_xyz, int32_t size, cudaStream_t stream);
-  int move_to_next_location_device(const double *d_origin, const double *d_dest,
-                                   const int8_t *d_flying, const double *d_weights, int32_t size,
-                                   cudaStream_t stream);
+  int move_to_next_location_device(const Move &m, cudaStream_t stream);
 
-  // Score filter: nbins flux arrays; a binned move tallies particle i into array bins[i] (outside
+  // Score filter: nbins flux arrays; a move with bins tallies particle i into array bins[i] (outside
   // [0, nbins): the particle flies unscored).  Resets the tally.  Before comm_init on multi-GPU runs.
   int set_score_bins(int32_t nbins);
   int32_t score_bins() const { return nbins_; }
-  int move_to_next_location_binned(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                                   const int32_t *bins, int32_t size);
-  int move_to_next_location_device_binned(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                                          const double *d_weights, const int32_t *d_bins, int32_t size, cudaStream_t stream);
   // Scores: nscores responses per particle and move, tallied in one walk (walk_core.cuh, ScoreParams).  A scored
   // move adds l * w[i] * r[i*nscores + k] to score k of the particle's bin for every segment of length l.
-  // Resets the tally; before comm_init.  With nscores > 1 only the scored moves are accepted.
+  // Resets the tally; before comm_init.  With nscores > 1 only the scored and timed moves are accepted.
   int set_scores(int32_t nscores);
   int32_t scores() const { return nscores_; }
-  int move_to_next_location_scored(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                                   const double *responses, const int32_t *bins, int32_t size);
-  int move_to_next_location_device_scored(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                                          const double *d_weights, const double *d_responses, const int32_t *d_bins,
-                                          int32_t size, cudaStream_t stream);
   // Time filter: edges T_0 < ... < T_nt (nt = nedges - 1, 1..kMaxTimeBins); a timed move splits every segment
   // between the time bins [T_j, T_j+1) it spans, by the time spent in each (walk_core.cuh, TimeParams).  edges ==
   // nullptr with nedges == 0 removes the filter.  Resets the tally; before comm_init.  While time bins are set only
   // the timed moves are accepted.
   int set_time_bins(const double *edges, int32_t nedges);
   int32_t time_bins() const { return ntime_; }
-  int move_to_next_location_timed(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                                  const double *times, const double *speeds, const double *responses,
-                                  const int32_t *bins, int32_t size);
-  int move_to_next_location_device_timed(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                                         const double *d_weights, const double *d_times, const double *d_speeds,
-                                         const double *d_responses, const int32_t *d_bins, int32_t size,
-                                         cudaStream_t stream);
   // Linear flux moments (walk_core.cuh, moment_tally): order 1 makes every move also tally the first spatial moment
   // of every score, order 0 stops it.  Resets the tally; before comm_init.  Combines with bins, scores and time bins.
   int set_moments(int32_t order);
@@ -132,12 +132,19 @@ class Engine {
   int exchange_tally();
 
  private:
+  // t: the move's tally with device arrays (bins only with several score bins); the default is a plain move
   int launch_range(const double *d_origin, const double *d_dest, const int8_t *d_flying,
                    const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
-                   bool timed);
-  int move_host(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size);
+                   const MoveTally &t = {});
+  int move_host(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size,
+                const MoveTally &dev, int32_t chunk);
+  // slice: doubles between time bins of d_flux; variant, tag: the kernel and its auto-tuner slot (-1: none)
   int launch_range_into(double *d_flux, const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                        const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, bool timed);
+                        const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, const MoveTally &t,
+                        int64_t slice, int variant, int tag);
+  // scored and timed moves, and every move with moments: a tallied walk kernel, never one of the auto-tuner's samples
+  bool scored_move(const MoveTally &t) const { return t.kind != MoveTally::kPlain || moments_ > 0; }
+  bool move_refused(const Move &m, bool device) const;  // with a message; checked before anything is uploaded
   // L2 partition of every SM (l2_partitions.cu), probed when option die_split is switched on; die0_sms_ == 0: no usable map
   uint32_t die_mask_[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   int die0_sms_ = 0, nsms_ = 0;
@@ -158,16 +165,7 @@ class Engine {
   int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments);
   int copy_moments(std::vector<double> &out, bool gradient);  // every result array, [time][bin][score][element][3]
   int get_moments_entry(double *out, int64_t n, bool gradient);
-  bool refuse_unscored(const char *what) const;
-  bool refuse_untimed(const char *what) const;
-  bool timed_args_ok(const char *what, const void *times, const void *speeds, const void *responses) const;
-  int move_host_entry(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size);
-  int move_device_entry(const double *d_origin, const double *d_dest, const int8_t *d_flying, const double *d_weights,
-                        int32_t size, cudaStream_t stream);
-  int move_binned_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                        const int32_t *bins, int32_t size);
-  int move_scored_entry(const double *origin, const double *dest, int8_t *flying, const double *weights,
-                        const double *responses, const int32_t *bins, int32_t size);
+  bool per_source_divisor(double *out);  // of the normalised results; false, with a message, while there is none
   int copy_results(std::vector<double> &out, bool normalized);
   // ---- point queries (locate_kernels.cu) ----
   LocateParams locate_params() const;
@@ -188,26 +186,21 @@ class Engine {
   double *d_eval_vals_ = nullptr, *d_eval_grads_ = nullptr, *d_eval_cen_ = nullptr;
   int build_eval_table();
   int write_scored_results();  // everything, [time][bin][score][element], caller's order
-  // per-particle doubles of a host-pointer move on their way to the device (upload_doubles)
+  // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
-    double *d = nullptr;  // device copy
-    double *h = nullptr;  // pinned copy of pageable caller arrays
-    size_t cap = 0;       // doubles allocated at d / h
+    void *d = nullptr;    // device copy
+    void *h = nullptr;    // pinned copy of pageable caller arrays
+    size_t cap = 0;       // bytes allocated at d / h
     cudaEvent_t ev = nullptr;
   };
-  int upload_doubles(AuxUpload &u, const double *a, const double *b, size_t cnt);
-  const double *cur_resp_ = nullptr;  // device responses of the scored move being launched
-  AuxUpload resp_up_;                 // [N * nscores_] responses of a host-pointer scored move
-  const double *cur_times_ = nullptr, *cur_speeds_ = nullptr;  // device arrays of the timed move being launched
+  int upload_aux(AuxUpload &u, const void *a, const void *b, size_t bytes);
+  void pool_copy(void *dst, const void *src, size_t bytes);  // on the staging workers once they exist
   AuxUpload time_up_;                 // [2N] times, then speeds, of a host-pointer timed move
+  AuxUpload resp_up_;                 // [N * nscores_] responses of a host-pointer scored or timed move
+  AuxUpload bins_up_;                 // [N] bins of a host-pointer move
   double *d_edges_ = nullptr;         // [ntime_ + 1] time bin edges
-  int64_t cur_slice_ = 0;             // doubles between time bins of the array the launch tallies into
-  uint64_t scored_moves_ = 0;         // scored and timed moves since the last reset (not the auto-tuner's samples)
-  const int32_t *cur_bins_ = nullptr; // device array of the move being launched (binned moves only)
+  uint64_t scored_moves_ = 0;         // scored_move() moves since the last reset (not the auto-tuner's samples)
   int8_t *d_mask_ = nullptr;          // [N] flying flags of one bin
-  int32_t *d_bins_ = nullptr;         // [N] bins of a host-pointer move
-  int32_t *h_bins_ = nullptr;         // [N] pinned copy of the caller's bins on their way to the device
-  cudaEvent_t ev_bins_ = nullptr, ev_bins_free_ = nullptr;
   bool host_is_pinned(const void *p) const;
   void maybe_register(const void *p, size_t bytes);
   void collect_timers(bool wait);
@@ -237,10 +230,10 @@ class Engine {
   int explore_pending_ = 0;
   bool explore_complete_ = false;
   uint64_t launches_ = 0;  // kernels launched by the move / localisation entry points
-  void begin_move();
+  void begin_move(bool scored);
   int block_ = 128;
   bool chunk_user_set_ = false;
-  int32_t chunk_ = 1 << 19;  // particles per H2D/compute pipeline stage
+  int32_t chunk_ = 1 << 19;  // particles per H2D/compute pipeline stage (a host move may raise its own, unless user-set)
   // Seed grid for relocation / localisation.  The reference walks straight from the particle's old
   // position to the new one and stops at the hull if that segment leaves the mesh -- on a mesh with
   // concavities or voids even when the new position is inside.  Starting from a seed cell instead
@@ -324,8 +317,9 @@ class Engine {
   int pool_node_ = -1;
   int ensure_stage_buffers(const void *caller_mem, size_t caller_bytes);
   void follow_caller_memory(const void *p, size_t bytes);
-  int ensure_patch_buffers(int nchunks);
-  int move_direct(const double *origin, const double *dest, int8_t *flying, const double *weights, int nchunks);
+  int ensure_patch_buffers(int nchunks, int32_t chunk);
+  int move_direct(const double *origin, const double *dest, int8_t *flying, const double *weights, int nchunks,
+                  const MoveTally &dev, int32_t chunk);
   // Page-locked caller arrays (pinned by the caller, or by option register_host): see move_pinned().
   // Off by default: the positions travelling back (24 B per particle, device->host) can slow the uploads
   // down more than the saved host work buys.
@@ -336,7 +330,8 @@ class Engine {
   std::vector<cudaEvent_t> pos_events_, walk_events_;  // per chunk: positions back on the host / walk + export done
   double d2h_bytes_ = 0.0;
   int ensure_position_mirror(int nchunks);
-  int move_pinned(const double *origin, const double *dest, int8_t *flying, const double *weights, int nchunks);
+  int move_pinned(const double *origin, const double *dest, int8_t *flying, const double *weights, int nchunks,
+                  int32_t chunk);
   int relocate_patches(const PatchEntry *d_list, int32_t count, cudaStream_t stream);
 
   // NCCL (resolved with dlopen at comm_init time)

@@ -19,6 +19,11 @@
 #include "walk_persist.cuh"
 
 namespace ptb {
+
+#ifdef PTB_EXPERIMENTS
+cudaError_t launch_walk_experiment(const WalkParams &p, int variant, int block, cudaStream_t stream);
+#endif
+
 namespace {
 
 // ---------------------------------------------------------------- variant 0
@@ -232,122 +237,55 @@ __global__ void sum_flying_weights_kernel(const int8_t *flying, const double *we
   if ((threadIdx.x & 31) == 0 && s != 0.0) atomicAdd(total, s);
 }
 
+// The product kernels of one instantiation of the walk: NS scores (0: the plain tally), TM the time filter, MO the
+// moments.  ldg is its thread-per-particle kernel, handed in because each instantiation has its own launch bounds.
+// Every other variant is refused, except that the plain walk hands it to the experiments when they are linked in.
+template <int NS, bool TM, bool MO>
+cudaError_t launch_product(const KernelParams<NS, TM> &p, int variant, int block, cudaStream_t stream,
+                           void (*ldg)(KernelParams<NS, TM>)) {
+  const long long n = (long long)p.end - p.begin;
+  if (n <= 0) return cudaSuccess;
+  if (block != 64 && block != 128 && block != 256) block = 128;
+  switch (variant) {
+    case kVariantLdg: {
+      const unsigned grid = (unsigned)((n + block - 1) / block);
+      ldg<<<grid, block, 0, stream>>>(p);
+      return cudaGetLastError();
+    }
+    case kVariantPersistRefill8:
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, NS, TM, MO>(p, n, stream);
+    case kVariantPersistGatherL1:
+      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, NS, TM, MO>(p, n, stream);
+    case kVariantPacked:
+      if (!p.rows) return cudaErrorInvalidValue;
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, NS, TM, MO>(p, n, stream);
+    default:
+#ifdef PTB_EXPERIMENTS
+      if constexpr (NS == 0) return launch_walk_experiment(p, variant, block, stream);
+#endif
+      return cudaErrorInvalidValue;  // the experiments have no scored, timed or moment instantiation
+  }
+}
+
 }  // namespace
 
-#ifdef PTB_EXPERIMENTS
-cudaError_t launch_walk_experiment(const WalkParams &p, int variant, int block, cudaStream_t stream);
-#endif
-
 cudaError_t launch_walk(const WalkParams &p, int variant, int block, cudaStream_t stream) {
-  const long long n = (long long)p.end - p.begin;
-  if (n <= 0) return cudaSuccess;
-  if (block != 64 && block != 128 && block != 256) block = 128;
-  switch (variant) {
-    case kVariantLdg: {
-      const unsigned grid = (unsigned)((n + block - 1) / block);
-      walk_ldg_kernel<<<grid, block, 0, stream>>>(p);
-      return cudaGetLastError();
-    }
-    case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8>(p, n, stream);
-    case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, true, 40>(p, n, stream);
-    case kVariantPacked:
-      if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2>(p, n, stream);
-    default:
-#ifdef PTB_EXPERIMENTS
-      return launch_walk_experiment(p, variant, block, stream);
-#else
-      return cudaErrorInvalidValue;
-#endif
-  }
+  return launch_product<0, false, false>(p, variant, block, stream, walk_ldg_kernel<0>);
 }
 
-cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block, cudaStream_t stream, bool moments) {
-  const long long n = (long long)p.end - p.begin;
-  if (n <= 0) return cudaSuccess;
+cudaError_t launch_walk_tallied(const TimedWalkParams &p, bool timed, bool moments, int variant, int block,
+                                cudaStream_t stream) {
   if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores ||
       p.sc.stride != score_stride(p.sc.nscores) * (moments ? kMomentSlots : 1) ||
-      (!p.sc.responses && !(moments && p.sc.nscores == 1)))
+      (!p.sc.responses && !(p.sc.nscores == 1 && (timed || moments))))
     return cudaErrorInvalidValue;
-  if (block != 64 && block != 128 && block != 256) block = 128;
-  if (moments) switch (variant) {
-    case kVariantLdg: {
-      const unsigned grid = (unsigned)((n + block - 1) / block);
-      walk_ldg_moments_kernel<<<grid, block, 0, stream>>>(p);
-      return cudaGetLastError();
-    }
-    case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores, false, true>(p, n, stream);
-    case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores, false, true>(p, n, stream);
-    case kVariantPacked:
-      if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores, false, true>(p, n, stream);
-    default:
-      return cudaErrorInvalidValue;  // the experiments have no moment instantiation
-  }
-  switch (variant) {
-    case kVariantLdg: {
-      const unsigned grid = (unsigned)((n + block - 1) / block);
-      walk_ldg_kernel<kMaxScores><<<grid, block, 0, stream>>>(p);
-      return cudaGetLastError();
-    }
-    case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores>(p, n, stream);
-    case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores>(p, n, stream);
-    case kVariantPacked:
-      if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores>(p, n, stream);
-    default:
-      return cudaErrorInvalidValue;  // the experiments have no scored instantiation
-  }
-}
-
-cudaError_t launch_walk_timed(const TimedWalkParams &p, int variant, int block, cudaStream_t stream, bool moments) {
-  const long long n = (long long)p.end - p.begin;
-  if (n <= 0) return cudaSuccess;
-  if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores ||
-      p.sc.stride != score_stride(p.sc.nscores) * (moments ? kMomentSlots : 1) ||
-      (!p.sc.responses && p.sc.nscores != 1))
+  if (timed && (p.tm.nt < 1 || p.tm.nt > kMaxTimeBins || p.tm.slice < 0 || !p.tm.edges || !p.tm.times || !p.tm.speeds))
     return cudaErrorInvalidValue;
-  if (p.tm.nt < 1 || p.tm.nt > kMaxTimeBins || p.tm.slice < 0 || !p.tm.edges || !p.tm.times || !p.tm.speeds)
-    return cudaErrorInvalidValue;
-  if (block != 64 && block != 128 && block != 256) block = 128;
-  if (moments) switch (variant) {
-    case kVariantLdg: {
-      const unsigned grid = (unsigned)((n + block - 1) / block);
-      walk_ldg_timed_moments_kernel<<<grid, block, 0, stream>>>(p);
-      return cudaGetLastError();
-    }
-    case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores, true, true>(p, n, stream);
-    case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores, true, true>(p, n, stream);
-    case kVariantPacked:
-      if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores, true, true>(p, n, stream);
-    default:
-      return cudaErrorInvalidValue;  // the experiments have no moment instantiation
-  }
-  switch (variant) {
-    case kVariantLdg: {
-      const unsigned grid = (unsigned)((n + block - 1) / block);
-      walk_ldg_timed_kernel<<<grid, block, 0, stream>>>(p);
-      return cudaGetLastError();
-    }
-    case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, kMaxScores, true>(p, n, stream);
-    case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, kMaxScores, true>(p, n, stream);
-    case kVariantPacked:
-      if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, kMaxScores, true>(p, n, stream);
-    default:
-      return cudaErrorInvalidValue;  // the experiments have no timed instantiation
-  }
+  if (timed)
+    return moments ? launch_product<kMaxScores, true, true>(p, variant, block, stream, walk_ldg_timed_moments_kernel)
+                   : launch_product<kMaxScores, true, false>(p, variant, block, stream, walk_ldg_timed_kernel);
+  return moments ? launch_product<kMaxScores, false, true>(p, variant, block, stream, walk_ldg_moments_kernel)
+                 : launch_product<kMaxScores, false, false>(p, variant, block, stream, walk_ldg_kernel<kMaxScores>);
 }
 
 int walk_blocks_per_sm() { return last_persist_occupancy(); }

@@ -56,18 +56,14 @@ inline bool variant_is_packed(int v) {
 
 cudaError_t launch_walk(const WalkParams &p, int variant, int block, cudaStream_t stream);
 bool walk_variant_available(int variant);  // compiled into this library?
-// Scored walk (walk_core.cuh, ScoreParams): same kernels, instantiated for up to kMaxScores scores; product
-// variants 0, 8, 16, 24 only.  p.flux is [element][p.sc.stride].
+// Tallied walk: the same kernels instantiated for up to kMaxScores scores (walk_core.cuh, ScoreParams; p.flux is
+// [element][p.sc.stride]); product variants 0, 8, 16, 24 only.  p.tm is read only when timed.
+// timed: the time filter (walk_core.cuh, TimeParams).  p.flux points at time bin 0 of the score bin; time bin j is at
+// p.flux + j * p.tm.slice.  p.sc.responses may be nullptr when p.sc.nscores == 1 (every response 1).
 // moments: the moment walk (walk_core.cuh, moment_tally): p.sc.stride is kMomentSlots * score_stride(nscores), and
 // p.sc.responses may be nullptr when p.sc.nscores == 1 (every response 1: the plain and binned moves).
-cudaError_t launch_walk_scored(const ScoredWalkParams &p, int variant, int block, cudaStream_t stream,
-                               bool moments = false);
-// Timed walk (walk_core.cuh, TimeParams): the scored walk plus a time filter, on the same four product variants.
-// p.flux points at time bin 0 of the score bin; time bin j is at p.flux + j * p.tm.slice.  p.sc.responses may be
-// nullptr when p.sc.nscores == 1 (every response 1).
-// moments: as for launch_walk_scored.
-cudaError_t launch_walk_timed(const TimedWalkParams &p, int variant, int block, cudaStream_t stream,
-                              bool moments = false);
+cudaError_t launch_walk_tallied(const TimedWalkParams &p, bool timed, bool moments, int variant, int block,
+                                cudaStream_t stream);
 // blocks per SM the occupancy calculator gave the last persistent walk kernel launched (0: none yet)
 int walk_blocks_per_sm();
 // origin == nullptr: the binning key is the stored position (state)

@@ -472,6 +472,54 @@ def test_pinned_caller_path_every_origin_changed_and_none_changed():
     np.testing.assert_array_equal(e.positions, orc.positions)
 
 
+def test_binned_and_scored_host_moves_leave_the_pinned_caller_options_alone():
+    """Binned and scored host moves never take the pinned-caller path, and they leave the options that choose it and
+    the stage size as the caller set them: a plain move after them takes the pinned-caller path again."""
+    import torch
+
+    nbins = 2
+    coords, t2v, wl = box_case((6, 6, 5), 40_000)
+    n = wl.n
+    e = gpu_engine(-1)(coords, t2v, n)
+    e.set_option("pinned_path", 1)
+    e.set_option("host_path", 1)
+    e.set_score_bins(nbins)
+    e.set_scores(1)
+    chunk = e.get_option("chunk")
+    orc = OraclePumiTally(coords, t2v, n)
+    init = wl.initial_positions()
+    for x in (e, orc):
+        x.CopyInitialPosition(init.reshape(-1).copy())
+    O, D, F, W = _host_buffers(n, "pinned")
+    B = torch.empty(n, dtype=torch.int32, pin_memory=True).numpy()
+    want = np.zeros((nbins, len(t2v)))
+    rng = np.random.default_rng(11)
+    for step, kind in enumerate(["binned", "scored", "plain"]):
+        o, d, f, w = wl.next_step()
+        O[:], D[:], W[:], F[:] = o.reshape(-1), d.reshape(-1), w, f
+        if kind == "binned":
+            B[:] = _bins_for_step(n, nbins, step)
+            e.MoveToNextLocationBinned(O, D, F, W, B)
+            oracle_binned_move(orc, want, o, d, f, w, B.copy())
+        else:
+            r = rng.uniform(0.5, 2.0, n) if kind == "scored" else np.ones(n)
+            if kind == "scored":
+                e.MoveToNextLocationScored(O, D, F, W, r)
+            else:
+                e.MoveToNextLocation(O, D, F, W)
+            before = orc.flux.copy()
+            orc.MoveToNextLocation(o.reshape(-1).copy(), d.reshape(-1).copy(), f.copy(), w * r)
+            want[0] += orc.flux - before  # no bins: the first bin
+        assert not F.any()
+        assert e.get_option("position_mirror") == (kind == "plain")
+        assert e.get_option("pinned_path") == 1 and e.get_option("chunk") == chunk
+        got = e.flux_bins
+        for b in range(nbins):
+            assert_flux_close(got[b], want[b], f"{kind} move, bin {b}")
+        np.testing.assert_array_equal(e.elem_ids, orc.elem_ids)
+        assert_positions_close(e.positions, orc.positions, f"{kind} move")
+
+
 def test_page_locked_caller_arrays_get_the_faster_of_staged_and_direct_uploads():
     """host_path=2 (default): with page-locked caller arrays moves 2-3 of every 256 are uploaded directly,
     the rest staged, and the faster path is kept; results are the oracle's whichever path a move took."""
