@@ -76,6 +76,25 @@ inline int EvaluatePoints(const PumiTally &tally, const double *xyz, int64_t npt
   return pumitally_evaluate_points(engine_of(tally), xyz, npts, out, n, out_elem);
 }
 
+// Collision estimator (see pumitally_set_collision_estimator in pumitally_c.h): a collision tally with the track-length
+// tally's configuration.  TallyCollisions scores events at arbitrary points (located as LocatePoints does),
+// TallyCollisionsAtParticles at the particles' positions after the last move, for every i with collided[i] != 0 (size
+// = num_particles).  Event i adds weights[i] * responses[i * nscores + k] to score k; responses may be nullptr with one
+// score, bins nullptr (bin 0), times nullptr without time bins.
+inline int SetCollisionEstimator(const PumiTally &tally, int32_t on) {
+  return pumitally_set_collision_estimator(engine_of(tally), on);
+}
+inline int TallyCollisions(const PumiTally &tally, const double *xyz, int64_t nevents, const double *weights,
+                           const double *responses = nullptr, const int32_t *bins = nullptr,
+                           const double *times = nullptr) {
+  return pumitally_tally_collisions(engine_of(tally), xyz, nevents, weights, responses, bins, times);
+}
+inline int TallyCollisionsAtParticles(const PumiTally &tally, const int8_t *collided, const double *weights,
+                                      int32_t size, const double *responses = nullptr, const int32_t *bins = nullptr,
+                                      const double *times = nullptr) {
+  return pumitally_tally_collisions_at_particles(engine_of(tally), collided, weights, responses, bins, times, size);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

@@ -345,6 +345,60 @@ int pumitally_locate_points_device(pumitally_engine *e, const double *d_xyz, int
 int pumitally_evaluate_points(pumitally_engine *e, const double *xyz, int64_t npts, double *out, int64_t n,
                               int32_t *out_elem);
 
+/* ---- additive: collision estimator (events scored at collision sites) ----
+ * Some scores can only be made at a collision (an analog absorption count, the energy a collision deposits) and only the
+ * caller knows what happened there; OpenMC's combined k-eff also wants a collision estimate next to the track-length
+ * one.  pumitally_set_collision_estimator(e, 1) adds a collision tally with the configuration of the track-length tally
+ * (score bins, scores, time bins, moment order) in arrays of its own, so the same scores are estimated both ways; 0
+ * (the default) removes it.  Any other value, or a flux array that cannot be allocated (twice the track-length one),
+ * returns non-zero and changes nothing.  The call resets the tally, combines with the other pumitally_set_* calls in any
+ * order and is refused after pumitally_comm_init.  pumitally_get_collision_estimator (or the read-only option
+ * "collision_estimator") returns 1 or 0.  With it off nothing differs from an engine without it.
+ * Event i in element e, score bin b = bins[i] and time bin j adds weights[i] * responses[i * nscores + k] to score k of
+ * (j, b, e); with moments it also adds that amount times (x_i - C), C the mesh centre, to the first-moment slots, as a
+ * move does for a segment's midpoint.  What weights carry is the caller's choice: w / Sigma_t for a collision
+ * estimate, w with 0/1 responses for an analog count.
+ * pumitally_tally_collisions: nevents events at AoS points xyz[3 * nevents], each located as pumitally_locate_points
+ * locates it; host calls work through device buffers of the option "chunk" events.  The _device variant takes device
+ * arrays and is enqueued on `stream`.
+ * pumitally_tally_collisions_at_particles: an event for every particle i with collided[i] != 0, at its stored position,
+ * in its parent element (no location step); n must be num_particles and collided is not zeroed.  Flag only flights that
+ * ended at their destination: a flight clipped at the hull stored the hull point.  The _device variant is enqueued on
+ * `stream` behind the last move, as a move on another stream is.
+ * responses may be NULL only with one score (every response 1); bins may be NULL (every event in bin 0); times are
+ * required while time bins are set and ignored otherwise.  A time on an edge belongs to the bin above it.  Not tallied:
+ * a bin outside [0, nbins), a time before T_0 or at or after T_n, a located event outside the mesh (counted as outside),
+ * and an event with a non-finite coordinate, weight * response or time (counted as rejected; this takes precedence).
+ * The read-only options "collisions", "collisions_outside" and "collisions_rejected" count the events tallied, outside
+ * and rejected since the last pumitally_reset_tally.  Refused (non-zero, nothing changes): the estimator is off,
+ * responses NULL with several scores, times NULL while time bins are set, nevents < 0, n != num_particles.  nevents == 0
+ * succeeds and does nothing.
+ * A collision call changes no particle, flying flag, track-length result, statistic or kernel choice; like a move it
+ * ends the validity of the last batch-end exchange.  Host calls have consumed their inputs when they return.
+ * pumitally_get_collision_results(e, kind, out, n): kind 0 raw, 1 normalised, 2 first moments m1, 3 gradient -- what
+ * pumitally_get_flux, _get_normalized_flux, _get_flux_moments and _get_flux_gradient return for the track-length tally,
+ * with the same n, layout, caller's numbering, volume, source normalisation and batch-end exchange (collective after
+ * pumitally_reduce_tally_to_owners).  Kinds 2 and 3 without moments, and any call with the estimator off, return
+ * non-zero.  pumitally_reset_tally zeroes the collision tally; both batch-end exchanges sum it with the track-length
+ * tally in the same collective.  WriteTallyResults writes, after the track-length arrays, every one of their names
+ * prefixed "collision_" ("collision_flux", "collision_flux_bin<b>", "collision_score<k>_t<j>", "collision_flux_grad",
+ * ...).  Behind pumitally_flux_device_ptr the collision tally directly follows the track-length one, same layout. */
+int pumitally_set_collision_estimator(pumitally_engine *e, int32_t on);
+int32_t pumitally_get_collision_estimator(const pumitally_engine *e);
+int pumitally_tally_collisions(pumitally_engine *e, const double *xyz, int64_t nevents, const double *weights,
+                               const double *responses, const int32_t *bins, const double *times);
+int pumitally_tally_collisions_device(pumitally_engine *e, const double *d_xyz, int64_t nevents,
+                                      const double *d_weights, const double *d_responses, const int32_t *d_bins,
+                                      const double *d_times, void *stream);
+int pumitally_tally_collisions_at_particles(pumitally_engine *e, const int8_t *collided, const double *weights,
+                                            const double *responses, const int32_t *bins, const double *times,
+                                            int32_t n);
+int pumitally_tally_collisions_at_particles_device(pumitally_engine *e, const int8_t *d_collided,
+                                                   const double *d_weights, const double *d_responses,
+                                                   const int32_t *d_bins, const double *d_times, int32_t n,
+                                                   void *stream);
+int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *out, int64_t n);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

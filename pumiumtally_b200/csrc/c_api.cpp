@@ -233,6 +233,44 @@ int pumitally_evaluate_points(pumitally_engine *e, const double *xyz, int64_t np
   return guarded(e, [&](ptb::Engine &g) { return g.evaluate_points(xyz, npts, out, n, out_elem); });
 }
 
+int pumitally_set_collision_estimator(pumitally_engine *e, int32_t on) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_collision_estimator(on); });
+}
+int32_t pumitally_get_collision_estimator(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "collision_estimator")) : 0;
+}
+int pumitally_tally_collisions(pumitally_engine *e, const double *xyz, int64_t nevents, const double *weights,
+                               const double *responses, const int32_t *bins, const double *times) {
+  return guarded(e, [&](ptb::Engine &g) { return g.tally_collisions(xyz, nevents, weights, responses, bins, times); });
+}
+int pumitally_tally_collisions_device(pumitally_engine *e, const double *d_xyz, int64_t nevents, const double *d_weights,
+                                      const double *d_responses, const int32_t *d_bins, const double *d_times,
+                                      void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_collisions_device(d_xyz, nevents, d_weights, d_responses, d_bins, d_times,
+                                     static_cast<cudaStream_t>(stream));
+  });
+}
+int pumitally_tally_collisions_at_particles(pumitally_engine *e, const int8_t *collided, const double *weights,
+                                            const double *responses, const int32_t *bins, const double *times,
+                                            int32_t n) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_collisions_at_particles(collided, weights, responses, bins, times, n);
+  });
+}
+int pumitally_tally_collisions_at_particles_device(pumitally_engine *e, const int8_t *d_collided,
+                                                   const double *d_weights, const double *d_responses,
+                                                   const int32_t *d_bins, const double *d_times, int32_t n,
+                                                   void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_collisions_at_particles_device(d_collided, d_weights, d_responses, d_bins, d_times, n,
+                                                  static_cast<cudaStream_t>(stream));
+  });
+}
+int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *out, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_collision_results(kind, out, n); });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

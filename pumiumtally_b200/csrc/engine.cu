@@ -77,6 +77,8 @@ Engine::Engine(HostMesh &&mesh, int32_t num_particles, int device)
   dev_alloc(&d_weights_, N, "weights staging");
   dev_alloc(&d_flying_, N, "flying staging");
   dev_alloc(&d_stats_, 1, "stats");
+  dev_alloc(&d_coll_counts_, 3, "collision counters");
+  cuda_or_throw(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)), "memset");
   dev_alloc(&d_initial_weight_, 1, "initial weight");
   cuda_or_throw(cudaMemset(d_initial_weight_, 0, sizeof(double)), "memset");
   dev_alloc(&d_tickets_, 2 * kTicketRing, "tickets");  // second half: the other L2 partition's tickets (die split)
@@ -184,6 +186,7 @@ Engine::~Engine() {
   cudaFree(d_cand_off_); cudaFree(d_cand_);
   cudaFree(d_qxyz_); cudaFree(d_qout_); cudaFree(d_qint_); cudaFree(d_qelem_);
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
+  cudaFree(d_coll_counts_); cudaFree(d_coll_buf_);
   if (compute_) cudaStreamDestroy(compute_);
   if (copy_) cudaStreamDestroy(copy_);
 }
@@ -311,13 +314,10 @@ int Engine::relocate_patches(const PatchEntry *d_list, int32_t count, cudaStream
   return 0;
 }
 
-int Engine::launch_range(const double *d_origin, const double *d_dest, const int8_t *d_flying,
-                         const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
-                         const MoveTally &t) {
-  if (end <= begin) return 0;
-  // Particle state, binning scratch and the ticket ring are shared by every launch: work enqueued on
-  // another stream than the previous launch's (a device-pointer move on the caller's stream after a
-  // host-pointer move on the engine's own, or the other way round) is ordered behind it by an event.
+// Particle state, binning scratch and the ticket ring are shared by every launch: work enqueued on
+// another stream than the previous launch's (a device-pointer move on the caller's stream after a
+// host-pointer move on the engine's own, or the other way round) is ordered behind it by an event.
+int Engine::follow_last_stream(cudaStream_t stream) {
   if (last_stream_set_ && stream != last_stream_) {
     if (!ev_order_) PTB_CUDA_OK(cudaEventCreateWithFlags(&ev_order_, cudaEventDisableTiming));
     PTB_CUDA_OK(cudaEventRecord(ev_order_, last_stream_));
@@ -325,6 +325,14 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   }
   last_stream_ = stream;
   last_stream_set_ = true;
+  return 0;
+}
+
+int Engine::launch_range(const double *d_origin, const double *d_dest, const int8_t *d_flying,
+                         const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
+                         const MoveTally &t) {
+  if (end <= begin) return 0;
+  if (follow_last_stream(stream)) return 1;
   if (d_dest) flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on; the last exchange no longer describes it
   const int64_t slice = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
   if (!(t.bins && d_dest))
@@ -344,7 +352,7 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
     if (launch_bin_mask(d_flying, t.bins, b, nbins_, d_mask_, begin, end, stream) != cudaSuccess) return 1;
     ++launches_;
     // the unreported array follows every reported one (with a time filter, all time bins of a bin-b pass go to it)
-    if (launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : flux_len()), d_origin, d_dest, d_mask_,
+    if (launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : reported_len()), d_origin, d_dest, d_mask_,
                           d_weights, begin, end, stream, t, b < nbins_ ? slice : 0, variant, tag))
       return 1;
   }
@@ -1104,7 +1112,7 @@ int Engine::set_score_bins(int32_t nbins) {
     fprintf(stderr, "[pumitally] ERROR: set_score_bins after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins, nscores_, ntime_, moments_);
+  return resize_flux(nbins, nscores_, ntime_, moments_, collision_);
 }
 
 // Scores (walk_core.cuh, ScoreParams): the flux array becomes [bin][element][score_stride(nscores)].
@@ -1114,7 +1122,7 @@ int Engine::set_scores(int32_t nscores) {
     fprintf(stderr, "[pumitally] ERROR: set_scores after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores, ntime_, moments_);
+  return resize_flux(nbins_, nscores, ntime_, moments_, collision_);
 }
 
 // Time filter (walk_core.cuh, TimeParams): the flux array becomes [time][bin][element][stride], the edges live on
@@ -1125,7 +1133,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (!edges && nedges == 0) {  // no time filter
-    if (resize_flux(nbins_, nscores_, 0, moments_)) return 1;
+    if (resize_flux(nbins_, nscores_, 0, moments_, collision_)) return 1;
     cudaFree(d_edges_);
     d_edges_ = nullptr;
     return 0;
@@ -1140,7 +1148,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (cudaMemcpy(ne, edges, size_t(nedges) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
-      resize_flux(nbins_, nscores_, nedges - 1, moments_)) {
+      resize_flux(nbins_, nscores_, nedges - 1, moments_, collision_)) {
     cudaGetLastError();
     cudaFree(ne);
     return 1;
@@ -1157,14 +1165,26 @@ int Engine::set_moments(int32_t order) {
     fprintf(stderr, "[pumitally] ERROR: set_moments after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores_, ntime_, order);
+  return resize_flux(nbins_, nscores_, ntime_, order, collision_);
 }
 
-int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments) {
+// Collision estimator (walk_core.cuh, collision_event): a second tally of the same layout after the track-length one.
+int Engine::set_collision_estimator(int32_t on) {
+  if (on != 0 && on != 1) return 1;
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_collision_estimator after comm_init (the exchange buffers are sized by then)\n");
+    return 1;
+  }
+  return resize_flux(nbins_, nscores_, ntime_, moments_, on != 0);
+}
+
+int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision) {
   if (synchronize()) return 1;
   const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores)) * (moments ? kMomentSlots : 1);
-  // [time][bin][element][stride], then the unreported array of the particles no bin matches
-  const size_t len = (size_t(ntime > 0 ? ntime : 1) * size_t(nbins) + (nbins > 1 ? 1 : 0)) * E * stride + kFluxPad;
+  // [time][bin][element][stride], the collision tally of the same layout, then the unreported array of the particles
+  // no bin matches
+  const size_t tally = size_t(ntime > 0 ? ntime : 1) * size_t(nbins) * (collision ? 2 : 1);
+  const size_t len = (tally + (nbins > 1 ? 1 : 0)) * E * stride + kFluxPad;
   double *nf = nullptr;
   const cudaError_t err = cudaMalloc(reinterpret_cast<void **>(&nf), len * sizeof(double));
   if (err != cudaSuccess) {
@@ -1181,6 +1201,7 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
   stride_ = int32_t(stride);
   ntime_ = ntime;
   moments_ = moments;
+  collision_ = collision;
   if (nbins > 1 && !d_mask_) PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
   return reset_tally();  // a new set of arrays starts from zero
 }
@@ -1296,7 +1317,7 @@ int Engine::get_flux_device(double *d_out, cudaStream_t stream) {
 
 // Every time bin, bin and score of the tally, [time][bin][score][element] in the caller's numbering: raw, or
 // normalised as get_normalized_flux does it.  (Time bin t of bin b is internal array t * nbins + b.)
-int Engine::copy_results(std::vector<double> &out, bool normalized) {
+int Engine::copy_results(std::vector<double> &out, bool normalized, size_t base) {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
   double per_source = 1.0;
   if (normalized && !per_source_divisor(&per_source)) return 1;
@@ -1307,7 +1328,7 @@ int Engine::copy_results(std::vector<double> &out, bool normalized) {
   std::vector<double> tmp(S * E);
   int rc = 0;
   for (size_t b = 0; b < B && !rc; ++b) {
-    const double *f = flux_view() + b * bin_len();
+    const double *f = flux_view() + base + b * bin_len();
     cudaError_t e = normalized ? launch_normalize_scores(f, d_volume_, d_tmp, int64_t(E), nscores_, stride_, per_source, compute_)
                                : launch_scores_to_caller_order(f, d_orig_of_internal_, d_tmp, int64_t(E), nscores_, stride_, compute_);
     if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
@@ -1347,13 +1368,13 @@ int Engine::get_flux(double *out, int64_t n) {
 
 // The linear moments of every result array, [time][bin][score][element][3] in the caller's numbering: m1 about each
 // element's centroid, or the gradient g = M^-1 m1 divided by the source normalisation (linear_moments()).
-int Engine::copy_moments(std::vector<double> &out, bool gradient) {
+int Engine::copy_moments(std::vector<double> &out, bool gradient, size_t base) {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
   const int slot = stride_ / kMomentSlots;
   double per_source = 1.0;
   if (gradient && !per_source_divisor(&per_source)) return 1;
   std::vector<double> raw(B * bin_len());
-  PTB_CUDA_OK(cudaMemcpy(raw.data(), flux_view(), raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  PTB_CUDA_OK(cudaMemcpy(raw.data(), flux_view() + base, raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
   out.resize(B * S * E * 3);
   const double *xyz = mesh_.coords.data();
 #pragma omp parallel for schedule(static)
@@ -1374,7 +1395,7 @@ int Engine::copy_moments(std::vector<double> &out, bool gradient) {
 }
 
 // n == 3E: time bin 0, bin 0, score 0; n == 3 * ntime * nbins * nscores * E: everything
-int Engine::get_moments_entry(double *out, int64_t n, bool gradient) {
+int Engine::get_moments_entry(double *out, int64_t n, bool gradient, size_t base) {
   const int64_t E = mesh_.ntets;
   if (!moments_) {
     fprintf(stderr, "[pumitally] ERROR: the engine tallies no moments (set_moments)\n");
@@ -1383,13 +1404,30 @@ int Engine::get_moments_entry(double *out, int64_t n, bool gradient) {
   if (n != 3 * E && n != 3 * int64_t(result_arrays()) * nscores_ * E) return 1;
   if (synchronize() || gather_shares()) return 1;
   std::vector<double> all;
-  if (copy_moments(all, gradient)) return 1;
+  if (copy_moments(all, gradient, base)) return 1;
   std::memcpy(out, all.data(), size_t(n) * sizeof(double));
   return 0;
 }
 
 int Engine::get_flux_moments(double *out, int64_t n) { return get_moments_entry(out, n, false); }
 int Engine::get_flux_gradient(double *out, int64_t n) { return get_moments_entry(out, n, true); }
+
+// The collision tally read as the track-length one is, through the general ([time][bin][score][element]) path.
+int Engine::get_collision_results(int32_t kind, double *out, int64_t n) {
+  if (!collision_) {
+    fprintf(stderr, "[pumitally] ERROR: the collision estimator is off (set_collision_estimator)\n");
+    return 1;
+  }
+  if (kind == 2 || kind == 3) return get_moments_entry(out, n, kind == 3, flux_len());
+  if (kind != 0 && kind != 1) return 1;
+  const int64_t E = mesh_.ntets;
+  if (n != E && n != int64_t(result_arrays()) * nscores_ * E) return 1;
+  if (synchronize() || gather_shares()) return 1;
+  std::vector<double> all;
+  if (copy_results(all, kind == 1, flux_len())) return 1;
+  std::memcpy(out, all.data(), size_t(n) * sizeof(double));
+  return 0;
+}
 
 // NormalizeFlux (PumiTallyImpl.cpp:382-409); n as for get_flux (the volumes are always E values)
 int Engine::get_normalized_flux(double *out_flux, double *out_volume, int64_t n) {
@@ -1483,6 +1521,7 @@ int Engine::reset_tally() {
   PTB_CUDA_OK(cudaMemset(d_flux_, 0, flux_alloc_ * sizeof(double)));
   scored_moves_ = 0;
   PTB_CUDA_OK(cudaMemset(d_stats_, 0, sizeof(DeviceStats)));
+  PTB_CUDA_OK(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)));
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
   kernel_ms_ = 0.0;
   h2d_bytes_ = 0.0;
@@ -1542,6 +1581,17 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "time_bins") return ntime_;
   if (name == "moments") return moments_;
   if (name == "locate_candidates") return int64_t(cand_entries_);  // entries of the point-location candidate lists
+  if (name == "collision_estimator") return collision_ ? 1 : 0;
+  // collision events since the last reset: tallied, located outside the mesh, rejected (non-finite inputs)
+  if (name == "collisions" || name == "collisions_outside" || name == "collisions_rejected") {
+    unsigned long long c[3] = {0, 0, 0};
+    if (cudaSetDevice(device_) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpy(c, d_coll_counts_, sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) {
+      cudaGetLastError();
+      return -1;
+    }
+    return int64_t(c[name == "collisions" ? 0 : name == "collisions_outside" ? 1 : 2]);
+  }
   if (name == "walk_blocks_per_sm") return walk_blocks_per_sm();  // occupancy of the last persistent walk kernel launched
   if (name == "die_split") return die_split_ ? 1 : 0;
   if (name == "l2_partition0_sms") return die0_sms_;  // SMs in the L2 partition of SM 0 (0: no map found)
@@ -1663,9 +1713,12 @@ int64_t Engine::debug_order(int32_t *out, int64_t n) {
   return cnt;
 }
 
-// FinalizeTallies (PumiTallyImpl.cpp:411-416)
+// FinalizeTallies (PumiTallyImpl.cpp:411-416).  With the collision estimator every array of the track-length tally is
+// followed by its collision twin, the same name prefixed "collision_".
 int Engine::write_tally_results() {
-  if (multi_results()) return write_scored_results();
+  VtkArrays coll;
+  if (collision_ && (synchronize() || gather_shares() || scored_arrays(flux_len(), "collision_", coll, nullptr))) return 1;
+  if (multi_results()) return write_scored_results(coll);
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
   if (get_normalized_flux(nf.data(), vol.data(), int64_t(nf.size()))) return 1;  // caller's element order
@@ -1680,6 +1733,7 @@ int Engine::write_tally_results() {
       for (size_t i = 0; i < E; ++i) nf[i] += nf[size_t(b) * E + i];
     nf.resize(E);
   }
+  extra.insert(extra.end(), coll.named.begin(), coll.named.end());  // (one component each: no moments here)
   std::string err;
   if (!write_vtk_dataset(output_name_, mesh_, nf, vol, rank_, nranks_, &err, extra)) {
     fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
@@ -1693,11 +1747,29 @@ int Engine::write_tally_results() {
 // these are sums over the time bins, and every time bin j adds the same arrays with "_t<j>" after the score name:
 // "flux_t<j>", "flux_t<j>_bin<b>", "score<k>_t<j>", "score<k>_t<j>_bin<b>".  With moments every one of these arrays
 // is followed by "<name>_grad", its normalised gradient (3 components; a sum's gradient is the sum of the gradients).
-int Engine::write_scored_results() {
+int Engine::write_scored_results(VtkArrays &coll) {
+  const size_t E = size_t(mesh_.ntets);
+  std::vector<double> vol(E), flux;
+  if (get_normalized_flux(nullptr, vol.data(), int64_t(E))) return 1;  // (synchronises and gathers the shares)
+  VtkArrays a;
+  if (scored_arrays(0, "", a, &flux)) return 1;
+  a.named.insert(a.named.end(), coll.named.begin(), coll.named.end());
+  a.ncomp.insert(a.ncomp.end(), coll.ncomp.begin(), coll.ncomp.end());
+  std::string err;
+  if (!write_vtk_dataset(output_name_, mesh_, flux, vol, rank_, nranks_, &err, a.named, a.ncomp)) {
+    fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
+    return 1;
+  }
+  return 0;
+}
+
+// The normalised results of the tally at `base` as write_scored_results names them (its data must be current: after
+// synchronize() and gather_shares()).
+int Engine::scored_arrays(size_t base, const std::string &prefix, VtkArrays &a, std::vector<double> *main) {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_), T = nslices();
-  std::vector<double> all(T * B * S * E), vol(E), grad;
-  if (get_normalized_flux(all.data(), vol.data(), int64_t(all.size()))) return 1;
-  if (moments_ && copy_moments(grad, true)) return 1;
+  std::vector<double> all, grad;
+  if (copy_results(all, true, base)) return 1;
+  if (moments_ && copy_moments(grad, true, base)) return 1;
   // the same sums for the gradients, 3 values per element: gsets[q] [bin][score][element][3], gsums[q * S + k]
   std::vector<std::vector<double>> gsets, gsums;
   if (moments_) {
@@ -1731,16 +1803,14 @@ int Engine::write_scored_results() {
       for (size_t b = 1; b < B; ++b)
         for (size_t i = 0; i < E; ++i) sum[i] += sets[q][(b * S + k) * E + i];
     }
-  std::vector<std::pair<std::string, const double *>> extra;
-  std::vector<int> ncomp;
-  auto add = [&](const std::string &name, const double *a, const double *g) {
-    if (a) {
-      extra.emplace_back(name, a);
-      ncomp.push_back(1);
+  auto add = [&](const std::string &name, const double *v, const double *g) {
+    if (v) {
+      a.named.emplace_back(prefix + name, v);
+      a.ncomp.push_back(1);
     }
     if (moments_) {
-      extra.emplace_back(name + "_grad", g);
-      ncomp.push_back(3);
+      a.named.emplace_back(prefix + name + "_grad", g);
+      a.ncomp.push_back(3);
     }
   };
   for (size_t q = 0; q < sets.size(); ++q) {
@@ -1748,18 +1818,17 @@ int Engine::write_scored_results() {
     for (size_t k = 0; k < S; ++k) {
       const std::string name = k == 0 ? "flux" + t : "score" + std::to_string(k) + t;
       // (set 0, score 0 is the main array)
-      add(name, (q > 0 || k > 0) ? sums[q * S + k].data() : nullptr, moments_ ? gsums[q * S + k].data() : nullptr);
+      add(name, (q > 0 || k > 0 || !main) ? sums[q * S + k].data() : nullptr, moments_ ? gsums[q * S + k].data() : nullptr);
       if (B > 1)
         for (size_t b = 0; b < B; ++b)
           add(name + "_bin" + std::to_string(b), sets[q].data() + (b * S + k) * E,
               moments_ ? gsets[q].data() + (b * S + k) * E * 3 : nullptr);
     }
   }
-  std::string err;
-  if (!write_vtk_dataset(output_name_, mesh_, sums[0], vol, rank_, nranks_, &err, extra, ncomp)) {
-    fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
-    return 1;
-  }
+  if (main) *main = sums[0];
+  // the pointers above point into these vectors' storage, which moving them keeps
+  for (auto *v : {&gsets, &gsums, &sets, &sums})
+    for (auto &x : *v) a.data.push_back(std::move(x));
   return 0;
 }
 
@@ -1920,6 +1989,162 @@ int Engine::evaluate_points(const double *xyz, int64_t npts, double *out, int64_
   return 0;
 }
 
+// ------------------------------------------------------------------ collision estimator
+
+CollisionParams Engine::collision_params() const {
+  CollisionParams c{};
+  c.flux = d_flux_ + flux_len();
+  c.edges = d_edges_;
+  c.nt = ntime_;
+  c.nbins = nbins_;
+  c.nscores = nscores_;
+  c.stride = stride_;
+  c.moments = moments_;
+  c.bin_stride = int64_t(bin_len());
+  c.slice = int64_t(nbins_) * int64_t(bin_len());
+  c.cx = mesh_.center[0]; c.cy = mesh_.center[1]; c.cz = mesh_.center[2];
+  return c;
+}
+
+// The refusals every collision call shares, checked before anything is uploaded.
+bool Engine::collision_refused(const double *responses, const double *times) const {
+  const char *why = !collision_                       ? "the collision estimator is off (set_collision_estimator)"
+                    : (!responses && nscores_ > 1)    ? "responses are required with several scores"
+                    : (!times && ntime_ > 0)          ? "times are required while time bins are set"
+                                                      : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: collision events refused: %s\n", why);
+  return why != nullptr;
+}
+
+int Engine::ensure_collision_buffer(size_t bytes) {
+  if (bytes <= coll_buf_bytes_) return 0;
+  cudaFree(d_coll_buf_);
+  d_coll_buf_ = nullptr;
+  coll_buf_bytes_ = 0;
+  PTB_CUDA_OK(cudaMalloc(&d_coll_buf_, bytes));
+  coll_buf_bytes_ = bytes;
+  return 0;
+}
+
+namespace {
+// The chunk-sized event arrays of a host-pointer collision call in one device buffer: xyz [3c] (located calls only),
+// weights [c], responses [nscores c], times [c], bins [c], collided [c] (at-particles calls only).  Per event that is
+// 24 + 8 + 8 nscores + 8 + 4 (+ 1) bytes.
+struct EventBuffers {
+  double *xyz, *w, *r, *t;
+  int32_t *bins;
+  int8_t *collided;
+  static size_t bytes(size_t c, size_t nscores) { return c * (24 + 8 + 8 * nscores + 8 + 4 + 1); }
+  EventBuffers(void *base, size_t c, size_t nscores) {
+    xyz = static_cast<double *>(base);
+    w = xyz + 3 * c;
+    r = w + c;
+    t = r + nscores * c;
+    bins = reinterpret_cast<int32_t *>(t + c);
+    collided = reinterpret_cast<int8_t *>(bins + c);
+  }
+};
+
+cudaError_t upload(void *dst, const void *src, size_t bytes, cudaStream_t s) {
+  return src ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+}
+}  // namespace
+
+int Engine::tally_collisions(const double *xyz, int64_t nevents, const double *weights, const double *responses,
+                             const int32_t *bins, const double *times) {
+  if (collision_refused(responses, times) || nevents < 0 || (nevents > 0 && (!xyz || !weights))) return 1;
+  if (nevents == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const int64_t chunk = std::min<int64_t>(chunk_, nevents);
+  const size_t S = size_t(nscores_);
+  if (ensure_candidates() || ensure_collision_buffer(EventBuffers::bytes(size_t(chunk), S))) return 1;
+  const EventBuffers d(d_coll_buf_, size_t(chunk), S);
+  const LocateParams l = locate_params();
+  const CollisionParams p = collision_params();
+  const double *t = ntime_ > 0 ? times : nullptr;
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on, as with a move
+  for (int64_t b = 0; b < nevents; b += chunk) {
+    const size_t cnt = size_t(std::min(chunk, nevents - b));
+    PTB_CUDA_OK(upload(d.xyz, xyz + 3 * b, 3 * cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.w, weights + b, cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.r, responses ? responses + S * size_t(b) : nullptr, S * cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.t, t ? t + b : nullptr, cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.bins, bins ? bins + b : nullptr, cnt * sizeof(int32_t), compute_));
+    PTB_CUDA_OK(launch_collide_located(l, p, d.xyz, int64_t(cnt), d.w, responses ? d.r : nullptr, bins ? d.bins : nullptr,
+                                       d.t, d_coll_counts_, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
+// The mesh tables location reads never change after construction, so located events need no ordering against moves.
+int Engine::tally_collisions_device(const double *d_xyz, int64_t nevents, const double *d_weights,
+                                    const double *d_responses, const int32_t *d_bins, const double *d_times,
+                                    cudaStream_t stream) {
+  if (collision_refused(d_responses, d_times) || nevents < 0 || (nevents > 0 && (!d_xyz || !d_weights))) return 1;
+  if (nevents == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_candidates()) return 1;
+  const LocateParams l = locate_params();
+  const CollisionParams p = collision_params();
+  const size_t S = size_t(nscores_);
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  const int64_t step = int64_t(1) << 30;  // events per launch
+  for (int64_t b = 0; b < nevents; b += step)
+    PTB_CUDA_OK(launch_collide_located(l, p, d_xyz + 3 * b, std::min(step, nevents - b), d_weights + b,
+                                       d_responses ? d_responses + S * size_t(b) : nullptr, d_bins ? d_bins + b : nullptr,
+                                       ntime_ > 0 ? d_times + b : nullptr, d_coll_counts_, stream));
+  return 0;
+}
+
+int Engine::tally_collisions_at_particles(const int8_t *collided, const double *weights, const double *responses,
+                                          const int32_t *bins, const double *times, int32_t n) {
+  if (collision_refused(responses, times)) return 1;
+  if (n != n_ || (n > 0 && (!collided || !weights))) {
+    fprintf(stderr, "[pumitally] ERROR: collision events at the particles: n must be num_particles (%d)\n", n_);
+    return 1;
+  }
+  if (n == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const int32_t chunk = std::min(chunk_, n);
+  const size_t S = size_t(nscores_);
+  if (ensure_collision_buffer(EventBuffers::bytes(size_t(chunk), S))) return 1;
+  const EventBuffers d(d_coll_buf_, size_t(chunk), S);
+  const CollisionParams p = collision_params();
+  const double *t = ntime_ > 0 ? times : nullptr;
+  if (follow_last_stream(compute_)) return 1;  // reads the particle state the last move wrote
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  for (int32_t b = 0; b < n; b += chunk) {
+    const size_t cnt = size_t(std::min(chunk, n - b));
+    PTB_CUDA_OK(upload(d.collided, collided + b, cnt, compute_));
+    PTB_CUDA_OK(upload(d.w, weights + b, cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.r, responses ? responses + S * size_t(b) : nullptr, S * cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.t, t ? t + b : nullptr, cnt * sizeof(double), compute_));
+    PTB_CUDA_OK(upload(d.bins, bins ? bins + b : nullptr, cnt * sizeof(int32_t), compute_));
+    PTB_CUDA_OK(launch_collide_particles(d_state_ + b, d.collided, int32_t(cnt), p, d.w, responses ? d.r : nullptr,
+                                         bins ? d.bins : nullptr, d.t, d_coll_counts_, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
+int Engine::tally_collisions_at_particles_device(const int8_t *d_collided, const double *d_weights,
+                                                 const double *d_responses, const int32_t *d_bins,
+                                                 const double *d_times, int32_t n, cudaStream_t stream) {
+  if (collision_refused(d_responses, d_times)) return 1;
+  if (n != n_ || (n > 0 && (!d_collided || !d_weights))) {
+    fprintf(stderr, "[pumitally] ERROR: collision events at the particles: n must be num_particles (%d)\n", n_);
+    return 1;
+  }
+  if (n == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  PTB_CUDA_OK(launch_collide_particles(d_state_, d_collided, n, collision_params(), d_weights, d_responses, d_bins,
+                                       ntime_ > 0 ? d_times : nullptr, d_coll_counts_, stream));
+  return 0;
+}
+
 // ------------------------------------------------------------------ multi-GPU
 
 int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
@@ -1931,7 +2156,7 @@ int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
   // NCCL sets up its NVLink connections lazily inside the first collective: pay that here,
   // on the scratch array, not in the first batch-end exchange
   if (nranks < 1 || size_t(nranks) > kFluxPad) return 1;
-  share_ = (flux_len() + size_t(nranks) - 1) / size_t(nranks);
+  share_ = (reported_len() + size_t(nranks) - 1) / size_t(nranks);
   PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_flux_global_), std::max<size_t>(share_ * size_t(nranks), 1) * sizeof(double)));
   PTB_CUDA_OK(cudaEventCreate(&ev_ar0_));
   PTB_CUDA_OK(cudaEventCreate(&ev_ar1_));
@@ -1951,7 +2176,7 @@ int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
   for (int rep = 0; rep < 3; ++rep)
     for (int which = 0; which < 2; ++which) {
       PTB_CUDA_OK(cudaEventRecord(ev_ar0_, compute_));
-      if (which == 0 ? nccl_allreduce_sum_f64(nccl_comm_, d_flux_, d_flux_global_, flux_len(), compute_)
+      if (which == 0 ? nccl_allreduce_sum_f64(nccl_comm_, d_flux_, d_flux_global_, reported_len(), compute_)
                      : nccl_reduce_scatter_sum_f64(nccl_comm_, d_flux_, d_flux_global_ + size_t(rank_) * share_, share_, compute_))
         return 1;
       PTB_CUDA_OK(cudaEventRecord(ev_ar1_, compute_));
@@ -1984,7 +2209,7 @@ int Engine::allreduce_tally() {
   PTB_CUDA_OK(cudaSetDevice(device_));
   PTB_CUDA_OK(cudaDeviceSynchronize());
   PTB_CUDA_OK(cudaEventRecord(ev_ar0_, compute_));
-  if (nccl_allreduce_sum_f64(nccl_comm_, d_flux_, d_flux_global_, flux_len(), compute_)) return 1;
+  if (nccl_allreduce_sum_f64(nccl_comm_, d_flux_, d_flux_global_, reported_len(), compute_)) return 1;
   PTB_CUDA_OK(cudaEventRecord(ev_ar1_, compute_));
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   float ms = 0.f;

@@ -95,6 +95,26 @@ class Engine {
   int locate_points(const double *xyz, int64_t npts, int32_t *out_elem);
   int locate_points_device(const double *d_xyz, int64_t npts, int32_t *d_elem, cudaStream_t stream);  // enqueue only
   int evaluate_points(const double *xyz, int64_t npts, double *out, int64_t n, int32_t *out_elem);
+  // Collision estimator (walk_core.cuh, collision_event): on == 1 adds a collision tally of the track-length tally's
+  // configuration, in its own region of d_flux_.  Resets the tally; before comm_init.  Event i adds weights[i] *
+  // responses[i * nscores + k] to score k of its element, bin bins[i] and time bin of times[i]; responses may be
+  // nullptr with one score, bins nullptr (bin 0), times is required while time bins are set.  tally_collisions: events
+  // at nevents points (AoS xyz), located as locate_points does; host calls work through chunk-sized buffers.
+  // tally_collisions_at_particles: the particles i with collided[i] != 0, at their stored positions and elements
+  // (n == num_particles).  Neither touches the particles, the track-length tally or the move statistics.
+  int set_collision_estimator(int32_t on);
+  int32_t collision_estimator() const { return collision_ ? 1 : 0; }
+  int tally_collisions(const double *xyz, int64_t nevents, const double *weights, const double *responses,
+                       const int32_t *bins, const double *times);
+  int tally_collisions_device(const double *d_xyz, int64_t nevents, const double *d_weights, const double *d_responses,
+                              const int32_t *d_bins, const double *d_times, cudaStream_t stream);  // enqueue only
+  int tally_collisions_at_particles(const int8_t *collided, const double *weights, const double *responses,
+                                    const int32_t *bins, const double *times, int32_t n);
+  int tally_collisions_at_particles_device(const int8_t *d_collided, const double *d_weights, const double *d_responses,
+                                           const int32_t *d_bins, const double *d_times, int32_t n, cudaStream_t stream);
+  // kind 0 raw, 1 normalised, 2 first moments, 3 gradient: get_flux, get_normalized_flux, get_flux_moments and
+  // get_flux_gradient of the collision tally (n as they take it)
+  int get_collision_results(int32_t kind, double *out, int64_t n);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -154,19 +174,23 @@ class Engine {
                                       // kMomentSlots with moments)
   int32_t ntime_ = 0;                 // time bins (0: no time filter)
   int32_t moments_ = 0;               // moment order (0: none, 1: linear; walk_core.cuh, moment_tally)
+  bool collision_ = false;            // the collision tally follows the track-length one in d_flux_
   size_t flux_alloc_ = 0;             // doubles allocated at d_flux_
-  // reported part of d_flux_: [time][bin][element][stride_]
+  // d_flux_: the track-length tally [time][bin][element][stride_] (flux_len()), with the collision estimator the
+  // collision tally of the same layout, then the unreported array of a binned move's unmatched particles and padding
   size_t nslices() const { return ntime_ > 0 ? size_t(ntime_) : 1; }
   size_t flux_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
+  size_t reported_len() const { return flux_len() * (collision_ ? 2 : 1); }  // what the exchange moves
   size_t bin_len() const { return size_t(mesh_.ntets) * size_t(stride_); }
   int32_t result_arrays() const { return int32_t(nslices()) * nbins_; }  // (time, bin) arrays of bin_len() doubles
   // results laid out [time][bin][score][element] (and read through the score-stride kernels)
   bool multi_results() const { return nscores_ > 1 || ntime_ > 0 || moments_ > 0; }
-  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments);
-  int copy_moments(std::vector<double> &out, bool gradient);  // every result array, [time][bin][score][element][3]
-  int get_moments_entry(double *out, int64_t n, bool gradient);
+  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision);
+  // base: doubles from d_flux_ (or the exchanged array) to the tally read, 0 (track length) or flux_len() (collision)
+  int copy_moments(std::vector<double> &out, bool gradient, size_t base = 0);  // [time][bin][score][element][3]
+  int get_moments_entry(double *out, int64_t n, bool gradient, size_t base = 0);
   bool per_source_divisor(double *out);  // of the normalised results; false, with a message, while there is none
-  int copy_results(std::vector<double> &out, bool normalized);
+  int copy_results(std::vector<double> &out, bool normalized, size_t base = 0);
   // ---- point queries (locate_kernels.cu) ----
   LocateParams locate_params() const;
   int ensure_candidates();  // non-convex hull: the cells' candidate lists, built and uploaded at the first query
@@ -185,7 +209,24 @@ class Engine {
   bool eval_valid_ = false;
   double *d_eval_vals_ = nullptr, *d_eval_grads_ = nullptr, *d_eval_cen_ = nullptr;
   int build_eval_table();
-  int write_scored_results();  // everything, [time][bin][score][element], caller's order
+  // named cell arrays of the VTK output; data owns them (a moved vector keeps its storage)
+  struct VtkArrays {
+    std::vector<std::vector<double>> data;
+    std::vector<std::pair<std::string, const double *>> named;
+    std::vector<int> ncomp;
+  };
+  // The arrays write_scored_results writes for the tally at `base`, every name prefixed.  main != nullptr: the sum of
+  // score 0 over the bins and time bins is returned there instead of being named prefix + "flux".
+  int scored_arrays(size_t base, const std::string &prefix, VtkArrays &a, std::vector<double> *main);
+  int write_scored_results(VtkArrays &a);  // everything, [time][bin][score][element], caller's order
+  // ---- collision estimator (locate_kernels.cu) ----
+  CollisionParams collision_params() const;
+  bool collision_refused(const double *responses, const double *times) const;  // with a message
+  int follow_last_stream(cudaStream_t stream);  // order work on the particle state behind the last such work
+  unsigned long long *d_coll_counts_ = nullptr;  // [3] events tallied, outside the mesh, rejected since the last reset
+  void *d_coll_buf_ = nullptr;                   // chunk-sized event arrays of the host-pointer calls
+  size_t coll_buf_bytes_ = 0;
+  int ensure_collision_buffer(size_t bytes);
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
     void *d = nullptr;    // device copy

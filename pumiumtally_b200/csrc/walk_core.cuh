@@ -788,4 +788,76 @@ PTB_HD int32_t locate_point(const LocateParams &P, double x, double y, double z,
   return locate_candidates(P, cell, x - P.cx, y - P.cy, z - P.cz, fetch);
 }
 
+// ---- collision estimator: events scored at a point --------------------------------------------------
+// The caller knows what happened at a collision (absorbed, scattered, the energy deposited), so it passes every event's
+// weight w, responses r[k], score bin and time, and the event adds w * r[k] to score k of its element, in a region of
+// d_flux_ laid out as the track-length tally ([time][bin][element][stride]).  With moments it also adds w * r[k] *
+// (x - C) to the moment slots, C the mesh centre, as moment_tally does for a segment's midpoint.
+struct CollisionParams {
+  double *flux;              // time bin 0, bin 0, element 0 of the collision region
+  const double *edges;       // [nt + 1] time bin edges (nt > 0)
+  int32_t nt;                // time bins (0: no time filter; times are not read)
+  int32_t nbins;             // score bins
+  int32_t nscores, stride;   // stride: score_stride(nscores), times kMomentSlots with moments
+  int32_t moments;           // 1: tally the first moments
+  int64_t bin_stride;        // doubles from one score bin to the next (E * stride)
+  int64_t slice;             // doubles from one time bin to the next (nbins * E * stride)
+  double cx, cy, cz;         // mesh centre
+};
+
+// What became of an event; the first three are counted.
+constexpr int kEventTallied = 0;
+constexpr int kEventOutside = 1;   // located outside the mesh
+constexpr int kEventRejected = 2;  // non-finite coordinate, weight * response or time
+constexpr int kEventSkipped = 3;   // bin outside [0, nbins), or time before T_0 or at or after T_nt
+
+// Time bin of t: the number of edges <= t, minus one (-1 before T_0, nt at or after T_nt): a time on an edge belongs
+// to the bin above it, as a track that starts there does (time_start).
+PTB_HD int time_bin(const double *ed, int nt, double t) {
+  int lo = 0, hi = nt + 1;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (PTB_LDG(ed + mid) <= t) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo - 1;
+}
+
+// One event in element e (internal id, -1: outside the mesh) at (x, y, z) (caller's coordinates) with weight w,
+// responses resp[0..nscores) (nullptr: every response 1), score bin `bin` and time t (read only with time bins).
+// Rejected takes precedence over outside, outside over skipped.
+PTB_HD int collision_event(const CollisionParams &P, int32_t e, double x, double y, double z, double w,
+                           const double *resp, int32_t bin, double t) {
+  double wr[kMaxScores];
+  bool bad = !all_finite(x, y, z) || (P.nt > 0 && !all_finite(t, 0.0, 0.0));
+PTB_UNROLL
+  for (int k = 0; k < kMaxScores; ++k)
+    if (k < P.nscores) {
+      wr[k] = w * (resp ? PTB_LDG(resp + k) : 1.0);
+      bad = bad || !all_finite(wr[k], 0.0, 0.0);
+    }
+  if (bad) return kEventRejected;
+  if (e < 0) return kEventOutside;
+  const int j = P.nt > 0 ? time_bin(P.edges, P.nt, t) : 0;
+  if (bin < 0 || bin >= P.nbins || j < 0 || (P.nt > 0 && j >= P.nt)) return kEventSkipped;
+  double *f = P.flux + (size_t)j * (size_t)P.slice + (size_t)bin * (size_t)P.bin_stride + (size_t)e * (size_t)P.stride;
+  if (P.moments) {
+    const int S = P.stride / kMomentSlots;
+    const double dx = x - P.cx, dy = y - P.cy, dz = z - P.cz;
+PTB_UNROLL
+    for (int k = 0; k < kMaxScores; ++k)
+      if (k < P.nscores) {
+        PTB_TALLY_ADD(f + k, wr[k]);
+        PTB_TALLY_ADD(f + S + k, wr[k] * dx);
+        PTB_TALLY_ADD(f + 2 * S + k, wr[k] * dy);
+        PTB_TALLY_ADD(f + 3 * S + k, wr[k] * dz);
+      }
+  } else {
+PTB_UNROLL
+    for (int k = 0; k < kMaxScores; ++k)
+      if (k < P.nscores) PTB_TALLY_ADD(f + k, wr[k]);
+  }
+  return kEventTallied;
+}
+
 }  // namespace ptb

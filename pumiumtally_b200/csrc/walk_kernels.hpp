@@ -130,5 +130,15 @@ cudaError_t launch_locate(const LocateParams &p, const double *xyz, int64_t n, i
 // r < R, e = internal[i]; NaN where e < 0.
 cudaError_t launch_evaluate(const double *xyz, const int32_t *internal, int64_t n, const double *vals, const double *grads,
                             const double *cen, int64_t E, int32_t R, double *out, int64_t pitch, cudaStream_t stream);
+// Collision estimator (walk_core.cuh, collision_event), thread per event.  Located: event i at xyz[3i..], located as
+// launch_locate does.  Particles: event i at particle i's stored position and element, for every i < n with
+// collided[i] != 0.  w[i], resp[i * c.nscores + k] (nullptr: every response 1), bins[i] (nullptr: bin 0), times[i]
+// (read only when c.nt > 0).  counts[0..2] += events tallied, outside the mesh, rejected.  n < 2^39.
+cudaError_t launch_collide_located(const LocateParams &l, const CollisionParams &c, const double *xyz, int64_t n,
+                                   const double *w, const double *resp, const int32_t *bins, const double *times,
+                                   unsigned long long *counts, cudaStream_t stream);
+cudaError_t launch_collide_particles(const ParticleState *state, const int8_t *collided, int32_t n,
+                                     const CollisionParams &c, const double *w, const double *resp, const int32_t *bins,
+                                     const double *times, unsigned long long *counts, cudaStream_t stream);
 
 }  // namespace ptb

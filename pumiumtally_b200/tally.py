@@ -63,6 +63,15 @@ C_API = {
     "pumitally_locate_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _ip]),
     "pumitally_locate_points_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "pumitally_evaluate_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, C.c_int64, _ip]),
+    "pumitally_set_collision_estimator": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_get_collision_estimator": (C.c_int32, [C.c_void_p]),
+    "pumitally_tally_collisions": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, _dp, _ip, _dp]),
+    "pumitally_tally_collisions_device": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pumitally_tally_collisions_at_particles": (C.c_int, [C.c_void_p, _bp, _dp, _dp, _ip, _dp, C.c_int32]),
+    "pumitally_tally_collisions_at_particles_device": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "pumitally_get_collision_results": (C.c_int, [C.c_void_p, C.c_int32, _dp, C.c_int64]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -432,6 +441,105 @@ class PumiTally:
                                              elem.ctypes.data_as(_ip)):
             raise RuntimeError("evaluate_points failed")
         return out, elem
+
+    # ---- collision estimator -------------------------------------------------------
+    def set_collision_estimator(self, on: bool):
+        """True: a collision tally with the track-length tally's configuration, in arrays of its own (resets the
+        tally); False removes it."""
+        if self._L.pumitally_set_collision_estimator(self._h, int(on)):
+            raise ValueError("set_collision_estimator failed")
+
+    @property
+    def collision_estimator(self) -> bool:
+        return bool(self._L.pumitally_get_collision_estimator(self._h))
+
+    def _event_args(self, n, weights, responses, bins, times):
+        """Host event arrays as contiguous numpy arrays (None stays None), checked against n events."""
+        w = _host_f64(weights, "weights")
+        if w.size != n:
+            raise TypeError("weights must hold one value per event")
+        r = t = b = None
+        if responses is not None:
+            r = _host_f64(responses, "responses")
+            if r.size != n * self.scores:
+                raise TypeError(f"responses must hold {self.scores} values per event")
+        if times is not None:
+            t = _host_f64(times, "times")
+            if t.size != n:
+                raise TypeError("times must hold one value per event")
+        if bins is not None:
+            b = np.ascontiguousarray(bins, dtype=np.int32).reshape(-1)
+            if b.size != n:
+                raise TypeError("bins must hold one value per event")
+        ptr = lambda a, p: None if a is None else a.ctypes.data_as(p)  # noqa: E731
+        return (w, r, b, t), (ptr(w, _dp), ptr(r, _dp), ptr(b, _ip), ptr(t, _dp))
+
+    def tally_collisions(self, points, weights, responses=None, bins=None, times=None):
+        """Collision events at ``points`` [n, 3], each located as locate() does: event i adds weights[i] *
+        responses[i, k] to score k of its element, bin bins[i] and the time bin of times[i]."""
+        p, n = self._points(points)
+        _keep, (w, r, b, t) = self._event_args(n, weights, responses, bins, times)
+        if self._L.pumitally_tally_collisions(self._h, p.ctypes.data_as(_dp), n, w, r, b, t):
+            raise RuntimeError("tally_collisions failed")
+
+    @staticmethod
+    def _tensor_ptr(x, dtype, numel, what):
+        if x is None:
+            return None
+        if not (x.is_cuda and x.dtype == dtype and x.is_contiguous() and x.numel() == numel):
+            raise TypeError(f"{what} must be a contiguous {dtype} CUDA tensor of {numel} values")
+        return x.data_ptr()
+
+    def _device_event_args(self, n, weights, responses, bins, times, stream, device):
+        import torch
+
+        args = (self._tensor_ptr(weights, torch.float64, n, "weights"),
+                self._tensor_ptr(responses, torch.float64, n * self.scores, "responses"),
+                self._tensor_ptr(bins, torch.int32, n, "bins"),
+                self._tensor_ptr(times, torch.float64, n, "times"))
+        if stream is None:
+            stream = torch.cuda.current_stream(device).cuda_stream
+        return args, stream
+
+    def tally_collisions_device(self, points, weights, responses=None, bins=None, times=None, stream=None):
+        """tally_collisions() on CUDA tensors (points float64 [n, 3], weights and times float64 [n], responses
+        float64 [n, nscores], bins int32 [n]); enqueued on ``stream`` (default: the current torch stream)."""
+        import torch
+
+        if not (points.is_cuda and points.dtype == torch.float64 and points.is_contiguous() and points.numel() % 3 == 0):
+            raise TypeError("points must be a contiguous float64 CUDA tensor of shape [n, 3]")
+        n = points.numel() // 3
+        (w, r, b, t), stream = self._device_event_args(n, weights, responses, bins, times, stream, points.device)
+        if self._L.pumitally_tally_collisions_device(self._h, points.data_ptr(), n, w, r, b, t, stream):
+            raise RuntimeError("tally_collisions_device failed")
+
+    def tally_collisions_at_particles(self, collided, weights, responses=None, bins=None, times=None):
+        """Collision events at the stored positions of the particles i with collided[i] != 0, in their elements."""
+        c = np.ascontiguousarray(collided, dtype=np.int8).reshape(-1)
+        _keep, (w, r, b, t) = self._event_args(c.size, weights, responses, bins, times)
+        if self._L.pumitally_tally_collisions_at_particles(self._h, c.ctypes.data_as(_bp), w, r, b, t, c.size):
+            raise RuntimeError("tally_collisions_at_particles failed")
+
+    def tally_collisions_at_particles_device(self, collided, weights, responses=None, bins=None, times=None,
+                                             stream=None):
+        """tally_collisions_at_particles() on CUDA tensors (collided int8 [num_particles]); enqueued on ``stream``."""
+        import torch
+
+        n = self.num_particles
+        c = self._tensor_ptr(collided, torch.int8, n, "collided")
+        (w, r, b, t), stream = self._device_event_args(n, weights, responses, bins, times, stream, collided.device)
+        if self._L.pumitally_tally_collisions_at_particles_device(self._h, c, w, r, b, t, n, stream):
+            raise RuntimeError("tally_collisions_at_particles_device failed")
+
+    def collision_results(self, kind=0):
+        """The collision tally: kind 0 raw, 1 normalised ([ntime, nbins, nscores, num_elements]), 2 first moments, 3
+        gradient ([..., 3]) -- what flux_time, normalized_flux_time()[0], flux_moments() and flux_gradient() give for
+        the track-length tally."""
+        shape = (max(self.time_bins, 1), self.score_bins, self.scores, self.num_elements) + ((3,) if kind in (2, 3) else ())
+        out = np.empty(shape)
+        if self._L.pumitally_get_collision_results(self._h, int(kind), out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError(f"get_collision_results({kind}) failed")
+        return out
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
