@@ -95,6 +95,23 @@ inline int TallyCollisionsAtParticles(const PumiTally &tally, const int8_t *coll
   return pumitally_tally_collisions_at_particles(engine_of(tally), collided, weights, responses, bins, times, size);
 }
 
+// Batch statistics (see pumitally_set_batch_statistics in pumitally_c.h): EndBatch folds the batch's per-source results
+// into a running mean and variance on the device and starts the next batch.  GetBatchResults: tally 0 track length, 1
+// collision; kind 0 mean, 1 standard error, 2 relative error, 3 gradient of the mean (n as pumitally_get_normalized_flux
+// / pumitally_get_flux_gradient take it).  GetBatchMaxRelErr: the largest relative error of one score and how many
+// results have a nonzero mean, for tally triggers.
+inline int SetBatchStatistics(const PumiTally &tally, int32_t on) {
+  return pumitally_set_batch_statistics(engine_of(tally), on);
+}
+inline int EndBatch(const PumiTally &tally) { return pumitally_end_batch(engine_of(tally)); }
+inline int GetBatchResults(const PumiTally &tally, int32_t which, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_batch_results(engine_of(tally), which, kind, out, n);
+}
+inline int GetBatchMaxRelErr(const PumiTally &tally, int32_t which, int32_t score, double *out_max,
+                             int64_t *out_nonzero) {
+  return pumitally_get_batch_max_rel_err(engine_of(tally), which, score, out_max, out_nonzero);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

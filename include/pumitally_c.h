@@ -399,6 +399,46 @@ int pumitally_tally_collisions_at_particles_device(pumitally_engine *e, const in
                                                    void *stream);
 int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *out, int64_t n);
 
+/* ---- additive: batch statistics (mean, standard and relative errors over batches, on the device) ----
+ * A Monte Carlo tally is reported as mean +- standard error over batches.  pumitally_set_batch_statistics(e, 1) keeps,
+ * for every reported result (the track-length tally and, with the estimator on, the collision tally: every time bin,
+ * score bin and score), a running mean and sum of squared deviations M2 on the device; 0 (the default) frees them.  Any
+ * other value, or statistics that cannot be allocated (2 doubles per double of the reported tallies), returns non-zero
+ * and changes nothing.  The call resets the tally, combines with the other pumitally_set_* calls in any order and is
+ * refused after pumitally_comm_init.  Calling it with 1 again discards the folded batches, and so does, while it is on,
+ * every other pumitally_set_* call that changes the configuration (the statistics take the new layout); so does
+ * pumitally_comm_init.  Read-only options: "batch_statistics" (0/1) and "batches" (batches folded).
+ * pumitally_end_batch(e) closes the open batch.  Its divisor d_b is, on one rank, exactly what
+ * pumitally_get_normalized_flux would divide by at that moment; on several ranks modes 1 and 3 use the sum of the ranks'
+ * divisors (the whole batch's source), mode 2 uses `value` and mode 0 uses 1.  A d_b that is not > 0 refuses the call
+ * and changes nothing.  Every reported double x of the batch tally is folded as x / d_b into its mean and M2 by Welford's
+ * update (which, unlike sum and sum of squares, does not cancel when the relative error is small); then the call does
+ * exactly what pumitally_reset_tally does, and synchronises as it does.  Refused while statistics are off.  With several
+ * ranks the call is collective: the batch tally is reduce-scattered to the element owners (as by
+ * pumitally_reduce_tally_to_owners) and every rank folds and keeps only its share.
+ * pumitally_get_batch_results(e, tally, kind, out, n): tally 0 track length, 1 collision; kind 0 the mean divided by
+ * volume (the per-source normalised result averaged over the batches), 1 its standard error sqrt(M2 / (B (B - 1))) /
+ * volume, 2 the relative error (1) / |(0)|, 0 where the mean is 0, 3 the gradient of the mean (what
+ * pumitally_get_flux_gradient computes, applied to the batch means; moments only).  n, the layout
+ * [time][bin][score][element] (times 3 for kind 3) and the caller's numbering are those of
+ * pumitally_get_normalized_flux / pumitally_get_flux_gradient.  Refused: no batch folded, fewer than two for kinds 1 and
+ * 2, kind 3 without moments, tally 1 without the estimator, a wrong n.  Collective with several ranks (the shares are
+ * gathered).  Statistics are of the m0 results only; moments and gradients get no variance (that needs covariances).
+ * pumitally_get_batch_max_rel_err(e, tally, score, out_max, out_nonzero): for tally triggers, the largest relative error
+ * of score `score` over every element, score bin and time bin with a nonzero mean, and how many such results there are,
+ * reduced on the device; refused with fewer than two batches.  Collective with several ranks (max and sum over ranks).
+ * WriteTallyResults with statistics on and at least one batch folded writes, after every array it writes without them,
+ * "<name>_mean" for every scalar array (for a sum over bins or time bins, such as "flux" with bins, the sum of the
+ * means) and, with two batches or more, "<name>_rel_err" for every scalar array that is exactly one (time bin, bin,
+ * score) result: "flux" / "score<k>" without bins or time bins, otherwise the "_bin<b>" / "_t<j>" arrays.  Sums over bins
+ * or time bins get no "_rel_err", their error needs covariances.  Collision arrays carry the same suffixes after their
+ * "collision_" names.  The other arrays are unchanged and hold the open batch. */
+int pumitally_set_batch_statistics(pumitally_engine *e, int32_t on);
+int pumitally_end_batch(pumitally_engine *e);
+int pumitally_get_batch_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
+int pumitally_get_batch_max_rel_err(pumitally_engine *e, int32_t tally, int32_t score, double *out_max,
+                                    int64_t *out_nonzero);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

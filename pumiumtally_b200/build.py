@@ -23,6 +23,7 @@ SOURCES = [
     "walk_kernels.cu",
     "bin_kernels.cu",
     "locate_kernels.cu",
+    "stats_kernels.cu",
     "l2_partitions.cu",
     "engine.cu",
     "host_stage.cpp",

@@ -271,6 +271,21 @@ int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *o
   return guarded(e, [&](ptb::Engine &g) { return g.get_collision_results(kind, out, n); });
 }
 
+int pumitally_set_batch_statistics(pumitally_engine *e, int32_t on) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_batch_statistics(on); });
+}
+int pumitally_end_batch(pumitally_engine *e) {
+  return guarded(e, [&](ptb::Engine &g) { return g.end_batch(); });
+}
+int pumitally_get_batch_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n) {
+  if (n > 0 && !out) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_batch_results(tally, kind, out, n); });
+}
+int pumitally_get_batch_max_rel_err(pumitally_engine *e, int32_t tally, int32_t score, double *out_max,
+                                    int64_t *out_nonzero) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_batch_max_rel_err(tally, score, out_max, out_nonzero); });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

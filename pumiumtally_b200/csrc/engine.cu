@@ -81,6 +81,8 @@ Engine::Engine(HostMesh &&mesh, int32_t num_particles, int device)
   cuda_or_throw(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)), "memset");
   dev_alloc(&d_initial_weight_, 1, "initial weight");
   cuda_or_throw(cudaMemset(d_initial_weight_, 0, sizeof(double)), "memset");
+  dev_alloc(&d_batch_div_, 2, "batch divisor");
+  dev_alloc(&d_stats_red_, 2, "batch statistics reduction");
   dev_alloc(&d_tickets_, 2 * kTicketRing, "tickets");  // second half: the other L2 partition's tickets (die split)
   dev_alloc(&d_pcell_, N, "particle cells");
   dev_alloc(&d_order_, N, "processing order");
@@ -187,6 +189,8 @@ Engine::~Engine() {
   cudaFree(d_qxyz_); cudaFree(d_qout_); cudaFree(d_qint_); cudaFree(d_qelem_);
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
   cudaFree(d_coll_counts_); cudaFree(d_coll_buf_);
+  free_stats();
+  cudaFree(d_batch_div_); cudaFree(d_stats_red_);
   if (compute_) cudaStreamDestroy(compute_);
   if (copy_) cudaStreamDestroy(copy_);
 }
@@ -1193,6 +1197,10 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
             cudaGetErrorString(err));
     return 1;
   }
+  if (batch_stats_ && alloc_stats(tally * E * stride)) {  // statistics of the new layout, no batch folded yet
+    cudaFree(nf);
+    return 1;
+  }
   cudaFree(d_flux_);
   d_flux_ = nf;
   flux_alloc_ = len;
@@ -1368,13 +1376,13 @@ int Engine::get_flux(double *out, int64_t n) {
 
 // The linear moments of every result array, [time][bin][score][element][3] in the caller's numbering: m1 about each
 // element's centroid, or the gradient g = M^-1 m1 divided by the source normalisation (linear_moments()).
-int Engine::copy_moments(std::vector<double> &out, bool gradient, size_t base) {
+int Engine::copy_moments(std::vector<double> &out, bool gradient, size_t base, const double *src) {
   const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(result_arrays());
   const int slot = stride_ / kMomentSlots;
   double per_source = 1.0;
-  if (gradient && !per_source_divisor(&per_source)) return 1;
+  if (gradient && !src && !per_source_divisor(&per_source)) return 1;
   std::vector<double> raw(B * bin_len());
-  PTB_CUDA_OK(cudaMemcpy(raw.data(), flux_view() + base, raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  PTB_CUDA_OK(cudaMemcpy(raw.data(), (src ? src : flux_view()) + base, raw.size() * sizeof(double), cudaMemcpyDeviceToHost));
   out.resize(B * S * E * 3);
   const double *xyz = mesh_.coords.data();
 #pragma omp parallel for schedule(static)
@@ -1582,6 +1590,8 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "moments") return moments_;
   if (name == "locate_candidates") return int64_t(cand_entries_);  // entries of the point-location candidate lists
   if (name == "collision_estimator") return collision_ ? 1 : 0;
+  if (name == "batch_statistics") return batch_stats_ ? 1 : 0;
+  if (name == "batches") return batches_;  // batches folded into the statistics
   // collision events since the last reset: tallied, located outside the mesh, rejected (non-finite inputs)
   if (name == "collisions" || name == "collisions_outside" || name == "collisions_rejected") {
     unsigned long long c[3] = {0, 0, 0};
@@ -1714,10 +1724,14 @@ int64_t Engine::debug_order(int32_t *out, int64_t n) {
 }
 
 // FinalizeTallies (PumiTallyImpl.cpp:411-416).  With the collision estimator every array of the track-length tally is
-// followed by its collision twin, the same name prefixed "collision_".
+// followed by its collision twin, the same name prefixed "collision_".  With batch statistics and at least one batch
+// folded, the "_mean" / "_rel_err" arrays (batch_arrays) of both tallies follow all of these.
 int Engine::write_tally_results() {
   VtkArrays coll;
   if (collision_ && (synchronize() || gather_shares() || scored_arrays(flux_len(), "collision_", coll, nullptr))) return 1;
+  if (batch_stats_ && batches_ > 0 &&
+      (synchronize() || batch_arrays(0, "", coll) || (collision_ && batch_arrays(1, "collision_", coll))))
+    return 1;
   if (multi_results()) return write_scored_results(coll);
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
@@ -2145,6 +2159,254 @@ int Engine::tally_collisions_at_particles_device(const int8_t *d_collided, const
   return 0;
 }
 
+// ------------------------------------------------------------------ batch statistics
+
+int Engine::alloc_stats(size_t len) {
+  double *nm = nullptr, *nq = nullptr;
+  const size_t bytes = std::max<size_t>(len, 1) * sizeof(double);
+  if (cudaMalloc(reinterpret_cast<void **>(&nm), bytes) != cudaSuccess ||
+      cudaMalloc(reinterpret_cast<void **>(&nq), bytes) != cudaSuccess || cudaMemset(nm, 0, bytes) != cudaSuccess ||
+      cudaMemset(nq, 0, bytes) != cudaSuccess) {
+    const cudaError_t err = cudaGetLastError();
+    cudaFree(nm);
+    cudaFree(nq);
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the batch statistics of %zu results (%s)\n", len,
+            cudaGetErrorString(err));
+    return 1;
+  }
+  free_stats();
+  d_mean_ = nm;
+  d_m2_ = nq;
+  return 0;
+}
+
+void Engine::free_stats() {
+  cudaFree(d_mean_);
+  cudaFree(d_m2_);
+  d_mean_ = d_m2_ = nullptr;
+  batches_ = 0;
+}
+
+int Engine::set_batch_statistics(int32_t on) {
+  if (on != 0 && on != 1) return 1;
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_batch_statistics after comm_init (the exchange buffers are sized by then)\n");
+    return 1;
+  }
+  if (synchronize()) return 1;
+  if (on) {
+    if (alloc_stats(reported_len())) return 1;  // (a second call with 1 discards the folded batches)
+  } else {
+    free_stats();
+  }
+  batch_stats_ = on != 0;
+  return reset_tally();
+}
+
+bool Engine::batch_refused(int32_t tally, int32_t kind) const {
+  const char *why = !batch_stats_                            ? "batch statistics are off (set_batch_statistics)"
+                    : (tally != 0 && tally != 1)             ? "tally must be 0 (track length) or 1 (collision)"
+                    : (tally == 1 && !collision_)            ? "the collision estimator is off (set_collision_estimator)"
+                    : (kind < 0 || kind > 3)                 ? "kind must be 0 (mean), 1 (standard error), 2 (relative "
+                                                               "error) or 3 (gradient of the mean)"
+                    : batches_ < 1                           ? "no batch has been folded yet (end_batch)"
+                    : (batches_ < 2 && (kind == 1 || kind == 2)) ? "errors need at least two batches"
+                    : (kind == 3 && !moments_)               ? "the engine tallies no moments (set_moments)"
+                                                             : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: batch results refused: %s\n", why);
+  return why != nullptr;
+}
+
+// Closes the open batch: its divisor d_b (as get_normalized_flux's, summed over the ranks for modes 1 and 3) goes to
+// d_batch_div_[0] on the device, every reported double x of the batch (this rank's share of the summed tally with
+// several ranks) is folded as x / d_b, and the tally is reset.
+int Engine::end_batch() {
+  if (!batch_stats_) {
+    fprintf(stderr, "[pumitally] ERROR: end_batch: batch statistics are off (set_batch_statistics)\n");
+    return 1;
+  }
+  if (synchronize()) return 1;
+  const double local = norm_mode_ == 1 ? double(std::max(n_, 1)) : norm_mode_ == 2 ? norm_value_ : 1.0;
+  if (norm_mode_ == 3)
+    PTB_CUDA_OK(cudaMemcpyAsync(d_batch_div_ + 1, d_initial_weight_, sizeof(double), cudaMemcpyDeviceToDevice, compute_));
+  else
+    PTB_CUDA_OK(cudaMemcpyAsync(d_batch_div_ + 1, &local, sizeof(double), cudaMemcpyHostToDevice, compute_));
+  if (sharded() && (norm_mode_ == 1 || norm_mode_ == 3)) {  // the whole batch's source
+    if (nccl_allreduce_sum_f64(nccl_comm_, d_batch_div_ + 1, d_batch_div_, 1, compute_)) return 1;
+  } else {
+    PTB_CUDA_OK(cudaMemcpyAsync(d_batch_div_, d_batch_div_ + 1, sizeof(double), cudaMemcpyDeviceToDevice, compute_));
+  }
+  double div = 0.0;
+  PTB_CUDA_OK(cudaMemcpyAsync(&div, d_batch_div_, sizeof(double), cudaMemcpyDeviceToHost, compute_));
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  if (!(div > 0.0)) {  // the same value on every rank: all of them refuse
+    fprintf(stderr, "[pumitally] ERROR: end_batch: the batch's source-normalisation divisor is %g\n", div);
+    return 1;
+  }
+  const size_t L = reported_len();
+  const double nb = double(batches_ + 1);
+  if (sharded()) {
+    const size_t lo = size_t(rank_) * share_;  // the last share ends in padding (or a binned move's unreported array)
+    if (nccl_reduce_scatter_sum_f64(nccl_comm_, d_flux_, d_flux_global_ + lo, share_, compute_)) return 1;
+    PTB_CUDA_OK(launch_batch_fold(d_flux_global_ + lo, d_mean_, d_m2_, lo < L ? int64_t(std::min(share_, L - lo)) : 0,
+                                  d_batch_div_, nb, compute_));
+  } else {
+    PTB_CUDA_OK(launch_batch_fold(d_flux_, d_mean_, d_m2_, int64_t(L), d_batch_div_, nb, compute_));
+  }
+  ++batches_;
+  return reset_tally();
+}
+
+int Engine::stats_view(const double **mean, const double **m2, double **tmp) {
+  *tmp = nullptr;
+  if (!sharded()) {
+    *mean = d_mean_;
+    *m2 = d_m2_;
+    return 0;
+  }
+  const size_t full = share_ * size_t(nranks_);
+  PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(tmp), 2 * full * sizeof(double)));
+  *mean = *tmp;
+  *m2 = *tmp + full;
+  if (nccl_all_gather_f64(nccl_comm_, d_mean_, *tmp, share_, compute_) ||
+      nccl_all_gather_f64(nccl_comm_, d_m2_, *tmp + full, share_, compute_))
+    return 1;
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
+int Engine::copy_batch_results(std::vector<double> &out, int32_t tally, int32_t kind) {
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), R = size_t(result_arrays());
+  if (ensure_element_maps()) return 1;
+  const double *mean = nullptr, *m2 = nullptr;
+  double *tmp = nullptr, *d_out = nullptr;
+  int rc = stats_view(&mean, &m2, &tmp);
+  if (!rc) {
+    const size_t base = size_t(tally) * flux_len();
+    out.resize(R * S * E);
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d_out), std::max<size_t>(out.size(), 1) * sizeof(double));
+    if (e == cudaSuccess)
+      e = launch_batch_readout(mean + base, m2 + base, d_volume_, d_orig_of_internal_, d_out, int64_t(E), int32_t(R),
+                               nscores_, stride_, double(batches_), kind, compute_);
+    if (e == cudaSuccess)
+      e = cudaMemcpyAsync(out.data(), d_out, out.size() * sizeof(double), cudaMemcpyDeviceToHost, compute_);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+    if (e != cudaSuccess) {
+      fprintf(stderr, "[pumitally] CUDA error %s reading the batch statistics\n", cudaGetErrorString(e));
+      rc = 1;
+    }
+  }
+  cudaFree(d_out);
+  cudaFree(tmp);
+  return rc;
+}
+
+int Engine::get_batch_results(int32_t tally, int32_t kind, double *out, int64_t n) {
+  if (batch_refused(tally, kind)) return 1;
+  const int64_t E = mesh_.ntets, m = kind == 3 ? 3 : 1;
+  if (n != m * E && n != m * int64_t(result_arrays()) * nscores_ * E) {
+    fprintf(stderr, "[pumitally] ERROR: get_batch_results: n must be %lld or %lld\n", (long long)(m * E),
+            (long long)(m * int64_t(result_arrays()) * nscores_ * E));
+    return 1;
+  }
+  if (synchronize()) return 1;
+  std::vector<double> all;
+  if (kind == 3) {  // the gradient of the mean records, which are already per source
+    const double *mean = nullptr, *m2 = nullptr;
+    double *tmp = nullptr;
+    const int rc = stats_view(&mean, &m2, &tmp) || copy_moments(all, true, size_t(tally) * flux_len(), mean);
+    cudaFree(tmp);
+    if (rc) return 1;
+  } else if (copy_batch_results(all, tally, kind)) {
+    return 1;
+  }
+  std::memcpy(out, all.data(), size_t(n) * sizeof(double));
+  return 0;
+}
+
+int Engine::get_batch_max_rel_err(int32_t tally, int32_t score, double *out_max, int64_t *out_nonzero) {
+  if (batch_refused(tally, 2)) return 1;
+  if (score < 0 || score >= nscores_ || !out_max || !out_nonzero) {
+    fprintf(stderr, "[pumitally] ERROR: get_batch_max_rel_err: score must be in [0, %d)\n", nscores_);
+    return 1;
+  }
+  if (synchronize()) return 1;
+  const size_t L = reported_len(), goff = sharded() ? size_t(rank_) * share_ : 0;
+  const int64_t n = goff < L ? int64_t(std::min(stats_len(), L - goff)) : 0;
+  PTB_CUDA_OK(launch_batch_max_rel_err(d_mean_, d_m2_, n, int64_t(goff), int64_t(size_t(tally) * flux_len()),
+                                       int64_t(flux_len()), stride_, score, double(batches_), d_stats_red_, compute_));
+  unsigned long long red[2] = {0, 0};
+  PTB_CUDA_OK(cudaMemcpyAsync(red, d_stats_red_, sizeof(red), cudaMemcpyDeviceToHost, compute_));
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  double mx = 0.0, cnt = double(red[1]);
+  std::memcpy(&mx, &red[0], sizeof(double));
+  if (sharded()) {  // max and sum over the ranks, from every rank's pair
+    std::vector<double> all(2 * size_t(nranks_) + 2);
+    all[0] = mx;
+    all[1] = cnt;
+    double *d = nullptr;
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d), all.size() * sizeof(double)));
+    cudaError_t e = cudaMemcpyAsync(d, all.data(), 2 * sizeof(double), cudaMemcpyHostToDevice, compute_);
+    const int rc = e != cudaSuccess || nccl_all_gather_f64(nccl_comm_, d, d + 2, 2, compute_);
+    if (!rc) e = cudaMemcpyAsync(all.data(), d, all.size() * sizeof(double), cudaMemcpyDeviceToHost, compute_);
+    if (!rc && e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+    cudaFree(d);
+    if (rc || e != cudaSuccess) return 1;
+    mx = cnt = 0.0;
+    for (int r = 0; r < nranks_; ++r) {
+      mx = std::max(mx, all[2 + 2 * size_t(r)]);
+      cnt += all[3 + 2 * size_t(r)];
+    }
+  }
+  *out_max = mx;
+  *out_nonzero = int64_t(cnt);
+  return 0;
+}
+
+// "<name>_mean" for every scalar array write_scored_results (or the plain writer) names, in its order: the sum of the
+// means where the array is a sum over bins or time bins.  With two batches or more, "<name>_rel_err" follows for every
+// such array that is exactly one (time bin, bin, score) result; a sum's error would need the covariances of its terms.
+int Engine::batch_arrays(int32_t tally, const std::string &prefix, VtkArrays &a) {
+  const size_t E = size_t(mesh_.ntets), S = size_t(nscores_), B = size_t(nbins_), T = nslices();
+  std::vector<double> mean, rel;
+  const bool errs = batches_ >= 2;
+  if (copy_batch_results(mean, tally, 0) || (errs && copy_batch_results(rel, tally, 2))) return 1;
+  auto add = [&](const std::string &name, std::vector<double> v) {
+    a.data.push_back(std::move(v));  // (moving a vector keeps its storage: earlier pointers stay valid)
+    a.named.emplace_back(prefix + name, a.data.back().data());
+    a.ncomp.push_back(1);
+  };
+  auto at = [&](const std::vector<double> &v, size_t t, size_t b, size_t k) { return v.data() + ((t * B + b) * S + k) * E; };
+  auto sum = [&](size_t t0, size_t t1, size_t b0, size_t b1, size_t k) {  // of the means
+    std::vector<double> s(E, 0.0);
+    for (size_t t = t0; t < t1; ++t)
+      for (size_t b = b0; b < b1; ++b) {
+        const double *p = at(mean, t, b, k);
+        for (size_t i = 0; i < E; ++i) s[i] += p[i];
+      }
+    return s;
+  };
+  // set 0: the sum over the time bins (time bin 0 itself without a time filter); set 1 + j: time bin j
+  const size_t nsets = ntime_ > 0 ? T + 1 : 1;
+  for (size_t q = 0; q < nsets; ++q) {
+    const std::string ts = q == 0 ? "" : "_t" + std::to_string(q - 1);
+    const size_t t0 = q == 0 ? 0 : q - 1, t1 = q == 0 ? T : q;
+    const bool single_time = ntime_ == 0 || q > 0;
+    for (size_t k = 0; k < S; ++k) {
+      const std::string name = (k == 0 ? "flux" : "score" + std::to_string(k)) + ts;
+      add(name + "_mean", sum(t0, t1, 0, B, k));
+      if (errs && single_time && B == 1) add(name + "_rel_err", std::vector<double>(at(rel, t0, 0, k), at(rel, t0, 0, k) + E));
+      if (B > 1)
+        for (size_t b = 0; b < B; ++b) {
+          const std::string bn = name + "_bin" + std::to_string(b);
+          add(bn + "_mean", sum(t0, t1, b, b + 1, k));
+          if (errs && single_time) add(bn + "_rel_err", std::vector<double>(at(rel, t0, b, k), at(rel, t0, b, k) + E));
+        }
+    }
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------ multi-GPU
 
 int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
@@ -2158,6 +2420,8 @@ int Engine::comm_init(int rank, int nranks, const uint8_t id[128]) {
   if (nranks < 1 || size_t(nranks) > kFluxPad) return 1;
   share_ = (reported_len() + size_t(nranks) - 1) / size_t(nranks);
   PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_flux_global_), std::max<size_t>(share_ * size_t(nranks), 1) * sizeof(double)));
+  // batch statistics from here on live sharded: this rank's share only, and no batch of the single-rank layout is kept
+  if (batch_stats_ && alloc_stats(stats_len())) return 1;
   PTB_CUDA_OK(cudaEventCreate(&ev_ar0_));
   PTB_CUDA_OK(cudaEventCreate(&ev_ar1_));
   PTB_CUDA_OK(cudaMemsetAsync(d_scratch_, 0, size_t(mesh_.ntets) * sizeof(double), compute_));

@@ -115,6 +115,17 @@ class Engine {
   // kind 0 raw, 1 normalised, 2 first moments, 3 gradient: get_flux, get_normalized_flux, get_flux_moments and
   // get_flux_gradient of the collision tally (n as they take it)
   int get_collision_results(int32_t kind, double *out, int64_t n);
+  // Batch statistics (batch_stats.cuh): on == 1 keeps a running mean and sum of squared deviations of every reported
+  // double (both tallies), folded by end_batch from the batch's results divided by its source-normalisation divisor;
+  // 0 frees them.  Resets the tally; before comm_init.  Any later set_* call discards the folded batches.
+  int set_batch_statistics(int32_t on);
+  // Collective with several ranks: the batch tally is reduce-scattered and each rank folds its share.  Then reset_tally.
+  int end_batch();
+  // tally 0 track length, 1 collision; kind 0 mean, 1 standard error (both / volume), 2 relative error, 3 gradient of
+  // the mean (n as get_normalized_flux / get_flux_gradient take it).  Collective with several ranks.
+  int get_batch_results(int32_t tally, int32_t kind, double *out, int64_t n);
+  // Largest relative error of score `score` over the results with a nonzero mean, and their number (device reduction).
+  int get_batch_max_rel_err(int32_t tally, int32_t score, double *out_max, int64_t *out_nonzero);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -187,7 +198,8 @@ class Engine {
   bool multi_results() const { return nscores_ > 1 || ntime_ > 0 || moments_ > 0; }
   int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision);
   // base: doubles from d_flux_ (or the exchanged array) to the tally read, 0 (track length) or flux_len() (collision)
-  int copy_moments(std::vector<double> &out, bool gradient, size_t base = 0);  // [time][bin][score][element][3]
+  // [time][bin][score][element][3]; src != nullptr: the records at src + base, gradients not divided by a source divisor
+  int copy_moments(std::vector<double> &out, bool gradient, size_t base = 0, const double *src = nullptr);
   int get_moments_entry(double *out, int64_t n, bool gradient, size_t base = 0);
   bool per_source_divisor(double *out);  // of the normalised results; false, with a message, while there is none
   int copy_results(std::vector<double> &out, bool normalized, size_t base = 0);
@@ -227,6 +239,25 @@ class Engine {
   void *d_coll_buf_ = nullptr;                   // chunk-sized event arrays of the host-pointer calls
   size_t coll_buf_bytes_ = 0;
   int ensure_collision_buffer(size_t bytes);
+  // ---- batch statistics (stats_kernels.cu) ----
+  bool batch_stats_ = false;
+  int64_t batches_ = 0;                            // batches folded
+  double *d_mean_ = nullptr, *d_m2_ = nullptr;     // [stats_len()] running mean and sum of squared deviations
+  double *d_batch_div_ = nullptr;                  // [2] divisor of the batch being folded, scratch of the exchange
+  unsigned long long *d_stats_red_ = nullptr;      // [2] result of the max-relative-error reduction
+  bool sharded() const { return nccl_comm_ && nranks_ > 1; }
+  // entries this rank keeps: the whole reported tally, or its share of it after comm_init with several ranks
+  size_t stats_len() const { return sharded() ? share_ : reported_len(); }
+  int alloc_stats(size_t len);  // zeroed, batches_ = 0; nothing changes when the allocation fails
+  void free_stats();
+  // the statistics of the whole reported tally: this rank's, or gathered from every rank's share into *tmp (collective,
+  // the caller frees *tmp)
+  int stats_view(const double **mean, const double **m2, double **tmp);
+  // [time][bin][score][element] of tally `tally`, kinds 0-2 of get_batch_results, caller's numbering
+  int copy_batch_results(std::vector<double> &out, int32_t tally, int32_t kind);
+  bool batch_refused(int32_t tally, int32_t kind) const;  // with a message
+  // the "<name>_mean" / "<name>_rel_err" arrays of the tally at `tally`, names prefixed
+  int batch_arrays(int32_t tally, const std::string &prefix, VtkArrays &a);
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
     void *d = nullptr;    // device copy

@@ -1,0 +1,140 @@
+// Batch statistics kernels (batch_stats.cuh; engine.cu, end_batch / get_batch_results / get_batch_max_rel_err).
+// All three are memory-bound flat passes over the [time][bin][element][stride] record of the reported tally.
+#include <cstdint>
+
+#include "batch_stats.cuh"
+#include "walk_kernels.hpp"
+
+namespace ptb {
+namespace {
+
+// Every double x of [0, n): (mean, m2) <- welford_fold(x / *divisor, nb).  Two doubles per thread and step when the
+// three arrays are 16-byte aligned (the rank shares of a reduce-scatter may start at an odd double).
+template <bool kVec>
+__global__ void batch_fold_kernel(const double *__restrict__ x, double *__restrict__ mean, double *__restrict__ m2,
+                                  int64_t n, const double *__restrict__ divisor, double nb) {
+  const double d = *divisor;
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x, t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  auto fold1 = [&](int64_t i) {
+    double mu = mean[i], q = m2[i];
+    welford_fold(x[i] / d, nb, mu, q);
+    mean[i] = mu;
+    m2[i] = q;
+  };
+  if (!kVec) {
+    for (int64_t i = t; i < n; i += stride) fold1(i);
+    return;
+  }
+  const int64_t pairs = n / 2;
+  for (int64_t p = t; p < pairs; p += stride) {
+    const double2 v = reinterpret_cast<const double2 *>(x)[p];
+    double2 mu = reinterpret_cast<double2 *>(mean)[p], q = reinterpret_cast<double2 *>(m2)[p];
+    welford_fold(v.x / d, nb, mu.x, q.x);
+    welford_fold(v.y / d, nb, mu.y, q.y);
+    reinterpret_cast<double2 *>(mean)[p] = mu;
+    reinterpret_cast<double2 *>(m2)[p] = q;
+  }
+  if (t == 0 && (n & 1)) fold1(n - 1);
+}
+
+// out[(r * nscores + k) * E + orig[e]] = batch_readout(...) of score k of element e in result array r
+__global__ void batch_readout_kernel(const double *__restrict__ mean, const double *__restrict__ m2,
+                                     const double *__restrict__ volume, const int32_t *__restrict__ orig_of_internal,
+                                     double *__restrict__ out, int64_t E, int32_t R, int32_t nscores, int32_t stride,
+                                     double nb, int kind) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= E * R) return;
+  const int64_t r = t / E, e = t - r * E;
+  const double v = volume[e];
+  const int32_t o = orig_of_internal[e];
+  const int64_t rec = t * stride;  // (r * E + e) * stride
+  for (int k = 0; k < nscores; ++k)
+    out[(r * nscores + k) * E + o] = batch_readout(mean[rec + k], kind == 0 ? 0.0 : m2[rec + k], nb, v, kind);
+}
+
+// Over local entries j of [0, n), global index g = goff + j: the entries of the tally [base, base + len) that are the
+// m0 slot of score `score` ((g - base) % stride == score) with a nonzero mean.  red[0] <- max of their relative errors
+// (as the bits of a non-negative double), red[1] += how many there are.
+__global__ void batch_max_rel_err_kernel(const double *__restrict__ mean, const double *__restrict__ m2, int64_t n,
+                                         int64_t goff, int64_t base, int64_t len, int32_t stride, int32_t score,
+                                         double nb, unsigned long long *red) {
+  double best = 0.0;
+  unsigned long long cnt = 0;
+  // first local entry of the tally's score slots at or after j = 0
+  int64_t g0 = goff > base ? goff : base;
+  const int64_t rem = (g0 - base) % stride;
+  g0 += rem <= score ? score - rem : stride - rem + score;
+  const int64_t gend = (goff + n < base + len) ? goff + n : base + len;
+  const int64_t step = int64_t(gridDim.x) * blockDim.x * stride;
+  for (int64_t g = g0 + (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) * stride; g < gend; g += step) {
+    const double mu = mean[g - goff];
+    if (mu != 0.0) {
+      best = fmax(best, batch_rel_err(mu, batch_std_err(m2[g - goff], nb)));
+      ++cnt;
+    }
+  }
+  for (int s = 16; s > 0; s >>= 1) {
+    best = fmax(best, __shfl_xor_sync(0xffffffffu, best, s));
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, s);
+  }
+  __shared__ double wbest[32];
+  __shared__ unsigned long long wcnt[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) {
+    wbest[warp] = best;
+    wcnt[warp] = cnt;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < int(blockDim.x >> 5); ++w) {
+      best = fmax(best, wbest[w]);
+      cnt += wcnt[w];
+    }
+    if (best > 0.0) atomicMax(red, (unsigned long long)__double_as_longlong(best));
+    if (cnt) atomicAdd(red + 1, cnt);
+  }
+}
+
+unsigned grid_for(int64_t work, int block) {
+  int dev = 0, sms = 132;
+  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int64_t want = (work + block - 1) / block, cap = int64_t(sms) * 8;
+  return unsigned(want < 1 ? 1 : want < cap ? want : cap);
+}
+
+}  // namespace
+
+cudaError_t launch_batch_fold(const double *x, double *mean, double *m2, int64_t n, const double *divisor, double nb,
+                              cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  auto aligned16 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
+  const int block = 256;
+  if (aligned16(x) && aligned16(mean) && aligned16(m2))
+    batch_fold_kernel<true><<<grid_for((n + 1) / 2, block), block, 0, stream>>>(x, mean, m2, n, divisor, nb);
+  else
+    batch_fold_kernel<false><<<grid_for(n, block), block, 0, stream>>>(x, mean, m2, n, divisor, nb);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_readout(const double *mean, const double *m2, const double *volume,
+                                 const int32_t *orig_of_internal, double *out, int64_t E, int32_t R, int32_t nscores,
+                                 int32_t stride, double nb, int kind, cudaStream_t stream) {
+  const int64_t n = E * int64_t(R);
+  if (n <= 0) return cudaSuccess;
+  batch_readout_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(mean, m2, volume, orig_of_internal, out, E, R,
+                                                                     nscores, stride, nb, kind);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_max_rel_err(const double *mean, const double *m2, int64_t n, int64_t goff, int64_t base,
+                                     int64_t len, int32_t stride, int32_t score, double nb, unsigned long long *red,
+                                     cudaStream_t stream) {
+  cudaError_t e = cudaMemsetAsync(red, 0, 2 * sizeof(unsigned long long), stream);
+  if (e != cudaSuccess || n <= 0) return e;
+  const int block = 256;
+  batch_max_rel_err_kernel<<<grid_for(n / stride + 1, block), block, 0, stream>>>(mean, m2, n, goff, base, len, stride,
+                                                                                  score, nb, red);
+  return cudaGetLastError();
+}
+
+}  // namespace ptb

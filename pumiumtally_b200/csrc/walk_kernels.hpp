@@ -141,4 +141,20 @@ cudaError_t launch_collide_particles(const ParticleState *state, const int8_t *c
                                      const CollisionParams &c, const double *w, const double *resp, const int32_t *bins,
                                      const double *times, unsigned long long *counts, cudaStream_t stream);
 
+// stats_kernels.cu.  Batch statistics (batch_stats.cuh).  fold: (mean[i], m2[i]) <- welford_fold(x[i] / *divisor, nb)
+// for i < n, nb the number of batches including this one; the divisor is read on the device.
+cudaError_t launch_batch_fold(const double *x, double *mean, double *m2, int64_t n, const double *divisor, double nb,
+                              cudaStream_t stream);
+// The m0 slots of R result arrays [R][E][stride] of means (and m2, unread for kind 0) of nb batches -> out[(r * nscores
+// + k) * E + caller's id of e] = batch_readout(..., volume[e], kind): 0 mean, 1 standard error, 2 relative error.
+cudaError_t launch_batch_readout(const double *mean, const double *m2, const double *volume,
+                                 const int32_t *orig_of_internal, double *out, int64_t E, int32_t R, int32_t nscores,
+                                 int32_t stride, double nb, int kind, cudaStream_t stream);
+// Local entries j < n of (mean, m2) are global entries goff + j.  Over the global entries of [base, base + len) that
+// are the m0 slot of `score` ((g - base) % stride == score) and have a nonzero mean: red[0] <- the bits of the largest
+// relative error (0.0 if none), red[1] <- their number.  red is zeroed first, on the stream.
+cudaError_t launch_batch_max_rel_err(const double *mean, const double *m2, int64_t n, int64_t goff, int64_t base,
+                                     int64_t len, int32_t stride, int32_t score, double nb, unsigned long long *red,
+                                     cudaStream_t stream);
+
 }  // namespace ptb

@@ -72,6 +72,10 @@ C_API = {
     "pumitally_tally_collisions_at_particles_device": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "pumitally_get_collision_results": (C.c_int, [C.c_void_p, C.c_int32, _dp, C.c_int64]),
+    "pumitally_set_batch_statistics": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_end_batch": (C.c_int, [C.c_void_p]),
+    "pumitally_get_batch_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
+    "pumitally_get_batch_max_rel_err": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.POINTER(C.c_int64)]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -540,6 +544,44 @@ class PumiTally:
         if self._L.pumitally_get_collision_results(self._h, int(kind), out.ctypes.data_as(_dp), out.size):
             raise RuntimeError(f"get_collision_results({kind}) failed")
         return out
+
+    # ---- batch statistics ----------------------------------------------------------
+    def set_batch_statistics(self, on: bool):
+        """True: keep a running mean and variance of every reported result over batches, on the device (resets the
+        tally, discards folded batches); False frees them."""
+        if self._L.pumitally_set_batch_statistics(self._h, int(on)):
+            raise ValueError("set_batch_statistics failed")
+
+    @property
+    def batch_statistics(self) -> bool:
+        return bool(self.get_option("batch_statistics"))
+
+    @property
+    def batches(self) -> int:
+        """Batches folded into the statistics."""
+        return self.get_option("batches")
+
+    def end_batch(self):
+        """Fold the open batch's per-source results into the statistics and start the next batch (collective with
+        several ranks)."""
+        if self._L.pumitally_end_batch(self._h):
+            raise RuntimeError("end_batch failed")
+
+    def batch_results(self, tally=0, kind=0):
+        """tally 0 track length, 1 collision; kind 0 mean, 1 standard error, 2 relative error
+        ([ntime, nbins, nscores, num_elements]), 3 gradient of the mean ([..., 3])."""
+        shape = (max(self.time_bins, 1), self.score_bins, self.scores, self.num_elements) + ((3,) if kind == 3 else ())
+        out = np.empty(shape)
+        if self._L.pumitally_get_batch_results(self._h, int(tally), int(kind), out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError(f"get_batch_results({tally}, {kind}) failed")
+        return out
+
+    def batch_max_rel_err(self, tally=0, score=0):
+        """(largest relative error of score ``score`` over the results with a nonzero mean, how many there are)."""
+        mx, cnt = C.c_double(0.0), C.c_int64(0)
+        if self._L.pumitally_get_batch_max_rel_err(self._h, int(tally), int(score), C.byref(mx), C.byref(cnt)):
+            raise RuntimeError(f"get_batch_max_rel_err({tally}, {score}) failed")
+        return mx.value, cnt.value
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
