@@ -137,7 +137,7 @@ def test_bins_scores_time_bins_and_moments_on_every_upload_path(path):
     # the caller's arrays stay alive and are reused for every move (what option register_host asks of the caller)
     o_buf, d_buf, w_buf = np.empty(3 * wl.n), np.empty(3 * wl.n), np.empty(wl.n)
     t_buf, v_buf = np.empty(wl.n), np.empty(wl.n)
-    r_buf, b_buf = np.empty((wl.n, nscores)), np.empty(wl.n, dtype=np.int32)
+    r_buf, b_buf, f_buf = np.empty((wl.n, nscores)), np.empty(wl.n, dtype=np.int32), np.empty(wl.n, dtype=np.int8)
     for step in range(2):
         o, d, f, w = wl.next_step()
         o_buf[:], d_buf[:], w_buf[:] = o.reshape(-1), d.reshape(-1), w
@@ -150,9 +150,9 @@ def test_bins_scores_time_bins_and_moments_on_every_upload_path(path):
             eng.move_device_timed(*(x.data_ptr() for x in dev), s)
             torch.cuda.synchronize()
         else:
-            f1 = f.copy()
-            eng.MoveToNextLocationTimed(o_buf, d_buf, f1, w_buf, t_buf, v_buf, r_buf, b_buf)
-            assert not f1.any()
+            f_buf[:] = f
+            eng.MoveToNextLocationTimed(o_buf, d_buf, f_buf, w_buf, t_buf, v_buf, r_buf, b_buf)
+            assert not f_buf.any()
         _move(twin, "timed", o, d, f, w, r, times, speeds, bins)
         assert_same_particles(eng, twin, f"{path} step {step}")
         for q in range(nbins):

@@ -182,7 +182,7 @@ def test_bins_times_scores_on_every_upload_path(path):
     s = torch.cuda.current_stream().cuda_stream
     # the same arrays every move (register_host pins the caller's buffers once)
     o_buf, d_buf, w_buf = np.empty(3 * wl.n), np.empty(3 * wl.n), np.empty(wl.n)
-    r_buf, b_buf = np.empty((wl.n, nscores)), np.empty(wl.n, dtype=np.int32)
+    r_buf, b_buf, f_buf = np.empty((wl.n, nscores)), np.empty(wl.n, dtype=np.int32), np.empty(wl.n, dtype=np.int8)
     h2d = 0.0
     for step in range(3):
         o, d, f, w = wl.next_step()
@@ -194,7 +194,8 @@ def test_bins_times_scores_on_every_upload_path(path):
             torch.cuda.synchronize()
         else:
             before = eng.stats()["h2d_bytes"]
-            eng.MoveToNextLocationScored(o_buf, d_buf, f.copy(), w_buf, r_buf, b_buf)
+            f_buf[:] = f
+            eng.MoveToNextLocationScored(o_buf, d_buf, f_buf, w_buf, r_buf, b_buf)
             h2d = eng.stats()["h2d_bytes"] - before
         for k, p in enumerate(plains):
             p.MoveToNextLocationBinned(o_buf.copy(), d_buf.copy(), f.copy(), w_buf * r_buf[:, k], b_buf.copy())

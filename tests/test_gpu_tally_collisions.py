@@ -1,11 +1,7 @@
 """Collision estimator (pumitally_set_collision_estimator): events scored at located points or at the particles'
 positions into a collision tally of the track-length tally's configuration.  Checked against the numpy reference
 (tests/collisions_ref.py); the collision calls must change nothing else, and on a homogeneous box the collision and
-track-length estimates of the same flux must agree.
-
-The module sorts after test_gpu_scores.py on purpose: that module's register_host case hands the engine temporary
-flying arrays, which stay page-locked after Python frees them, and whether a later pageable copy of another engine starts
-inside one of those ranges (and fails) depends on the heap that earlier tests in the process left behind."""
+track-length estimates of the same flux must agree."""
 import ctypes as C
 import os
 import subprocess

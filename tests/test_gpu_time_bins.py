@@ -123,7 +123,7 @@ def test_bins_times_scores_on_every_upload_path(path):
     s = torch.cuda.current_stream().cuda_stream
     o_buf, d_buf, w_buf = np.empty(3 * wl.n), np.empty(3 * wl.n), np.empty(wl.n)
     t_buf, v_buf = np.empty(wl.n), np.empty(wl.n)
-    r_buf, b_buf = np.empty((wl.n, nscores)), np.empty(wl.n, dtype=np.int32)
+    r_buf, b_buf, f_buf = np.empty((wl.n, nscores)), np.empty(wl.n, dtype=np.int32), np.empty(wl.n, dtype=np.int8)
     want = np.zeros((len(edges) - 1, nbins, nscores, len(t2v)))
     h2d = 0.0
     for step in range(2):
@@ -137,7 +137,8 @@ def test_bins_times_scores_on_every_upload_path(path):
             torch.cuda.synchronize()
         else:
             before = eng.stats()["h2d_bytes"]
-            eng.MoveToNextLocationTimed(o_buf, d_buf, f.copy(), w_buf, t_buf, v_buf, r_buf, b_buf)
+            f_buf[:] = f
+            eng.MoveToNextLocationTimed(o_buf, d_buf, f_buf, w_buf, t_buf, v_buf, r_buf, b_buf)
             h2d = eng.stats()["h2d_bytes"] - before
         twin.MoveToNextLocationScored(o_buf.copy(), d_buf.copy(), f.copy(), w_buf.copy(), r_buf, b_buf.copy())
         for b in range(nbins):
