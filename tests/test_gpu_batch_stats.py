@@ -150,6 +150,62 @@ def test_eight_batches_match_numpy(case, mode, path):
     np.testing.assert_array_equal(first, b.eng.batch_results(0, 1)[0, 0, 0])
 
 
+@pytest.mark.parametrize("path", ["host", "device"])
+@pytest.mark.parametrize("mode", [0, 3])
+@pytest.mark.parametrize("collision", [False, True], ids=["track", "collision"])
+def test_odd_element_count(collision, mode, path):
+    """One score, no bins and an odd number of elements: without the collision estimator the folded length L = E is
+    odd, so the double2 fold ends in its odd tail; with it the collision tally starts at the odd offset E.  Every
+    element is scored in every batch (a flight starts at each centroid), so a result the fold or readout skipped
+    would show as a zero mean."""
+    import torch
+
+    from pumiumtally_b200.mesh import delaunay_box
+
+    c, t = delaunay_box(60, seed=1)
+    E = len(t)
+    assert E % 2 == 1
+    cen = c[t].mean(axis=1)
+    n = E + 1000
+    rng = np.random.default_rng(7 + mode)
+    eng = PumiTally.from_arrays(c, t, n)
+    eng.set_collision_estimator(collision)
+    eng.set_batch_statistics(True)
+    eng.set_source_normalization(mode, MODES[mode])
+    start = np.vstack([cen, rng.uniform(0.05, 0.95, (n - E, 3))])
+    eng.CopyInitialPosition(start.reshape(-1).copy())
+    caps = []
+    for _ in range(6):
+        o = np.vstack([cen, eng.positions[E:]])  # the first E re-start at the centroids
+        d = rng.uniform(0.0, 1.0, (n, 3))
+        f = np.ones(n, dtype=np.int8)
+        w = rng.uniform(0.5, 1.5, n)
+        if path == "host":
+            _move(eng, "plain", o, d, f, w)
+        else:
+            do, dd, df, dw = (torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in (o.reshape(-1), d.reshape(-1), f, w))
+            eng.move_device(do.data_ptr(), dd.data_ptr(), df.data_ptr(), dw.data_ptr(),
+                            torch.cuda.current_stream().cuda_stream)
+            torch.cuda.synchronize()
+        cap = [eng.normalized_flux()[0]]
+        if collision:
+            eng.tally_collisions(cen, rng.uniform(0.5, 1.5, E))
+            cap.append(eng.collision_results(1)[0, 0, 0])
+        caps.append(cap)
+        eng.end_batch()
+    for tally in range(len(caps[0])):
+        x = np.array([cp[tally] for cp in caps])
+        assert (x != 0).all()
+        want = numpy_stats(x)
+        for kind in range(3):
+            got = eng.batch_results(tally, kind)[0, 0, 0]
+            assert_stats(got, want[kind], f"tally {tally} kind {kind}")
+            assert got[E - 1] != 0 and abs(got[E - 1] - want[kind][E - 1]) <= 1e-12 * abs(want[kind][E - 1])
+        mx, cnt = eng.batch_max_rel_err(tally, 0)
+        assert cnt == E
+        np.testing.assert_allclose(mx, want[2].max(), rtol=1e-12, atol=0)
+
+
 def test_ill_conditioned_batches():
     """The same flights every batch with weights scaled by 1 + 1e-9 b: the standard error is 1e-9 of the mean, and
     still matches numpy's two-pass result to 1e-6."""
@@ -449,3 +505,171 @@ def test_two_gpus_fold_the_summed_batches():
                 mx, cnt = res[rank][5][2 * tally + k]
                 assert cnt == int((m != 0).sum())
                 np.testing.assert_allclose(mx, rel[m != 0].max(), rtol=1e-12)
+
+
+# Uneven rank shares: share_ = ceil(L / nranks) odd and not a multiple of the record stride, so every rank after the
+# first folds from an odd double (the scalar fold) and its max-relative-error window starts inside a record.  On the
+# Delaunay mesh below (E = 731 = 5 mod 6) with the collision estimator on:
+#   "s2": 2 scores (stride 2), L = 4 E;  3 ranks: share 975, rank 1 holds the end of the track-length tally and the
+#         start of the collision tally;  4 ranks: share 731, rank 2 starts exactly at the collision tally.
+#   "s1_b2_mo": 1 score, 2 bins, moments (stride 4), L = 16 E;  3 ranks: share 3899, rank 1 holds both tallies.
+UNEVEN = {"s2": (2, 1, 0), "s1_b2_mo": (1, 2, 1)}  # nscores, nbins, moments
+UNEVEN_N, UNEVEN_BATCHES = 2500, 5
+
+
+def _uneven_inputs(rank, nscores, nbins):
+    """Every rank's initial positions and, per batch (one more than UNEVEN_BATCHES: the last stays open), its move
+    and collision events."""
+    wl = SyntheticWorkload(box=(1.0, 1.0, 1.0), num_particles=UNEVEN_N, mean_length=0.3, seed=300 + rank)
+    rng = np.random.default_rng(rank)
+    init, steps = wl.initial_positions().reshape(-1).copy(), []
+    for _ in range(UNEVEN_BATCHES + 1):
+        o, d, f, w = wl.next_step()
+        k = 1500
+        steps.append(dict(o=o, d=d, f=f, w=w * rng.uniform(0.5, 1.5), r=responses(rng, UNEVEN_N, nscores),
+                          bins=rng.integers(0, nbins, UNEVEN_N).astype(np.int32), pts=rng.uniform(0.0, 1.0, (k, 3)),
+                          cw=rng.uniform(0.5, 1.5, k), cr=rng.uniform(0.0, 1.0, (k, nscores)),
+                          cb=rng.integers(0, nbins, k).astype(np.int32)))
+    return init, steps
+
+
+def _uneven_engine(c, t, n, nscores, nbins, moments, device=-1):
+    eng = PumiTally.from_arrays(c, t, n, device=device)
+    _configure(eng, nscores, moments=moments, nbins=nbins)
+    eng.set_collision_estimator(True)
+    eng.set_batch_statistics(True)
+    eng.set_source_normalization(3)
+    return eng
+
+
+def _uneven_step(eng, s, nscores):
+    if nscores > 1:
+        _move(eng, "scored", s["o"], s["d"], s["f"], s["w"], s["r"], bins=s["bins"])
+    else:
+        _move(eng, "binned", s["o"], s["d"], s["f"], s["w"], bins=s["bins"])
+    eng.tally_collisions(s["pts"], s["cw"], s["cr"], s["cb"])
+
+
+def _exchanged(eng, moments, pts):
+    """What the accessors return after a batch-end exchange (raw results and point values, mode 0)."""
+    out = [eng.flux_time, eng.collision_results(0), eng.evaluate(pts)[0]]
+    if moments:
+        out += [eng.flux_moments(), eng.collision_results(2)]
+    return out
+
+
+def _uneven_worker(rank, world, port, q, case):
+    import sys
+
+    import torch
+    import torch.distributed as dist
+
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    from pumiumtally_b200.distributed import broadcast_unique_id
+    from pumiumtally_b200.mesh import delaunay_box
+
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+    torch.cuda.set_device(rank)
+    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nscores, nbins, moments = UNEVEN[case]
+    c, t = delaunay_box(120, seed=6)
+    eng = _uneven_engine(c, t, UNEVEN_N, nscores, nbins, moments, device=rank)
+    eng.comm_init(rank, world, broadcast_unique_id(dist, PumiTally.nccl_unique_id, device=torch.device("cuda", rank)))
+    init, steps = _uneven_inputs(rank, nscores, nbins)
+    eng.CopyInitialPosition(init)
+    local, weights = [], []
+    for s in steps[:-1]:
+        _uneven_step(eng, s, nscores)
+        local.append((eng.flux_time.copy(), eng.collision_results(0).copy()))
+        weights.append(float((s["w"] * (s["f"] == 1)).sum()))
+        eng.end_batch()
+    kinds = range(4) if moments else range(3)
+    results = [[eng.batch_results(tally, kind) for kind in kinds] for tally in (0, 1)]
+    trig = [eng.batch_max_rel_err(tally, k) for tally in (0, 1) for k in range(nscores)]
+    _uneven_step(eng, steps[-1], nscores)  # an open batch, exchanged both ways
+    eng.set_source_normalization(0)
+    pts = np.random.default_rng(99).uniform(0.0, 1.0, (500, 3))
+    eng.reduce_tally_to_owners()
+    owners = _exchanged(eng, moments, pts)
+    eng.allreduce_tally()
+    summed = _exchanged(eng, moments, pts)
+    q.put((rank, local, weights, results, trig, owners, summed))
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("case,world,straddle", [("s2", 3, True), ("s2", 4, False), ("s1_b2_mo", 3, True)],
+                         ids=["s2-3ranks", "s2-4ranks", "s1_b2_mo-3ranks"])
+def test_uneven_rank_shares(case, world, straddle):
+    import torch
+
+    from pumiumtally_b200.mesh import delaunay_box
+    from test_gpu_stats_kernels import score_stride
+
+    nscores, nbins, moments = UNEVEN[case]
+    c, t = delaunay_box(120, seed=6)
+    E = len(t)
+    stride = score_stride(nscores) * (4 if moments else 1)
+    flux_len = nbins * E * stride
+    L = 2 * flux_len
+    share = -(-L // world)
+    # the layout this test is about
+    assert share % 2 == 1 and share % stride != 0
+    los = [r * share for r in range(world)]
+    if straddle:  # one share holds the end of the track-length tally and the start of the collision tally
+        assert any(lo < flux_len < lo + share for lo in los)
+    else:  # a share starts exactly at the collision tally
+        assert flux_len in los
+    if torch.cuda.device_count() < world:
+        pytest.skip(f"needs {world} GPUs")
+    import torch.multiprocessing as mp
+
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    port = 29900 + (os.getpid() + 17 * world + len(case)) % 1000
+    procs = [ctx.Process(target=_uneven_worker, args=(r, world, port, q, case)) for r in range(world)]
+    for p in procs:
+        p.start()
+    res = sorted([q.get(timeout=600) for _ in range(world)], key=lambda x: x[0])
+    for p in procs:
+        p.join(timeout=60)
+        assert p.exitcode == 0
+    vol = _geometry(c, t)[1]
+    div = np.sum([r[2] for r in res], axis=0)  # mode 3: the whole batch's first-track weight
+    # the same particles and events on one GPU
+    one = _uneven_engine(c, t, world * UNEVEN_N, nscores, nbins, moments)
+    inputs = [_uneven_inputs(r, nscores, nbins) for r in range(world)]
+    one.CopyInitialPosition(np.concatenate([i for i, _ in inputs]))
+    for b in range(UNEVEN_BATCHES + 1):
+        s = {k: np.concatenate([steps[b][k] for _, steps in inputs]) for k in inputs[0][1][b]}
+        _uneven_step(one, s, nscores)
+        if b < UNEVEN_BATCHES:
+            one.end_batch()
+    for tally in (0, 1):
+        x = np.array([sum(r[1][b][tally] for r in res) / vol / div[b] for b in range(UNEVEN_BATCHES)])
+        want = numpy_stats(x)
+        for rank in range(world):
+            for kind in range(3):
+                assert_stats(res[rank][3][tally][kind], want[kind], f"rank {rank} tally {tally} kind {kind}")
+                assert_stats(res[rank][3][tally][kind], one.batch_results(tally, kind), f"one GPU {tally} {kind}")
+            if moments:
+                g = one.batch_results(tally, 3)
+                np.testing.assert_allclose(res[rank][3][tally][3], g, rtol=1e-9, atol=1e-12 * np.abs(g).max(),
+                                           err_msg=f"rank {rank} gradient {tally}")
+            for k in range(nscores):
+                m, _, rel = (w[:, :, k] for w in want)
+                mx, cnt = res[rank][4][nscores * tally + k]
+                assert cnt == int((m != 0).sum()) > 0
+                np.testing.assert_allclose(mx, rel[m != 0].max(), rtol=1e-12)
+                one_mx, one_cnt = one.batch_max_rel_err(tally, k)
+                assert cnt == one_cnt
+                np.testing.assert_allclose(mx, one_mx, rtol=1e-12, atol=0)
+    one.set_source_normalization(0)
+    want = _exchanged(one, moments, np.random.default_rng(99).uniform(0.0, 1.0, (500, 3)))
+    for rank in range(world):
+        for how, got in (("reduce_tally_to_owners", res[rank][5]), ("allreduce_tally", res[rank][6])):
+            for j, (g, w) in enumerate(zip(got, want)):
+                fin = np.isfinite(w)
+                np.testing.assert_array_equal(np.isfinite(g), fin)
+                tol = 1e-12 * np.abs(w[fin]) + 1e-15 * np.abs(w[fin]).sum()
+                assert (np.abs(g[fin] - w[fin]) <= tol).all(), f"rank {rank} {how} array {j}"
