@@ -112,6 +112,24 @@ inline int GetBatchMaxRelErr(const PumiTally &tally, int32_t which, int32_t scor
   return pumitally_get_batch_max_rel_err(engine_of(tally), which, score, out_max, out_nonzero);
 }
 
+// Region tallies (see pumitally_set_regions in pumitally_c.h): SetRegions groups the elements into nregions regions
+// (one id per element in [-1, nregions), -1 for none; nullptr with 0 removes them).  GetRegionResults: tally 0 track
+// length, 1 collision; kind 0 the raw sum over each region, 1 sum / volume / the per-source divisor.
+// GetRegionBatchResults: kind 0 mean, 1 standard error, 2 relative error of the region sums over the batches.  n is
+// nregions (time bin 0, bin 0, score 0) or ntime * nbins * nscores * nregions, [time][bin][score][region].
+inline int SetRegions(const PumiTally &tally, const int32_t *region_of_element, int64_t n, int32_t nregions) {
+  return pumitally_set_regions(engine_of(tally), region_of_element, n, nregions);
+}
+inline int GetRegionVolumes(const PumiTally &tally, double *out, int64_t n) {
+  return pumitally_get_region_volumes(engine_of(tally), out, n);
+}
+inline int GetRegionResults(const PumiTally &tally, int32_t which, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_region_results(engine_of(tally), which, kind, out, n);
+}
+inline int GetRegionBatchResults(const PumiTally &tally, int32_t which, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_region_batch_results(engine_of(tally), which, kind, out, n);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

@@ -439,6 +439,37 @@ int pumitally_get_batch_results(pumitally_engine *e, int32_t tally, int32_t kind
 int pumitally_get_batch_max_rel_err(pumitally_engine *e, int32_t tally, int32_t score, double *out_max,
                                     int64_t *out_nonzero);
 
+/* ---- additive: region tallies (sums over caller-defined groups of elements, with batch statistics) ----
+ * A region is a group of elements, such as a material or a CAD part (a Gmsh physical group, an Omega_h class id).
+ * pumitally_set_regions(e, region_of_element, n, nregions): region_of_element holds one id per element in the caller's
+ * numbering (n == pumitally_num_elements), each in [-1, nregions), -1 for an element in no region, and
+ * 1 <= nregions <= n.  Regions may be empty.  region_of_element == NULL with nregions == 0 removes the regions; any
+ * other input returns non-zero and changes nothing.  The call resets the tally and discards the folded batches, as
+ * every pumitally_set_* call does, and is refused after pumitally_comm_init.  pumitally_get_regions returns nregions, 0
+ * without regions.
+ * pumitally_get_region_volumes(e, out, n == nregions): V_G, the sum of the region's element volumes.
+ * pumitally_get_region_results(e, tally, kind, out, n): tally 0 track length, 1 collision (estimator on); kind 0 the raw
+ * sum sum_{e in G} x_e of every result (m0 only: moments are not summed), kind 1 the normalised value sum / V_G / d,
+ * d the divisor pumitally_get_normalized_flux uses.  Layout [time][bin][score][region]; n == nregions gives time bin 0,
+ * bin 0, score 0, n == ntime * nbins * nscores * nregions everything.  It reads the tally the flux accessors read
+ * (after a batch-end exchange the summed one; collective after pumitally_reduce_tally_to_owners, as they are).
+ * Sums are formed on the device in a fixed order (ascending internal element id in chunks of 32, then the chunk sums
+ * in chunks of 32, and so on), so the same tally gives the same bits; a one-element region gives exactly the element's
+ * pumitally_get_flux / pumitally_get_normalized_flux value, and its volume is the element's.  An empty region has
+ * volume 0 and sum 0; its kind 1 value and all of its batch results are NaN (0 / 0).
+ * Batch statistics: while pumitally_set_batch_statistics is on and regions are set, pumitally_end_batch also sums the
+ * batch's raw tally (both tallies) into regions before it is folded, adds those sums over the ranks (one
+ * ncclAllReduce of nregions * results doubles) and folds sum / d_b as it folds every element.  The variance of a
+ * region sum needs the covariances of its elements, which per-element statistics cannot give afterwards: this does.
+ * pumitally_get_region_batch_results(e, tally, kind, out, n): kind 0 the mean / V_G, 1 the standard error / V_G, 2 the
+ * relative error; layout and n as pumitally_get_region_results.  Refused as pumitally_get_batch_results is (kind 3 does
+ * not exist here), and without regions.  Not collective: every rank holds the same region statistics. */
+int pumitally_set_regions(pumitally_engine *e, const int32_t *region_of_element, int64_t n, int32_t nregions);
+int32_t pumitally_get_regions(const pumitally_engine *e);
+int pumitally_get_region_volumes(pumitally_engine *e, double *out, int64_t n);
+int pumitally_get_region_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
+int pumitally_get_region_batch_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

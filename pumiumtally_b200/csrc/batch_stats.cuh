@@ -9,6 +9,9 @@
 #if !defined(__CUDACC__)
 #include <cmath>
 #endif
+#include <algorithm>
+#include <cstdint>
+#include <vector>
 
 namespace ptb {
 
@@ -32,6 +35,99 @@ PTB_HD double batch_readout(double mean, double m2, double nb, double volume, in
   if (kind == 0) return m;
   const double s = batch_std_err(m2, nb) / volume;
   return kind == 1 ? s : batch_rel_err(m, s);
+}
+
+// ---- region sums (engine.cu, set_regions / get_region_results / end_batch; stats_kernels.cu, launch_region_sums) ----
+// A region's sum is formed in levels.  Level 0 cuts the region's elements (ascending internal id) into chunks of at most
+// kRegionChunk consecutive elements and sums each chunk left to right; every later level does the same to the region's
+// chunk sums of the level before, until one sum per region is left.  The order depends on the region sizes only: the
+// same tally always gives the same bits, and a one-element region's sum is its element's value itself.
+constexpr int kRegionChunk = 32;
+
+// Chunks a region of n inputs is cut into at one level; an empty region keeps one empty chunk, whose sum is 0.
+PTB_HD int64_t region_chunks(int64_t n) { return n > kRegionChunk ? (n + kRegionChunk - 1) / kRegionChunk : 1; }
+
+// acc[k] = x(0, k) + x(1, k) + ... + x(n - 1, k), left to right, for k < nscores: 0 for n == 0, x(0, k) for n == 1.
+// (x is a device lambda in the kernel and a host one in region_sums_host)
+#if defined(__CUDACC__)
+#pragma nv_exec_check_disable
+#endif
+template <class F>
+PTB_HD void chunk_sum(int64_t n, int nscores, F x, double (&acc)[kMaxScores]) {
+  PTB_UNROLL
+  for (int k = 0; k < kMaxScores; ++k) acc[k] = (k < nscores && n > 0) ? x(0, k) : 0.0;
+  for (int64_t i = 1; i < n; ++i) {
+    PTB_UNROLL
+    for (int k = 0; k < kMaxScores; ++k)
+      if (k < nscores) acc[k] += x(i, k);
+  }
+}
+
+// One level of the plan: its chunk c covers inputs [starts[start_off + c], starts[start_off + c + 1]).
+struct RegionLevel {
+  int64_t start_off;  // first of its chunks + 1 entries in RegionPlan::starts
+  int64_t chunks;     // the last level has one chunk per region, in region order
+  int64_t inputs;     // level 0: the elements in a region; later levels: the chunks of the level before
+};
+
+struct RegionPlan {
+  std::vector<int32_t> elems;   // level 0's inputs: internal element ids, ascending region, then ascending id
+  std::vector<int32_t> starts;  // every level's chunk starts
+  std::vector<RegionLevel> levels;
+};
+
+// The plan of region_of_internal[e] in [-1, nregions) for e < E (-1: in no region).
+inline RegionPlan build_region_plan(const int32_t *region_of_internal, int64_t E, int32_t nregions) {
+  RegionPlan p;
+  std::vector<int64_t> n(size_t(nregions), 0), off(size_t(nregions) + 1, 0);
+  for (int64_t e = 0; e < E; ++e)
+    if (region_of_internal[e] >= 0) ++n[size_t(region_of_internal[e])];
+  for (size_t g = 0; g < n.size(); ++g) off[g + 1] = off[g] + n[g];
+  p.elems.resize(size_t(off.back()));
+  for (int64_t e = 0; e < E; ++e)  // ascending id within each region
+    if (region_of_internal[e] >= 0) p.elems[size_t(off[size_t(region_of_internal[e])]++)] = int32_t(e);
+  for (bool done = false; !done;) {
+    RegionLevel l{int64_t(p.starts.size()), 0, 0};
+    done = true;
+    for (int64_t &m : n) {
+      const int64_t c = region_chunks(m);
+      for (int64_t j = 0; j < c; ++j) p.starts.push_back(int32_t(l.inputs + std::min<int64_t>(j * kRegionChunk, m)));
+      l.inputs += m;
+      l.chunks += c;
+      m = c;
+      done = done && c == 1;
+    }
+    p.starts.push_back(int32_t(l.inputs));
+    p.levels.push_back(l);
+  }
+  return p;
+}
+
+// Doubles of the scratch launch_region_sums needs for narrays arrays of nscores results: two buffers of the largest
+// level output before the last.
+inline int64_t region_scratch_len(const RegionPlan &p, int64_t narrays, int32_t nscores) {
+  int64_t m = 0;
+  for (size_t l = 0; l + 1 < p.levels.size(); ++l) m = std::max(m, p.levels[l].chunks);
+  return 2 * m * narrays * nscores;
+}
+
+// The region sums of one value per element, values[internal id], in the order above: what launch_region_sums computes,
+// on the host (the region volumes; tests/host_emul/emul_regions.cpp).
+inline std::vector<double> region_sums_host(const RegionPlan &p, const double *values) {
+  std::vector<double> in, out;
+  for (size_t l = 0; l < p.levels.size(); ++l) {
+    const RegionLevel &v = p.levels[l];
+    out.assign(size_t(v.chunks), 0.0);
+    for (int64_t c = 0; c < v.chunks; ++c) {
+      const int32_t lo = p.starts[size_t(v.start_off + c)], hi = p.starts[size_t(v.start_off + c + 1)];
+      double acc[kMaxScores];
+      chunk_sum(hi - lo, 1, [&](int64_t i, int) { return l == 0 ? values[p.elems[size_t(lo + i)]] : in[size_t(lo + i)]; },
+                acc);
+      out[size_t(c)] = acc[0];
+    }
+    in.swap(out);
+  }
+  return in;
 }
 
 }  // namespace ptb

@@ -286,6 +286,25 @@ int pumitally_get_batch_max_rel_err(pumitally_engine *e, int32_t tally, int32_t 
   return guarded(e, [&](ptb::Engine &g) { return g.get_batch_max_rel_err(tally, score, out_max, out_nonzero); });
 }
 
+int pumitally_set_regions(pumitally_engine *e, const int32_t *region_of_element, int64_t n, int32_t nregions) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_regions(region_of_element, n, nregions); });
+}
+int32_t pumitally_get_regions(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "regions")) : 0;
+}
+int pumitally_get_region_volumes(pumitally_engine *e, double *out, int64_t n) {
+  if (n > 0 && !out) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_region_volumes(out, n); });
+}
+int pumitally_get_region_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n) {
+  if (n > 0 && !out) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_region_results(tally, kind, out, n); });
+}
+int pumitally_get_region_batch_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n) {
+  if (n > 0 && !out) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_region_batch_results(tally, kind, out, n); });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

@@ -190,6 +190,7 @@ Engine::~Engine() {
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
   cudaFree(d_coll_counts_); cudaFree(d_coll_buf_);
   free_stats();
+  free_regions();
   cudaFree(d_batch_div_); cudaFree(d_stats_red_);
   if (compute_) cudaStreamDestroy(compute_);
   if (copy_) cudaStreamDestroy(copy_);
@@ -1592,6 +1593,7 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "collision_estimator") return collision_ ? 1 : 0;
   if (name == "batch_statistics") return batch_stats_ ? 1 : 0;
   if (name == "batches") return batches_;  // batches folded into the statistics
+  if (name == "regions") return nregions_;
   // collision events since the last reset: tallied, located outside the mesh, rejected (non-finite inputs)
   if (name == "collisions" || name == "collisions_outside" || name == "collisions_rejected") {
     unsigned long long c[3] = {0, 0, 0};
@@ -2183,7 +2185,8 @@ int Engine::alloc_stats(size_t len) {
 void Engine::free_stats() {
   cudaFree(d_mean_);
   cudaFree(d_m2_);
-  d_mean_ = d_m2_ = nullptr;
+  cudaFree(d_region_stats_);
+  d_mean_ = d_m2_ = d_region_stats_ = nullptr;
   batches_ = 0;
 }
 
@@ -2225,7 +2228,7 @@ int Engine::end_batch() {
     fprintf(stderr, "[pumitally] ERROR: end_batch: batch statistics are off (set_batch_statistics)\n");
     return 1;
   }
-  if (synchronize()) return 1;
+  if (synchronize() || (nregions_ > 0 && (ensure_region_work() || ensure_region_stats()))) return 1;
   const double local = norm_mode_ == 1 ? double(std::max(n_, 1)) : norm_mode_ == 2 ? norm_value_ : 1.0;
   if (norm_mode_ == 3)
     PTB_CUDA_OK(cudaMemcpyAsync(d_batch_div_ + 1, d_initial_weight_, sizeof(double), cudaMemcpyDeviceToDevice, compute_));
@@ -2245,6 +2248,13 @@ int Engine::end_batch() {
   }
   const size_t L = reported_len();
   const double nb = double(batches_ + 1);
+  if (nregions_ > 0) {  // region sums of this rank's batch, summed over the ranks: the same statistics on every rank
+    const size_t RL = region_len();
+    double *sums = d_region_stats_;
+    if (region_sums(d_flux_, int64_t(collision_ ? 2 : 1) * result_arrays(), sums)) return 1;
+    if (sharded() && nccl_allreduce_sum_f64(nccl_comm_, sums, sums, RL, compute_)) return 1;
+    PTB_CUDA_OK(launch_batch_fold(sums, sums + RL, sums + 2 * RL, int64_t(RL), d_batch_div_, nb, compute_));
+  }
   if (sharded()) {
     const size_t lo = size_t(rank_) * share_;  // the last share ends in padding (or a binned move's unreported array)
     if (nccl_reduce_scatter_sum_f64(nccl_comm_, d_flux_, d_flux_global_ + lo, share_, compute_)) return 1;
@@ -2403,6 +2413,196 @@ int Engine::batch_arrays(int32_t tally, const std::string &prefix, VtkArrays &a)
           if (errs && single_time) add(bn + "_rel_err", std::vector<double>(at(rel, t0, b, k), at(rel, t0, b, k) + E));
         }
     }
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------ region tallies
+
+void Engine::free_regions() {
+  cudaFree(d_region_elems_);
+  cudaFree(d_region_starts_);
+  cudaFree(d_region_ident_);
+  cudaFree(d_region_volume_);
+  cudaFree(d_region_work_);
+  cudaFree(d_region_stats_);
+  d_region_elems_ = d_region_starts_ = d_region_ident_ = nullptr;
+  d_region_volume_ = d_region_work_ = d_region_stats_ = nullptr;
+  region_scratch_ = 0;
+  region_levels_.clear();
+  region_volume_.clear();
+  nregions_ = 0;
+}
+
+int Engine::set_regions(const int32_t *region_of_element, int64_t n, int32_t nregions) {
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_regions after comm_init (the batch statistics are sized by then)\n");
+    return 1;
+  }
+  const int64_t E = mesh_.ntets;
+  const bool remove = !region_of_element && nregions == 0;
+  if (!remove) {
+    const char *why = !region_of_element                  ? "the region map is null (remove the regions with nregions 0)"
+                      : n != E                            ? "n must be the number of elements"
+                      : (nregions < 1 || nregions > E)    ? "nregions must be in [1, number of elements]"
+                                                          : nullptr;
+    for (int64_t e = 0; !why && e < n; ++e)
+      if (region_of_element[e] < -1 || region_of_element[e] >= nregions) why = "a region id is outside [-1, nregions)";
+    if (why) {
+      fprintf(stderr, "[pumitally] ERROR: set_regions: %s\n", why);
+      return 1;
+    }
+  }
+  if (synchronize()) return 1;
+  // the new plan's device arrays first: nothing changes unless all of them (and fresh statistics) can be had
+  RegionPlan plan;
+  std::vector<double> vol;
+  int32_t *elems = nullptr, *starts = nullptr, *ident = nullptr;
+  double *dvol = nullptr;
+  if (!remove) {
+    std::vector<int32_t> region_of_internal(static_cast<size_t>(E));
+    for (int64_t i = 0; i < E; ++i) region_of_internal[size_t(i)] = region_of_element[mesh_.orig_of_internal[size_t(i)]];
+    plan = build_region_plan(region_of_internal.data(), E, nregions);
+    vol = region_sums_host(plan, mesh_.volume.data());
+    std::vector<int32_t> id(static_cast<size_t>(nregions));
+    for (int32_t g = 0; g < nregions; ++g) id[size_t(g)] = g;
+    auto up = [](auto **d, const auto &h) {
+      const size_t bytes = std::max<size_t>(h.size(), 1) * sizeof(h[0]);
+      return cudaMalloc(reinterpret_cast<void **>(d), bytes) == cudaSuccess &&
+             cudaMemcpy(*d, h.data(), h.size() * sizeof(h[0]), cudaMemcpyHostToDevice) == cudaSuccess;
+    };
+    if (!up(&elems, plan.elems) || !up(&starts, plan.starts) || !up(&ident, id) || !up(&dvol, vol)) {
+      const cudaError_t err = cudaGetLastError();
+      cudaFree(elems); cudaFree(starts); cudaFree(ident); cudaFree(dvol);
+      fprintf(stderr, "[pumitally] ERROR: no device memory for the regions (%s)\n", cudaGetErrorString(err));
+      return 1;
+    }
+  }
+  if (batch_stats_ && alloc_stats(reported_len())) {  // discards the folded batches (element and region)
+    cudaFree(elems); cudaFree(starts); cudaFree(ident); cudaFree(dvol);
+    return 1;
+  }
+  free_regions();
+  if (!remove) {
+    nregions_ = nregions;
+    region_levels_ = plan.levels;
+    region_volume_ = std::move(vol);
+    d_region_elems_ = elems;
+    d_region_starts_ = starts;
+    d_region_ident_ = ident;
+    d_region_volume_ = dvol;
+  }
+  return reset_tally();
+}
+
+int Engine::ensure_region_work() {
+  const int64_t A = 2 * int64_t(result_arrays());  // (both tallies)
+  RegionPlan p;
+  p.levels = region_levels_;
+  const int64_t scratch = region_scratch_len(p, A, nscores_);
+  const size_t need = size_t(scratch) + size_t(A) * size_t(nregions_) * size_t(nscores_);
+  if (d_region_work_ && scratch == region_scratch_ && need <= region_work_len_) return 0;
+  cudaFree(d_region_work_);
+  d_region_work_ = nullptr;
+  region_work_len_ = 0;
+  if (cudaMalloc(reinterpret_cast<void **>(&d_region_work_), std::max<size_t>(need, 1) * sizeof(double)) != cudaSuccess) {
+    const cudaError_t err = cudaGetLastError();
+    d_region_work_ = nullptr;
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the region sums (%s)\n", cudaGetErrorString(err));
+    return 1;
+  }
+  region_scratch_ = scratch;
+  region_work_len_ = need;
+  return 0;
+}
+
+int Engine::ensure_region_stats() {
+  if (d_region_stats_) return 0;
+  const size_t bytes = std::max<size_t>(3 * region_len(), 1) * sizeof(double);
+  if (cudaMalloc(reinterpret_cast<void **>(&d_region_stats_), bytes) != cudaSuccess ||
+      cudaMemset(d_region_stats_, 0, bytes) != cudaSuccess) {
+    const cudaError_t err = cudaGetLastError();
+    cudaFree(d_region_stats_);
+    d_region_stats_ = nullptr;
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the region statistics (%s)\n", cudaGetErrorString(err));
+    return 1;
+  }
+  return 0;
+}
+
+int Engine::region_sums(const double *flux, int64_t narrays, double *out) {
+  PTB_CUDA_OK(launch_region_sums(flux, int64_t(bin_len()), stride_, nscores_, narrays, d_region_elems_,
+                                 d_region_starts_, region_levels_.data(), int(region_levels_.size()), d_region_work_,
+                                 region_scratch_, out, compute_));
+  return 0;
+}
+
+bool Engine::region_refused(int32_t tally, int32_t kind, int32_t max_kind, int64_t n) const {
+  const int64_t one = nregions_, all = int64_t(result_arrays()) * nscores_ * nregions_;
+  const char *why = nregions_ == 0                          ? "no regions are set (set_regions)"
+                    : (tally != 0 && tally != 1)            ? "tally must be 0 (track length) or 1 (collision)"
+                    : (tally == 1 && !collision_)           ? "the collision estimator is off (set_collision_estimator)"
+                    : (kind < 0 || kind > max_kind)         ? "kind out of range"
+                    : (n != one && n != all)                ? "n must be nregions or ntime * nbins * nscores * nregions"
+                                                            : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: region results refused: %s\n", why);
+  return why != nullptr;
+}
+
+int Engine::get_region_volumes(double *out, int64_t n) {
+  if (nregions_ == 0 || n != nregions_) {
+    fprintf(stderr, "[pumitally] ERROR: get_region_volumes: %s\n", nregions_ ? "n must be nregions" : "no regions are set");
+    return 1;
+  }
+  std::memcpy(out, region_volume_.data(), size_t(n) * sizeof(double));
+  return 0;
+}
+
+// The region sums of the open tally, read where copy_results reads it (flux_view(), after gather_shares()).  Kind 1
+// divides as normalize_scores does, sum / V_G / d: a one-element region gives get_normalized_flux's bits.
+int Engine::get_region_results(int32_t tally, int32_t kind, double *out, int64_t n) {
+  if (region_refused(tally, kind, 1, n)) return 1;
+  if (synchronize() || gather_shares() || ensure_region_work()) return 1;
+  double per_source = 1.0;
+  if (kind == 1 && !per_source_divisor(&per_source)) return 1;
+  const size_t R = size_t(result_arrays()), S = size_t(nscores_), G = size_t(nregions_);
+  double *d_out = d_region_work_ + region_scratch_;
+  if (region_sums(flux_view() + size_t(tally) * flux_len(), int64_t(R), d_out)) return 1;
+  const int64_t rows = n / int64_t(G);  // (r, k) pairs asked for: 1, or all of them
+  std::vector<double> sums(size_t(n) == G ? G * S : R * G * S);
+  PTB_CUDA_OK(cudaMemcpyAsync(sums.data(), d_out, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  const double *vol = region_volume_.data();
+#pragma omp parallel for schedule(static)
+  for (int64_t q = 0; q < rows; ++q) {  // [r][g][k] -> [r][k][g]
+    const size_t r = size_t(q) / S, k = size_t(q) % S;
+    const double *src = sums.data() + r * G * S + k;
+    double *dst = out + size_t(q) * G;
+    if (kind == 1)
+      for (size_t g = 0; g < G; ++g) dst[g] = src[g * S] / vol[g] / per_source;
+    else
+      for (size_t g = 0; g < G; ++g) dst[g] = src[g * S];
+  }
+  return 0;
+}
+
+int Engine::get_region_batch_results(int32_t tally, int32_t kind, double *out, int64_t n) {
+  if (region_refused(tally, kind, 2, n) || batch_refused(tally, kind)) return 1;
+  if (synchronize()) return 1;
+  const size_t R = size_t(result_arrays()), S = size_t(nscores_), G = size_t(nregions_), RL = region_len();
+  const size_t base = size_t(tally) * R * G * S;
+  double *d_out = nullptr;
+  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d_out), R * S * G * sizeof(double));
+  if (e == cudaSuccess)
+    e = launch_batch_readout(d_region_stats_ + RL + base, d_region_stats_ + 2 * RL + base, d_region_volume_,
+                             d_region_ident_, d_out, int64_t(G), int32_t(R), nscores_, nscores_, double(batches_), kind,
+                             compute_);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, compute_);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+  cudaFree(d_out);
+  if (e != cudaSuccess) {
+    fprintf(stderr, "[pumitally] CUDA error %s reading the region statistics\n", cudaGetErrorString(e));
+    return 1;
   }
   return 0;
 }

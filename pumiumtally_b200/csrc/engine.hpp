@@ -13,6 +13,7 @@
 
 #include <cuda_runtime.h>
 
+#include "batch_stats.cuh"
 #include "host_stage.hpp"
 #include "tet_mesh.hpp"
 #include "walk_kernels.hpp"
@@ -126,6 +127,17 @@ class Engine {
   int get_batch_results(int32_t tally, int32_t kind, double *out, int64_t n);
   // Largest relative error of score `score` over the results with a nonzero mean, and their number (device reduction).
   int get_batch_max_rel_err(int32_t tally, int32_t score, double *out_max, int64_t *out_nonzero);
+  // Region tallies (batch_stats.cuh, RegionPlan): region_of_element[n == E] in [-1, nregions) in the caller's numbering
+  // (-1: in no region), 1 <= nregions <= E; nullptr with nregions == 0 removes the regions.  Resets the tally, discards
+  // the folded batches; before comm_init.  Anything else is refused and changes nothing.
+  int set_regions(const int32_t *region_of_element, int64_t n, int32_t nregions);
+  int32_t regions() const { return nregions_; }
+  int get_region_volumes(double *out, int64_t n);  // n == nregions
+  // tally 0 track length, 1 collision; kind 0 the raw sum over each region, 1 sum / V_G / the per-source divisor;
+  // [time][bin][score][region] (n == nregions: time bin 0, bin 0, score 0).  Collective with several ranks, as get_flux.
+  int get_region_results(int32_t tally, int32_t kind, double *out, int64_t n);
+  // kinds 0-2 of get_batch_results for the region sums, folded by end_batch while regions are set; not collective
+  int get_region_batch_results(int32_t tally, int32_t kind, double *out, int64_t n);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -258,6 +270,25 @@ class Engine {
   bool batch_refused(int32_t tally, int32_t kind) const;  // with a message
   // the "<name>_mean" / "<name>_rel_err" arrays of the tally at `tally`, names prefixed
   int batch_arrays(int32_t tally, const std::string &prefix, VtkArrays &a);
+  // ---- region tallies (stats_kernels.cu, launch_region_sums) ----
+  int32_t nregions_ = 0;                           // 0: no regions
+  std::vector<RegionLevel> region_levels_;         // of the plan set_regions built
+  std::vector<double> region_volume_;              // [nregions_], summed in the plan's order
+  int32_t *d_region_elems_ = nullptr, *d_region_starts_ = nullptr;  // the plan's elems and starts
+  int32_t *d_region_ident_ = nullptr;              // [nregions_] 0, 1, ...: the readout's order map
+  double *d_region_volume_ = nullptr;              // [nregions_]
+  double *d_region_work_ = nullptr;                // scratch of launch_region_sums, then one tally's region sums
+  int64_t region_scratch_ = 0;                     // doubles of that scratch
+  size_t region_work_len_ = 0;                     // doubles at d_region_work_
+  double *d_region_stats_ = nullptr;               // [3 * region_len()]: the batch's sums, running mean, M2
+  // region results of every reported tally: [tally][time][bin][region][score]
+  size_t region_len() const { return (collision_ ? 2 : 1) * size_t(result_arrays()) * size_t(nregions_) * size_t(nscores_); }
+  void free_regions();
+  int ensure_region_work();   // d_region_work_ for the current layout
+  int ensure_region_stats();  // d_region_stats_ (zeroed when allocated: it is freed whenever the batches are discarded)
+  // the region sums of `narrays` result arrays from `flux` (the arrays of one or both tallies) into out, on compute_
+  int region_sums(const double *flux, int64_t narrays, double *out);
+  bool region_refused(int32_t tally, int32_t kind, int32_t max_kind, int64_t n) const;  // with a message
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
     void *d = nullptr;    // device copy

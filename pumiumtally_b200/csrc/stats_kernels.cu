@@ -95,6 +95,27 @@ __global__ void batch_max_rel_err_kernel(const double *__restrict__ mean, const 
   }
 }
 
+// One level of the region sums (batch_stats.cuh, chunk_sum): unit u = a * nchunks + c sums chunk c of array a, one
+// lane per score (2^lane_bits >= nscores lanes per unit), into out[u * nscores + k].  Input i of array a is the record
+// src + a * pitch + (idx ? idx[i] : i) * stride.  The lanes of a unit read one record together, and neighbouring units
+// take neighbouring chunks, so single-element regions read neighbouring records.
+__global__ void region_level_kernel(const double *__restrict__ src, const int32_t *__restrict__ idx, int64_t pitch,
+                                    int32_t stride, const int32_t *__restrict__ starts, int64_t nchunks,
+                                    int64_t narrays, int32_t nscores, int lane_bits, double *__restrict__ out) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x, u = t >> lane_bits;
+  const int k = int(t & ((1 << lane_bits) - 1));
+  if (u >= nchunks * narrays || k >= nscores) return;
+  const int64_t a = u / nchunks, c = u - a * nchunks;
+  const int32_t lo = __ldg(starts + c), hi = __ldg(starts + c + 1);
+  const double *s = src + a * pitch + k;
+  double acc[kMaxScores];
+  chunk_sum(hi - lo, 1, [&](int64_t i, int) {
+    const int64_t rec = idx ? int64_t(__ldg(idx + lo + i)) : lo + i;
+    return __ldg(s + rec * stride);
+  }, acc);
+  out[u * nscores + k] = acc[0];
+}
+
 unsigned grid_for(int64_t work, int block) {
   int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -135,6 +156,28 @@ cudaError_t launch_batch_max_rel_err(const double *mean, const double *m2, int64
   batch_max_rel_err_kernel<<<grid_for(n / stride + 1, block), block, 0, stream>>>(mean, m2, n, goff, base, len, stride,
                                                                                   score, nb, red);
   return cudaGetLastError();
+}
+
+cudaError_t launch_region_sums(const double *flux, int64_t array_len, int32_t stride, int32_t nscores, int64_t narrays,
+                               const int32_t *elems, const int32_t *starts, const RegionLevel *levels, int nlevels,
+                               double *scratch, int64_t scratch_len, double *out, cudaStream_t stream) {
+  if (narrays <= 0 || nlevels <= 0) return cudaSuccess;
+  const int block = 256;
+  int lane_bits = 0;
+  while ((1 << lane_bits) < nscores) ++lane_bits;
+  const double *src = flux;
+  for (int l = 0; l < nlevels; ++l) {
+    const RegionLevel &v = levels[l];
+    double *dst = l + 1 == nlevels ? out : scratch + (l & 1) * (scratch_len / 2);
+    const int64_t n = (v.chunks * narrays) << lane_bits;
+    region_level_kernel<<<unsigned((n + block - 1) / block), block, 0, stream>>>(
+        src, l == 0 ? elems : nullptr, l == 0 ? array_len : v.inputs * nscores, l == 0 ? stride : nscores,
+        starts + v.start_off, v.chunks, narrays, nscores, lane_bits, dst);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    src = dst;
+  }
+  return cudaSuccess;
 }
 
 }  // namespace ptb

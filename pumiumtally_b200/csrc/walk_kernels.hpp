@@ -156,5 +156,13 @@ cudaError_t launch_batch_readout(const double *mean, const double *m2, const dou
 cudaError_t launch_batch_max_rel_err(const double *mean, const double *m2, int64_t n, int64_t goff, int64_t base,
                                      int64_t len, int32_t stride, int32_t score, double nb, unsigned long long *red,
                                      cudaStream_t stream);
+// Region sums (batch_stats.cuh, RegionPlan) of the m0 slots [0, nscores) of narrays result arrays [a][E][stride] at
+// flux (array a at flux + a * array_len), over a plan's levels[nlevels] with its elems and starts on the device:
+// out[(a * nregions + g) * nscores + k] is the sum of score k of array a over region g.  scratch holds
+// region_scratch_len doubles (scratch_len), which may be 0 with one level.
+struct RegionLevel;
+cudaError_t launch_region_sums(const double *flux, int64_t array_len, int32_t stride, int32_t nscores, int64_t narrays,
+                               const int32_t *elems, const int32_t *starts, const RegionLevel *levels, int nlevels,
+                               double *scratch, int64_t scratch_len, double *out, cudaStream_t stream);
 
 }  // namespace ptb

@@ -76,6 +76,11 @@ C_API = {
     "pumitally_end_batch": (C.c_int, [C.c_void_p]),
     "pumitally_get_batch_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
     "pumitally_get_batch_max_rel_err": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.POINTER(C.c_int64)]),
+    "pumitally_set_regions": (C.c_int, [C.c_void_p, _ip, C.c_int64, C.c_int32]),
+    "pumitally_get_regions": (C.c_int32, [C.c_void_p]),
+    "pumitally_get_region_volumes": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pumitally_get_region_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
+    "pumitally_get_region_batch_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -582,6 +587,48 @@ class PumiTally:
         if self._L.pumitally_get_batch_max_rel_err(self._h, int(tally), int(score), C.byref(mx), C.byref(cnt)):
             raise RuntimeError(f"get_batch_max_rel_err({tally}, {score}) failed")
         return mx.value, cnt.value
+
+    # ---- region tallies ------------------------------------------------------------
+    def set_regions(self, region_of_element, nregions=None):
+        """Group the elements into regions: region_of_element[e] in [-1, nregions) for every element (caller's
+        numbering; -1: in no region).  nregions None: max + 1.  None as the map removes the regions.  Resets the
+        tally and discards the folded batches."""
+        if region_of_element is None:
+            rc = self._L.pumitally_set_regions(self._h, None, 0, 0)
+        else:
+            m = np.ascontiguousarray(region_of_element, dtype=np.int32).reshape(-1)
+            if nregions is None:
+                nregions = int(m.max()) + 1 if m.size else 0
+            rc = self._L.pumitally_set_regions(self._h, m.ctypes.data_as(_ip), m.size, int(nregions))
+        if rc:
+            raise ValueError("set_regions failed")
+
+    @property
+    def regions(self) -> int:
+        """Number of regions, 0 without regions."""
+        return int(self._L.pumitally_get_regions(self._h))
+
+    def region_volumes(self):
+        out = np.empty(self.regions)
+        if self._L.pumitally_get_region_volumes(self._h, out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError("get_region_volumes failed")
+        return out
+
+    def _region_call(self, fn, tally, kind, what):
+        out = np.empty((max(self.time_bins, 1), self.score_bins, self.scores, self.regions))
+        if fn(self._h, int(tally), int(kind), out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError(f"{what}({tally}, {kind}) failed")
+        return out
+
+    def region_results(self, tally=0, kind=1):
+        """tally 0 track length, 1 collision; kind 0 raw sum over each region, 1 sum / region volume / per-source
+        divisor: [ntime, nbins, nscores, nregions]."""
+        return self._region_call(self._L.pumitally_get_region_results, tally, kind, "get_region_results")
+
+    def region_batch_results(self, tally=0, kind=0):
+        """kind 0 mean, 1 standard error (both / region volume), 2 relative error of the region sums over the
+        batches: [ntime, nbins, nscores, nregions]."""
+        return self._region_call(self._L.pumitally_get_region_batch_results, tally, kind, "get_region_batch_results")
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
