@@ -130,6 +130,20 @@ inline int GetRegionBatchResults(const PumiTally &tally, int32_t which, int32_t 
   return pumitally_get_region_batch_results(engine_of(tally), which, kind, out, n);
 }
 
+// Checkpoints (see pumitally_save_checkpoint in pumitally_c.h): SaveCheckpoint writes the tally state and the batch
+// statistics to a file atomically; LoadCheckpoint restores them into an engine set up with the same configuration;
+// MergeCheckpoint adds another run's folded batches.  No particle state is saved: after LoadCheckpoint, call
+// CopyInitialPosition before the next move.  A refusal returns 1 and changes nothing.
+inline int SaveCheckpoint(const PumiTally &tally, const char *path) {
+  return pumitally_save_checkpoint(engine_of(tally), path);
+}
+inline int LoadCheckpoint(const PumiTally &tally, const char *path) {
+  return pumitally_load_checkpoint(engine_of(tally), path);
+}
+inline int MergeCheckpoint(const PumiTally &tally, const char *path) {
+  return pumitally_merge_checkpoint(engine_of(tally), path);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

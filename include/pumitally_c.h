@@ -470,6 +470,37 @@ int pumitally_get_region_volumes(pumitally_engine *e, double *out, int64_t n);
 int pumitally_get_region_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
 int pumitally_get_region_batch_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
 
+/* ---- additive: checkpoints (save the tally state to a file, restart from it, merge independent runs) ----
+ * A checkpoint holds the engine's tally state: the open batch (the raw tally, the first-track weight, the collision
+ * counters, the pumitally_get_stats counts and the move counters), included only when something was moved, collided
+ * or localised since the last reset (right after pumitally_end_batch it is the statistics alone); and, while batch
+ * statistics are on, the number of folded batches, this rank's running mean and M2 of every reported double and the
+ * region statistics.  It also holds a fingerprint of everything their layout and meaning depend on: the mesh (counts
+ * and a hash of coordinates and t2v), the internal element order, score bins, scores, time-bin edges (bit for bit),
+ * moment order, collision estimator, batch statistics on/off, the region map, the source-normalisation mode (and its
+ * value in mode 2), and rank, number of ranks and rank share.  It holds no particle state, kernel or host-path option,
+ * timer or output name: after a load the caller places the particles (CopyInitialPosition, as OpenMC does at every
+ * batch start) before the next move.  All three calls return 0 on success; a refusal returns 1, prints the reason and
+ * changes nothing in the engine.  None is collective: with several ranks every rank saves, loads or merges its own
+ * share under a path the caller makes unique per rank (the region statistics, the same on every rank, are in each).
+ * pumitally_save_checkpoint(e, path) synchronises, writes path + ".tmp", flushes, fsyncs and renames it over path: a
+ * failed or killed save leaves the previous file at path intact.  It changes nothing in the engine, and the same state
+ * always gives the same bytes.
+ * pumitally_load_checkpoint(e, path) replaces the tally state with the file's.  It never reconfigures: set up the
+ * configuration the file was saved with first (then pumitally_comm_init with several ranks, which discards folded
+ * batches), then load.  The header and fingerprint are checked before anything is allocated; every section is
+ * checked against its CRC-32 before the engine's buffers are replaced.
+ * pumitally_merge_checkpoint(e, path) adds the file's folded batches to the engine's (Chan's parallel update of mean
+ * and M2, on the device; element and region statistics): B becomes B_a + B_b.  It needs batch statistics on and the
+ * same fingerprint, except the mode-2 normalisation value (the folded values are already per source), and refuses a
+ * file that holds an open batch (save it at a batch end).  The engine's open batch, particles and counters are left
+ * alone.
+ * Device memory: load and merge hold a second copy of what they read until the swap or the merge is done, up to
+ * 2 * (statistics doubles) + (tally doubles); when that cannot be allocated they refuse. */
+int pumitally_save_checkpoint(pumitally_engine *e, const char *path);
+int pumitally_load_checkpoint(pumitally_engine *e, const char *path);
+int pumitally_merge_checkpoint(pumitally_engine *e, const char *path);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

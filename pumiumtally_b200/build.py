@@ -26,6 +26,7 @@ SOURCES = [
     "stats_kernels.cu",
     "l2_partitions.cu",
     "engine.cu",
+    "checkpoint.cpp",
     "host_stage.cpp",
     "tet_mesh.cpp",
     "osh_reader.cpp",

@@ -22,6 +22,16 @@ PTB_HD void welford_fold(double x, double nb, double &mean, double &m2) {
   m2 += d * (x - mean);
 }
 
+// Combines the statistics (mean_b, m2_b) of nb batches into (mean, m2) of na other batches (Chan et al.'s parallel
+// update): with n = na + nb and d = mean_b - mean, mean + d (nb / n) and m2 + m2_b + d^2 na nb / n.  An empty side
+// gives the other side's values bit for bit (engine.cu, merge_checkpoint).
+PTB_HD void welford_merge(double mean_b, double m2_b, double na, double nb, double &mean, double &m2) {
+  const double n = na + nb, d = mean_b - mean;
+  const double mu = mean + d * (nb / n), q = m2 + m2_b + d * d * (na * nb / n);
+  mean = nb == 0.0 ? mean : na == 0.0 ? mean_b : mu;
+  m2 = nb == 0.0 ? m2 : na == 0.0 ? m2_b : q;
+}
+
 // Standard error of the mean of nb >= 2 batches: sqrt(m2 / (nb (nb - 1))).
 PTB_HD double batch_std_err(double m2, double nb) { return sqrt(m2 / (nb * (nb - 1.0))); }
 

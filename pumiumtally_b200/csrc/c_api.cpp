@@ -305,6 +305,19 @@ int pumitally_get_region_batch_results(pumitally_engine *e, int32_t tally, int32
   return guarded(e, [&](ptb::Engine &g) { return g.get_region_batch_results(tally, kind, out, n); });
 }
 
+int pumitally_save_checkpoint(pumitally_engine *e, const char *path) {
+  if (!path) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.save_checkpoint(path); });
+}
+int pumitally_load_checkpoint(pumitally_engine *e, const char *path) {
+  if (!path) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.load_checkpoint(path); });
+}
+int pumitally_merge_checkpoint(pumitally_engine *e, const char *path) {
+  if (!path) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.merge_checkpoint(path); });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

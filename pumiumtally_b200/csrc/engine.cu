@@ -2,13 +2,16 @@
 #include "engine.hpp"
 
 #include <sys/mman.h>
+#include <sys/stat.h>
 #include <sys/syscall.h>
 #include <unistd.h>
 
 #include <algorithm>
 #include <atomic>
+#include <cerrno>
 #include <chrono>
 #include <climits>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -522,6 +525,7 @@ int Engine::copy_initial_position(const double *xyz, int32_t size) {
   }
   PTB_CUDA_OK(cudaMemcpyAsync(d_xyz, src, size_t(size) * sizeof(double), cudaMemcpyHostToDevice, compute_));
   h2d_bytes_ += double(size) * sizeof(double);
+  tallied_ = true;  // the localisation walk counts relocations and lost walks
   move_variant_ = variant_;
   move_tag_ = -1;
   if (launch_range(d_xyz, nullptr, nullptr, nullptr, 0, n_, compute_)) return 1;
@@ -536,6 +540,7 @@ int Engine::copy_initial_position_device(const double *d_xyz, int32_t size, cuda
     return 1;
   }
   PTB_CUDA_OK(cudaSetDevice(device_));
+  tallied_ = true;  // the localisation walk counts relocations and lost walks
   move_variant_ = variant_;
   move_tag_ = -1;
   if (launch_range(d_xyz, nullptr, nullptr, nullptr, 0, n_, stream)) return 1;
@@ -680,6 +685,7 @@ int Engine::ensure_patch_buffers(int nchunks, int32_t chunk) {
 int Engine::move_to_next_location(const Move &m) {
   if (move_refused(m, false)) return 1;
   PTB_CUDA_OK(cudaSetDevice(device_));
+  tallied_ = true;
   const MoveTally &t = m.tally;
   const size_t N = size_t(n_);
   MoveTally dev;  // t with the device copies of its arrays
@@ -1094,6 +1100,7 @@ bool Engine::move_refused(const Move &m, bool device) const {
 int Engine::move_to_next_location_device(const Move &m, cudaStream_t stream) {
   if (move_refused(m, true)) return 1;
   PTB_CUDA_OK(cudaSetDevice(device_));
+  tallied_ = true;
   const bool scored = scored_move(m.tally);
   begin_move(scored);
   // (the staging arrays are not touched: "pinned dest slots == device dest array" keeps holding, and the
@@ -1531,7 +1538,7 @@ int Engine::reset_tally() {
   scored_moves_ = 0;
   PTB_CUDA_OK(cudaMemset(d_stats_, 0, sizeof(DeviceStats)));
   PTB_CUDA_OK(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)));
-  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = tallied_ = false;
   kernel_ms_ = 0.0;
   h2d_bytes_ = 0.0;
   moves_ = 0;
@@ -2079,6 +2086,7 @@ int Engine::tally_collisions(const double *xyz, int64_t nevents, const double *w
   const CollisionParams p = collision_params();
   const double *t = ntime_ > 0 ? times : nullptr;
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on, as with a move
+  tallied_ = true;
   for (int64_t b = 0; b < nevents; b += chunk) {
     const size_t cnt = size_t(std::min(chunk, nevents - b));
     PTB_CUDA_OK(upload(d.xyz, xyz + 3 * b, 3 * cnt * sizeof(double), compute_));
@@ -2105,6 +2113,7 @@ int Engine::tally_collisions_device(const double *d_xyz, int64_t nevents, const 
   const CollisionParams p = collision_params();
   const size_t S = size_t(nscores_);
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  tallied_ = true;
   const int64_t step = int64_t(1) << 30;  // events per launch
   for (int64_t b = 0; b < nevents; b += step)
     PTB_CUDA_OK(launch_collide_located(l, p, d_xyz + 3 * b, std::min(step, nevents - b), d_weights + b,
@@ -2130,6 +2139,7 @@ int Engine::tally_collisions_at_particles(const int8_t *collided, const double *
   const double *t = ntime_ > 0 ? times : nullptr;
   if (follow_last_stream(compute_)) return 1;  // reads the particle state the last move wrote
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  tallied_ = true;
   for (int32_t b = 0; b < n; b += chunk) {
     const size_t cnt = size_t(std::min(chunk, n - b));
     PTB_CUDA_OK(upload(d.collided, collided + b, cnt, compute_));
@@ -2156,6 +2166,7 @@ int Engine::tally_collisions_at_particles_device(const int8_t *d_collided, const
   PTB_CUDA_OK(cudaSetDevice(device_));
   if (follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  tallied_ = true;
   PTB_CUDA_OK(launch_collide_particles(d_state_, d_collided, n, collision_params(), d_weights, d_responses, d_bins,
                                        ntime_ > 0 ? d_times : nullptr, d_coll_counts_, stream));
   return 0;
@@ -2483,6 +2494,7 @@ int Engine::set_regions(const int32_t *region_of_element, int64_t n, int32_t nre
     return 1;
   }
   free_regions();
+  region_hash_ = remove ? 0 : ckpt::hash64(region_of_element, size_t(E) * sizeof(int32_t), uint64_t(nregions));
   if (!remove) {
     nregions_ = nregions;
     region_levels_ = plan.levels;
@@ -2604,6 +2616,354 @@ int Engine::get_region_batch_results(int32_t tally, int32_t kind, double *out, i
     fprintf(stderr, "[pumitally] CUDA error %s reading the region statistics\n", cudaGetErrorString(e));
     return 1;
   }
+  return 0;
+}
+
+// ------------------------------------------------------------------ checkpoints
+
+namespace {
+
+constexpr size_t kCheckpointChunk = size_t(64) << 20;  // bytes per pinned chunk buffer; two per call
+
+// The two pinned chunk buffers of one save, load or merge, each with the event of its last device copy.
+struct ChunkBuffers {
+  void *h[2] = {nullptr, nullptr};
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  size_t bytes = 0;
+  bool ok = true;
+  explicit ChunkBuffers(size_t b) : bytes(b) {
+    for (int i = 0; i < 2; ++i)
+      ok = ok && cudaHostAlloc(&h[i], b, cudaHostAllocDefault) == cudaSuccess &&
+           cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) == cudaSuccess;
+    if (!ok) cudaGetLastError();
+  }
+  ~ChunkBuffers() {
+    for (int i = 0; i < 2; ++i) {
+      if (h[i]) cudaFreeHost(h[i]);
+      if (ev[i]) cudaEventDestroy(ev[i]);
+    }
+  }
+};
+
+// chunk size for sections of at most `largest` bytes: no 128 MB of pinned memory for a small tally
+size_t chunk_bytes_for(uint64_t largest) {
+  return size_t(std::max<uint64_t>(4096, std::min<uint64_t>(kCheckpointChunk, largest)));
+}
+
+}  // namespace
+
+ckpt::Fingerprint Engine::fingerprint() {
+  const size_t E = size_t(mesh_.ntets);
+  if (!mesh_hashed_) {  // computed once: the mesh never changes
+    std::vector<int32_t> t2v(4 * E);  // in the caller's numbering
+    for (size_t i = 0; i < E; ++i)
+      std::memcpy(&t2v[4 * size_t(mesh_.orig_of_internal[i])], &mesh_.t2v[4 * i], 4 * sizeof(int32_t));
+    mesh_hash_ = ckpt::hash64(t2v.data(), t2v.size() * sizeof(int32_t),
+                              ckpt::hash64(mesh_.coords.data(), mesh_.coords.size() * sizeof(double)));
+    order_hash_ = ckpt::hash64(mesh_.orig_of_internal.data(), E * sizeof(int32_t));
+    mesh_hashed_ = true;
+  }
+  ckpt::Fingerprint f;
+  f.nelems = mesh_.ntets;
+  f.nverts = mesh_.nverts;
+  f.mesh_hash = mesh_hash_;
+  f.order_hash = order_hash_;
+  f.nbins = nbins_;
+  f.nscores = nscores_;
+  f.stride = stride_;
+  f.moments = moments_;
+  f.collision = collision_ ? 1 : 0;
+  f.batch_stats = batch_stats_ ? 1 : 0;
+  f.nregions = nregions_;
+  f.region_hash = region_hash_;
+  f.norm_mode = norm_mode_;
+  f.norm_value = norm_mode_ == 2 ? norm_value_ : 0.0;
+  f.rank = sharded() ? rank_ : 0;
+  f.nranks = sharded() ? nranks_ : 1;
+  f.share = sharded() ? share_ : 0;
+  if (ntime_ > 0) {
+    f.edges.resize(size_t(ntime_) + 1);
+    if (cudaMemcpy(f.edges.data(), d_edges_, f.edges.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess)
+      f.edges.assign(f.edges.size(), std::nan(""));  // (compares unequal to every file's edges)
+  }
+  return f;
+}
+
+int Engine::save_checkpoint(const std::string &path) {
+  if (synchronize()) return 1;
+  auto refuse = [&](const std::string &why) {
+    fprintf(stderr, "[pumitally] ERROR: save_checkpoint: %s: %s\n", path.c_str(), why.c_str());
+    return 1;
+  };
+  const ckpt::Fingerprint f = fingerprint();
+  ckpt::Header h;
+  const size_t RL = batch_stats_ && nregions_ ? region_len() : 0;
+  h.batches = batch_stats_ ? batches_ : 0;
+  h.open = tallied_ ? 1 : 0;
+  h.open_len = tallied_ ? reported_len() : 0;
+  h.stats_len = batch_stats_ ? stats_len() : 0;
+  h.region_len = RL;
+  std::vector<uint8_t> scalars;
+  if (tallied_) {
+    ckpt::OpenScalars s;
+    DeviceStats ds;
+    unsigned long long cc[3];
+    PTB_CUDA_OK(cudaMemcpy(&s.initial_weight, d_initial_weight_, sizeof(double), cudaMemcpyDeviceToHost));
+    PTB_CUDA_OK(cudaMemcpy(&ds, d_stats_, sizeof(ds), cudaMemcpyDeviceToHost));
+    PTB_CUDA_OK(cudaMemcpy(cc, d_coll_counts_, sizeof(cc), cudaMemcpyDeviceToHost));
+    s.initial_weight_pending = initial_weight_pending_ ? 1 : 0;
+    for (int i = 0; i < 3; ++i) s.coll_counts[i] = cc[i];
+    s.segments = ds.segments;
+    s.tracks = ds.tracks;
+    s.relocations = ds.relocations;
+    s.lost = ds.lost;
+    s.fallbacks = ds.fallbacks;
+    s.moves = moves_;
+    s.scored_moves = scored_moves_;
+    scalars = ckpt::pack_open_scalars(s);
+  }
+  // the arrays of the sections, in file order (nullptr: zeros -- region statistics before the first end_batch)
+  struct Src { uint32_t id; const double *d; const uint8_t *host; uint64_t bytes; };
+  std::vector<Src> src;
+  if (h.open) {
+    src.push_back({ckpt::kOpenTally, d_flux_, nullptr, 8 * h.open_len});
+    src.push_back({ckpt::kOpenScalars, nullptr, scalars.data(), scalars.size()});
+  }
+  if (h.stats_len) {
+    src.push_back({ckpt::kMean, d_mean_, nullptr, 8 * h.stats_len});
+    src.push_back({ckpt::kM2, d_m2_, nullptr, 8 * h.stats_len});
+  }
+  if (RL) {
+    src.push_back({ckpt::kRegionMean, d_region_stats_ ? d_region_stats_ + RL : nullptr, nullptr, 8 * RL});
+    src.push_back({ckpt::kRegionM2, d_region_stats_ ? d_region_stats_ + 2 * RL : nullptr, nullptr, 8 * RL});
+  }
+  uint64_t largest = 0;
+  for (const Src &s : src) largest = std::max(largest, s.bytes);
+  ChunkBuffers buf(chunk_bytes_for(largest));
+  if (!buf.ok) return refuse("no pinned host memory for the chunk buffers");
+  const std::string tmp = path + ".tmp";
+  FILE *fp = std::fopen(tmp.c_str(), "wb");
+  if (!fp) return refuse(std::string("cannot create ") + tmp + " (" + std::strerror(errno) + ")");
+  ckpt::Writer w([&](const void *p, size_t n) { return std::fwrite(p, 1, n, fp) == n; },
+                 [&](uint64_t off, const void *p, size_t n) {
+                   return fseeko(fp, off_t(off), SEEK_SET) == 0 && std::fwrite(p, 1, n, fp) == n &&
+                          fseeko(fp, 0, SEEK_END) == 0;
+                 });
+  bool ok = w.begin(h, f);
+  for (const Src &s : src) {
+    if (!ok) break;
+    const size_t C = buf.bytes;
+    // Chunk k + 1 is copied into the other buffer (whose chunk k - 1 has been written) while chunk k is checksummed
+    // and written.
+    auto issue = [&](size_t k) {
+      const uint64_t off = uint64_t(k) * C;
+      if (off >= s.bytes) return true;
+      const size_t n = size_t(std::min<uint64_t>(C, s.bytes - off));
+      if (!s.d) {
+        std::memset(buf.h[k & 1], 0, n);
+        return true;
+      }
+      return cudaMemcpyAsync(buf.h[k & 1], reinterpret_cast<const char *>(s.d) + off, n, cudaMemcpyDeviceToHost,
+                             copy_) == cudaSuccess &&
+             cudaEventRecord(buf.ev[k & 1], copy_) == cudaSuccess;
+    };
+    if (s.host) {
+      ok = w.section(s.id, s.bytes, C, [&](size_t, uint64_t off, size_t) -> const void * { return s.host + off; });
+    } else {
+      ok = w.section(s.id, s.bytes, C, [&](size_t k, uint64_t, size_t) -> const void * {
+        if ((k == 0 && !issue(0)) || !issue(k + 1)) return nullptr;
+        if (s.d && cudaEventSynchronize(buf.ev[k & 1]) != cudaSuccess) return nullptr;
+        return buf.h[k & 1];
+      });
+    }
+  }
+  cudaStreamSynchronize(copy_);  // (nothing may still be copying into the buffers when they are freed)
+  std::string why = ok ? "" : (w.error().empty() ? "write failed" : w.error());
+  if (ok && (std::fflush(fp) != 0 || fsync(fileno(fp)) != 0)) {
+    ok = false;
+    why = std::string("flush failed (") + std::strerror(errno) + ")";
+  }
+  if (std::fclose(fp) != 0 && ok) {
+    ok = false;
+    why = std::string("close failed (") + std::strerror(errno) + ")";
+  }
+  if (ok && std::rename(tmp.c_str(), path.c_str()) != 0) {
+    ok = false;
+    why = std::string("cannot rename ") + tmp + " (" + std::strerror(errno) + ")";
+  }
+  if (!ok) {
+    std::remove(tmp.c_str());
+    cudaGetLastError();
+    return refuse(why);
+  }
+  return 0;
+}
+
+int Engine::load_checkpoint(const std::string &path) { return read_checkpoint(path, false); }
+int Engine::merge_checkpoint(const std::string &path) { return read_checkpoint(path, true); }
+
+// Load: every section arrives in new device buffers, which replace the engine's only once all of them arrived intact.
+// Merge: the file's statistics arrive in device scratch and are merged into the engine's by one launch per array.
+int Engine::read_checkpoint(const std::string &path, bool merge) {
+  const char *what = merge ? "merge_checkpoint" : "load_checkpoint";
+  auto refuse = [&](const std::string &why) {
+    fprintf(stderr, "[pumitally] ERROR: %s: %s: %s\n", what, path.c_str(), why.c_str());
+    return 1;
+  };
+  if (merge && !batch_stats_) return refuse("batch statistics are off (set_batch_statistics)");
+  if (synchronize()) return 1;
+  FILE *fp = std::fopen(path.c_str(), "rb");
+  if (!fp) return refuse(std::strerror(errno));
+  std::unique_ptr<FILE, int (*)(FILE *)> closer(fp, std::fclose);
+  struct stat st;
+  if (fstat(fileno(fp), &st) != 0 || !S_ISREG(st.st_mode)) return refuse("not a regular file");
+  ckpt::Reader r([&](void *p, size_t n) { return std::fread(p, 1, n, fp) == n; }, uint64_t(st.st_size));
+  ckpt::Header h;
+  ckpt::Fingerprint ff;
+  if (!r.begin(&h, &ff)) return refuse(r.error());
+  if (const char *field = ckpt::fingerprint_mismatch(fingerprint(), ff, merge))
+    return refuse(std::string("the checkpoint differs from this engine in: ") + field);
+  const size_t SL = batch_stats_ ? stats_len() : 0, RL = batch_stats_ && nregions_ ? region_len() : 0;
+  if (h.stats_len != SL || h.region_len != RL || (h.open && h.open_len != reported_len()) ||
+      (!batch_stats_ && h.batches != 0))
+    return refuse("the declared lengths do not match this engine's configuration");
+  if (merge && h.open)
+    return refuse("the checkpoint holds an open batch, which a merge would drop (save at a batch end)");
+  // new buffers: the open tally (whole allocation, zero past the reported part), the statistics, the region statistics
+  // (load: the engine's [sums][mean][M2] layout; merge: [mean][M2] scratch)
+  double *nflux = nullptr, *nmean = nullptr, *nm2 = nullptr, *nreg = nullptr;
+  auto release = [&] {
+    cudaFree(nflux);
+    cudaFree(nmean);
+    cudaFree(nm2);
+    cudaFree(nreg);
+    cudaGetLastError();
+  };
+  auto alloc = [&](double **p, size_t n) {
+    return cudaMalloc(reinterpret_cast<void **>(p), std::max<size_t>(n, 1) * sizeof(double)) == cudaSuccess &&
+           cudaMemset(*p, 0, std::max<size_t>(n, 1) * sizeof(double)) == cudaSuccess;
+  };
+  const size_t reg_off = merge ? 0 : RL;  // where the region means go in nreg
+  if ((!merge && h.open && !alloc(&nflux, flux_alloc_)) || (SL && (!alloc(&nmean, SL) || !alloc(&nm2, SL))) ||
+      (RL && !alloc(&nreg, (merge ? 2 : 3) * RL))) {
+    release();
+    return refuse("no device memory for a second copy of the checkpoint's arrays");
+  }
+  std::vector<uint8_t> scalars(8 * ckpt::kOpenScalarWords);
+  struct Dst { uint32_t id; double *d; uint64_t bytes; };
+  std::vector<Dst> dst;
+  if (h.open) {
+    dst.push_back({ckpt::kOpenTally, nflux, 8 * h.open_len});
+    dst.push_back({ckpt::kOpenScalars, nullptr, scalars.size()});
+  }
+  if (SL) {
+    dst.push_back({ckpt::kMean, nmean, 8 * SL});
+    dst.push_back({ckpt::kM2, nm2, 8 * SL});
+  }
+  if (RL) {
+    dst.push_back({ckpt::kRegionMean, nreg + reg_off, 8 * RL});
+    dst.push_back({ckpt::kRegionM2, nreg + reg_off + RL, 8 * RL});
+  }
+  uint64_t largest = 0;
+  for (const Dst &d : dst) largest = std::max(largest, d.bytes);
+  bool ok = true;
+  std::string why;
+  {
+    ChunkBuffers buf(chunk_bytes_for(largest));
+    if (!buf.ok) {
+      ok = false;
+      why = "no pinned host memory for the chunk buffers";
+    }
+    for (const Dst &d : dst) {
+      if (!ok) break;
+      if (!d.d) {
+        ok = r.section(d.id, d.bytes, buf.bytes, [&](size_t) -> void * { return scalars.data(); },
+                       [](size_t, uint64_t, const void *, size_t) { return true; });
+      } else {
+        // chunk k is read into the buffer whose last copy (chunk k - 2, or a chunk of the section before) has finished;
+        // its own copy then overlaps the reading and checksumming of chunk k + 1
+        ok = r.section(
+            d.id, d.bytes, buf.bytes,
+            [&](size_t k) -> void * {
+              return cudaEventSynchronize(buf.ev[k & 1]) == cudaSuccess ? buf.h[k & 1] : nullptr;
+            },
+            [&](size_t k, uint64_t off, const void *p, size_t n) {
+              return cudaMemcpyAsync(reinterpret_cast<char *>(d.d) + off, p, n, cudaMemcpyHostToDevice, copy_) ==
+                         cudaSuccess &&
+                     cudaEventRecord(buf.ev[k & 1], copy_) == cudaSuccess;
+            });
+      }
+      if (!ok) why = r.error();
+    }
+    if (cudaStreamSynchronize(copy_) != cudaSuccess && ok) {
+      ok = false;
+      why = "a copy to the device failed";
+    }
+  }
+  ckpt::OpenScalars sc;
+  if (ok && !r.at_end()) {
+    ok = false;
+    why = "data after the last section";
+  }
+  if (ok && h.open && !ckpt::unpack_open_scalars(scalars.data(), scalars.size(), &sc)) {
+    ok = false;
+    why = "corrupt open-batch counters";
+  }
+  if (ok && merge && RL && ensure_region_stats()) {
+    ok = false;
+    why = "no device memory for the region statistics";
+  }
+  if (!ok) {
+    release();
+    return refuse(why);
+  }
+  if (merge) {  // in place, (na, nb) -> na + nb batches; a file of no batches changes nothing
+    if (h.batches > 0) {
+      const double na = double(batches_), nb = double(h.batches);
+      cudaError_t e = launch_batch_merge(nmean, nm2, d_mean_, d_m2_, int64_t(SL), na, nb, compute_);
+      if (e == cudaSuccess && RL)
+        e = launch_batch_merge(nreg, nreg + RL, d_region_stats_ + RL, d_region_stats_ + 2 * RL, int64_t(RL), na, nb,
+                               compute_);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+      release();
+      PTB_CUDA_OK(e);
+      batches_ += h.batches;
+    } else {
+      release();
+    }
+    return 0;
+  }
+  // load: swap the new state in
+  if (h.open) {
+    cudaFree(d_flux_);
+    d_flux_ = nflux;
+    nflux = nullptr;
+  } else {
+    PTB_CUDA_OK(cudaMemset(d_flux_, 0, flux_alloc_ * sizeof(double)));  // (sc: a reset tally's counters)
+  }
+  if (SL) {
+    cudaFree(d_mean_);
+    cudaFree(d_m2_);
+    d_mean_ = nmean;
+    d_m2_ = nm2;
+    nmean = nm2 = nullptr;
+  }
+  if (RL) {
+    cudaFree(d_region_stats_);
+    d_region_stats_ = nreg;
+    nreg = nullptr;
+  }
+  batches_ = h.batches;
+  DeviceStats ds{sc.segments, sc.tracks, sc.relocations, sc.lost, sc.fallbacks};
+  const unsigned long long cc[3] = {sc.coll_counts[0], sc.coll_counts[1], sc.coll_counts[2]};
+  PTB_CUDA_OK(cudaMemcpy(d_initial_weight_, &sc.initial_weight, sizeof(double), cudaMemcpyHostToDevice));
+  PTB_CUDA_OK(cudaMemcpy(d_stats_, &ds, sizeof(ds), cudaMemcpyHostToDevice));
+  PTB_CUDA_OK(cudaMemcpy(d_coll_counts_, cc, sizeof(cc), cudaMemcpyHostToDevice));
+  initial_weight_pending_ = sc.initial_weight_pending != 0;
+  moves_ = sc.moves;
+  scored_moves_ = sc.scored_moves;
+  tallied_ = h.open != 0;
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
   return 0;
 }
 

@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 
 #include "batch_stats.cuh"
+#include "checkpoint.hpp"
 #include "host_stage.hpp"
 #include "tet_mesh.hpp"
 #include "walk_kernels.hpp"
@@ -138,6 +139,17 @@ class Engine {
   int get_region_results(int32_t tally, int32_t kind, double *out, int64_t n);
   // kinds 0-2 of get_batch_results for the region sums, folded by end_batch while regions are set; not collective
   int get_region_batch_results(int32_t tally, int32_t kind, double *out, int64_t n);
+  // Checkpoints (checkpoint.hpp): the tally state -- the open batch, if anything was tallied since the last reset, and
+  // the batch statistics (element and region) -- with a fingerprint of the configuration.  No particle state: after a
+  // load the caller places the particles (CopyInitialPosition) before the next move.  Save changes nothing in the
+  // engine and writes path + ".tmp", then renames it over path.  Load replaces the tally state after the same
+  // configuration was set up (and comm_init, with several ranks); merge adds the file's folded batches to this
+  // engine's (batch statistics on, no open batch in the file) and leaves the open batch alone.  Both refuse a
+  // different fingerprint, a corrupt or truncated file, or too little device memory for a second copy of what they
+  // read (up to 2 stats_len() + reported_len() doubles), and then change nothing.  Not collective.
+  int save_checkpoint(const std::string &path);
+  int load_checkpoint(const std::string &path);
+  int merge_checkpoint(const std::string &path);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -289,6 +301,14 @@ class Engine {
   // the region sums of `narrays` result arrays from `flux` (the arrays of one or both tallies) into out, on compute_
   int region_sums(const double *flux, int64_t narrays, double *out);
   bool region_refused(int32_t tally, int32_t kind, int32_t max_kind, int64_t n) const;  // with a message
+  uint64_t region_hash_ = 0;                       // of the map set_regions took (caller's numbering), 0 without
+  // ---- checkpoints (checkpoint.hpp) ----
+  bool tallied_ = false;  // a move, collision or localisation since the last reset: a checkpoint holds the open batch
+  bool mesh_hashed_ = false;
+  uint64_t mesh_hash_ = 0, order_hash_ = 0;  // coordinates and t2v (caller's numbering); orig_of_internal
+  ckpt::Fingerprint fingerprint();
+  // load (merge == false) or merge the checkpoint at path, with a message on refusal
+  int read_checkpoint(const std::string &path, bool merge);
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
     void *d = nullptr;    // device copy

@@ -37,6 +37,34 @@ __global__ void batch_fold_kernel(const double *__restrict__ x, double *__restri
   if (t == 0 && (n & 1)) fold1(n - 1);
 }
 
+// Every entry i of [0, n): (mean[i], m2[i]) <- welford_merge(mean_b[i], m2_b[i], na, nb), in place.  Two doubles per
+// thread and step when the four arrays are 16-byte aligned, as batch_fold_kernel.
+template <bool kVec>
+__global__ void batch_merge_kernel(const double *__restrict__ mean_b, const double *__restrict__ m2_b,
+                                   double *__restrict__ mean, double *__restrict__ m2, int64_t n, double na, double nb) {
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x, t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  auto merge1 = [&](int64_t i) {
+    double mu = mean[i], q = m2[i];
+    welford_merge(mean_b[i], m2_b[i], na, nb, mu, q);
+    mean[i] = mu;
+    m2[i] = q;
+  };
+  if (!kVec) {
+    for (int64_t i = t; i < n; i += stride) merge1(i);
+    return;
+  }
+  const int64_t pairs = n / 2;
+  for (int64_t p = t; p < pairs; p += stride) {
+    const double2 mb = reinterpret_cast<const double2 *>(mean_b)[p], qb = reinterpret_cast<const double2 *>(m2_b)[p];
+    double2 mu = reinterpret_cast<double2 *>(mean)[p], q = reinterpret_cast<double2 *>(m2)[p];
+    welford_merge(mb.x, qb.x, na, nb, mu.x, q.x);
+    welford_merge(mb.y, qb.y, na, nb, mu.y, q.y);
+    reinterpret_cast<double2 *>(mean)[p] = mu;
+    reinterpret_cast<double2 *>(m2)[p] = q;
+  }
+  if (t == 0 && (n & 1)) merge1(n - 1);
+}
+
 // out[(r * nscores + k) * E + orig[e]] = batch_readout(...) of score k of element e in result array r
 __global__ void batch_readout_kernel(const double *__restrict__ mean, const double *__restrict__ m2,
                                      const double *__restrict__ volume, const int32_t *__restrict__ orig_of_internal,
@@ -134,6 +162,18 @@ cudaError_t launch_batch_fold(const double *x, double *mean, double *m2, int64_t
     batch_fold_kernel<true><<<grid_for((n + 1) / 2, block), block, 0, stream>>>(x, mean, m2, n, divisor, nb);
   else
     batch_fold_kernel<false><<<grid_for(n, block), block, 0, stream>>>(x, mean, m2, n, divisor, nb);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_batch_merge(const double *mean_b, const double *m2_b, double *mean, double *m2, int64_t n, double na,
+                               double nb, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  auto aligned16 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
+  const int block = 256;
+  if (aligned16(mean_b) && aligned16(m2_b) && aligned16(mean) && aligned16(m2))
+    batch_merge_kernel<true><<<grid_for((n + 1) / 2, block), block, 0, stream>>>(mean_b, m2_b, mean, m2, n, na, nb);
+  else
+    batch_merge_kernel<false><<<grid_for(n, block), block, 0, stream>>>(mean_b, m2_b, mean, m2, n, na, nb);
   return cudaGetLastError();
 }
 

@@ -145,6 +145,10 @@ cudaError_t launch_collide_particles(const ParticleState *state, const int8_t *c
 // for i < n, nb the number of batches including this one; the divisor is read on the device.
 cudaError_t launch_batch_fold(const double *x, double *mean, double *m2, int64_t n, const double *divisor, double nb,
                               cudaStream_t stream);
+// merge: (mean[i], m2[i]) of na batches <- welford_merge(mean_b[i], m2_b[i], na, nb) for i < n, in place: the statistics
+// of the na + nb batches together.
+cudaError_t launch_batch_merge(const double *mean_b, const double *m2_b, double *mean, double *m2, int64_t n, double na,
+                               double nb, cudaStream_t stream);
 // The m0 slots of R result arrays [R][E][stride] of means (and m2, unread for kind 0) of nb batches -> out[(r * nscores
 // + k) * E + caller's id of e] = batch_readout(..., volume[e], kind): 0 mean, 1 standard error, 2 relative error.
 cudaError_t launch_batch_readout(const double *mean, const double *m2, const double *volume,

@@ -81,6 +81,9 @@ C_API = {
     "pumitally_get_region_volumes": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pumitally_get_region_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
     "pumitally_get_region_batch_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
+    "pumitally_save_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "pumitally_load_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "pumitally_merge_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -629,6 +632,26 @@ class PumiTally:
         """kind 0 mean, 1 standard error (both / region volume), 2 relative error of the region sums over the
         batches: [ntime, nbins, nscores, nregions]."""
         return self._region_call(self._L.pumitally_get_region_batch_results, tally, kind, "get_region_batch_results")
+
+    # ---- checkpoints -------------------------------------------------------------
+    def save_checkpoint(self, path):
+        """Write the tally state (the open batch if anything was tallied since the last reset, the batch statistics,
+        the region statistics) and a fingerprint of the configuration to `path`, atomically (path + ".tmp", then a
+        rename).  Changes nothing in the engine.  No particle state: after a load, place the particles first."""
+        if self._L.pumitally_save_checkpoint(self._h, os.fsencode(os.fspath(path))):
+            raise RuntimeError(f"save_checkpoint({path!r}) failed")
+
+    def load_checkpoint(self, path):
+        """Replace the tally state with the checkpoint's; the engine must have the configuration it was saved with
+        (and the same ranks, after comm_init).  A refusal changes nothing."""
+        if self._L.pumitally_load_checkpoint(self._h, os.fsencode(os.fspath(path))):
+            raise RuntimeError(f"load_checkpoint({path!r}) failed")
+
+    def merge_checkpoint(self, path):
+        """Add the checkpoint's folded batches to this engine's (batch statistics on, the checkpoint saved at a batch
+        end).  The open batch is left alone.  A refusal changes nothing."""
+        if self._L.pumitally_merge_checkpoint(self._h, os.fsencode(os.fspath(path))):
+            raise RuntimeError(f"merge_checkpoint({path!r}) failed")
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
