@@ -208,8 +208,13 @@ __device__ __forceinline__ uint64_t l2_policy_stream() {
   asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-// same value, created where it is used: keeps the policy out of the registers that stay live
-// across the crossing loop of the compact-layout kernel
+// same values, created where they are used (volatile: not hoisted out of the loop): keeps the
+// policies out of the registers that stay live across the crossing loop of the persistent kernel
+__device__ __forceinline__ uint64_t l2_policy_keep_now() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
 __device__ __forceinline__ uint64_t l2_policy_stream_now() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -280,6 +285,13 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst, const void *src, uint6
 __device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
+// The ticket ids of gather mode: 4-byte copies committed as one group per ticket and waited for with
+// cp_async_wait_ids() when the ticket becomes current (the stage copies complete on their mbarriers instead).
+__device__ __forceinline__ void cp_async_4(uint32_t dst, const void *src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_ids() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 // `id` = this lane's particle for the chunk (lanes >= count hold garbage and copy nothing)
 __device__ __forceinline__ void stage_gather(const WalkParams &P, int id, int count, ParticleStage *st,
                                              uint32_t bar, int lane, uint64_t pol) {
@@ -303,16 +315,38 @@ __device__ __forceinline__ void stage_gather(const WalkParams &P, int id, int co
   cp_async_arrive_noinc(bar);
 }
 
+// The ray target (Ray::tx,ty,tz) and the particle id live in the lane's shared-memory slots `tgt` and
+// `id`, not in registers across the crossing loop: only end_ray() reads them.  target_in() returns the
+// id and puts the target into the ray in the step that ends the ray -- the test is advance()'s own --
+// and target_out() saves the target of a ray that starts in that step (phase 2 after phase 1, or
+// phase 1 again from the stored position).
+__device__ __forceinline__ int target_in(const WalkParams &P, Ray &r, double texit, int32_t next,
+                                         const double *tgt, const int32_t *id) {
+  int i = 0;
+  if (!(texit < 1.0) || next < 0 || r.iters + 1 >= P.max_iters) {
+    r.tx = tgt[0]; r.ty = tgt[1]; r.tz = tgt[2];
+    i = *id;
+  }
+  return i;
+}
+__device__ __forceinline__ void target_out(const Ray &r, double *tgt) {
+  if (r.iters == 0 && r.stage != kStageDone) {
+    tgt[0] = r.tx; tgt[1] = r.ty; tgt[2] = r.tz;
+  }
+}
+
 // One crossing on the plane records.  Entry-face elision: after a crossing the face the ray came
 // in through is known (r.entry) and can never be the exit, so only the other three 32-byte
-// sectors of the record are fetched; the first tet of a ray needs all four.
+// sectors of the record are fetched; the first tet of a ray needs all four.  tgt, id: the lane's slots.
 template <int FETCH, int NS = 0, bool TM = false, bool MO = false>
-__device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r, Counters &c, uint64_t pol,
-                                           const ScoreLane *sl = nullptr) {
+__device__ __forceinline__ void plane_step(const WalkParams &P, Ray &r, Counters &c, uint64_t pol, double *tgt,
+                                           const int32_t *id, const ScoreLane *sl = nullptr) {
   ExitScan sc;
   const double *rec = P.tets[r.e].d;
   const int en = r.entry;
-  double q[3][4], q3[4];
+  // q3, the fourth face of a ray's first tet, is zero when it is not loaded: left undefined, it would be
+  // carried round the crossing loop in registers (or on the stack) from the last first tet.
+  double q[3][4], q3[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     const int fk = k + ((en >= 0 && k >= en) ? 1 : 0);
@@ -331,8 +365,11 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, int my_i, Ray &r
     face_payload(q3[0], q3[1], q3[2], q3[3], r.e, 3, nb, bk);
     scan_face(sc, q3[0], q3[1], q3[2], q3[3], nb, bk, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
   }
-  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM, MO>(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back,
+  const double texit = exit_parameter(sc);
+  const int my_i = target_in(P, r, texit, sc.nbr, tgt, id);
+  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM, MO>(P, my_i, r, texit, sc.nbr, sc.back,
                                                                                   c, true, sl);
+  target_out(r, tgt);
 }
 
 // Lean crossing step.  The compiler can sink the third record load of plane_step() below the arithmetic on
@@ -522,6 +559,23 @@ __device__ __forceinline__ void edge_persist_step(const WalkParams &P, int my_i,
 
 constexpr int kClaimRun = 4;  // gather mode: a warp takes up to this many consecutive chunks per ticket
 
+// Scheduling state of a persistent warp.  It is warp-uniform and only the refill branch of the kernel uses
+// it, once per several crossings, so it lives in a per-warp shared-memory record instead of registers: the
+// branch reads it on entry and writes the cursor back on exit, and none of it is live across a crossing.
+struct SchedFixed {  // set once per launch
+  int total, nchunks, claim_run;
+  int own_lo, own_hi, oth_lo, oth_hi;  // die split: chunk ranges of this SM's L2 partition and of the other one
+  unsigned int *own_cnt, *oth_cnt;     // die split: their chunk tickets
+};
+struct SchedCursor {
+  int run_base, run_next, run_end, pend_base;  // gather mode: current ticket run, and the next ticket's first chunk
+  int tk;                                      // gather mode: the current ticket's ids are ids[tk], the next one's ids[tk ^ 1]
+  int split_phase;                             // die split: 0 own chunks, 1 the other partition's, 3 none left, 2 off
+  int cur, cursor, cur_count;                  // stage being handed out, its next slot, its particles (0: none)
+  int chunk_cur, chunk_next;                   // chunks in the two stages (-1: none)
+  uint32_t parity;                             // bit b = phase parity of particle-stage barrier b
+};
+
 // REFILL_T: idle lanes are topped up only when at least this many have finished -- the
 // refill code then runs with REFILL_T+ active lanes instead of the ~3 that finish per
 // iteration, at the price of a few idle lanes in the walk step.
@@ -578,7 +632,14 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
   __shared__ __align__(8) unsigned long long bars[WARPS][3];
   __shared__ __align__(128) unsigned char rows[kRows ? WARPS : 1][kRows ? 32 * kRowBytes : 16];
   constexpr bool kEdge = FETCH == kFetchEdge;
-  __shared__ double targets[kEdge ? BLOCK : 1][3];  // compact layout: each lane's ray target
+  // each lane's ray target (plane_step, edge_persist_step) and particle id (plane_step); the whole-record
+  // and lean steps keep their own
+  constexpr bool kTargetSlot = !kRows && FETCH != kFetchLean && FETCH != kFetchLeanL1;
+  __shared__ double targets[kTargetSlot ? BLOCK : 1][3];
+  __shared__ int32_t lane_ids[kTargetSlot ? BLOCK : 1];
+  __shared__ SchedFixed sched_fixed[WARPS];
+  __shared__ SchedCursor sched_cursor[WARPS];
+  __shared__ int32_t ticket_ids[GATHER ? WARPS : 1][2][kClaimRun * kChunk];  // gather mode: current and next ticket
   static_assert(NS == 0 || (!kEdge && !kRows), "scored walks run on the plane records");
   static_assert(!TM || NS > 0, "the timed walk is a scored walk");
   __shared__ double score_wl[kLaneSlots<NS, TM>][NS > 0 ? BLOCK : 1];  // scored walk: ScoreLane::wl of each lane
@@ -595,17 +656,19 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncwarp();
-  const uint64_t keep = FETCH != kFetchPlain ? l2_policy_keep() : 0;
-  const uint64_t strm = (FETCH == kFetchEdge) ? 0 : ((FETCH != kFetchPlain || GATHER) ? l2_policy_stream() : 0);
-  const int total = (GATHER || PACKED) ? (int)__ldg(P.work_count) : P.end - P.begin;
-  const int nchunks = (total + kChunk - 1) / kChunk;
-  // Gather mode: a ticket is a run of kClaimRun chunks = 64 particles whose ids sit in two
-  // registers per lane.  The *next* ticket is claimed, and its ids requested, one run ahead, so
-  // neither the atomic nor the id loads are ever waited for.
-  static_assert(kClaimRun * kChunk == 64, "two id registers per lane cover the largest ticket");
-  const int claim_run = GATHER ? min(max(P.claim_run, 1), kClaimRun) : 1;
-  int run_base = 0, run_next = 0, run_end = 0, ids0 = 0, ids1 = 0;
-  int pend_base = -1, pend0 = 0, pend1 = 0;
+  // The L2 policies are made where they are used (one createpolicy each): none is held across the loop.
+  SchedFixed fx;
+  SchedCursor s;
+  fx.total = (GATHER || PACKED) ? (int)__ldg(P.work_count) : P.end - P.begin;
+  fx.nchunks = (fx.total + kChunk - 1) / kChunk;
+  // Gather mode: a ticket is a run of kClaimRun chunks = 64 particles whose ids are copied to the
+  // warp's ticket_ids.  The *next* ticket is claimed, and its ids requested, one run ahead, so the
+  // id copies are never waited for.
+  static_assert(kClaimRun * kChunk == 64, "two ids per lane cover the largest ticket");
+  fx.claim_run = GATHER ? min(max(P.claim_run, 1), kClaimRun) : 1;
+  s.run_base = s.run_next = s.run_end = 0;
+  s.pend_base = -1;
+  s.tk = 0;
   // Die split (sorted modes only).  On a GPU whose L2 is two partitions that each cache the lines their own SMs
   // touch, a line only the other partition holds costs a longer trip.  When all SMs
   // work through the sorted particles front to back, both partitions hold the same window of the mesh.  Here
@@ -614,100 +677,109 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
   // own window; a partition that runs out of chunks helps the other finish.
   constexpr bool kSplit = GATHER || PACKED;
   constexpr int kNoChunk = 0x3fffffff;
-  int split_phase = 2, own_lo = 0, own_hi = 0, oth_lo = 0, oth_hi = 0;
-  unsigned int *own_cnt = P.work_counter, *oth_cnt = P.work_counter;
+  s.split_phase = 2;
+  fx.own_lo = fx.own_hi = fx.oth_lo = fx.oth_hi = 0;
+  fx.own_cnt = fx.oth_cnt = P.work_counter;
   if constexpr (kSplit) {
     if (P.die0_sms > 0 && P.die0_sms < P.nsms) {
       unsigned sm;
       asm("mov.u32 %0, %%smid;" : "=r"(sm));
       const int die = (P.die_mask[(sm >> 5) & 7] >> (sm & 31)) & 1;
-      const int mid = (int)((long long)nchunks * P.die0_sms / P.nsms) & ~(kClaimRun - 1);  // tickets never straddle it
-      own_lo = die ? mid : 0; own_hi = die ? nchunks : mid;
-      oth_lo = die ? 0 : mid; oth_hi = die ? mid : nchunks;
-      own_cnt = die ? P.work_counter2 : P.work_counter;
-      oth_cnt = die ? P.work_counter : P.work_counter2;
-      split_phase = 0;
+      const int mid = (int)((long long)fx.nchunks * P.die0_sms / P.nsms) & ~(kClaimRun - 1);  // tickets never straddle it
+      fx.own_lo = die ? mid : 0; fx.own_hi = die ? fx.nchunks : mid;
+      fx.oth_lo = die ? 0 : mid; fx.oth_hi = die ? mid : fx.nchunks;
+      fx.own_cnt = die ? P.work_counter2 : P.work_counter;
+      fx.oth_cnt = die ? P.work_counter : P.work_counter2;
+      s.split_phase = 0;
     }
   }
   // next ticket of `run` chunks: its first chunk, or a value >= nchunks when nothing is left (warp-uniform)
   auto take = [&](int run) -> int {
     int c = 0;
     if constexpr (kSplit) {
-      if (split_phase < 2) {
+      if (s.split_phase < 2) {
         if (lane == 0) {
           c = kNoChunk;
-          if (split_phase == 0) {
-            c = own_lo + (int)atomicAdd(own_cnt, (unsigned)run);
-            if (c >= own_hi) { c = kNoChunk; split_phase = 1; }
+          if (s.split_phase == 0) {
+            c = fx.own_lo + (int)atomicAdd(fx.own_cnt, (unsigned)run);
+            if (c >= fx.own_hi) { c = kNoChunk; s.split_phase = 1; }
           }
           if (c == kNoChunk) {
-            c = oth_lo + (int)atomicAdd(oth_cnt, (unsigned)run);
-            if (c >= oth_hi) { c = kNoChunk; split_phase = 3; }
+            c = fx.oth_lo + (int)atomicAdd(fx.oth_cnt, (unsigned)run);
+            if (c >= fx.oth_hi) { c = kNoChunk; s.split_phase = 3; }
           }
         }
-        split_phase = __shfl_sync(0xffffffffu, split_phase, 0);
+        s.split_phase = __shfl_sync(0xffffffffu, s.split_phase, 0);
         return __shfl_sync(0xffffffffu, c, 0);
       }
-      if (split_phase == 3) return kNoChunk;
+      if (s.split_phase == 3) return kNoChunk;
     }
     if (lane == 0) c = (int)atomicAdd(P.work_counter, (unsigned)run);
     return __shfl_sync(0xffffffffu, c, 0);
   };
+  // claims the next ticket and starts the copies of its ids into ticket_ids[warp][s.tk ^ 1]
   auto fetch_ticket = [&]() {
-    pend_base = take(claim_run);
-    const long long p0 = (long long)pend_base * kChunk + lane, p1 = p0 + 32;
-    const long long pe = min((long long)total, ((long long)pend_base + claim_run) * kChunk);
-    pend0 = p0 < pe ? __ldg(P.order + p0) : 0;
-    pend1 = p1 < pe ? __ldg(P.order + p1) : 0;
+    s.pend_base = take(fx.claim_run);
+    const long long p0 = (long long)s.pend_base * kChunk + lane, p1 = p0 + 32;
+    const long long pe = min((long long)fx.total, ((long long)s.pend_base + fx.claim_run) * kChunk);
+    int32_t *ids = ticket_ids[GATHER ? warp : 0][s.tk ^ 1];
+    if (p0 < pe) cp_async_4(smem_u32(ids + lane), P.order + p0);
+    if (p1 < pe) cp_async_4(smem_u32(ids + lane + 32), P.order + p1);
+    cp_async_commit();
   };
   auto load_stage = [&](int chunk, ParticleStage *st, uint32_t bar) {
     if constexpr (PACKED) {
       // one bulk copy: the chunk's rows are contiguous and every row is 64 bytes, ragged tail included
       if (lane == 0) {
-        const uint32_t bytes = 64u * (uint32_t)min(kChunk, total - chunk * kChunk);
+        const uint32_t bytes = 64u * (uint32_t)min(kChunk, fx.total - chunk * kChunk);
         mbar_expect_tx(bar, bytes);
-        bulk_g2s_hint(smem_u32(st), P.rows + (size_t)chunk * kChunk, bytes, bar, strm);
+        bulk_g2s_hint(smem_u32(st), P.rows + (size_t)chunk * kChunk, bytes, bar, l2_policy_stream_now());
       }
     } else if constexpr (GATHER) {
-      const int k = chunk - run_base;  // chunk's position in the current ticket (warp-uniform)
-      const int id = __shfl_sync(0xffffffffu, (k >> 1) ? ids1 : ids0, ((k & 1) << 4) | (lane & 15));
-      stage_gather(P, id, min(kChunk, total - chunk * kChunk), st, bar, lane,
-                   FETCH == kFetchEdge ? l2_policy_stream_now() : strm);
+      const int k = chunk - s.run_base;  // chunk's position in the current ticket (warp-uniform)
+      const int id = ticket_ids[warp][s.tk][k * kChunk + (lane & (kChunk - 1))];
+      stage_gather(P, id, min(kChunk, fx.total - chunk * kChunk), st, bar, lane, l2_policy_stream_now());
     } else if constexpr (FETCH == kFetchPlain) {
       stage_load(P, chunk, st, bar, lane);
     } else {
-      stage_load_hint(P, chunk, st, bar, lane, FETCH == kFetchEdge ? l2_policy_stream_now() : strm);
+      stage_load_hint(P, chunk, st, bar, lane, l2_policy_stream_now());
     }
   };
   auto claim = [&]() -> int {
     int c = 0;
     if constexpr (GATHER) {
-      if (run_next >= run_end) {
-        if (pend_base < 0) fetch_ticket();
-        run_base = run_next = pend_base;
-        run_end = pend_base + claim_run;
-        ids0 = pend0;
-        ids1 = pend1;
+      if (s.run_next >= s.run_end) {
+        if (s.pend_base < 0) fetch_ticket();
+        s.run_base = s.run_next = s.pend_base;
+        s.run_end = s.pend_base + fx.claim_run;
+        s.tk ^= 1;
+        cp_async_wait_ids();  // this lane's copies of the ticket's ids have landed...
+        __syncwarp();         // ...and every lane's are visible to the warp
         fetch_ticket();
       }
-      c = run_next++;
+      c = s.run_next++;
     } else {
       c = take(1);
     }
-    return c < nchunks ? c : -1;
+    return c < fx.nchunks ? c : -1;
   };
 
-  int cur = 0, cursor = 0, cur_count = 0;
-  uint32_t parity = 0;  // bit b = phase parity of barrier b (0,1 particle stages; 2 tet rows)
-  int chunk_cur = claim();
-  if (chunk_cur >= 0) load_stage(chunk_cur, &stages[warp][0], bar0);
-  int chunk_next = chunk_cur >= 0 ? claim() : -1;
-  if (chunk_next >= 0) load_stage(chunk_next, &stages[warp][1], bar0 + 8);
-  if (chunk_cur >= 0) {
+  s.cur = s.cursor = s.cur_count = 0;
+  s.parity = 0;
+  s.chunk_cur = claim();
+  if (s.chunk_cur >= 0) load_stage(s.chunk_cur, &stages[warp][0], bar0);
+  s.chunk_next = s.chunk_cur >= 0 ? claim() : -1;
+  if (s.chunk_next >= 0) load_stage(s.chunk_next, &stages[warp][1], bar0 + 8);
+  if (s.chunk_cur >= 0) {
     mbar_wait(bar0, 0);
-    parity ^= 1u;
-    cur_count = min(kChunk, total - chunk_cur * kChunk);
+    s.parity ^= 1u;
+    s.cur_count = min(kChunk, fx.total - s.chunk_cur * kChunk);
   }
+  if (lane == 0) {
+    sched_fixed[warp] = fx;
+    sched_cursor[warp] = s;
+  }
+  __syncwarp();
 
   Counters c;
   Ray r;
@@ -715,61 +787,81 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
   g.dv = 0;
   r.stage = kStageDone;
   int my_i = 0;
+  uint32_t row_parity = 0;  // phase parity of the tet-row barrier (kBulkTets)
+  double *const tgt = &targets[kTargetSlot ? threadIdx.x : 0][0];
   for (;;) {
     unsigned idle = __ballot_sync(0xffffffffu, r.stage == kStageDone);
-    while (cur_count > 0 && (int)__popc(idle) >= REFILL_T) {
-      const int slot = cursor + __popc(idle & ((1u << lane) - 1u));
-      if (r.stage == kStageDone && slot < cur_count) {
-        if constexpr (PACKED) {
-          const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-          my_i = begin_from_row<NS, TM, MO>(P, reinterpret_cast<const PackedRow *>(&stages[warp][cur]) + slot, r, c,
-                                    NS > 0 ? &sl : nullptr);
-        } else {
-          my_i = GATHER ? stages[warp][cur].id[slot] : P.begin + chunk_cur * kChunk + slot;
-          const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-          begin_from_stage<NS, TM, MO>(P, &stages[warp][cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
-        }
-        if constexpr (FETCH == kFetchEdge) {
-          g.dv = 0;
-          if (r.stage != kStageDone) {
-            targets[threadIdx.x][0] = r.tx; targets[threadIdx.x][1] = r.ty; targets[threadIdx.x][2] = r.tz;
+    if ((int)__popc(idle) >= REFILL_T && sched_cursor[warp].cur_count > 0) {
+      fx = sched_fixed[warp];
+      s = sched_cursor[warp];
+      while (s.cur_count > 0 && (int)__popc(idle) >= REFILL_T) {
+        const int slot = s.cursor + __popc(idle & ((1u << lane) - 1u));
+        if (r.stage == kStageDone && slot < s.cur_count) {
+          if constexpr (PACKED) {
+            const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
+            my_i = begin_from_row<NS, TM, MO>(P, reinterpret_cast<const PackedRow *>(&stages[warp][s.cur]) + slot, r,
+                                              c, NS > 0 ? &sl : nullptr);
+          } else {
+            my_i = GATHER ? stages[warp][s.cur].id[slot] : P.begin + s.chunk_cur * kChunk + slot;
+            const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
+            begin_from_stage<NS, TM, MO>(P, &stages[warp][s.cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
+          }
+          if constexpr (FETCH == kFetchEdge) g.dv = 0;
+          if constexpr (kTargetSlot) {
+            if (r.stage != kStageDone) {
+              tgt[0] = r.tx; tgt[1] = r.ty; tgt[2] = r.tz;
+              lane_ids[threadIdx.x] = my_i;
+            }
           }
         }
+        __syncwarp();
+        s.cursor += __popc(idle);
+        if (s.cursor >= s.cur_count) {
+          // every slot of this stage has been handed out: recycle it for the chunk after next
+          const int recycled = s.cur;
+          s.chunk_cur = s.chunk_next;
+          s.cur ^= 1;
+          s.cursor = 0;
+          s.cur_count = 0;
+          s.chunk_next = -1;
+          if (s.chunk_cur >= 0) {
+            mbar_wait(bar0 + 8 * s.cur, (s.parity >> s.cur) & 1u);
+            s.parity ^= 1u << s.cur;
+            s.cur_count = min(kChunk, fx.total - s.chunk_cur * kChunk);
+            s.chunk_next = claim();
+            if (s.chunk_next >= 0) {
+              if (lane == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+              load_stage(s.chunk_next, &stages[warp][recycled], bar0 + 8 * recycled);
+            }
+          }
+        }
+        idle = __ballot_sync(0xffffffffu, r.stage == kStageDone);
+      }
+      // write back what this mode can have changed (the rest need not stay live through the branch)
+      __syncwarp();
+      if (lane == 0) {
+        SchedCursor &d = sched_cursor[warp];
+        d.cur = s.cur; d.cursor = s.cursor; d.cur_count = s.cur_count;
+        d.chunk_cur = s.chunk_cur; d.chunk_next = s.chunk_next; d.parity = s.parity;
+        if constexpr (GATHER) {
+          d.run_base = s.run_base; d.run_next = s.run_next; d.run_end = s.run_end;
+          d.pend_base = s.pend_base; d.tk = s.tk;
+        }
+        if constexpr (kSplit) d.split_phase = s.split_phase;
       }
       __syncwarp();
-      cursor += __popc(idle);
-      if (cursor >= cur_count) {
-        // every slot of this stage has been handed out: recycle it for the chunk after next
-        const int recycled = cur;
-        chunk_cur = chunk_next;
-        cur ^= 1;
-        cursor = 0;
-        cur_count = 0;
-        chunk_next = -1;
-        if (chunk_cur >= 0) {
-          mbar_wait(bar0 + 8 * cur, (parity >> cur) & 1u);
-          parity ^= 1u << cur;
-          cur_count = min(kChunk, total - chunk_cur * kChunk);
-          chunk_next = claim();
-          if (chunk_next >= 0) {
-            if (lane == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            load_stage(chunk_next, &stages[warp][recycled], bar0 + 8 * recycled);
-          }
-        }
-      }
-      idle = __ballot_sync(0xffffffffu, r.stage == kStageDone);
     }
     if (idle == 0xffffffffu) break;  // no lane active and nothing left to hand out
     if constexpr (kBulkTets) {
       const unsigned act = ~idle;
       if (lane == __ffs(act) - 1) mbar_expect_tx(bar_row, 128u * __popc(act));
-      if (r.stage != kStageDone) bulk_g2s_hint(row, P.tets + r.e, 128u, bar_row, keep);
-      mbar_wait(bar_row, (parity >> 2) & 1u);
-      parity ^= 4u;
+      if (r.stage != kStageDone) bulk_g2s_hint(row, P.tets + r.e, 128u, bar_row, l2_policy_keep_now());
+      mbar_wait(bar_row, row_parity);
+      row_parity ^= 1u;
     }
     if (r.stage != kStageDone) {
       if constexpr (FETCH == kFetchEdge) {
-        edge_persist_step(P, my_i, r, g, c, keep, &targets[kEdge ? threadIdx.x : 0][0]);
+        edge_persist_step(P, my_i, r, g, c, l2_policy_keep_now(), tgt);
       } else if constexpr (kRows) {
         ExitScan sc;
         double raw[16];
@@ -781,10 +873,11 @@ __global__ void __launch_bounds__(BLOCK, MINB) walk_persist_kernel(const KernelP
         scan_record(raw, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
         advance(P, my_i, r, exit_parameter(sc), sc.nbr, sc.back, c, true);
       } else if constexpr (FETCH == kFetchLean || FETCH == kFetchLeanL1) {
-        plane_step_lean<FETCH>(P, my_i, r, c, keep);
+        plane_step_lean<FETCH>(P, my_i, r, c, l2_policy_keep_now());
       } else {
         const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-        plane_step<FETCH, NS, TM, MO>(P, my_i, r, c, keep, NS > 0 ? &sl : nullptr);
+        plane_step<FETCH, NS, TM, MO>(P, r, c, FETCH != kFetchPlain ? l2_policy_keep_now() : 0, tgt,
+                                      &lane_ids[kTargetSlot ? threadIdx.x : 0], NS > 0 ? &sl : nullptr);
       }
     }
   }
@@ -806,8 +899,9 @@ cudaError_t launch_persist(const KernelParams<NS, TM> &p, long long n, cudaStrea
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int carve = CARVE < 0 ? (int)cudaSharedmemCarveoutMaxShared : CARVE;
-    if (NS > 0 && CARVE >= 0) {
-      // the scores' slots must not cost resident blocks: widen the carveout to what MINB blocks need
+    if (CARVE >= 0) {
+      // the lane slots (targets, ids, scores) must not cost resident blocks: widen the carveout to what
+      // MINB blocks need
       cudaFuncAttributes fa{};
       int per_sm = 0, reserved = 0;
       cudaFuncGetAttributes(&fa, walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>);
