@@ -144,6 +144,31 @@ inline int MergeCheckpoint(const PumiTally &tally, const char *path) {
   return pumitally_merge_checkpoint(engine_of(tally), path);
 }
 
+// Weight windows (see pumitally_set_weight_windows in pumitally_c.h): ngroups (lower, upper) pairs per element,
+// [group][element] in the caller's numbering; lower <= 0 is no window, read back as (-1, -1).  GenerateWeightWindows
+// makes them from the batch statistics of one result by the MAGIC method, the score bins as groups.
+// WeightWindowsAtParticles gives the window of each particle's parent element (size = num_particles), WeightWindowsAtPoints
+// the window at located points; groups may be nullptr (group 0).
+inline int SetWeightWindows(const PumiTally &tally, const double *lower, const double *upper, int64_t n,
+                            int32_t ngroups) {
+  return pumitally_set_weight_windows(engine_of(tally), lower, upper, n, ngroups);
+}
+inline int GetWeightWindows(const PumiTally &tally, double *lower, double *upper, int64_t n) {
+  return pumitally_get_weight_windows(engine_of(tally), lower, upper, n);
+}
+inline int GenerateWeightWindows(const PumiTally &tally, int32_t which, int32_t score, int32_t time_bin, double ratio,
+                                 double max_rel_err) {
+  return pumitally_generate_weight_windows(engine_of(tally), which, score, time_bin, ratio, max_rel_err);
+}
+inline int WeightWindowsAtParticles(const PumiTally &tally, const int32_t *groups, double *lower, double *upper,
+                                    int32_t size) {
+  return pumitally_get_weight_windows_at_particles(engine_of(tally), groups, lower, upper, size);
+}
+inline int WeightWindowsAtPoints(const PumiTally &tally, const double *xyz, int64_t npts, const int32_t *groups,
+                                 double *lower, double *upper) {
+  return pumitally_get_weight_windows_at_points(engine_of(tally), xyz, npts, groups, lower, upper);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

@@ -501,6 +501,56 @@ int pumitally_save_checkpoint(pumitally_engine *e, const char *path);
 int pumitally_load_checkpoint(pumitally_engine *e, const char *path);
 int pumitally_merge_checkpoint(pumitally_engine *e, const char *path);
 
+/* ---- additive: weight windows (MAGIC generation from the batch statistics, lookups on the GPU) ----
+ * Deep-penetration and shielding tallies converge only with weight windows, and the usual way to get them is the MAGIC
+ * method: run, turn the mesh flux tally into per-element, per-energy-group bounds, run again with those bounds.  The
+ * engine holds one window table: ngroups (lower, upper) pairs per element, 16 * ngroups * num_elements bytes of device
+ * memory; a call that cannot allocate it is refused.  Windows are not tally state: pumitally_reset_tally,
+ * pumitally_end_batch, every pumitally_set_* call, pumitally_comm_init and checkpoint save, load and merge leave them
+ * alone, and checkpoints do not hold them (get them and set them back).  A missing window reads (-1, -1).  Refusals
+ * print the reason, return non-zero and change nothing.
+ * pumitally_set_weight_windows(e, lower, upper, n, ngroups): host arrays [group][element] in the caller's numbering,
+ * n == ngroups * num_elements.  An entry with lower <= 0 means no window; any other entry must be finite with
+ * upper > lower, or (a NaN, an infinity, upper <= lower) the whole call is refused.  lower == NULL with ngroups == 0
+ * removes the windows.  Not collective.  pumitally_get_weight_window_groups returns ngroups (0 without windows);
+ * pumitally_get_weight_windows(e, lower, upper, n) returns what set stored, in the same layout (n == ngroups *
+ * num_elements; 0 without windows).
+ * pumitally_generate_weight_windows(e, tally, score, time_bin, ratio, max_rel_err) replaces the table with the MAGIC
+ * windows of one result, the score bins as energy groups (ngroups = nbins).  It needs batch statistics on and at least
+ * two folded batches; tally is 0 (track length) or 1 (collision, estimator on), 0 <= score < nscores,
+ * 0 <= time_bin < max(ntime, 1), ratio finite and > 1, max_rel_err > 0 (+inf accepts every error).  For group b and
+ * element e, phi and r are what pumitally_get_batch_results kinds 0 and 2 return for (time_bin, b, score, e).  The
+ * element is eligible when phi is finite and > 0 and r <= max_rel_err; phimax_b is the largest eligible phi of group b.
+ * An eligible element gets lower = (phi / phimax_b) * c with c = 2 / (ratio + 1), and upper = lower * ratio, in that
+ * order of operations: the window's centre is phi / phimax_b, weight 1 where the flux is largest.  Every other element,
+ * and every element of a group without an eligible one, gets (-1, -1).  Collective with several ranks: every rank
+ * gathers the whole statistics and computes the same table.
+ * pumitally_get_weight_windows_at_particles(e, groups, lower, upper, n): the window of each particle's current parent
+ * element, n == num_particles; groups int32[n] is each particle's energy group, NULL for group 0.  A group outside
+ * [0, ngroups) or an element without a window gives (-1, -1).  Refused before CopyInitialPosition.  The _device variant
+ * takes device arrays and is enqueued on `stream` behind the last move, as pumitally_tally_collisions_at_particles_device.
+ * pumitally_get_weight_windows_at_points(e, xyz, npts, groups, lower, upper): the window at each of npts AoS points,
+ * located as pumitally_locate_points locates them; a point outside the mesh or with a non-finite coordinate gives
+ * (-1, -1).  Host calls work through device buffers of the option "chunk" points; the _device variant is enqueued on
+ * `stream`.  No lookup changes a particle, the tally, a statistic, a counter or the kernel auto-tuner.
+ * WriteTallyResults with windows set writes, after every other array, "ww_lower" and "ww_upper" (one group) or
+ * "ww_lower_g<g>" and "ww_upper_g<g>" for every group g. */
+int pumitally_set_weight_windows(pumitally_engine *e, const double *lower, const double *upper, int64_t n,
+                                 int32_t ngroups);
+int32_t pumitally_get_weight_window_groups(const pumitally_engine *e);
+int pumitally_get_weight_windows(pumitally_engine *e, double *lower, double *upper, int64_t n);
+int pumitally_generate_weight_windows(pumitally_engine *e, int32_t tally, int32_t score, int32_t time_bin, double ratio,
+                                      double max_rel_err);
+int pumitally_get_weight_windows_at_particles(pumitally_engine *e, const int32_t *groups, double *lower, double *upper,
+                                              int32_t n);
+int pumitally_get_weight_windows_at_particles_device(pumitally_engine *e, const int32_t *d_groups, double *d_lower,
+                                                     double *d_upper, int32_t n, void *stream);
+int pumitally_get_weight_windows_at_points(pumitally_engine *e, const double *xyz, int64_t npts, const int32_t *groups,
+                                           double *lower, double *upper);
+int pumitally_get_weight_windows_at_points_device(pumitally_engine *e, const double *d_xyz, int64_t npts,
+                                                  const int32_t *d_groups, double *d_lower, double *d_upper,
+                                                  void *stream);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

@@ -24,6 +24,7 @@ SOURCES = [
     "bin_kernels.cu",
     "locate_kernels.cu",
     "stats_kernels.cu",
+    "ww_kernels.cu",
     "l2_partitions.cu",
     "engine.cu",
     "checkpoint.cpp",

@@ -318,6 +318,42 @@ int pumitally_merge_checkpoint(pumitally_engine *e, const char *path) {
   return guarded(e, [&](ptb::Engine &g) { return g.merge_checkpoint(path); });
 }
 
+int pumitally_set_weight_windows(pumitally_engine *e, const double *lower, const double *upper, int64_t n,
+                                 int32_t ngroups) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_weight_windows(lower, upper, n, ngroups); });
+}
+int32_t pumitally_get_weight_window_groups(const pumitally_engine *e) {
+  return (e && e->impl) ? e->impl->weight_window_groups() : 0;
+}
+int pumitally_get_weight_windows(pumitally_engine *e, double *lower, double *upper, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_weight_windows(lower, upper, n); });
+}
+int pumitally_generate_weight_windows(pumitally_engine *e, int32_t tally, int32_t score, int32_t time_bin, double ratio,
+                                      double max_rel_err) {
+  return guarded(e, [&](ptb::Engine &g) { return g.generate_weight_windows(tally, score, time_bin, ratio, max_rel_err); });
+}
+int pumitally_get_weight_windows_at_particles(pumitally_engine *e, const int32_t *groups, double *lower, double *upper,
+                                              int32_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.weight_windows_at_particles(groups, lower, upper, n); });
+}
+int pumitally_get_weight_windows_at_particles_device(pumitally_engine *e, const int32_t *d_groups, double *d_lower,
+                                                     double *d_upper, int32_t n, void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.weight_windows_at_particles_device(d_groups, d_lower, d_upper, n, static_cast<cudaStream_t>(stream));
+  });
+}
+int pumitally_get_weight_windows_at_points(pumitally_engine *e, const double *xyz, int64_t npts, const int32_t *groups,
+                                           double *lower, double *upper) {
+  return guarded(e, [&](ptb::Engine &g) { return g.weight_windows_at_points(xyz, npts, groups, lower, upper); });
+}
+int pumitally_get_weight_windows_at_points_device(pumitally_engine *e, const double *d_xyz, int64_t npts,
+                                                  const int32_t *d_groups, double *d_lower, double *d_upper,
+                                                  void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.weight_windows_at_points_device(d_xyz, npts, d_groups, d_lower, d_upper, static_cast<cudaStream_t>(stream));
+  });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cerrno>
+#include <cfloat>
 #include <chrono>
 #include <climits>
 #include <cmath>
@@ -20,6 +21,7 @@
 #include "host_stage.hpp"
 #include "seed_grid.hpp"
 #include "vtk_writer.hpp"
+#include "weight_windows.cuh"
 
 namespace ptb {
 
@@ -194,6 +196,7 @@ Engine::~Engine() {
   cudaFree(d_coll_counts_); cudaFree(d_coll_buf_);
   free_stats();
   free_regions();
+  free_weight_windows();
   cudaFree(d_batch_div_); cudaFree(d_stats_red_);
   if (compute_) cudaStreamDestroy(compute_);
   if (copy_) cudaStreamDestroy(copy_);
@@ -1734,13 +1737,15 @@ int64_t Engine::debug_order(int32_t *out, int64_t n) {
 
 // FinalizeTallies (PumiTallyImpl.cpp:411-416).  With the collision estimator every array of the track-length tally is
 // followed by its collision twin, the same name prefixed "collision_".  With batch statistics and at least one batch
-// folded, the "_mean" / "_rel_err" arrays (batch_arrays) of both tallies follow all of these.
+// folded, the "_mean" / "_rel_err" arrays (batch_arrays) of both tallies follow all of these, and with weight windows
+// their bounds (ww_arrays) come last.
 int Engine::write_tally_results() {
   VtkArrays coll;
   if (collision_ && (synchronize() || gather_shares() || scored_arrays(flux_len(), "collision_", coll, nullptr))) return 1;
   if (batch_stats_ && batches_ > 0 &&
       (synchronize() || batch_arrays(0, "", coll) || (collision_ && batch_arrays(1, "collision_", coll))))
     return 1;
+  if (ww_groups_ > 0 && ww_arrays(coll)) return 1;
   if (multi_results()) return write_scored_results(coll);
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
@@ -2964,6 +2969,231 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
   scored_moves_ = sc.scored_moves;
   tallied_ = h.open != 0;
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
+  return 0;
+}
+
+// ------------------------------------------------------------------ weight windows
+
+void Engine::free_weight_windows() {
+  cudaFree(d_ww_);
+  d_ww_ = nullptr;
+  ww_groups_ = 0;
+}
+
+int Engine::alloc_weight_windows(int32_t ngroups, double2 **out) {
+  const size_t bytes = size_t(ngroups) * size_t(std::max<int64_t>(mesh_.ntets, 1)) * sizeof(double2);
+  if (cudaMalloc(reinterpret_cast<void **>(out), bytes) != cudaSuccess) {
+    const cudaError_t err = cudaGetLastError();
+    *out = nullptr;
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the weight windows (%zu bytes: %s)\n", bytes,
+            cudaGetErrorString(err));
+    return 1;
+  }
+  return 0;
+}
+
+int Engine::set_weight_windows(const double *lower, const double *upper, int64_t n, int32_t ngroups) {
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (!lower && ngroups == 0) {
+    if (synchronize()) return 1;  // a device lookup may still read the table
+    free_weight_windows();
+    return 0;
+  }
+  const int64_t E = mesh_.ntets;
+  const char *why = ngroups < 1                       ? "ngroups must be >= 1 (0 with lower == NULL removes the windows)"
+                    : (!lower || !upper)              ? "null bound array"
+                    : n != int64_t(ngroups) * E       ? "n must be ngroups * num_elements"
+                                                      : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_weight_windows refused: %s\n", why);
+    return 1;
+  }
+  std::vector<double2> h = std::vector<double2>(size_t(n));
+  for (int64_t g = 0; g < ngroups; ++g)
+    for (int64_t o = 0; o < E; ++o) {
+      const size_t i = size_t(g * E + o);
+      const int k = ww_entry(lower[i], upper[i]);
+      if (k < 0) {
+        fprintf(stderr,
+                "[pumitally] ERROR: set_weight_windows refused: group %lld, element %lld: lower %g, upper %g (a window "
+                "needs finite bounds with upper > lower; lower <= 0 means no window)\n",
+                (long long)g, (long long)o, lower[i], upper[i]);
+        return 1;
+      }
+      h[size_t(g * E + mesh_.internal_of_orig[size_t(o)])] =
+          k ? make_double2(lower[i], upper[i]) : make_double2(kNoWindow, kNoWindow);
+    }
+  double2 *d = nullptr;
+  if (synchronize() || alloc_weight_windows(ngroups, &d)) return 1;
+  const cudaError_t e = cudaMemcpy(d, h.data(), h.size() * sizeof(double2), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(d);
+    fprintf(stderr, "[pumitally] CUDA error %s uploading the weight windows\n", cudaGetErrorString(e));
+    return 1;
+  }
+  free_weight_windows();
+  d_ww_ = d;
+  ww_groups_ = ngroups;
+  return 0;
+}
+
+int Engine::get_weight_windows(double *lower, double *upper, int64_t n) {
+  const int64_t E = mesh_.ntets, want = int64_t(ww_groups_) * E;
+  if (n != want || (n > 0 && (!lower || !upper))) {
+    fprintf(stderr, "[pumitally] ERROR: get_weight_windows: n must be ngroups * num_elements (%lld)\n", (long long)want);
+    return 1;
+  }
+  if (n == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  std::vector<double2> h = std::vector<double2>(size_t(n));
+  PTB_CUDA_OK(cudaMemcpy(h.data(), d_ww_, h.size() * sizeof(double2), cudaMemcpyDeviceToHost));
+  for (int64_t g = 0; g < ww_groups_; ++g)
+    for (int64_t i = 0; i < E; ++i) {
+      const size_t o = size_t(g * E + mesh_.orig_of_internal[size_t(i)]);
+      lower[o] = h[size_t(g * E + i)].x;
+      upper[o] = h[size_t(g * E + i)].y;
+    }
+  return 0;
+}
+
+// The statistics of (tally, time_bin, bin b, score) for every element are at base + b * bin_len() + e * stride_ of the
+// whole reported tally, which stats_view gives every rank.
+int Engine::generate_weight_windows(int32_t tally, int32_t score, int32_t time_bin, double ratio, double max_rel_err) {
+  const char *why = !batch_stats_                          ? "batch statistics are off (set_batch_statistics)"
+                    : batches_ < 2                         ? "at least two batches must be folded (end_batch)"
+                    : (tally != 0 && tally != 1)           ? "tally must be 0 (track length) or 1 (collision)"
+                    : (tally == 1 && !collision_)          ? "the collision estimator is off (set_collision_estimator)"
+                    : (score < 0 || score >= nscores_)     ? "score must be in [0, nscores)"
+                    : (time_bin < 0 || time_bin >= int32_t(nslices())) ? "time_bin must be in [0, max(ntime, 1))"
+                    : !(ratio > 1.0 && ratio <= DBL_MAX)   ? "ratio must be finite and > 1"
+                    : !(max_rel_err > 0.0)                 ? "max_rel_err must be > 0"
+                                                           : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: generate_weight_windows refused: %s\n", why);
+    return 1;
+  }
+  if (synchronize()) return 1;
+  const double *mean = nullptr, *m2 = nullptr;
+  double *tmp = nullptr;
+  double2 *d = nullptr;
+  unsigned long long *red = nullptr;
+  int rc = stats_view(&mean, &m2, &tmp);
+  if (!rc) rc = alloc_weight_windows(nbins_, &d);
+  if (!rc && cudaMalloc(reinterpret_cast<void **>(&red), size_t(nbins_) * sizeof(unsigned long long)) != cudaSuccess) {
+    fprintf(stderr, "[pumitally] ERROR: generate_weight_windows: %s\n", cudaGetErrorString(cudaGetLastError()));
+    rc = 1;
+  }
+  if (!rc) {
+    const size_t base = size_t(tally) * flux_len() + size_t(time_bin) * size_t(nbins_) * bin_len() + size_t(score);
+    const double c = 2.0 / (ratio + 1.0);
+    cudaError_t e = launch_ww_generate(mean + base, m2 + base, d_volume_, mesh_.ntets, nbins_, int64_t(bin_len()),
+                                       stride_, double(batches_), max_rel_err, c, ratio, red, d, compute_);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+    if (e != cudaSuccess) {
+      fprintf(stderr, "[pumitally] CUDA error %s generating the weight windows\n", cudaGetErrorString(e));
+      rc = 1;
+    }
+  }
+  cudaFree(red);
+  cudaFree(tmp);
+  if (rc) {
+    cudaFree(d);
+    return 1;
+  }
+  free_weight_windows();
+  d_ww_ = d;
+  ww_groups_ = nbins_;
+  return 0;
+}
+
+bool Engine::ww_lookup_refused(const char *what, bool particles, int64_t n) {
+  const char *why = !particles ? (n < 0 ? "npts must be >= 0" : nullptr)
+                    : n != n_  ? "n must be num_particles"
+                    : !initialized_ ? "called before CopyInitialPosition"
+                                    : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: weight windows %s refused: %s\n", what, why);
+  return why != nullptr;
+}
+
+int Engine::weight_windows_at_particles(const int32_t *groups, double *lower, double *upper, int32_t n) {
+  if (ww_lookup_refused("at the particles", true, n) || (n > 0 && (!lower || !upper))) return 1;
+  if (n == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const int32_t chunk = std::min(chunk_, n);
+  if (ensure_query_buffers(size_t(chunk), 2 * size_t(chunk))) return 1;
+  if (follow_last_stream(compute_)) return 1;  // reads the particle state the last move wrote
+  for (int32_t b = 0; b < n; b += chunk) {
+    const int32_t cnt = std::min(chunk, n - b);
+    if (groups)
+      PTB_CUDA_OK(cudaMemcpyAsync(d_qint_, groups + b, size_t(cnt) * sizeof(int32_t), cudaMemcpyHostToDevice, compute_));
+    PTB_CUDA_OK(launch_ww_particles(d_state_ + b, cnt, groups ? d_qint_ : nullptr, d_ww_, ww_groups_, mesh_.ntets,
+                                    d_qout_, d_qout_ + cnt, compute_));
+    PTB_CUDA_OK(cudaMemcpyAsync(lower + b, d_qout_, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+    PTB_CUDA_OK(cudaMemcpyAsync(upper + b, d_qout_ + cnt, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
+int Engine::weight_windows_at_particles_device(const int32_t *d_groups, double *d_lower, double *d_upper, int32_t n,
+                                               cudaStream_t stream) {
+  if (ww_lookup_refused("at the particles", true, n) || (n > 0 && (!d_lower || !d_upper))) return 1;
+  if (n == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
+  PTB_CUDA_OK(launch_ww_particles(d_state_, n, d_groups, d_ww_, ww_groups_, mesh_.ntets, d_lower, d_upper, stream));
+  return 0;
+}
+
+int Engine::weight_windows_at_points(const double *xyz, int64_t npts, const int32_t *groups, double *lower,
+                                     double *upper) {
+  if (ww_lookup_refused("at points", false, npts) || (npts > 0 && (!xyz || !lower || !upper))) return 1;
+  if (npts == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const int64_t chunk = std::min<int64_t>(chunk_, npts);
+  if (ensure_candidates() || ensure_query_buffers(size_t(chunk), 2 * size_t(chunk))) return 1;
+  const LocateParams p = locate_params();
+  for (int64_t b = 0; b < npts; b += chunk) {
+    const int64_t cnt = std::min(chunk, npts - b);
+    PTB_CUDA_OK(cudaMemcpyAsync(d_qxyz_, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
+    if (groups)
+      PTB_CUDA_OK(cudaMemcpyAsync(d_qint_, groups + b, size_t(cnt) * sizeof(int32_t), cudaMemcpyHostToDevice, compute_));
+    PTB_CUDA_OK(launch_ww_points(p, d_qxyz_, cnt, groups ? d_qint_ : nullptr, d_ww_, ww_groups_, mesh_.ntets, d_qout_,
+                                 d_qout_ + cnt, compute_));
+    PTB_CUDA_OK(cudaMemcpyAsync(lower + b, d_qout_, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+    PTB_CUDA_OK(cudaMemcpyAsync(upper + b, d_qout_ + cnt, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  return 0;
+}
+
+// The mesh tables location reads never change after construction, so a point lookup needs no ordering against moves.
+int Engine::weight_windows_at_points_device(const double *d_xyz, int64_t npts, const int32_t *d_groups, double *d_lower,
+                                            double *d_upper, cudaStream_t stream) {
+  if (ww_lookup_refused("at points", false, npts) || (npts > 0 && (!d_xyz || !d_lower || !d_upper))) return 1;
+  if (npts == 0) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_candidates()) return 1;
+  const LocateParams p = locate_params();
+  const int64_t step = int64_t(1) << 30;  // points per launch
+  for (int64_t b = 0; b < npts; b += step)
+    PTB_CUDA_OK(launch_ww_points(p, d_xyz + 3 * b, std::min(step, npts - b), d_groups ? d_groups + b : nullptr, d_ww_,
+                                 ww_groups_, mesh_.ntets, d_lower + b, d_upper + b, stream));
+  return 0;
+}
+
+int Engine::ww_arrays(VtkArrays &a) {
+  const size_t E = size_t(mesh_.ntets), G = size_t(ww_groups_);
+  std::vector<double> lo(G * E), hi(G * E);
+  if (get_weight_windows(lo.data(), hi.data(), int64_t(G * E))) return 1;
+  for (size_t g = 0; g < G; ++g) {
+    const std::string suffix = G == 1 ? "" : "_g" + std::to_string(g);
+    for (auto &[name, v] : {std::make_pair("ww_lower", &lo), std::make_pair("ww_upper", &hi)}) {
+      a.data.emplace_back(v->begin() + g * E, v->begin() + (g + 1) * E);  // (a moved vector keeps its storage)
+      a.named.emplace_back(name + suffix, a.data.back().data());
+      a.ncomp.push_back(1);
+    }
+  }
   return 0;
 }
 

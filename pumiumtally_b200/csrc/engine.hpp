@@ -150,6 +150,25 @@ class Engine {
   int save_checkpoint(const std::string &path);
   int load_checkpoint(const std::string &path);
   int merge_checkpoint(const std::string &path);
+  // Weight windows (weight_windows.cuh): ngroups (lower, upper) pairs per element, not tally state (no reset, set_*,
+  // end_batch, comm_init or checkpoint touches them).  set: host arrays [group][element] in the caller's numbering,
+  // n == ngroups * E; lower <= 0 is no window, stored (-1, -1); any other entry must be finite with upper > lower, or the
+  // call is refused and changes nothing.  lower == nullptr with ngroups == 0 removes them.  get: what set stored.
+  int set_weight_windows(const double *lower, const double *upper, int64_t n, int32_t ngroups);
+  int32_t weight_window_groups() const { return ww_groups_; }
+  int get_weight_windows(double *lower, double *upper, int64_t n);
+  // The MAGIC step over the batch statistics of (tally, score, time_bin), the score bins as groups: replaces the table.
+  // Collective with several ranks (stats_view).
+  int generate_weight_windows(int32_t tally, int32_t score, int32_t time_bin, double ratio, double max_rel_err);
+  // The window of group groups[i] (nullptr: 0) in particle i's parent element (n == num_particles) or at point i (located
+  // as locate_points does); (-1, -1) for a group outside [0, ngroups), an element without a window or a point outside.
+  // Nothing changes.  Host calls work through chunk-sized device buffers; the device calls are enqueued only.
+  int weight_windows_at_particles(const int32_t *groups, double *lower, double *upper, int32_t n);
+  int weight_windows_at_particles_device(const int32_t *d_groups, double *d_lower, double *d_upper, int32_t n,
+                                         cudaStream_t stream);
+  int weight_windows_at_points(const double *xyz, int64_t npts, const int32_t *groups, double *lower, double *upper);
+  int weight_windows_at_points_device(const double *d_xyz, int64_t npts, const int32_t *d_groups, double *d_lower,
+                                      double *d_upper, cudaStream_t stream);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -309,6 +328,14 @@ class Engine {
   ckpt::Fingerprint fingerprint();
   // load (merge == false) or merge the checkpoint at path, with a message on refusal
   int read_checkpoint(const std::string &path, bool merge);
+  // ---- weight windows (ww_kernels.cu) ----
+  int32_t ww_groups_ = 0;     // 0: no windows
+  double2 *d_ww_ = nullptr;   // [ww_groups_][internal element] (lower, upper), (-1, -1) where there is none
+  void free_weight_windows();
+  int alloc_weight_windows(int32_t ngroups, double2 **out);  // 16 ngroups E bytes; nothing changes when it fails
+  bool ww_lookup_refused(const char *what, bool particles, int64_t n);  // with a message
+  // the "ww_lower" / "ww_upper" arrays (with several groups "_g<g>" after each name), caller's numbering
+  int ww_arrays(VtkArrays &a);
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
     void *d = nullptr;    // device copy

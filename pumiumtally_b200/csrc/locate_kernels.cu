@@ -4,22 +4,11 @@
 // event; nothing here writes the particle state, the track-length tally or the statistics.
 #include <cmath>
 
+#include "fetch_record.cuh"
 #include "walk_kernels.hpp"
 
 namespace ptb {
 namespace {
-
-// One tet record as four 32-byte sectors, two 128-bit read-only loads each.
-__device__ __forceinline__ void fetch_record(const TetRecord *tets, int32_t e, double (&r)[16]) {
-  const double *p = tets[e].d;
-#pragma unroll
-  for (int f = 0; f < 4; ++f)
-    asm volatile(
-        "ld.global.nc.v2.f64 {%0,%1}, [%4];\n\t"
-        "ld.global.nc.v2.f64 {%2,%3}, [%4+16];"
-        : "=d"(r[4 * f]), "=d"(r[4 * f + 1]), "=d"(r[4 * f + 2]), "=d"(r[4 * f + 3])
-        : "l"(p + 4 * f));
-}
 
 // internal[i]: the internal element id of point i (for the evaluation kernel), out[i]: the caller's element id; either
 // may be nullptr.

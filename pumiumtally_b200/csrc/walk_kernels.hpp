@@ -169,4 +169,18 @@ cudaError_t launch_region_sums(const double *flux, int64_t array_len, int32_t st
                                const int32_t *elems, const int32_t *starts, const RegionLevel *levels, int nlevels,
                                double *scratch, int64_t scratch_len, double *out, cudaStream_t stream);
 
+// ww_kernels.cu.  Weight windows (weight_windows.cuh).  generate: table[b * E + e] <- ww_generate of the m0 value of
+// group b and element e of nb batches, at mean[b * pitch + e * stride] and m2 alike, with phimax the largest eligible
+// phi of the group; red [ngroups] is scratch (zeroed first, on the stream).
+cudaError_t launch_ww_generate(const double *mean, const double *m2, const double *volume, int64_t E, int32_t ngroups,
+                               int64_t pitch, int32_t stride, double nb, double max_rel_err, double c, double ratio,
+                               unsigned long long *red, double2 *table, cudaStream_t stream);
+// (lower[i], upper[i]) <- the window of group groups[i] (nullptr: 0) in particle i's parent element, for i < n
+cudaError_t launch_ww_particles(const ParticleState *state, int32_t n, const int32_t *groups, const double2 *table,
+                                int32_t ngroups, int64_t E, double *lower, double *upper, cudaStream_t stream);
+// the same at n points (AoS xyz) located as launch_locate locates them; n < 2^39
+cudaError_t launch_ww_points(const LocateParams &p, const double *xyz, int64_t n, const int32_t *groups,
+                             const double2 *table, int32_t ngroups, int64_t E, double *lower, double *upper,
+                             cudaStream_t stream);
+
 }  // namespace ptb

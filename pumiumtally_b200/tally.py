@@ -84,6 +84,17 @@ C_API = {
     "pumitally_save_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
     "pumitally_load_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
     "pumitally_merge_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "pumitally_set_weight_windows": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_int32]),
+    "pumitally_get_weight_window_groups": (C.c_int32, [C.c_void_p]),
+    "pumitally_get_weight_windows": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64]),
+    "pumitally_generate_weight_windows": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                                    C.c_double]),
+    "pumitally_get_weight_windows_at_particles": (C.c_int, [C.c_void_p, _ip, _dp, _dp, C.c_int32]),
+    "pumitally_get_weight_windows_at_particles_device": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "pumitally_get_weight_windows_at_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _ip, _dp, _dp]),
+    "pumitally_get_weight_windows_at_points_device": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -652,6 +663,105 @@ class PumiTally:
         end).  The open batch is left alone.  A refusal changes nothing."""
         if self._L.pumitally_merge_checkpoint(self._h, os.fsencode(os.fspath(path))):
             raise RuntimeError(f"merge_checkpoint({path!r}) failed")
+
+    # ---- weight windows ------------------------------------------------------------
+    def set_weight_windows(self, lower, upper=None):
+        """Set the window table: lower and upper [ngroups, num_elements] (caller's numbering; one group may be given as
+        [num_elements]).  lower <= 0 means no window; every other entry must be finite with upper > lower.  None as
+        lower removes the windows."""
+        if lower is None:
+            rc = self._L.pumitally_set_weight_windows(self._h, None, None, 0, 0)
+        else:
+            lo, hi = _host_f64(lower, "lower"), _host_f64(upper, "upper")
+            if lo.size != hi.size or lo.size % max(self.num_elements, 1):
+                raise TypeError("lower and upper must both hold ngroups * num_elements values")
+            ngroups = lo.size // max(self.num_elements, 1)
+            rc = self._L.pumitally_set_weight_windows(self._h, lo.ctypes.data_as(_dp), hi.ctypes.data_as(_dp), lo.size,
+                                                      ngroups)
+        if rc:
+            raise ValueError("set_weight_windows failed")
+
+    @property
+    def weight_window_groups(self) -> int:
+        """Number of energy groups of the window table, 0 without windows."""
+        return int(self._L.pumitally_get_weight_window_groups(self._h))
+
+    def weight_windows(self):
+        """(lower, upper), each [ngroups, num_elements] in the caller's numbering; (-1, -1) where there is no window."""
+        lo, hi = (np.empty((self.weight_window_groups, self.num_elements)) for _ in range(2))
+        if self._L.pumitally_get_weight_windows(self._h, lo.ctypes.data_as(_dp), hi.ctypes.data_as(_dp), lo.size):
+            raise RuntimeError("get_weight_windows failed")
+        return lo, hi
+
+    def generate_weight_windows(self, tally=0, score=0, time_bin=0, ratio=5.0, max_rel_err=float("inf")):
+        """Replace the window table by the MAGIC windows of the batch means of (tally, score, time_bin), the score bins
+        as energy groups: lower = phi / phimax * 2 / (ratio + 1), upper = lower * ratio where phi > 0 and its relative
+        error is <= max_rel_err (collective with several ranks)."""
+        if self._L.pumitally_generate_weight_windows(self._h, int(tally), int(score), int(time_bin), float(ratio),
+                                                     float(max_rel_err)):
+            raise RuntimeError("generate_weight_windows failed")
+
+    def weight_windows_at_particles(self, groups=None):
+        """(lower, upper) [num_particles] of each particle's parent element in energy group groups[i] (None: 0)."""
+        lo, hi = np.empty(self.num_particles), np.empty(self.num_particles)
+        g = None
+        if groups is not None:
+            g = np.ascontiguousarray(groups, dtype=np.int32).reshape(-1)
+            if g.size != self.num_particles:
+                raise TypeError("groups must hold one value per particle")
+        if self._L.pumitally_get_weight_windows_at_particles(self._h, None if g is None else g.ctypes.data_as(_ip),
+                                                             lo.ctypes.data_as(_dp), hi.ctypes.data_as(_dp), lo.size):
+            raise RuntimeError("get_weight_windows_at_particles failed")
+        return lo, hi
+
+    def weight_windows_at_particles_device(self, groups=None, stream=None, device=None):
+        """weight_windows_at_particles() into float64 CUDA tensors (groups: an int32 CUDA tensor or None), enqueued on
+        ``stream`` (default: the current torch stream) behind the last move."""
+        import torch
+
+        n = self.num_particles
+        dev = groups.device if groups is not None else torch.device("cuda", torch.cuda.current_device()
+                                                                     if device is None else device)
+        g = self._tensor_ptr(groups, torch.int32, n, "groups")
+        lo, hi = torch.empty(n, dtype=torch.float64, device=dev), torch.empty(n, dtype=torch.float64, device=dev)
+        if stream is None:
+            stream = torch.cuda.current_stream(dev).cuda_stream
+        if self._L.pumitally_get_weight_windows_at_particles_device(self._h, g, lo.data_ptr(), hi.data_ptr(), n, stream):
+            raise RuntimeError("get_weight_windows_at_particles_device failed")
+        return lo, hi
+
+    def weight_windows_at_points(self, points, groups=None):
+        """(lower, upper) [npts] at ``points`` [npts, 3], each located as locate() does; (-1, -1) outside the mesh."""
+        p, npts = self._points(points)
+        lo, hi = np.empty(npts), np.empty(npts)
+        g = None
+        if groups is not None:
+            g = np.ascontiguousarray(groups, dtype=np.int32).reshape(-1)
+            if g.size != npts:
+                raise TypeError("groups must hold one value per point")
+        if self._L.pumitally_get_weight_windows_at_points(self._h, p.ctypes.data_as(_dp), npts,
+                                                          None if g is None else g.ctypes.data_as(_ip),
+                                                          lo.ctypes.data_as(_dp), hi.ctypes.data_as(_dp)):
+            raise RuntimeError("get_weight_windows_at_points failed")
+        return lo, hi
+
+    def weight_windows_at_points_device(self, points, groups=None, stream=None):
+        """weight_windows_at_points() on a contiguous float64 CUDA tensor [npts, 3]: float64 CUDA tensors, enqueued on
+        ``stream`` (default: the current torch stream)."""
+        import torch
+
+        if not (points.is_cuda and points.dtype == torch.float64 and points.is_contiguous() and points.numel() % 3 == 0):
+            raise TypeError("points must be a contiguous float64 CUDA tensor of shape [npts, 3]")
+        npts = points.numel() // 3
+        g = self._tensor_ptr(groups, torch.int32, npts, "groups")
+        lo = torch.empty(npts, dtype=torch.float64, device=points.device)
+        hi = torch.empty(npts, dtype=torch.float64, device=points.device)
+        if stream is None:
+            stream = torch.cuda.current_stream(points.device).cuda_stream
+        if self._L.pumitally_get_weight_windows_at_points_device(self._h, points.data_ptr(), npts, g, lo.data_ptr(),
+                                                                 hi.data_ptr(), stream):
+            raise RuntimeError("get_weight_windows_at_points_device failed")
+        return lo, hi
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
