@@ -2,6 +2,7 @@
 written to a file, restored into a fresh engine and merged across independent runs.  A loaded engine must answer every
 accessor with the saving engine's bits; merged statistics must match numpy statistics of all the batches; every refusal
 must leave every accessor bit-identical."""
+import json
 import os
 import struct
 import subprocess
@@ -248,6 +249,93 @@ def test_merge_of_three_and_five_batches(tmp_path):
     z.eng.save_checkpoint(fz)
     a.eng.merge_checkpoint(fz)
     assert_same(after, snapshot(a), "merging 0 batches")
+
+
+K_MEAN, K_M2, K_REGION_MEAN, K_REGION_M2 = 3, 4, 5, 6  # checkpoint.hpp, SectionId
+
+
+def sections(path):
+    """{section id: payload} of a checkpoint file: after the header CRC, every section is id (u32), byte length (u64),
+    CRC-32 (u32) and the payload (checkpoint.hpp).  Every section's CRC is checked."""
+    data = read_bytes(path)
+    off = 156 + 8 * struct.unpack_from("<I", data, 152)[0] + 4
+    out = {}
+    while off < len(data):
+        sid, n, crc = struct.unpack_from("<IQI", data, off)
+        payload = data[off + 16:off + 16 + n]
+        assert len(payload) == n and zlib.crc32(payload) == crc, sid
+        out[sid] = payload
+        off += 16 + n
+    return out
+
+
+ODD_NREGIONS = 5
+
+
+def odd_engine(seed, batches):
+    """An engine whose statistics have odd lengths: no collision estimator, one score and no bins on the odd number
+    of elements of delaunay_box(60, seed=1), and ODD_NREGIONS slab regions.  The first E flights of every batch start
+    at the element centroids, so every element is scored in every batch."""
+    from pumiumtally_b200.mesh import delaunay_box
+
+    c, t = delaunay_box(60, seed=1)
+    E = len(t)
+    cen = c[t].mean(axis=1)
+    n = E + 1000
+    rng = np.random.default_rng(seed)
+    eng = PumiTally.from_arrays(c, t, n)
+    eng.set_collision_estimator(False)
+    eng.set_batch_statistics(True)
+    eng.set_regions(slab_map(c, t, ODD_NREGIONS))
+    eng.CopyInitialPosition(np.vstack([cen, rng.uniform(0.05, 0.95, (n - E, 3))]).reshape(-1).copy())
+    for _ in range(batches):
+        o = np.vstack([cen, eng.positions[E:]])
+        _move(eng, "plain", o, rng.uniform(0.0, 1.0, (n, 3)), np.ones(n, dtype=np.int8), rng.uniform(0.5, 1.5, n))
+        eng.end_batch()
+    return eng
+
+
+def print_merge_kernels(fa, fr, fm):
+    """(run by run_in_fresh_process) fa loaded into an odd_engine, fr merged into it under the profiler, the result
+    saved to fm; prints the names of the merge kernels that ran"""
+    from test_gpu_stats_kernels import kernels_launched
+
+    eng = odd_engine(0, 0)
+    eng.load_checkpoint(fa)
+    names = kernels_launched(lambda: eng.merge_checkpoint(fr), "batch_merge_kernel")
+    eng.save_checkpoint(fm)
+    print(json.dumps(names))
+
+
+def test_merge_of_odd_lengths_is_exact(tmp_path):
+    """Without the collision estimator, one score and no bins on an odd number of elements, the statistics have an odd
+    length (the double2 merge ends in its odd tail), and an odd number of regions puts the region M2 at an odd double
+    (the scalar merge).  The merged sections must equal merge_ref of the two files' sections bit for bit, and both
+    kernels must have run."""
+    from test_gpu_stats_kernels import merge_ref, run_in_fresh_process
+
+    a, r = odd_engine(61, 3), odd_engine(62, 4)
+    E = len(a.positions) - 1000
+    fa, fr, fm, fm2 = (str(tmp_path / f) for f in ("a.ckpt", "r.ckpt", "merged.ckpt", "merged_elsewhere.ckpt"))
+    a.save_checkpoint(fa)
+    r.save_checkpoint(fr)
+    a.merge_checkpoint(fr)
+    assert a.batches == 7
+    a.save_checkpoint(fm)
+    # the same merge after a load, in a process of its own, where the profiler sees which kernels ran
+    names = run_in_fresh_process("test_gpu_checkpoint", "print_merge_kernels", fa, fr, fm2)
+    assert any("batch_merge_kernel<true>" in x for x in names), names
+    assert any("batch_merge_kernel<false>" in x for x in names), names
+    assert read_bytes(fm2) == read_bytes(fm)
+    sa, sr, sm = (sections(f) for f in (fa, fr, fm))
+    f64 = lambda b: np.frombuffer(b, dtype="<f8")  # noqa: E731
+    for km, kq, length in ((K_MEAN, K_M2, E), (K_REGION_MEAN, K_REGION_M2, ODD_NREGIONS)):
+        assert len(sa[km]) == len(sr[km]) == 8 * length and length % 2 == 1
+        want = merge_ref(f64(sr[km]), f64(sr[kq]), 3.0, 4.0, f64(sa[km]), f64(sa[kq]))
+        np.testing.assert_array_equal(bits(f64(sm[km])), bits(want[0]), err_msg=f"section {km}")
+        np.testing.assert_array_equal(bits(f64(sm[kq])), bits(want[1]), err_msg=f"section {kq}")
+        # the last entry (the double2 kernel's odd tail for the element statistics) was merged
+        assert f64(sm[km])[-1] != f64(sa[km])[-1] and f64(sm[kq])[-1] != f64(sa[kq])[-1]
 
 
 def patched(data, off, new):

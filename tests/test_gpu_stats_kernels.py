@@ -1,12 +1,16 @@
-"""The batch-statistics kernels (stats_kernels.cu) called directly, through a test-only C wrapper of their launchers
-(tests/gpu_harness/stats_harness.cpp), at the lengths, offsets and rank shares that the engine only reaches on several
-GPUs: odd lengths, shares that start at an odd double (the scalar fold), shares that start inside a score record or
-hold only padding.  Every result must equal an exactly rounded host reference bit for bit, and every device buffer
-carries canaries on both sides that must come back untouched."""
+"""The batch-statistics kernels (stats_kernels.cu) and the weight-window generation (ww_kernels.cu) called directly,
+through a test-only C wrapper of their launchers (tests/gpu_harness/stats_harness.cpp), at the lengths, offsets and
+rank shares that the engine only reaches on several GPUs: odd lengths, shares that start at an odd double (the scalar
+fold and merge), shares that start inside a score record or hold only padding, region plans of several levels, and
+weight-window groups up to the engine's limit.  Every result must equal an exactly rounded host reference bit for
+bit, and every device buffer carries canaries on both sides that must come back untouched."""
 import ctypes as C
 import functools
+import json
+import math
 import os
 import subprocess
+import sys
 from fractions import Fraction
 
 import numpy as np
@@ -77,6 +81,25 @@ def fold_ref(x, mean, m2, div, nb):
     return mean, fma_exact(d, v - mean, m2)
 
 
+def merge_ref(mean_b, m2_b, na, nb, mean, m2):
+    """welford_merge(mean_b, m2_b, na, nb, mean, m2) as the device rounds it (the merge section below)."""
+    if nb == 0.0:
+        return mean.copy(), m2.copy()
+    if na == 0.0:
+        return mean_b.copy(), m2_b.copy()
+    n = na + nb
+    kb, kab = nb / n, (na * nb) / n
+    d = mean_b - mean
+    return fma_exact(d, kb, mean), fma_exact(d * d, kab, m2 + m2_b)
+
+
+def merge_unfused(mean_b, m2_b, na, nb, mean, m2):
+    """the same update with every product rounded before its sum: what the data must tell apart from merge_ref"""
+    n = na + nb
+    d = mean_b - mean
+    return mean + d * (nb / n), (m2 + m2_b) + (d * d) * ((na * nb) / n)
+
+
 def std_err_ref(m2, nb):
     return np.sqrt(m2 / (nb * (nb - 1.0)))
 
@@ -131,17 +154,25 @@ def harness(tmp_path_factory):
     from pumiumtally_b200 import build as pbuild
 
     lib = pbuild.build_library()
-    cuda_inc = os.path.join(os.path.dirname(os.path.dirname(pbuild._nvcc())), "include")
+    cuda = os.path.dirname(os.path.dirname(pbuild._nvcc()))
     so = str(tmp_path_factory.mktemp("stats_harness") / "libstats_harness.so")
     subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-O1", "-fPIC", "-shared",
                            "-I", os.path.join(ROOT, "pumiumtally_b200", "csrc"), "-I", os.path.join(ROOT, "include"),
-                           "-I", cuda_inc, os.path.join(HERE, "gpu_harness", "stats_harness.cpp"), "-o", so,
-                           "-L", os.path.dirname(lib), "-lpumitally", "-Wl,-rpath," + os.path.dirname(lib)])
+                           "-I", os.path.join(cuda, "include"), os.path.join(HERE, "gpu_harness", "stats_harness.cpp"),
+                           "-o", so, "-L", os.path.dirname(lib), "-lpumitally", "-Wl,-rpath," + os.path.dirname(lib),
+                           "-L", os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + os.path.join(cuda, "lib64")])
+    return _load_harness(so)
+
+
+def _load_harness(so):
     L = C.CDLL(so)
     p, i64, i32, f64 = C.c_void_p, C.c_int64, C.c_int32, C.c_double
     L.ptb_test_batch_fold.argtypes = [p, p, p, i64, p, f64, p]
     L.ptb_test_batch_readout.argtypes = [p, p, p, p, p, i64, i32, i32, i32, f64, C.c_int, p]
     L.ptb_test_batch_max_rel_err.argtypes = [p, p, i64, i64, i64, i64, i32, i32, f64, p, p]
+    L.ptb_test_batch_merge.argtypes = [p, p, p, p, i64, f64, f64, p]
+    L.ptb_test_region_sums.argtypes = [p, i64, i32, i32, i32, i64, i64, p, p, C.POINTER(C.c_int), p]
+    L.ptb_test_ww_generate.argtypes = [p, p, p, i64, i32, i64, i32, f64, f64, f64, f64, p, p, p]
     return L
 
 
@@ -155,6 +186,33 @@ def _sms():
     import torch
 
     return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def run_in_fresh_process(module, func, *args):
+    """module.func(*args) (str arguments) run in a new Python process; returns the JSON it printed last.
+
+    The tests that check which kernel a launcher chose use torch.profiler, and in a process that has been running for
+    more than about a minute it stops reporting kernels (torch 2.11 on an H100: the runtime API calls are still
+    recorded, the kernel launches they made are not).  So such a check cannot run inside a long test session; it runs
+    in a process of its own."""
+    cmd = [sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c",
+           f"import sys; sys.path[:0] = {[ROOT, HERE]!r}; import {module}; {module}.{func}(*sys.argv[1:])",
+           *map(str, args)]
+    r = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-3000:]
+    return json.loads(r.stdout.strip().splitlines()[-1])
+
+
+def kernels_launched(fn, pattern):
+    """names of the kernels containing `pattern` that fn() launched (in this process: see run_in_fresh_process)"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    return [e.name for e in prof.events() if pattern in e.name]
 
 
 class Guarded:
@@ -297,27 +355,167 @@ def test_fold_is_exact(harness, n, data, offs):
     if data == "zeros":
         assert not mean.values().any() and not m2.values().any()
 
-
-@gpu
-@pytest.mark.parametrize("offs", OFFSETS, ids=[f"x{a}m{b}q{c}" for a, b, c in OFFSETS])
-def test_fold_path_follows_alignment(harness, offs):
-    """The double2 kernel runs only when x, mean and m2 all start on a 16-byte boundary; otherwise the scalar one."""
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-
+def _fold_path_case(offs):
     n = 257
     x, div, states = _fold_case(n, "random")
     ox, om, oq = offs
     xg, dv = Guarded(x[0], ox), Guarded(div)
     mean, m2 = Guarded(np.zeros(n), om), Guarded(np.zeros(n), oq)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        assert harness.ptb_test_batch_fold(xg.ptr(), mean.ptr(), m2.ptr(), n, dv.ptr(), 1.0, _stream()) == 0
-        torch.cuda.synchronize()
-    names = [e.name for e in prof.events() if "batch_fold_kernel" in e.name]
+    return lambda L: L.ptb_test_batch_fold(xg.ptr(), mean.ptr(), m2.ptr(), n, dv.ptr(), 1.0, _stream()), mean, \
+        states[0][0]
+
+
+@gpu
+@pytest.mark.parametrize("offs", OFFSETS, ids=[f"x{a}m{b}q{c}" for a, b, c in OFFSETS])
+def test_fold_path_follows_alignment(harness, offs):
+    """The double2 kernel runs only when x, mean and m2 all start on a 16-byte boundary; otherwise the scalar one."""
+    names = _path_kernels(harness._name)["fold"][str(offs)]
     want = "batch_fold_kernel<true>" if offs == (0, 0, 0) else "batch_fold_kernel<false>"
     assert len(names) == 1 and want in names[0], names
-    assert_bits(mean.values(), states[0][0], "mean")
+    launch, mean, want_mean = _fold_path_case(offs)
+    assert launch(harness) == 0
+    assert_bits(mean.values(), want_mean, "mean")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Merge (merge_checkpoint: Chan's parallel update of two runs' statistics, in place)
+#
+# cuobjdump -sass of stats_kernels.cu.o (nvcc -O3, sm_90a, default flags), welford_merge in batch_merge_kernel<false>,
+# and in <true> both in its double2 loop and in its odd tail:
+#   n = na + nb, then nb / n and (na * nb) / n    DADD; correctly rounded divisions (MUFU.RCP64H + Newton DFMAs with
+#                                                 the slow-path call), na * nb a DMUL; hoisted out of the loop
+#   s = m2 + m2_b                                 DADD
+#   d = mean_b - mean                             DADD
+#   mean' = fma(d, nb / n, mean)                  DFMA
+#   m2' = fma(d * d, (na * nb) / n, s)            DMUL for d * d, then DFMA
+# The nb == 0 and na == 0 selects are FSELs in the tail; in the loops they are branches, hoisted out, to a loop that
+# keeps the arrays or copies mean_b and m2_b.  So merge_ref rounds the two updates once each.
+# ---------------------------------------------------------------------------------------------------------------------
+MERGE_DATA = ["random", "negative", "zeros", "opposite", "ill"]
+MERGE_COUNTS = [(0.0, 5.0), (5.0, 0.0), (1.0, 1.0), (3.0, 5.0), (1e6, 1.0), (2.0 ** 40, 3.0)]
+OFFSETS4 = [(a, b, c, d) for a in (0, 1) for b in (0, 1) for c in (0, 1) for d in (0, 1)]
+FULL_OFFSETS = (257, "scalar")  # every alignment of the four arrays; other lengths: all aligned, or all not
+MERGE_CASES = [(n, offs) for n in FOLD_N for offs in (OFFSETS4 if n in FULL_OFFSETS else [(0,) * 4, (1,) * 4])]
+
+
+@functools.lru_cache(maxsize=2)
+def _merge_data(n, data):
+    """(mean_b, m2_b, mean, m2): the statistics of the merged run and of the run it is merged into"""
+    rng = np.random.default_rng([n, MERGE_DATA.index(data)])
+    ln = lambda s: rng.lognormal(0.0, s, n)  # noqa: E731
+    if data == "random":
+        mean = rng.normal(0.0, 1.0, n) * ln(2.0)
+        mean_b = mean * rng.uniform(0.5, 1.5, n) + rng.normal(0.0, 1.0, n)
+        m2, m2_b = ln(2.0), ln(2.0)
+        mean[::13], m2_b[5::17] = 0.0, 0.0
+    elif data == "negative":
+        mean, mean_b, m2, m2_b = -ln(2.0), -ln(2.0), ln(2.0), ln(2.0)
+    elif data == "zeros":
+        mean, mean_b, m2, m2_b = (np.zeros(n) for _ in range(4))
+    elif data == "opposite":  # means of opposite sign: d is larger than either
+        mean, mean_b, m2, m2_b = ln(1.0), -ln(1.0), ln(2.0), ln(2.0)
+    else:  # the spread is 1e-9 of the mean, as in the fold
+        mean, mean_b = (1e8 * (1.0 + 1e-9 * rng.uniform(-1.0, 1.0, n)) for _ in range(2))
+        m2, m2_b = (0.1 * rng.uniform(0.0, 1.0, n) for _ in range(2))
+    return mean_b, m2_b, mean, m2
+
+
+def test_exact_fma_matches_fractions_on_merges():
+    """merge_ref's two fused operations on every kind of merge data, against the exact rational result; and the data
+    has elements where one rounding differs from two, so a merge that rounds the product first cannot pass."""
+    for data in MERGE_DATA:
+        mean_b, m2_b, mean, m2 = _merge_data(4097, data)
+        dm = dq = 0
+        for na, nb in MERGE_COUNTS:
+            if not na or not nb:
+                continue
+            n = na + nb
+            d = mean_b - mean
+            args_m, args_q = (d, np.full_like(d, nb / n), mean), (d * d, np.full_like(d, na * nb / n), m2 + m2_b)
+            assert_bits(fma_exact(*args_m), fma_fraction(*args_m), f"{data} ({na}, {nb}) mean")
+            assert_bits(fma_exact(*args_q), fma_fraction(*args_q), f"{data} ({na}, {nb}) m2")
+            got, un = merge_ref(mean_b, m2_b, na, nb, mean, m2), merge_unfused(mean_b, m2_b, na, nb, mean, m2)
+            dm += int((got[0] != un[0]).sum())
+            dq += int((got[1] != un[1]).sum())
+        if data != "zeros":
+            assert dq > 0, data
+            assert dm > 0 or data == "ill", data  # mean ~ 1e8 against d nb / n ~ 1e-1: the product's rounding is lost
+
+
+@gpu
+@pytest.mark.parametrize("n, offs", MERGE_CASES, ids=[f"{n}-b{a}{b}a{c}{d}" for n, (a, b, c, d) in MERGE_CASES])
+@pytest.mark.parametrize("data", MERGE_DATA)  # the offsets of one length vary fastest and share one _merge_data
+def test_merge_is_exact(harness, n, offs, data):
+    n = _fold_len(n)
+    mean_b, m2_b, mean, m2 = _merge_data(n, data)
+    ob, qb, om, oq = offs
+    gmb, gqb = Guarded(mean_b, ob, seed=1), Guarded(m2_b, qb, seed=2)
+    dm = dq = 0
+    for na, nb in MERGE_COUNTS:
+        label = f"n {n} offsets {offs} {data} (na, nb) = ({na}, {nb})"
+        gm, gq = Guarded(mean, om, seed=3), Guarded(m2, oq, seed=4)
+        assert harness.ptb_test_batch_merge(gmb.ptr(), gqb.ptr(), gm.ptr(), gq.ptr(), n, na, nb, _stream()) == 0
+        want = merge_ref(mean_b, m2_b, na, nb, mean, m2)
+        assert_bits(gm.values(), want[0], label + " mean")
+        assert_bits(gq.values(), want[1], label + " m2")
+        if nb == 0.0:  # a file of no batches: the arrays keep their bits
+            assert_bits(gm.values(), mean, label + " kept mean")
+            assert_bits(gq.values(), m2, label + " kept m2")
+        elif na == 0.0:  # merged into no batches: the file's bits
+            assert_bits(gm.values(), mean_b, label + " copied mean")
+            assert_bits(gq.values(), m2_b, label + " copied m2")
+        else:
+            un = merge_unfused(mean_b, m2_b, na, nb, mean, m2)
+            dm += int((want[0] != un[0]).sum())
+            dq += int((want[1] != un[1]).sum())
+        gm.assert_unchanged_outside(0, n, label + " mean")
+        gq.assert_unchanged_outside(0, n, label + " m2")
+    for g in (gmb, gqb):
+        g.assert_unchanged_outside(0, 0, "read-only input")
+    if n >= 255 and data != "zeros":  # the data tells the fused update from the twice-rounded one
+        assert dq > 0 and (dm > 0 or data == "ill"), (dm, dq)
+
+
+def _merge_path_case(offs):
+    n = 257
+    mean_b, m2_b, mean, m2 = _merge_data(n, "random")
+    ob, qb, om, oq = offs
+    gmb, gqb, gm, gq = Guarded(mean_b, ob), Guarded(m2_b, qb), Guarded(mean, om), Guarded(m2, oq)
+    return lambda L: L.ptb_test_batch_merge(gmb.ptr(), gqb.ptr(), gm.ptr(), gq.ptr(), n, 3.0, 5.0, _stream()), gq, \
+        merge_ref(mean_b, m2_b, 3.0, 5.0, mean, m2)[1]
+
+
+PATH_CASES = {"fold": (_fold_path_case, OFFSETS), "merge": (_merge_path_case, OFFSETS4)}
+
+
+def print_path_kernels(so):
+    """(run by run_in_fresh_process) {fold / merge: {offsets: the kernels one launch at those offsets ran}}"""
+    L = _load_harness(so)
+    res = {}
+    for which, (case, offsets) in PATH_CASES.items():
+        res[which] = {}
+        for offs in offsets:
+            launch, _, _ = case(offs)
+            res[which][str(offs)] = kernels_launched(lambda: launch(L), f"batch_{which}_kernel")
+    print(json.dumps(res))
+
+
+@functools.lru_cache(maxsize=1)
+def _path_kernels(so):
+    return run_in_fresh_process("test_gpu_stats_kernels", "print_path_kernels", so)
+
+
+@gpu
+@pytest.mark.parametrize("offs", OFFSETS4, ids=[f"b{a}{b}a{c}{d}" for a, b, c, d in OFFSETS4])
+def test_merge_path_follows_alignment(harness, offs):
+    """The double2 kernel runs only when mean_b, m2_b, mean and m2 all start on a 16-byte boundary; otherwise the
+    scalar one."""
+    names = _path_kernels(harness._name)["merge"][str(offs)]
+    want = "batch_merge_kernel<true>" if offs == (0, 0, 0, 0) else "batch_merge_kernel<false>"
+    assert len(names) == 1 and want in names[0], names
+    launch, m2, want_m2 = _merge_path_case(offs)
+    assert launch(harness) == 0
+    assert_bits(m2.values(), want_m2, "m2")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -327,14 +525,22 @@ def score_stride(nscores):
     return 1 if nscores <= 1 else 2 if nscores <= 2 else 4 if nscores <= 4 else 8
 
 
+READOUT_STRIDES = {  # the record stride of nscores results
+    "m0": score_stride,  # the tally's padded records
+    "moments": lambda s: 4 * score_stride(s),  # with the three moment slots of each score
+    "unpadded": lambda s: s,  # the region statistics: nscores results per record, no padding
+}
+# (unpadded only where it differs from m0)
+READOUT_CASES = [(s, lay) for s in range(1, 9) for lay in READOUT_STRIDES if lay != "unpadded" or score_stride(s) != s]
+
+
 @gpu
-@pytest.mark.parametrize("moments", [False, True], ids=["m0", "moments"])
-@pytest.mark.parametrize("nscores", range(1, 9))
+@pytest.mark.parametrize("nscores, layout", READOUT_CASES, ids=[f"{s}-{lay}" for s, lay in READOUT_CASES])
 @pytest.mark.parametrize("R", [1, 3, 6])
 @pytest.mark.parametrize("E", [1, 7, 719, 100_003])
-def test_readout_is_exact(harness, E, R, nscores, moments):
-    stride = score_stride(nscores) * (4 if moments else 1)
-    rng = np.random.default_rng([E, R, nscores, int(moments)])
+def test_readout_is_exact(harness, E, R, nscores, layout):
+    stride = READOUT_STRIDES[layout](nscores)
+    rng = np.random.default_rng([E, R, nscores, list(READOUT_STRIDES).index(layout)])
     size = R * E * stride
     mean = np.full(size, np.nan)  # padding and moment slots: NaN, so reading one shows
     m2 = np.full(size, np.nan)
@@ -574,3 +780,271 @@ def test_sharded_fold_and_readout_equal_unsharded(harness, layout):
             assert_bits(got[j], unsharded[j], f"{nranks} ranks: readout {j}")
     for g in xs + [dv, gv, go]:
         g.assert_unchanged_outside(0, 0, "read-only input")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Region sums (batch_stats.cuh, the documented order; launch_region_sums through the product's build_region_plan)
+# ---------------------------------------------------------------------------------------------------------------------
+CHUNK = 32  # kRegionChunk
+U = 2.0 ** -53
+
+
+def region_sums_ref(region, nregions, values, reverse=False):
+    """values [E, K] summed over the regions of region[E] in the documented order: a region's elements in ascending
+    internal id, cut into chunks of CHUNK consecutive inputs, each chunk summed left to right (reverse: right to
+    left), level after level until one value per region is left.  Returns ([nregions, K], levels)."""
+    values = np.asarray(values, dtype=np.float64).reshape(len(region), -1)
+    ids = np.flatnonzero(region >= 0)
+    ids = ids[np.argsort(region[ids], kind="stable")]  # ascending region, then ascending id
+    x, n = values[ids], np.bincount(region[ids], minlength=nregions)
+    levels = 0
+    while True:
+        levels += 1
+        c = np.where(n > CHUNK, -(-n // CHUNK), 1)
+        g = np.repeat(np.arange(nregions), c)  # region of every chunk
+        j = np.arange(c.sum()) - np.repeat(np.cumsum(c) - c, c)  # its index within the region
+        lo = (np.cumsum(n) - n)[g] + CHUNK * j
+        ln = np.clip(n[g] - CHUNK * j, 0, CHUNK)
+        acc = np.zeros((len(g), x.shape[1]))
+        acc[ln > 0] = x[lo[ln > 0] + (ln[ln > 0] - 1 if reverse else 0)]
+        for i in range(1, CHUNK):
+            t = ln > i
+            acc[t] = acc[t] + x[lo[t] + (ln[t] - 1 - i if reverse else i)]
+        x, n = acc, c
+        if (c == 1).all():
+            return x, levels
+
+
+def _shuffled_map(rng, sizes, unassigned):
+    """region of every internal id: sizes[g] elements in region g and `unassigned` in none (-1), shuffled"""
+    region = np.concatenate([np.repeat(np.arange(len(sizes), dtype=np.int32), sizes),
+                             np.full(unassigned, -1, dtype=np.int32)])
+    return rng.permutation(region), len(sizes)
+
+
+REGION_SIZES = [0, 1, 31, 32, 33, 1023, 1024, 1025, 32769]  # 32769 takes four levels
+
+
+@functools.lru_cache(maxsize=1)
+def _region_map(name):
+    """(region of every internal id, nregions, levels)"""
+    rng = np.random.default_rng(len(name))
+    if name == "sizes":
+        region, nreg = _shuffled_map(rng, REGION_SIZES, 501)
+        return region, nreg, 4
+    if name == "singletons":
+        return rng.permutation(4099).astype(np.int32), 4099, 1
+    return np.zeros(33 * 1024 + 7, dtype=np.int32), 1, 4  # one region of every element
+
+
+def _cancelling(rng, shape):
+    """O(1) terms with +-1e16 among them: the order of a sum decides which of them survive"""
+    v = rng.normal(0.0, 1.0, shape) * rng.lognormal(0.0, 1.0, shape)
+    big = rng.random(shape) < 0.03
+    v[big] = np.where(rng.random(int(big.sum())) < 0.5, 1e16, -1e16)
+    return v
+
+
+def test_region_reference_within_the_fsum_bound():
+    """region_sums_ref against math.fsum: each level adds at most CHUNK terms left to right, so the error is at most
+    h u / (1 - h u) * sum |x| with h = levels * (CHUNK - 1); and the order is not fsum's, nor the reversed one."""
+    rng = np.random.default_rng(11)
+    for name in ("sizes", "singletons", "one"):
+        region, nreg, levels = _region_map(name)
+        x = _cancelling(rng, len(region))
+        got, lv = region_sums_ref(region, nreg, x)
+        rev, _ = region_sums_ref(region, nreg, x, reverse=True)
+        assert lv == levels, name
+        h = levels * (CHUNK - 1)
+        apart = 0
+        for g in range(nreg):
+            xs = x[region == g]
+            want = math.fsum(xs)
+            assert abs(got[g, 0] - want) <= h * U / (1 - h * U) * math.fsum(np.abs(xs)), (name, g)
+            apart += got[g, 0] != want and got[g, 0] != rev[g, 0]
+        assert apart > 0 or name != "sizes", name  # (one region may happen to agree with one of them)
+    # one region of 33 elements in two chunks: ((x0 + ... + x31) + x32), summed left to right within the first
+    x = np.array([1e16, 1.0, -1e16] + [0.5] * 29 + [3.0])
+    got, lv = region_sums_ref(np.zeros(33, dtype=np.int32), 1, x)
+    assert lv == 2 and got[0, 0] == ((1e16 + 1.0) - 1e16 + 0.5 * 29) + 3.0
+
+
+@gpu
+@pytest.mark.parametrize("gap", [False, True], ids=["packed", "gap"])
+@pytest.mark.parametrize("narrays", [1, 3, 6])
+@pytest.mark.parametrize("nscores", range(1, 9))
+@pytest.mark.parametrize("name", ["sizes", "singletons", "one"])
+def test_region_sums_are_exact(harness, name, nscores, narrays, gap):
+    region, nreg, levels = _region_map(name)
+    E = len(region)
+    stride = score_stride(nscores)
+    pitch = E * stride + (5 if gap else 0)
+    rng = np.random.default_rng([levels, nscores, narrays, int(gap)])
+    vals = _cancelling(rng, (narrays, E, nscores))
+    vals[:, region < 0] = np.nan  # elements in no region must not reach a sum
+    if name == "sizes":  # the one-element region is its value, -0.0 included
+        vals[0, np.flatnonzero(region == 1)[0], 0] = -0.0
+    src = np.full(narrays * pitch, np.nan)  # padding slots and the gap: NaN
+    for a in range(narrays):
+        src[a * pitch:a * pitch + E * stride].reshape(E, stride)[:, :nscores] = vals[a]
+    gs = Guarded(src, 1, seed=1)
+    out = Guarded(np.full(narrays * nreg * nscores, np.nan), seed=2)
+    nlevels = C.c_int(-1)
+    assert harness.ptb_test_region_sums(region.ctypes.data, E, nreg, nscores, stride, narrays, pitch, gs.ptr(),
+                                        out.ptr(), C.byref(nlevels), _stream()) == 0, "scratch canary"
+    assert nlevels.value == levels
+    want, lv = region_sums_ref(region, nreg, vals.transpose(1, 0, 2))  # [nregions, narrays * nscores]
+    assert lv == levels
+    want = want.reshape(nreg, narrays, nscores).transpose(1, 0, 2).reshape(-1)
+    got = out.values()
+    assert_bits(got, want, f"{name} nscores {nscores} narrays {narrays} gap {gap}")
+    out.assert_unchanged_outside(0, out.n, "out")
+    gs.assert_unchanged_outside(0, 0, "read-only input")
+    assert not np.isnan(got).any()
+    got = got.reshape(narrays, nreg, nscores)
+    if name == "sizes":
+        assert np.signbit(got[0, 1, 0]) and got[0, 1, 0] == 0.0
+        empty = got[:, 0, :]  # region 0 holds no element: +0.0
+        assert (empty.view(np.int64) == 0).all()
+        rev, _ = region_sums_ref(region, nreg, vals.transpose(1, 0, 2), reverse=True)
+        rev = rev.reshape(nreg, narrays, nscores).transpose(1, 0, 2)
+        fs = np.array([[[math.fsum(vals[a, region == g, k]) for k in range(nscores)] for g in range(nreg)]
+                       for a in range(narrays)])
+        assert ((got != rev) & (got != fs)).any()  # the order is checked, not just a sum
+    if name == "singletons":
+        assert_bits(got, vals[:, np.argsort(region), :], "every element its own region")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Weight windows (weight_windows.cuh, ww_kernels.cu): the MAGIC step over raw mean, m2 and volume
+# ---------------------------------------------------------------------------------------------------------------------
+def ww_ref(mean, m2, vol, nb, max_rel_err, ratio):
+    """(phimax [G], lower [G, E], upper [G, E]) of the m0 values mean, m2 [G, E]: phi and r are batch_readout kinds
+    0 and 2, eligible where phi is finite and > 0 and r <= max_rel_err; lower = (phi / phimax) * c, upper =
+    lower * ratio with c = 2 / (ratio + 1); (-1, -1) where not eligible, phimax 0 for a group with no eligible
+    element."""
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        phi = mean / vol
+        r = rel_ref(phi, std_err_ref(m2, nb) / vol)
+        ok = (phi > 0.0) & (phi <= np.finfo(np.float64).max) & (r <= max_rel_err)
+        pm = np.where(ok, phi, 0.0).max(axis=1)
+        lo = (phi / pm[:, None]) * (2.0 / (ratio + 1.0))
+        hi = lo * ratio
+    return pm, np.where(ok, lo, -1.0), np.where(ok, hi, -1.0)
+
+
+WW_GROUPS = [1, 3, 16, 4096]
+WW_E = [1, 5, 31, 257, 100_003]
+WW_CASES = [(G, E) for G in WW_GROUPS for E in WW_E if (G, E) != (4096, 100_003)]  # 4096 x 100003 x 16 B: 6.5 GB
+WW_CALLS = [(5.0, float("inf")), (2.0, 0.3), (1.0 + 2.0 ** -40, 0.05), (1e6, 1.0)]  # (ratio, max_rel_err)
+NB_WW = 6.0
+
+
+def _peak(g, E):
+    """where group g's largest phi lies.  Group 0: the last element, in the last grid-stride step when one block
+    strides over the mesh.  Group g > 0: the last element at thread 255 - 33 ((g - 1) % 8) of a 256-thread block,
+    so that the maxima of groups 1 to 8 lie in warps 7 down to 0."""
+    o = 255 - 33 * ((g - 1) % 8)
+    if g == 0 or E - 1 < o:
+        return (E - 1) if g == 0 else (g - 1) % E
+    return (E - 1) - ((E - 1 - o) % 256)
+
+
+def _ww_case(rng, G, E, stride, score, gap, base):
+    """(mean array, m2 array, volumes, mean [G, E], m2 [G, E], pitch): mean and m2 of group b and element e at
+    base + b * pitch + e * stride + score, NaN in every other slot.  phi spans 6 decades across groups.  A tenth of
+    the elements have a phi of 0, -0.0, -1, NaN or +-inf, a tenth a relative error of 10; the others up to 0.25.
+    Each group's largest phi is at _peak, with a relative error of 0.01: eligible under every limit of WW_CALLS."""
+    pitch = E * stride + gap
+    vol = rng.uniform(0.05, 3.0, E)
+    phi = rng.uniform(0.5, 1.0, (G, E)) * 10.0 ** rng.integers(-3, 3, (G, 1))
+    rel = rng.uniform(0.0, 0.25, (G, E))
+    special, high_r = rng.random((G, E)) < 0.1, rng.random((G, E)) < 0.1
+    for g in range(G):
+        p = _peak(g, E)
+        phi[g, p], rel[g, p], special[g, p], high_r[g, p] = 1.5 * phi[g].max(), 0.01, False, False
+    rel[high_r] = 10.0
+    mean = phi * vol
+    m2 = (rel * mean) ** 2 * NB_WW * (NB_WW - 1.0)
+    mean[special] = rng.choice(np.array([0.0, -0.0, -1.0, np.nan, np.inf, -np.inf]), int(special.sum()))
+    arr, arr2 = np.full(base + G * pitch, np.nan), np.full(base + G * pitch, np.nan)
+    idx = base + np.arange(G)[:, None] * pitch + np.arange(E)[None, :] * stride + score
+    arr[idx], arr2[idx] = mean, m2
+    return arr, arr2, vol, mean, m2, pitch
+
+
+def _ww_run(harness, gm, gq, gv, base, score, E, G, pitch, stride, mean, m2, vol, mre, ratio, label):
+    """one launch_ww_generate on the m0 values at gm / gq + base + score, checked bit for bit against ww_ref, with
+    canaries on red and the table; returns ww_ref's (phimax, lower, upper)"""
+    red = Guarded(np.random.default_rng(G).integers(0, 2 ** 63, G).astype(np.uint64), seed=7)  # zeroed first
+    table = Guarded(np.full(2 * G * E, np.nan), seed=8)
+    assert harness.ptb_test_ww_generate(gm.ptr(base + score), gq.ptr(base + score), gv.ptr(), E, G, pitch, stride,
+                                        NB_WW, mre, 2.0 / (ratio + 1.0), ratio, red.ptr(), table.ptr(),
+                                        _stream()) == 0
+    pm, lo, hi = ww_ref(mean, m2, vol, NB_WW, mre, ratio)
+    assert_bits(red.values().view(np.float64), pm, label + " group maxima")
+    got = table.values().reshape(G, E, 2)
+    assert_bits(got[:, :, 0], lo, label + " lower")
+    assert_bits(got[:, :, 1], hi, label + " upper")
+    red.assert_unchanged_outside(0, G, label + " red")
+    table.assert_unchanged_outside(0, table.n, label + " table")
+    return pm, lo, hi
+
+
+@gpu
+@pytest.mark.parametrize("stride", [1, 2, 4, 8])
+@pytest.mark.parametrize("G, E", WW_CASES, ids=[f"g{G}-e{E}" for G, E in WW_CASES])
+def test_ww_generate_is_exact(harness, G, E, stride):
+    rng = np.random.default_rng([G, E, stride])
+    score = (G + E) % stride
+    gap = 3 if stride % 2 else 0  # a pitch with a gap, or E * stride
+    base = 2 * E * stride + 1  # a time bin's base, taken by pointer: odd, so the arrays start at an odd double
+    arr, arr2, vol, mean, m2, pitch = _ww_case(rng, G, E, stride, score, gap, base)
+    gm, gq, gv = Guarded(arr, 0, seed=1), Guarded(arr2, 1, seed=2), Guarded(vol, 1, seed=3)
+    for ratio, mre in WW_CALLS:
+        label = f"G {G} E {E} stride {stride} ratio {ratio} max_rel_err {mre}"
+        pm, lo, _ = _ww_run(harness, gm, gq, gv, base, score, E, G, pitch, stride, mean, m2, vol, mre, ratio, label)
+        peaks = [_peak(g, E) for g in range(G)]
+        assert (pm == mean[range(G), peaks] / vol[peaks]).all(), label
+        assert (lo[range(G), peaks] == 2.0 / (ratio + 1.0)).all(), label
+    for g in (gm, gq, gv):
+        g.assert_unchanged_outside(0, 0, "read-only input")
+
+
+@gpu
+@pytest.mark.parametrize("E", [1, 5, 257, 100_003])
+def test_ww_generate_edges(harness, E):
+    """r at the limit and one ulp below it; an infinite limit with an infinite r; phi of 0, -0.0, negative, NaN and
+    +-inf; a group whose only eligible element is the last; a group with none; tied maxima."""
+    G = 5
+    rng = np.random.default_rng(E)
+    vol = rng.uniform(0.5, 2.0, E)
+    vol[-1] = vol[0]  # the tie of group 3: equal means in equal volumes
+    mean = rng.uniform(0.1, 1.0, (G, E)) * vol
+    specials = np.array([0.0, -0.0, -2.0, np.nan, np.inf, -np.inf])
+    for g in (1, 2):  # group 1: every element ineligible but the last; group 2: none eligible
+        mean[g] = specials[np.arange(E) % len(specials)]
+    mean[1, -1] = 0.25 * vol[-1]
+    mean[3, 0] = mean[3, -1] = 4.0 * vol[0]  # group 3: the largest phi twice, at the first and the last element
+    # group 4: the largest phi has an infinite relative error (m2 = inf), the next largest is element k, whose relative
+    # error of 0.1 is the largest of all the others (0.01)
+    k = E // 2
+    mean[4, -1], mean[4, k] = 8.0 * vol[-1], 6.0 * vol[k]
+    with np.errstate(invalid="ignore", over="ignore"):
+        m2 = (0.01 * mean) ** 2 * NB_WW * (NB_WW - 1.0)
+    m2[4, k] = (0.1 * mean[4, k]) ** 2 * NB_WW * (NB_WW - 1.0)
+    m2[4, -1] = np.inf
+    phi_k = mean[4, k] / vol[k]
+    r_k = float(rel_ref(np.array([phi_k]), std_err_ref(np.array([m2[4, k]]), NB_WW) / vol[k])[0])
+    gm, gq, gv = Guarded(mean.reshape(-1), 1, seed=1), Guarded(m2.reshape(-1), 0, seed=2), Guarded(vol, 0, seed=3)
+    seen = []
+    for mre in (float("inf"), r_k, np.nextafter(r_k, 0.0)):
+        label = f"E {E} max_rel_err {mre!r}"
+        pm, lo, hi = _ww_run(harness, gm, gq, gv, 0, 0, E, G, E, 1, mean, m2, vol, mre, 3.0, label)
+        assert pm[1] == 0.25 and (lo[1, :-1] == -1.0).all() and lo[1, -1] == 0.5, label
+        assert pm[2] == 0.0 and (lo[2] == -1.0).all() and (hi[2] == -1.0).all(), label
+        if E > 1:
+            assert pm[3] == 4.0 and lo[3, 0] == lo[3, -1] == 0.5, label
+        seen.append(pm[4])
+    if E > 1:  # inf: the infinite r counts; r_k: the element at the limit does; one ulp below r_k: it does not
+        assert seen[0] == 8.0 and seen[1] == phi_k and seen[2] < phi_k, seen
