@@ -65,6 +65,19 @@ inline int MoveToNextLocationTimed(const PumiTally &tally, double *particle_orig
 // gives the gradient of the flux's linear projection.
 inline int SetMoments(const PumiTally &tally, int32_t order) { return pumitally_set_moments(engine_of(tally), order); }
 
+// Face currents (see pumitally_set_face_currents in pumitally_c.h): the weight crossing every element face in the walk,
+// per score bin and time bin.  GetFaceCurrentResults: direction 0 outgoing, 1 incoming; kind 0 value, 1 batch mean,
+// 2 standard error, 3 relative error; n = ntime * nbins * E * 4, [time][bin][element][face].  GetLeakage: the outgoing
+// current summed over the hull faces, n = ntime * nbins.
+inline int SetFaceCurrents(const PumiTally &tally, int32_t on) { return pumitally_set_face_currents(engine_of(tally), on); }
+inline int32_t GetFaceCurrents(const PumiTally &tally) { return pumitally_get_face_currents(engine_of(tally)); }
+inline int GetFaceCurrentResults(const PumiTally &tally, int32_t direction, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_face_current_results(engine_of(tally), direction, kind, out, n);
+}
+inline int GetLeakage(const PumiTally &tally, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_leakage(engine_of(tally), kind, out, n);
+}
+
 // Point queries (see pumitally_locate_points in pumitally_c.h): the element containing each of npts points (AoS xyz),
 // -1 outside the mesh; and every normalised result at the points, [time][bin][score][point], n = npts or
 // ntime * nbins * nscores * npts (the linear reconstruction with moments, NaN outside).  out_elem may be nullptr.

@@ -399,6 +399,30 @@ int pumitally_tally_collisions_at_particles_device(pumitally_engine *e, const in
                                                    void *stream);
 int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *out, int64_t n);
 
+/* ---- additive: face currents (the weight crossing every element face, and the leakage through the hull) ----
+ * pumitally_set_face_currents(e, 1) makes every move -- plain, binned, scored and timed, host and device pointers --
+ * also tally, for each face a track crosses in the tally phase of a move, the particle's weight (weights[i], no
+ * response) as the outgoing partial current of the face of the element it leaves, which is the incoming partial
+ * current of the same face of the neighbour.  A flight that leaves through the hull counts as outgoing through that
+ * hull face (leakage); nothing enters through the hull.  A relocation, the end of a flight, a face the iteration limit
+ * stopped the walk at and a bad track add nothing.  Currents are kept per score bin (particles whose bin is outside
+ * [0, nbins) add nothing) and per time bin (the bin that holds the crossing time; a crossing exactly on an edge belongs
+ * to the bin below), not per score.  0 (the default) stops them; any other value is refused.  The call resets the tally
+ * and discards the folded batches; refused after pumitally_comm_init.  Currents change no other result.
+ *
+ * pumitally_get_face_current_results(e, direction, kind, out, n): direction 0 outgoing, 1 incoming; kind 0 the open
+ * tally divided by the per-source divisor of the source normalisation (not by an area or volume), 1 the batch mean,
+ * 2 its standard error, 3 its relative error (kinds 1-3 need batch statistics, 2-3 two batches).  n = ntime * nbins *
+ * E * 4, [time][bin][element][face] in the caller's numbering, face f opposite local vertex f of the element (the
+ * convention of pumitally_get_adjacency).  pumitally_get_leakage(e, kind, out, n): the outgoing current summed over all
+ * hull faces, summed on the device in a fixed order, kinds as above, n = ntime * nbins, [time][bin].  A wrong n or
+ * kind is refused and changes nothing.  Both are collective after pumitally_reduce_tally_to_owners, as pumitally_get_flux.
+ * Checkpoints carry the currents; a checkpoint saved with the other setting is refused. */
+int pumitally_set_face_currents(pumitally_engine *e, int32_t on);
+int32_t pumitally_get_face_currents(const pumitally_engine *e);
+int pumitally_get_face_current_results(pumitally_engine *e, int32_t direction, int32_t kind, double *out, int64_t n);
+int pumitally_get_leakage(pumitally_engine *e, int32_t kind, double *out, int64_t n);
+
 /* ---- additive: batch statistics (mean, standard and relative errors over batches, on the device) ----
  * A Monte Carlo tally is reported as mean +- standard error over batches.  pumitally_set_batch_statistics(e, 1) keeps,
  * for every reported result (the track-length tally and, with the estimator on, the collision tally: every time bin,

@@ -271,6 +271,19 @@ int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *o
   return guarded(e, [&](ptb::Engine &g) { return g.get_collision_results(kind, out, n); });
 }
 
+int pumitally_set_face_currents(pumitally_engine *e, int32_t on) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_face_currents(on); });
+}
+int32_t pumitally_get_face_currents(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "face_currents")) : 0;
+}
+int pumitally_get_face_current_results(pumitally_engine *e, int32_t direction, int32_t kind, double *out, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_face_current_results(direction, kind, out, n); });
+}
+int pumitally_get_leakage(pumitally_engine *e, int32_t kind, double *out, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_leakage(kind, out, n); });
+}
+
 int pumitally_set_batch_statistics(pumitally_engine *e, int32_t on) {
   return guarded(e, [&](ptb::Engine &g) { return g.set_batch_statistics(on); });
 }

@@ -158,6 +158,8 @@ Engine::~Engine() {
     if (u->ev) cudaEventDestroy(u->ev);
   }
   cudaFree(d_edges_);
+  cudaFree(d_face_opp_);
+  cudaFree(d_hull_slots_);
   if (ev_copy0_) cudaEventDestroy(ev_copy0_);
   if (ev_copy1_) cudaEventDestroy(ev_copy1_);
   if (ev_ar0_) cudaEventDestroy(ev_ar0_);
@@ -346,9 +348,13 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   if (follow_last_stream(stream)) return 1;
   if (d_dest) flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on; the last exchange no longer describes it
   const int64_t slice = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
+  // face currents: [time][bin][element][4] after the tallies; a binned move's unmatched particles cross into the scratch
+  // array after the unreported flux array
+  const int64_t E4 = 4 * int64_t(mesh_.ntets), cur_slice = int64_t(nbins_) * E4;
+  double *cur = currents_ ? d_flux_ + current_base() : nullptr;
   if (!(t.bins && d_dest))
     return launch_range_into(d_flux_, d_origin, d_dest, d_flying, d_weights, begin, end, stream, t, slice, move_variant_,
-                             move_tag_);
+                             move_tag_, cur, cur_slice);
   // Score filter: particles are independent and a particle that does not fly is not touched, so the range
   // is walked once per bin with the flying flags masked down to that bin's particles and the tally pointed
   // at that bin's flux array -- the walk kernels themselves are the unfiltered ones.  One more pass (array
@@ -364,7 +370,9 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
     ++launches_;
     // the unreported array follows every reported one (with a time filter, all time bins of a bin-b pass go to it)
     if (launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : reported_len()), d_origin, d_dest, d_mask_,
-                          d_weights, begin, end, stream, t, b < nbins_ ? slice : 0, variant, tag))
+                          d_weights, begin, end, stream, t, b < nbins_ ? slice : 0, variant, tag,
+                          cur ? (b < nbins_ ? cur + b * E4 : d_flux_ + reported_len() + bin_len()) : nullptr,
+                          b < nbins_ ? cur_slice : 0))
       return 1;
   }
   return 0;
@@ -372,16 +380,18 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
 
 int Engine::launch_range_into(double *d_flux, const double *d_origin, const double *d_dest, const int8_t *d_flying,
                               const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
-                              const MoveTally &t, int64_t slice, int variant, int tag) {
+                              const MoveTally &t, int64_t slice, int variant, int tag, double *d_cur,
+                              int64_t cur_slice) {
   if (d_dest && d_weights && initial_weight_pending_)  // first tracks of the batch: their total weight
     PTB_CUDA_OK(launch_sum_flying_weights(d_flying, d_weights, begin, end, d_initial_weight_, stream));
-  TimedWalkParams tp{};
+  CurrentWalkParams tp{};
   WalkParams &p = tp;
   const bool timed_walk = t.kind == MoveTally::kTimed && d_dest;
   // with moments every tallying move is a scored one; the plain and binned moves have one score and no responses
   const bool scored = scored_move(t) && d_dest;
   if (scored) tp.sc = ScoreParams{t.responses, nscores_, stride_};
   if (timed_walk) tp.tm = TimeParams{d_edges_, t.times, t.speeds, ntime_, slice};
+  if (scored && currents_) tp.cu = CurrentParams{d_cur, cur_slice};
   p.tets = d_tets_;
   p.links = d_links_;
   p.verts = d_verts_;
@@ -466,7 +476,7 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
     launches_ += 5;  // count, 3-kernel scan, scatter
     p.flying = nullptr;  // order[] holds flying particles only
   }
-  const cudaError_t err = scored ? launch_walk_tallied(tp, timed_walk, moments_ > 0, variant, block_, stream)
+  const cudaError_t err = scored ? launch_walk_tallied(tp, timed_walk, moments_ > 0, currents_, variant, block_, stream)
                                  : launch_walk(p, variant, block_, stream);
   if (err != cudaSuccess) {
     fprintf(stderr, "[pumitally] ERROR: walk kernel %d: %s (scored, timed and moment moves run on the kernels 0, 8, 16 "
@@ -1127,7 +1137,7 @@ int Engine::set_score_bins(int32_t nbins) {
     fprintf(stderr, "[pumitally] ERROR: set_score_bins after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins, nscores_, ntime_, moments_, collision_);
+  return resize_flux(nbins, nscores_, ntime_, moments_, collision_, currents_);
 }
 
 // Scores (walk_core.cuh, ScoreParams): the flux array becomes [bin][element][score_stride(nscores)].
@@ -1137,7 +1147,7 @@ int Engine::set_scores(int32_t nscores) {
     fprintf(stderr, "[pumitally] ERROR: set_scores after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores, ntime_, moments_, collision_);
+  return resize_flux(nbins_, nscores, ntime_, moments_, collision_, currents_);
 }
 
 // Time filter (walk_core.cuh, TimeParams): the flux array becomes [time][bin][element][stride], the edges live on
@@ -1148,7 +1158,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (!edges && nedges == 0) {  // no time filter
-    if (resize_flux(nbins_, nscores_, 0, moments_, collision_)) return 1;
+    if (resize_flux(nbins_, nscores_, 0, moments_, collision_, currents_)) return 1;
     cudaFree(d_edges_);
     d_edges_ = nullptr;
     return 0;
@@ -1163,7 +1173,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (cudaMemcpy(ne, edges, size_t(nedges) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
-      resize_flux(nbins_, nscores_, nedges - 1, moments_, collision_)) {
+      resize_flux(nbins_, nscores_, nedges - 1, moments_, collision_, currents_)) {
     cudaGetLastError();
     cudaFree(ne);
     return 1;
@@ -1180,7 +1190,7 @@ int Engine::set_moments(int32_t order) {
     fprintf(stderr, "[pumitally] ERROR: set_moments after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores_, ntime_, order, collision_);
+  return resize_flux(nbins_, nscores_, ntime_, order, collision_, currents_);
 }
 
 // Collision estimator (walk_core.cuh, collision_event): a second tally of the same layout after the track-length one.
@@ -1190,16 +1200,28 @@ int Engine::set_collision_estimator(int32_t on) {
     fprintf(stderr, "[pumitally] ERROR: set_collision_estimator after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores_, ntime_, moments_, on != 0);
+  return resize_flux(nbins_, nscores_, ntime_, moments_, on != 0, currents_);
 }
 
-int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision) {
+// Face currents (walk_core.cuh, CurrentParams): the current slots and the leakage slots after both tallies.
+int Engine::set_face_currents(int32_t on) {
+  if (on != 0 && on != 1) return 1;
+  if (nccl_comm_) {
+    fprintf(stderr, "[pumitally] ERROR: set_face_currents after comm_init (the exchange buffers are sized by then)\n");
+    return 1;
+  }
+  return resize_flux(nbins_, nscores_, ntime_, moments_, collision_, on != 0);
+}
+
+int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents) {
   if (synchronize()) return 1;
   const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores)) * (moments ? kMomentSlots : 1);
-  // [time][bin][element][stride], the collision tally of the same layout, then the unreported array of the particles
-  // no bin matches
-  const size_t tally = size_t(ntime > 0 ? ntime : 1) * size_t(nbins) * (collision ? 2 : 1);
-  const size_t len = (tally + (nbins > 1 ? 1 : 0)) * E * stride + kFluxPad;
+  // [time][bin][element][stride], the collision tally of the same layout, with face currents [time][bin][element][4]
+  // and [time][bin] leakage slots, then the unreported array of the particles no bin matches (and its currents)
+  const size_t arrays = size_t(ntime > 0 ? ntime : 1) * size_t(nbins);
+  const size_t tally = arrays * (collision ? 2 : 1);
+  const size_t reported = tally * E * stride + (currents ? arrays * (4 * E + 1) : 0);
+  const size_t len = reported + (nbins > 1 ? E * stride + (currents ? 4 * E : 0) : 0) + kFluxPad;
   double *nf = nullptr;
   const cudaError_t err = cudaMalloc(reinterpret_cast<void **>(&nf), len * sizeof(double));
   if (err != cudaSuccess) {
@@ -1208,7 +1230,7 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
             cudaGetErrorString(err));
     return 1;
   }
-  if (batch_stats_ && alloc_stats(tally * E * stride)) {  // statistics of the new layout, no batch folded yet
+  if (batch_stats_ && alloc_stats(reported)) {  // statistics of the new layout, no batch folded yet
     cudaFree(nf);
     return 1;
   }
@@ -1221,6 +1243,7 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
   ntime_ = ntime;
   moments_ = moments;
   collision_ = collision;
+  currents_ = currents;
   if (nbins > 1 && !d_mask_) PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
   return reset_tally();  // a new set of arrays starts from zero
 }
@@ -1601,6 +1624,7 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "moments") return moments_;
   if (name == "locate_candidates") return int64_t(cand_entries_);  // entries of the point-location candidate lists
   if (name == "collision_estimator") return collision_ ? 1 : 0;
+  if (name == "face_currents") return currents_ ? 1 : 0;
   if (name == "batch_statistics") return batch_stats_ ? 1 : 0;
   if (name == "batches") return batches_;  // batches folded into the statistics
   if (name == "regions") return nregions_;
@@ -1746,6 +1770,7 @@ int Engine::write_tally_results() {
       (synchronize() || batch_arrays(0, "", coll) || (collision_ && batch_arrays(1, "collision_", coll))))
     return 1;
   if (ww_groups_ > 0 && ww_arrays(coll)) return 1;
+  if (currents_ && current_arrays(coll)) return 1;
   if (multi_results()) return write_scored_results(coll);
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
@@ -1761,9 +1786,11 @@ int Engine::write_tally_results() {
       for (size_t i = 0; i < E; ++i) nf[i] += nf[size_t(b) * E + i];
     nf.resize(E);
   }
-  extra.insert(extra.end(), coll.named.begin(), coll.named.end());  // (one component each: no moments here)
+  std::vector<int> ncomp(extra.size(), 1);  // (the face currents have four components, everything else one)
+  extra.insert(extra.end(), coll.named.begin(), coll.named.end());
+  ncomp.insert(ncomp.end(), coll.ncomp.begin(), coll.ncomp.end());
   std::string err;
-  if (!write_vtk_dataset(output_name_, mesh_, nf, vol, rank_, nranks_, &err, extra)) {
+  if (!write_vtk_dataset(output_name_, mesh_, nf, vol, rank_, nranks_, &err, extra, ncomp)) {
     fprintf(stderr, "[pumitally] ERROR: %s\n", err.c_str());
     return 1;
   }
@@ -2264,6 +2291,8 @@ int Engine::end_batch() {
   }
   const size_t L = reported_len();
   const double nb = double(batches_ + 1);
+  // the batch's leakage: its hull slots summed into the leakage slots, which the exchange and the fold then carry
+  if (currents_ && leakage_sums(d_flux_ + current_base(), d_flux_ + leak_base())) return 1;
   if (nregions_ > 0) {  // region sums of this rank's batch, summed over the ranks: the same statistics on every rank
     const size_t RL = region_len();
     double *sums = d_region_stats_;
@@ -2429,6 +2458,154 @@ int Engine::batch_arrays(int32_t tally, const std::string &prefix, VtkArrays &a)
           if (errs && single_time) add(bn + "_rel_err", std::vector<double>(at(rel, t0, b, k), at(rel, t0, b, k) + E));
         }
     }
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------ face currents
+
+int Engine::ensure_face_maps() {
+  if (d_face_opp_) return 0;
+  const int64_t E = mesh_.ntets;
+  std::vector<uint32_t> opp(size_t(4 * E)), hull;
+  for (int64_t e = 0; e < E; ++e)
+    for (int f = 0; f < 4; ++f) {
+      const int32_t nb = mesh_.t2t[size_t(4 * e + f)];
+      int back = f;  // the neighbour's local index of the shared face, found as the packer finds it (tet_mesh.cpp)
+      if (nb >= 0)
+        for (int q = 0; q < 4; ++q)
+          if (mesh_.t2t[4 * size_t(nb) + q] == int32_t(e)) back = q;
+      opp[size_t(4 * e + f)] = nb >= 0 ? 4 * uint32_t(nb) + uint32_t(back) : kNoFace;
+      if (nb < 0) hull.push_back(uint32_t(4 * e + f));
+    }
+  uint32_t *dopp = nullptr, *dhull = nullptr;
+  if (cudaMalloc(reinterpret_cast<void **>(&dopp), opp.size() * sizeof(uint32_t)) != cudaSuccess ||
+      cudaMalloc(reinterpret_cast<void **>(&dhull), std::max<size_t>(hull.size(), 1) * sizeof(uint32_t)) != cudaSuccess ||
+      cudaMemcpy(dopp, opp.data(), opp.size() * sizeof(uint32_t), cudaMemcpyHostToDevice) != cudaSuccess ||
+      (!hull.empty() &&
+       cudaMemcpy(dhull, hull.data(), hull.size() * sizeof(uint32_t), cudaMemcpyHostToDevice) != cudaSuccess)) {
+    const cudaError_t err = cudaGetLastError();
+    cudaFree(dopp);
+    cudaFree(dhull);
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the face maps (%s)\n", cudaGetErrorString(err));
+    return 1;
+  }
+  d_face_opp_ = dopp;
+  d_hull_slots_ = dhull;
+  nhull_ = int64_t(hull.size());
+  return 0;
+}
+
+int Engine::leakage_sums(const double *cur, double *out) {
+  if (ensure_face_maps()) return 1;
+  PTB_CUDA_OK(launch_leakage(cur, mesh_.ntets, result_arrays(), d_hull_slots_, nhull_, out, compute_));
+  return 0;
+}
+
+int Engine::get_face_current_results(int32_t direction, int32_t kind, double *out, int64_t n) {
+  const int64_t E = mesh_.ntets, R = result_arrays();
+  const char *why = !currents_                               ? "face currents are off (set_face_currents)"
+                    : (direction != 0 && direction != 1)     ? "direction must be 0 (outgoing) or 1 (incoming)"
+                    : (kind < 0 || kind > 3)                 ? "kind must be 0 (value), 1 (batch mean), 2 (standard "
+                                                               "error) or 3 (relative error)"
+                    : (n != R * E * 4 || !out)               ? "n must be ntime * nbins * E * 4"
+                                                             : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: get_face_current_results: %s\n", why);
+    return 1;
+  }
+  if (kind > 0 && batch_refused(0, kind - 1)) return 1;
+  if (synchronize() || ensure_element_maps() || ensure_face_maps()) return 1;
+  double div = 1.0;
+  const double *mean = nullptr, *m2 = nullptr;
+  double *tmp = nullptr, *d_out = nullptr;
+  if (kind == 0) {
+    if (gather_shares() || !per_source_divisor(&div)) return 1;
+    mean = flux_view();
+  } else if (stats_view(&mean, &m2, &tmp)) {
+    cudaFree(tmp);
+    return 1;
+  }
+  const size_t base = current_base();
+  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d_out), size_t(n) * sizeof(double));
+  if (e == cudaSuccess)
+    e = launch_current_readout(mean + base, m2 ? m2 + base : nullptr, d_face_opp_, d_orig_of_internal_, d_out, E,
+                               int32_t(R), direction, kind - 1, double(batches_), div, compute_);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, compute_);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+  cudaFree(d_out);
+  cudaFree(tmp);
+  if (e != cudaSuccess) {
+    fprintf(stderr, "[pumitally] CUDA error %s reading the face currents\n", cudaGetErrorString(e));
+    return 1;
+  }
+  return 0;
+}
+
+// The open tally's leakage is summed from its hull slots (its leakage slots fill only at end_batch); the batch kinds
+// read the folded leakage slots.
+int Engine::get_leakage(int32_t kind, double *out, int64_t n) {
+  const int64_t R = result_arrays();
+  const char *why = !currents_                 ? "face currents are off (set_face_currents)"
+                    : (kind < 0 || kind > 3)   ? "kind must be 0 (value), 1 (batch mean), 2 (standard error) or 3 "
+                                                 "(relative error)"
+                    : (n != R || !out)         ? "n must be ntime * nbins"
+                                               : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: get_leakage: %s\n", why);
+    return 1;
+  }
+  if (kind > 0 && batch_refused(0, kind - 1)) return 1;
+  if (synchronize()) return 1;
+  std::vector<double> mean(static_cast<size_t>(R)), m2(static_cast<size_t>(R));
+  if (kind == 0) {
+    double div = 1.0, *d_sum = nullptr;
+    if (gather_shares() || !per_source_divisor(&div)) return 1;
+    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_sum), size_t(R) * sizeof(double)));
+    int rc = leakage_sums(flux_view() + current_base(), d_sum);
+    if (!rc && (cudaMemcpyAsync(mean.data(), d_sum, size_t(R) * sizeof(double), cudaMemcpyDeviceToHost, compute_) !=
+                    cudaSuccess ||
+                cudaStreamSynchronize(compute_) != cudaSuccess))
+      rc = 1;
+    cudaFree(d_sum);
+    if (rc) {
+      fprintf(stderr, "[pumitally] CUDA error %s reading the leakage\n", cudaGetErrorString(cudaGetLastError()));
+      return 1;
+    }
+    for (int64_t r = 0; r < R; ++r) out[r] = mean[size_t(r)] / div;
+    return 0;
+  }
+  const double *dm = nullptr, *dq = nullptr;
+  double *tmp = nullptr;
+  int rc = stats_view(&dm, &dq, &tmp);
+  if (!rc && (cudaMemcpy(mean.data(), dm + leak_base(), size_t(R) * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess ||
+              cudaMemcpy(m2.data(), dq + leak_base(), size_t(R) * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess))
+    rc = 1;
+  cudaFree(tmp);
+  if (rc) return 1;
+  for (int64_t r = 0; r < R; ++r)
+    out[r] = batch_readout(mean[size_t(r)], kind == 1 ? 0.0 : m2[size_t(r)], double(batches_), 1.0, kind - 1);
+  return 0;
+}
+
+int Engine::current_arrays(VtkArrays &a) {
+  const size_t E = size_t(mesh_.ntets), R = size_t(result_arrays());
+  for (int32_t dir = 0; dir < 2; ++dir) {
+    std::vector<double> all(R * E * 4);
+    if (get_face_current_results(dir, 0, all.data(), int64_t(all.size()))) return 1;
+    for (size_t r = 1; r < R; ++r)
+      for (size_t i = 0; i < E * 4; ++i) all[i] += all[r * E * 4 + i];
+    all.resize(E * 4);
+    // component k is the face opposite vertex k of the cell as written, which swaps vertices 2 and 3 of a negatively
+    // oriented tet
+    for (size_t i = 0; i < E; ++i)
+      if (vtk_cell_flipped(mesh_, mesh_.t2v.data() + 4 * i)) {
+        double *c = all.data() + 4 * size_t(mesh_.orig_of_internal[i]);
+        std::swap(c[2], c[3]);
+      }
+    a.data.push_back(std::move(all));
+    a.named.emplace_back(dir == 0 ? "current_out" : "current_in", a.data.back().data());
+    a.ncomp.push_back(4);
   }
   return 0;
 }
@@ -2828,10 +3005,19 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
   if (!r.begin(&h, &ff)) return refuse(r.error());
   if (const char *field = ckpt::fingerprint_mismatch(fingerprint(), ff, merge))
     return refuse(std::string("the checkpoint differs from this engine in: ") + field);
-  const size_t SL = batch_stats_ ? stats_len() : 0, RL = batch_stats_ && nregions_ ? region_len() : 0;
-  if (h.stats_len != SL || h.region_len != RL || (h.open && h.open_len != reported_len()) ||
-      (!batch_stats_ && h.batches != 0))
-    return refuse("the declared lengths do not match this engine's configuration");
+  const size_t RL = batch_stats_ && nregions_ ? region_len() : 0;
+  // the lengths this engine would have with face currents on or off (the fingerprint does not hold the setting)
+  auto lengths_match = [&](bool currents) {
+    const size_t rep = reported_len_for(currents);
+    const size_t SL = !batch_stats_ ? 0 : sharded() ? (rep + size_t(nranks_) - 1) / size_t(nranks_) : rep;
+    return h.stats_len == SL && h.region_len == RL && (!h.open || h.open_len == rep) && (batch_stats_ || h.batches == 0);
+  };
+  if (!lengths_match(currents_))
+    return refuse(lengths_match(!currents_)
+                      ? std::string("the face currents differ: the checkpoint was saved with them ") +
+                            (currents_ ? "off" : "on") + " (set_face_currents)"
+                      : std::string("the declared lengths do not match this engine's configuration"));
+  const size_t SL = batch_stats_ ? stats_len() : 0;
   if (merge && h.open)
     return refuse("the checkpoint holds an open batch, which a merge would drop (save at a batch end)");
   // new buffers: the open tally (whole allocation, zero past the reported part), the statistics, the region statistics

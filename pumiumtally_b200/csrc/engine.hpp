@@ -117,6 +117,17 @@ class Engine {
   // kind 0 raw, 1 normalised, 2 first moments, 3 gradient: get_flux, get_normalized_flux, get_flux_moments and
   // get_flux_gradient of the collision tally (n as they take it)
   int get_collision_results(int32_t kind, double *out, int64_t n);
+  // Face currents (walk_core.cuh, CurrentParams): on == 1 makes every move also tally the weight crossing each face,
+  // per score bin and time bin, and the leakage through the hull; 0 stops it.  Resets the tally, discards the folded
+  // batches; before comm_init.  Combines with everything else and changes none of its results.
+  int set_face_currents(int32_t on);
+  int32_t face_currents() const { return currents_ ? 1 : 0; }
+  // direction 0 outgoing, 1 incoming partial current of face f (opposite the caller's local vertex f) of every element;
+  // kind 0 the open tally / the per-source divisor, 1 batch mean, 2 standard error, 3 relative error (neither divided
+  // by an area or volume).  n == ntime * nbins * E * 4, [time][bin][element][face] in the caller's numbering.
+  int get_face_current_results(int32_t direction, int32_t kind, double *out, int64_t n);
+  // the outgoing current summed over every hull face, kinds as above; n == ntime * nbins, [time][bin]
+  int get_leakage(int32_t kind, double *out, int64_t n);
   // Batch statistics (batch_stats.cuh): on == 1 keeps a running mean and sum of squared deviations of every reported
   // double (both tallies), folded by end_batch from the batch's results divided by its source-normalisation divisor;
   // 0 frees them.  Resets the tally; before comm_init.  Any later set_* call discards the folded batches.
@@ -213,11 +224,13 @@ class Engine {
   int move_host(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size,
                 const MoveTally &dev, int32_t chunk);
   // slice: doubles between time bins of d_flux; variant, tag: the kernel and its auto-tuner slot (-1: none)
+  // d_cur, cur_slice: the face currents of the score bin and the doubles between their time bins (read with currents)
   int launch_range_into(double *d_flux, const double *d_origin, const double *d_dest, const int8_t *d_flying,
                         const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, const MoveTally &t,
-                        int64_t slice, int variant, int tag);
-  // scored and timed moves, and every move with moments: a tallied walk kernel, never one of the auto-tuner's samples
-  bool scored_move(const MoveTally &t) const { return t.kind != MoveTally::kPlain || moments_ > 0; }
+                        int64_t slice, int variant, int tag, double *d_cur = nullptr, int64_t cur_slice = 0);
+  // scored and timed moves, and every move with moments or face currents: a tallied walk kernel, never one of the
+  // auto-tuner's samples
+  bool scored_move(const MoveTally &t) const { return t.kind != MoveTally::kPlain || moments_ > 0 || currents_; }
   bool move_refused(const Move &m, bool device) const;  // with a message; checked before anything is uploaded
   // L2 partition of every SM (l2_partitions.cu), probed when option die_split is switched on; die0_sms_ == 0: no usable map
   uint32_t die_mask_[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -229,17 +242,26 @@ class Engine {
   int32_t ntime_ = 0;                 // time bins (0: no time filter)
   int32_t moments_ = 0;               // moment order (0: none, 1: linear; walk_core.cuh, moment_tally)
   bool collision_ = false;            // the collision tally follows the track-length one in d_flux_
+  bool currents_ = false;             // face currents and leakage follow both tallies in d_flux_
   size_t flux_alloc_ = 0;             // doubles allocated at d_flux_
   // d_flux_: the track-length tally [time][bin][element][stride_] (flux_len()), with the collision estimator the
   // collision tally of the same layout, then the unreported array of a binned move's unmatched particles and padding
   size_t nslices() const { return ntime_ > 0 ? size_t(ntime_) : 1; }
   size_t flux_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
-  size_t reported_len() const { return flux_len() * (collision_ ? 2 : 1); }  // what the exchange moves
+  // With face currents the reported part goes on: the current slots [time][bin][element][4] (walk_core.cuh,
+  // CurrentParams) from current_base(), then one leakage slot per [time][bin], filled by end_batch.
+  size_t current_base() const { return flux_len() * (collision_ ? 2 : 1); }
+  size_t current_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * 4; }
+  size_t leak_base() const { return current_base() + current_len(); }
+  size_t reported_len_for(bool currents) const {
+    return current_base() + (currents ? current_len() + size_t(result_arrays()) : 0);
+  }
+  size_t reported_len() const { return reported_len_for(currents_); }  // what the exchange moves
   size_t bin_len() const { return size_t(mesh_.ntets) * size_t(stride_); }
   int32_t result_arrays() const { return int32_t(nslices()) * nbins_; }  // (time, bin) arrays of bin_len() doubles
   // results laid out [time][bin][score][element] (and read through the score-stride kernels)
   bool multi_results() const { return nscores_ > 1 || ntime_ > 0 || moments_ > 0; }
-  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision);
+  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents);
   // base: doubles from d_flux_ (or the exchanged array) to the tally read, 0 (track length) or flux_len() (collision)
   // [time][bin][score][element][3]; src != nullptr: the records at src + base, gradients not divided by a source divisor
   int copy_moments(std::vector<double> &out, bool gradient, size_t base = 0, const double *src = nullptr);
@@ -328,6 +350,16 @@ class Engine {
   ckpt::Fingerprint fingerprint();
   // load (merge == false) or merge the checkpoint at path, with a message on refusal
   int read_checkpoint(const std::string &path, bool merge);
+  // ---- face currents (stats_kernels.cu, launch_current_readout / launch_leakage) ----
+  // [4E] per internal element and face: 4 * neighbour + back, kNoFace on the hull; the hull slots 4 e + f, ascending
+  // (30-bit element ids: every slot index fits 32 bits).  Built and uploaded at the first use.
+  uint32_t *d_face_opp_ = nullptr, *d_hull_slots_ = nullptr;
+  int64_t nhull_ = 0;
+  int ensure_face_maps();
+  // leakage of the R = result_arrays() current arrays at cur (R * 4E doubles) into out[R], on compute_
+  int leakage_sums(const double *cur, double *out);
+  // the "current_out" / "current_in" arrays (4 components, summed over time and score bins, per source)
+  int current_arrays(VtkArrays &a);
   // ---- weight windows (ww_kernels.cu) ----
   int32_t ww_groups_ = 0;     // 0: no windows
   double2 *d_ww_ = nullptr;   // [ww_groups_][internal element] (lower, upper), (-1, -1) where there is none

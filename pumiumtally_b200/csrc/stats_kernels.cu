@@ -80,6 +80,45 @@ __global__ void batch_readout_kernel(const double *__restrict__ mean, const doub
     out[(r * nscores + k) * E + o] = batch_readout(mean[rec + k], kind == 0 ? 0.0 : m2[rec + k], nb, v, kind);
 }
 
+// Face currents (walk_kernels.hpp, launch_current_readout): thread per (array r, internal element e), four faces each.
+__global__ void current_readout_kernel(const double *__restrict__ mean, const double *__restrict__ m2,
+                                       const uint32_t *__restrict__ opp, const int32_t *__restrict__ orig_of_internal,
+                                       double *__restrict__ out, int64_t E, int32_t R, int direction, int kind, double nb,
+                                       double div) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= E * R) return;
+  const int64_t r = t / E, e = t - r * E;
+  const double *mu = mean + r * E * 4, *q = m2 ? m2 + r * E * 4 : nullptr;
+  double *o = out + (r * E + orig_of_internal[e]) * 4;
+  for (int f = 0; f < 4; ++f) {
+    const uint32_t o4 = opp[4 * e + f];
+    const int64_t s = o4 == kNoFace ? -1 : int64_t(o4), own = 4 * e + f;
+    // the slot that holds the current asked for: -1 for the incoming current of a hull face
+    const int64_t src = direction == 0 ? (s >= 0 ? s : own) : (s >= 0 ? own : -1);
+    const double x = src >= 0 ? mu[src] : 0.0;
+    o[f] = kind < 0 ? x / div : batch_readout(x, (kind == 0 || src < 0) ? 0.0 : q[src], nb, 1.0, kind);
+  }
+}
+
+// Leakage (walk_kernels.hpp, launch_leakage): block r sums array r's hull slots, thread k taking slots k, k + kLeakBlock,
+// ... left to right, then a fixed tree over the threads.
+constexpr int kLeakBlock = 256;
+__global__ void __launch_bounds__(kLeakBlock) leakage_kernel(const double *__restrict__ cur, int64_t E,
+                                                             const uint32_t *__restrict__ hull, int64_t nhull,
+                                                             double *__restrict__ out) {
+  __shared__ double part[kLeakBlock];
+  const double *c = cur + int64_t(blockIdx.x) * E * 4;
+  double s = 0.0;
+  for (int64_t k = threadIdx.x; k < nhull; k += kLeakBlock) s += c[hull[k]];
+  part[threadIdx.x] = s;
+  __syncthreads();
+  for (int h = kLeakBlock / 2; h > 0; h >>= 1) {
+    if (int(threadIdx.x) < h) part[threadIdx.x] += part[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[blockIdx.x] = part[0];
+}
+
 // Over local entries j of [0, n), global index g = goff + j: the entries of the tally [base, base + len) that are the
 // m0 slot of score `score` ((g - base) % stride == score) with a nonzero mean.  red[0] <- max of their relative errors
 // (as the bits of a non-negative double), red[1] += how many there are.
@@ -195,6 +234,23 @@ cudaError_t launch_batch_max_rel_err(const double *mean, const double *m2, int64
   const int block = 256;
   batch_max_rel_err_kernel<<<grid_for(n / stride + 1, block), block, 0, stream>>>(mean, m2, n, goff, base, len, stride,
                                                                                   score, nb, red);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_current_readout(const double *mean, const double *m2, const uint32_t *opp, const int32_t *orig_of_internal,
+                                   double *out, int64_t E, int32_t R, int direction, int kind, double nb, double div,
+                                   cudaStream_t stream) {
+  const int64_t n = E * int64_t(R);
+  if (n <= 0) return cudaSuccess;
+  current_readout_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(mean, m2, opp, orig_of_internal, out, E, R,
+                                                                       direction, kind, nb, div);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_leakage(const double *cur, int64_t E, int32_t R, const uint32_t *hull, int64_t nhull, double *out,
+                           cudaStream_t stream) {
+  if (R <= 0) return cudaSuccess;
+  leakage_kernel<<<unsigned(R), kLeakBlock, 0, stream>>>(cur, E, hull, nhull, out);
   return cudaGetLastError();
 }
 

@@ -24,6 +24,16 @@ struct Block {
 
 }  // namespace
 
+bool vtk_cell_flipped(const HostMesh &m, const int32_t *v) {
+  const double *a = m.coords.data() + 3 * size_t(v[0]), *b = m.coords.data() + 3 * size_t(v[1]);
+  const double *c = m.coords.data() + 3 * size_t(v[2]), *d = m.coords.data() + 3 * size_t(v[3]);
+  const double ab[3] = {b[0] - a[0], b[1] - a[1], b[2] - a[2]}, ac[3] = {c[0] - a[0], c[1] - a[1], c[2] - a[2]},
+               ad[3] = {d[0] - a[0], d[1] - a[1], d[2] - a[2]};
+  const double det = ab[0] * (ac[1] * ad[2] - ac[2] * ad[1]) - ab[1] * (ac[0] * ad[2] - ac[2] * ad[0]) +
+                     ab[2] * (ac[0] * ad[1] - ac[1] * ad[0]);
+  return det < 0.0;
+}
+
 bool write_vtk_dataset(const std::string &path, const HostMesh &m, const std::vector<double> &flux,
                        const std::vector<double> &volume, int rank, int nranks, std::string *err,
                        const std::vector<std::pair<std::string, const double *>> &extra,
@@ -44,13 +54,7 @@ bool write_vtk_dataset(const std::string &path, const HostMesh &m, const std::ve
   std::vector<int32_t> conn = m.to_original(m.t2v.data(), 4);
   for (uint64_t e = e0; e < e1; ++e) {
     int32_t *v = conn.data() + 4 * e;
-    const double *a = m.coords.data() + 3 * size_t(v[0]), *b = m.coords.data() + 3 * size_t(v[1]);
-    const double *c = m.coords.data() + 3 * size_t(v[2]), *d = m.coords.data() + 3 * size_t(v[3]);
-    const double ab[3] = {b[0] - a[0], b[1] - a[1], b[2] - a[2]}, ac[3] = {c[0] - a[0], c[1] - a[1], c[2] - a[2]},
-                 ad[3] = {d[0] - a[0], d[1] - a[1], d[2] - a[2]};
-    const double det = ab[0] * (ac[1] * ad[2] - ac[2] * ad[1]) - ab[1] * (ac[0] * ad[2] - ac[2] * ad[0]) +
-                       ab[2] * (ac[0] * ad[1] - ac[1] * ad[0]);
-    if (det < 0.0) std::swap(v[2], v[3]);
+    if (vtk_cell_flipped(m, v)) std::swap(v[2], v[3]);
   }
   std::vector<Block> blocks = {{m.coords.data(), V * 24}, {conn.data() + 4 * e0, E * 16},
                                {offsets.data(), E * 4},   {types.data(), E},

@@ -18,6 +18,10 @@ namespace ptb {
 // `extra`: further named Float64 cell arrays of the same shape (the per-bin fluxes of a filtered tally).
 // `extra_ncomp[i]`: components per element of extra[i], interleaved (3 for the flux gradients); 1 where the vector
 // is shorter.
+// The writer stores every tet positively oriented, as VTK expects: a tet whose caller's vertices v[0..3] are
+// negatively oriented is written with v[2] and v[3] swapped.
+bool vtk_cell_flipped(const HostMesh &mesh, const int32_t *v);
+
 bool write_vtk_dataset(const std::string &path, const HostMesh &mesh,
                        const std::vector<double> &flux, const std::vector<double> &volume,
                        int rank, int nranks, std::string *err,

@@ -375,6 +375,29 @@ struct TimeLane : ScoreLane {
   int32_t *bin;
 };
 
+// ---- face currents: the weight crossing every face --------------------------------------------------
+// Each crossing of the tally phase adds the particle's weight w (not a response) to one double per (element, local
+// face): for an interior face, the slot (next, back) of the element entered, so the slot holds the weight *entering*
+// through it; for a hull face, the slot (e, f) of the element left, so the slot holds the weight *leaving* through it
+// (nothing enters through the hull: the tally phase ends there).  Four doubles per element are one 32-byte sector; a
+// crossing costs one more reduction and no fetch, since the neighbour and `back` are already decoded.  With a time
+// filter the crossing goes to the bin that holds its time (time_tally's bin after the segment: a crossing exactly on
+// an edge stays in the bin below).
+struct CurrentParams {
+  double *cur;    // [E][4] of time bin 0 of the score bin
+  int64_t slice;  // doubles from time bin j to j + 1 of cur (0: every time bin into one array)
+};
+
+// Parameters of a launch with face currents: the timed ones, unchanged, followed by the currents.
+struct CurrentWalkParams : TimedWalkParams {
+  CurrentParams cu;
+};
+
+// The lane slot that holds w, after the scores and the time slots: written when the tally phase starts (0 for a bad
+// track), read at every crossing.
+template <int NS, bool TM>
+constexpr int kCurrentSlot = NS + (TM ? 3 : 0);
+
 // ---- linear flux moments: the first spatial moment of every score ---------------------------------
 // A segment of length l from ray parameter p to q adds w * r * l to score k and, with moments, w * r * l * (mid - C)
 // to its first moment, mid = o + (p + q) / 2 * u the segment midpoint: the integral of (x - C) along a straight
@@ -508,10 +531,13 @@ PTB_UNROLL
 // or a speed that is not finite and > 0 is a bad track like a non-finite weight.  No responses (nullptr):
 // every r[i,k] is 1.
 // MO: moment walk (NS > 0); responses may be nullptr here too (every r[i,k] 1), for the plain and binned moves.
-template <int NS = 0, bool TM = false, bool MO = false>
+// CU: face currents (NS > 0; P is a CurrentWalkParams): w goes to the lane's kCurrentSlot, 0 for a bad track; responses may
+// be nullptr as with MO.
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
 PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, double z, double tx, double ty,
                            double tz, double w, Counters &c, bool writer, int i = 0,
                            const ScoreLane *sl = nullptr) {
+  static_assert(!CU || NS > 0, "face currents run on the tallied walk");
   if constexpr (NS == 0) {
     if (!all_finite(tx, ty, tz) || !all_finite(w, 0.0, 0.0)) {
       tx = x; ty = y; tz = z;
@@ -534,7 +560,7 @@ PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, doub
 PTB_UNROLL
     for (int k = 0; k < NS; ++k)
       if (k < sl->n) {
-        const double wr = w * ((!(TM || MO) || sl->responses) ? PTB_LDG(rp + k) : 1.0);
+        const double wr = w * ((!(TM || MO || CU) || sl->responses) ? PTB_LDG(rp + k) : 1.0);
         bad = bad || !all_finite(wr, 0.0, 0.0);
         sl->wl[k * sl->step] = wr;
       }
@@ -550,15 +576,16 @@ PTB_UNROLL
       if (k < sl->n) sl->wl[k * sl->step] = bad ? 0.0 : sl->wl[k * sl->step] * len;
     if constexpr (TM)
       time_start<NS>(static_cast<const TimedWalkParams &>(P), static_cast<const TimeLane *>(sl), t0, len / v, bad);
+    if constexpr (CU) sl->wl[kCurrentSlot<NS, TM> * sl->step] = bad ? 0.0 : w;
   }
   r.stage = kStageTally;
   if (writer) c.tracks++;
 }
 
-template <int NS = 0, bool TM = false, bool MO = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
 PTB_HD void start_tally(const WalkParams &P, int i, Ray &r, double x, double y, double z,
                         Counters &c, bool writer, const ScoreLane *sl = nullptr) {
-  start_tally_to<NS, TM, MO>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
+  start_tally_to<NS, TM, MO, CU>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
                      PTB_LDG(P.dest + 3 * (size_t)i + 2), PTB_LDG(P.weights + i), c, writer, i, sl);
 }
 
@@ -589,7 +616,7 @@ PTB_HD void start_reloc(const WalkParams &P, Ray &r, double x, double y, double 
 }
 
 // K1/K2/K3 of the reference folded into the prologue: pick the walk target.
-template <int NS = 0, bool TM = false, bool MO = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
 PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool writer,
                            const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -610,14 +637,14 @@ PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool
       return;
     }
   }
-  if (P.dest) start_tally<NS, TM, MO>(P, i, r, x, y, z, c, writer, sl);
+  if (P.dest) start_tally<NS, TM, MO, CU>(P, i, r, x, y, z, c, writer, sl);
 }
 
 // The current ray ended (target reached, hull hit, or iteration limit).
 // kReloadTarget: the caller does not keep Ray::tx,ty,tz alive in registers (the compact-layout
 // kernel); the target is read back from the caller's array, where it came from: dest[] in the
 // tally phase, origin[] in phase 1.  Same values, six registers fewer in the crossing loop.
-template <bool kReloadTarget = false, int NS = 0, bool TM = false, bool MO = false>
+template <bool kReloadTarget = false, int NS = 0, bool TM = false, bool MO = false, bool CU = false>
 PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tnew, Counters &c,
                     bool writer, const ScoreLane *sl = nullptr) {
   // crossings of the ray that just ended: tally contributions in the tally phase, relocation crossings
@@ -647,7 +674,7 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
     x = fma(tnew, r.ux, r.ox) + P.cx; y = fma(tnew, r.uy, r.oy) + P.cy; z = fma(tnew, r.uz, r.oz) + P.cz;
   }
   if (r.stage != kStageTally && P.dest) {
-    start_tally<NS, TM, MO>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
+    start_tally<NS, TM, MO, CU>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
   } else {
     if (writer) {
       store_state(P.state + i, x, y, z, r.e);
@@ -660,7 +687,10 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
 // NS > 0: scored walk (start_tally_to); one reduction per score into the element's scores.
 // TM: timed walk (time_tally); the same reductions, into the time bins the segment spans.
 // MO: moment walk (NS > 0): each of those reductions comes with the three of its first moment (moment_tally).
-template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0, bool TM = false, bool MO = false>
+// CU: face currents (NS > 0): a crossing of the tally phase -- not the end of a flight, not a face the iteration limit
+// stopped the walk at -- adds w to the slot of the face (CurrentParams).
+template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0, bool TM = false, bool MO = false,
+          bool CU = false>
 PTB_HD void advance(const WalkParams &P, int i, Ray &r, double texit, int32_t next, int32_t back,
                     Counters &c, bool writer, const ScoreLane *sl = nullptr) {
   const bool reached = !(texit < 1.0);  // last_exit == -1: destination inside this tet
@@ -691,9 +721,19 @@ PTB_UNROLL
   const bool hull = !reached && next < 0;  // next_elems == -1 (Impl.cpp:270-271)
   r.iters++;
   const bool over = r.iters >= P.max_iters;
+  if constexpr (CU) {
+    if (r.stage == kStageTally && writer && !reached && (hull || !over)) {
+      const CurrentWalkParams &Q = static_cast<const CurrentWalkParams &>(P);
+      int j = 0;
+      if constexpr (TM) j = *static_cast<const TimeLane *>(sl)->bin;
+      const double w = sl->wl[kCurrentSlot<NS, TM> * sl->step];
+      if (!TM || (j >= 0 && j < Q.tm.nt))
+        PTB_TALLY_ADD(Q.cu.cur + (size_t)j * (size_t)Q.cu.slice + (size_t)(hull ? r.e : next) * 4 + back, w);
+    }
+  }
   if (reached || hull || over) {
     if (over && !reached && !hull && writer && r.stage != kStageSeed) c.lost++;
-    end_ray<kReloadTarget, NS, TM, MO>(P, i, r, reached, tnew, c, writer, sl);
+    end_ray<kReloadTarget, NS, TM, MO, CU>(P, i, r, reached, tnew, c, writer, sl);
   } else {
     r.e = next;  // UpdateCurrentElement (Impl.cpp:247-253)
     r.entry = back;

@@ -33,16 +33,17 @@ namespace {
 // NS > 0: scored walk (walk_persist.cuh); the lanes' score slots are sized for the largest block.
 // TM: timed walk (NS > 0); the lanes' time slots sit next to the scores.
 // MO: moment walk (NS > 0; walk_core.cuh, moment_tally).
-template <int NS, bool TM, bool MO = false>
-__device__ __forceinline__ void ldg_walk(const KernelParams<NS, TM> &P) {
+// CU: face currents (NS > 0; walk_core.cuh, CurrentParams); the lane's weight slot follows the others.
+template <int NS, bool TM, bool MO = false, bool CU = false>
+__device__ __forceinline__ void ldg_walk(const KernelParamsCU<NS, TM, CU> &P) {
   const int i = P.begin + blockIdx.x * blockDim.x + threadIdx.x;
-  __shared__ double score_wl[kLaneSlots<NS, TM>][NS > 0 ? 256 : 1];
+  __shared__ double score_wl[kLaneSlots<NS, TM, CU>][NS > 0 ? 256 : 1];
   __shared__ int32_t time_bin[TM ? 256 : 1];
   const auto sl = walk_lane<NS, 256, TM>(P, &score_wl[0][0], &time_bin[0]);
   Counters c;
   Ray r;
   r.stage = kStageDone;
-  if (i < P.end) begin_particle<NS, TM, MO>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
+  if (i < P.end) begin_particle<NS, TM, MO, CU>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
   while (r.stage != kStageDone) {
     const double *rec = P.tets[r.e].d;
     double raw[16];
@@ -51,7 +52,7 @@ __device__ __forceinline__ void ldg_walk(const KernelParams<NS, TM> &P) {
       load_face_256(rec + 4 * f, raw[4 * f], raw[4 * f + 1], raw[4 * f + 2], raw[4 * f + 3]);
     ExitScan sc;
     scan_record(raw, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
-    advance<false, false, NS, TM, MO>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
+    advance<false, false, NS, TM, MO, CU>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
   }
   flush_counters(P, c);
 }
@@ -69,6 +70,20 @@ __global__ void __launch_bounds__(256, 4) walk_ldg_moments_kernel(const ScoredWa
 }
 __global__ void __launch_bounds__(256, 4) walk_ldg_timed_moments_kernel(const TimedWalkParams P) {
   ldg_walk<kMaxScores, true, true>(P);
+}
+
+// The same four walks with face currents, under names of their own and held to the same four blocks.
+__global__ void __launch_bounds__(256, 4) walk_ldg_current_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, false, false, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_timed_current_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, true, false, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_moments_current_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, false, true, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_timed_moments_current_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, true, true, true>(P);
 }
 
 // ------------------------------------------------------------ small kernels
@@ -238,11 +253,12 @@ __global__ void sum_flying_weights_kernel(const int8_t *flying, const double *we
 }
 
 // The product kernels of one instantiation of the walk: NS scores (0: the plain tally), TM the time filter, MO the
-// moments.  ldg is its thread-per-particle kernel, handed in because each instantiation has its own launch bounds.
-// Every other variant is refused, except that the plain walk hands it to the experiments when they are linked in.
-template <int NS, bool TM, bool MO>
-cudaError_t launch_product(const KernelParams<NS, TM> &p, int variant, int block, cudaStream_t stream,
-                           void (*ldg)(KernelParams<NS, TM>)) {
+// moments, CU the face currents.  ldg is its thread-per-particle kernel, handed in because each instantiation has its
+// own launch bounds.  Every other variant is refused, except that the plain walk hands it to the experiments when they
+// are linked in.
+template <int NS, bool TM, bool MO, bool CU = false>
+cudaError_t launch_product(const KernelParamsCU<NS, TM, CU> &p, int variant, int block, cudaStream_t stream,
+                           void (*ldg)(KernelParamsCU<NS, TM, CU>)) {
   const long long n = (long long)p.end - p.begin;
   if (n <= 0) return cudaSuccess;
   if (block != 64 && block != 128 && block != 256) block = 128;
@@ -253,12 +269,12 @@ cudaError_t launch_product(const KernelParams<NS, TM> &p, int variant, int block
       return cudaGetLastError();
     }
     case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, NS, TM, MO>(p, n, stream);
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, NS, TM, MO, CU>(p, n, stream);
     case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, NS, TM, MO>(p, n, stream);
+      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, NS, TM, MO, CU>(p, n, stream);
     case kVariantPacked:
       if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, NS, TM, MO>(p, n, stream);
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, NS, TM, MO, CU>(p, n, stream);
     default:
 #ifdef PTB_EXPERIMENTS
       if constexpr (NS == 0) return launch_walk_experiment(p, variant, block, stream);
@@ -273,14 +289,23 @@ cudaError_t launch_walk(const WalkParams &p, int variant, int block, cudaStream_
   return launch_product<0, false, false>(p, variant, block, stream, walk_ldg_kernel<0>);
 }
 
-cudaError_t launch_walk_tallied(const TimedWalkParams &p, bool timed, bool moments, int variant, int block,
-                                cudaStream_t stream) {
+cudaError_t launch_walk_tallied(const CurrentWalkParams &p, bool timed, bool moments, bool currents, int variant,
+                                int block, cudaStream_t stream) {
   if (p.sc.nscores < 1 || p.sc.nscores > kMaxScores ||
       p.sc.stride != score_stride(p.sc.nscores) * (moments ? kMomentSlots : 1) ||
-      (!p.sc.responses && !(p.sc.nscores == 1 && (timed || moments))))
+      (!p.sc.responses && !(p.sc.nscores == 1 && (timed || moments || currents))))
     return cudaErrorInvalidValue;
   if (timed && (p.tm.nt < 1 || p.tm.nt > kMaxTimeBins || p.tm.slice < 0 || !p.tm.edges || !p.tm.times || !p.tm.speeds))
     return cudaErrorInvalidValue;
+  if (currents && (!p.cu.cur || p.cu.slice < 0)) return cudaErrorInvalidValue;
+  if (currents) {
+    if (timed)
+      return moments ? launch_product<kMaxScores, true, true, true>(p, variant, block, stream,
+                                                                    walk_ldg_timed_moments_current_kernel)
+                     : launch_product<kMaxScores, true, false, true>(p, variant, block, stream, walk_ldg_timed_current_kernel);
+    return moments ? launch_product<kMaxScores, false, true, true>(p, variant, block, stream, walk_ldg_moments_current_kernel)
+                   : launch_product<kMaxScores, false, false, true>(p, variant, block, stream, walk_ldg_current_kernel);
+  }
   if (timed)
     return moments ? launch_product<kMaxScores, true, true>(p, variant, block, stream, walk_ldg_timed_moments_kernel)
                    : launch_product<kMaxScores, true, false>(p, variant, block, stream, walk_ldg_timed_kernel);

@@ -62,8 +62,10 @@ bool walk_variant_available(int variant);  // compiled into this library?
 // p.flux + j * p.tm.slice.  p.sc.responses may be nullptr when p.sc.nscores == 1 (every response 1).
 // moments: the moment walk (walk_core.cuh, moment_tally): p.sc.stride is kMomentSlots * score_stride(nscores), and
 // p.sc.responses may be nullptr when p.sc.nscores == 1 (every response 1: the plain and binned moves).
-cudaError_t launch_walk_tallied(const TimedWalkParams &p, bool timed, bool moments, int variant, int block,
-                                cudaStream_t stream);
+// currents: face currents (walk_core.cuh, CurrentParams) into p.cu.cur ([E][4] per time bin, p.cu.slice apart); p.cu is
+// read only then, and p.sc.responses may be nullptr when p.sc.nscores == 1 here too.
+cudaError_t launch_walk_tallied(const CurrentWalkParams &p, bool timed, bool moments, bool currents, int variant,
+                                int block, cudaStream_t stream);
 // blocks per SM the occupancy calculator gave the last persistent walk kernel launched (0: none yet)
 int walk_blocks_per_sm();
 // origin == nullptr: the binning key is the stored position (state)
@@ -168,6 +170,18 @@ struct RegionLevel;
 cudaError_t launch_region_sums(const double *flux, int64_t array_len, int32_t stride, int32_t nscores, int64_t narrays,
                                const int32_t *elems, const int32_t *starts, const RegionLevel *levels, int nlevels,
                                double *scratch, int64_t scratch_len, double *out, cudaStream_t stream);
+// Face currents (walk_core.cuh, CurrentParams) of R arrays [r][E][4] (internal order), opp [4E] as the engine keeps it
+// (4 * neighbour + back, kNoFace on the hull).  out[(r * E + caller's id of e) * 4 + f] is, for direction 0 (outgoing) the
+// slot of the neighbour across f (interior) or of (e, f) itself (hull), for direction 1 (incoming) the slot (e, f)
+// (interior) or nothing (hull).  kind -1: the value / div (nothing: 0); kind 0-2: batch_readout of mean and m2 at the
+// slot with volume 1 (nothing: mean and m2 0).  m2 is read for kinds 1 and 2 only.
+constexpr uint32_t kNoFace = 0xffffffffu;
+cudaError_t launch_current_readout(const double *mean, const double *m2, const uint32_t *opp, const int32_t *orig_of_internal,
+                                   double *out, int64_t E, int32_t R, int direction, int kind, double nb, double div,
+                                   cudaStream_t stream);
+// out[r] = sum of cur[r * 4E + hull[k]] over k < nhull, for r < R, in a fixed order (the same bits every time)
+cudaError_t launch_leakage(const double *cur, int64_t E, int32_t R, const uint32_t *hull, int64_t nhull, double *out,
+                           cudaStream_t stream);
 
 // ww_kernels.cu.  Weight windows (weight_windows.cuh).  generate: table[b * E + e] <- ww_generate of the m0 value of
 // group b and element e of nb batches, at mean[b * pitch + e * stride] and m2 alike, with phimax the largest eligible

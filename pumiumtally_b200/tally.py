@@ -65,6 +65,10 @@ C_API = {
     "pumitally_evaluate_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, C.c_int64, _ip]),
     "pumitally_set_collision_estimator": (C.c_int, [C.c_void_p, C.c_int32]),
     "pumitally_get_collision_estimator": (C.c_int32, [C.c_void_p]),
+    "pumitally_set_face_currents": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_get_face_currents": (C.c_int32, [C.c_void_p]),
+    "pumitally_get_face_current_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
+    "pumitally_get_leakage": (C.c_int, [C.c_void_p, C.c_int32, _dp, C.c_int64]),
     "pumitally_tally_collisions": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, _dp, _ip, _dp]),
     "pumitally_tally_collisions_device": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -464,6 +468,34 @@ class PumiTally:
                                              elem.ctypes.data_as(_ip)):
             raise RuntimeError("evaluate_points failed")
         return out, elem
+
+    # ---- face currents ---------------------------------------------------------------
+    def set_face_currents(self, on: bool):
+        """True: every move also tallies the weight crossing each element face, per score bin and time bin, and the
+        leakage through the hull; False stops it (the default).  Resets the tally and discards the folded batches."""
+        if self._L.pumitally_set_face_currents(self._h, int(on)):
+            raise ValueError("set_face_currents failed")
+
+    @property
+    def face_currents(self) -> bool:
+        return bool(self._L.pumitally_get_face_currents(self._h))
+
+    def face_current_results(self, direction=0, kind=0):
+        """Partial currents [ntime, nbins, num_elements, 4] in the caller's numbering, face f opposite local vertex f:
+        direction 0 outgoing, 1 incoming; kind 0 the open tally / the per-source divisor, 1 batch mean, 2 standard
+        error, 3 relative error."""
+        out = np.empty((max(self.time_bins, 1), self.score_bins, self.num_elements, 4))
+        if self._L.pumitally_get_face_current_results(self._h, int(direction), int(kind), out.ctypes.data_as(_dp),
+                                                      out.size):
+            raise RuntimeError("get_face_current_results failed")
+        return out
+
+    def leakage(self, kind=0):
+        """The outgoing current summed over the hull faces, [ntime, nbins]; kinds as face_current_results."""
+        out = np.empty((max(self.time_bins, 1), self.score_bins))
+        if self._L.pumitally_get_leakage(self._h, int(kind), out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError("get_leakage failed")
+        return out
 
     # ---- collision estimator -------------------------------------------------------
     def set_collision_estimator(self, on: bool):
