@@ -182,6 +182,23 @@ inline int WeightWindowsAtPoints(const PumiTally &tally, const double *xyz, int6
   return pumitally_get_weight_windows_at_points(engine_of(tally), xyz, npts, groups, lower, upper);
 }
 
+// Mesh source (see pumitally_set_source in pumitally_c.h): strengths [group][element] in the caller's numbering, bias
+// optional (nullptr), per_volume multiplies each by its element's volume.  SampleSource draws samples first .. first +
+// n - 1 of seed (outputs may be nullptr); place != 0 (n == num_particles) puts sample j at particle j without a walk.
+// GetSourceStrength gives Q, the unbiased total the caller normalises by.
+inline int SetSource(const PumiTally &tally, const double *strength, const double *bias, int64_t n, int32_t ngroups,
+                     int32_t per_volume) {
+  return pumitally_set_source(engine_of(tally), strength, bias, n, ngroups, per_volume);
+}
+inline int32_t GetSourceGroups(const PumiTally &tally) { return pumitally_get_source_groups(engine_of(tally)); }
+inline int GetSourceStrength(const PumiTally &tally, double *total) {
+  return pumitally_get_source_strength(engine_of(tally), total);
+}
+inline int SampleSource(const PumiTally &tally, uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem,
+                        int32_t *group, double *weight, int32_t place) {
+  return pumitally_sample_source(engine_of(tally), seed, first, n, xyz, elem, group, weight, place);
+}
+
 }  // namespace pumitally
 
 #endif  // PUMITALLY_PUMITALLYEXTRAS_H

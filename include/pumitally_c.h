@@ -575,6 +575,42 @@ int pumitally_get_weight_windows_at_points_device(pumitally_engine *e, const dou
                                                   const int32_t *d_groups, double *d_lower, double *d_upper,
                                                   void *stream);
 
+/* ---- additive: mesh source (per-element, per-group strengths sampled on the GPU, with source biasing) ----
+ * A volumetric source on the tally mesh, e.g. the decay photons of a shutdown-dose-rate run: one strength per element
+ * and group.  A sample picks an entry in proportion to its (biased) strength and then a uniform point inside the
+ * element.  The engine holds one source table: 8 bytes per entry (16 with bias) and, from the first set on, the
+ * elements' vertices (96 bytes per element).  The source is not tally state: pumitally_reset_tally, pumitally_end_batch,
+ * every other pumitally_set_* call, pumitally_comm_init and checkpoints leave it alone, and checkpoints do not hold it.
+ * Refusals print the reason, return non-zero and change nothing.
+ * pumitally_set_source(e, strength, bias, n, ngroups, per_volume): host arrays [group][element] in the caller's
+ * numbering, n == ngroups * num_elements; bias may be NULL.  Entry k = g * E + e gets p[k] = (q[k] * V[e] if per_volume
+ * else q[k]) * (b[k] if bias else 1), each product rounded separately, V the element's volume; the CDF is the
+ * sequential sum C[k] = C[k-1] + p[k], T = C[K-1], and Q the same sum of the unbiased q V (or q).  Refused: a strength
+ * or bias that is negative or not finite, a bias of 0 where the strength is > 0, T or Q 0 or not finite, ngroups < 1
+ * or a wrong n.  strength == NULL with ngroups == 0 removes the source.  pumitally_get_source_groups returns ngroups
+ * (0 without a source); pumitally_get_source_strength returns Q, by which the caller normalises.
+ * pumitally_sample_source(e, seed, first, n, xyz, elem, group, weight, place): samples i = first .. first + n - 1.
+ * Sample i takes four uniforms u_k = ((z_k >> 12) + 0.5) * 2^-52, z_k the SplitMix64 mix of (seed, i, stream k), so it
+ * depends on (seed, i) alone.  Its entry k is the first with C[k] > u_0 * T (the last entry with p > 0 if x rounded up
+ * to T): group k / E, element k % E.  Its point is the Rocchini-Cignoni fold of (u_1, u_2, u_3) applied to the
+ * element's vertices in the caller's local order, every operation rounded separately.  Its weight is 1 without bias and
+ * (T / Q) / b[k] with bias (mean 1).  The outputs -- AoS xyz [3n], elem (caller's numbering), group, weight -- may each
+ * be NULL.  place != 0 needs n == num_particles: sample j becomes particle j's position and parent element, without a
+ * walk, as pumitally_set_state_device stores them; it counts as the initial placement (CopyInitialPosition is refused
+ * afterwards).  Without place nothing in the engine changes.  The host call works through device buffers of the option
+ * "chunk" samples and synchronises; the _device variant takes device arrays and is enqueued on `stream`, behind the
+ * last work on the particle state.
+ * WriteTallyResults with a source set writes, after every other array, "source" (one group) or "source_g<g>" for every
+ * group g: the strengths as the caller gave them. */
+int pumitally_set_source(pumitally_engine *e, const double *strength, const double *bias, int64_t n, int32_t ngroups,
+                         int32_t per_volume);
+int32_t pumitally_get_source_groups(const pumitally_engine *e);
+int pumitally_get_source_strength(pumitally_engine *e, double *total);
+int pumitally_sample_source(pumitally_engine *e, uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem,
+                            int32_t *group, double *weight, int32_t place);
+int pumitally_sample_source_device(pumitally_engine *e, uint64_t seed, int64_t first, int64_t n, double *d_xyz,
+                                   int32_t *d_elem, int32_t *d_group, double *d_weight, int32_t place, void *stream);
+
 /* test hook: processing order produced by the last binning pass (ids of flying particles
  * grouped by seed-grid cell); returns the number of entries, copies at most n of them */
 int64_t pumitally_debug_order(pumitally_engine *e, int32_t *out, int64_t n);

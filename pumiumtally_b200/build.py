@@ -25,6 +25,7 @@ SOURCES = [
     "locate_kernels.cu",
     "stats_kernels.cu",
     "ww_kernels.cu",
+    "source_kernels.cu",
     "l2_partitions.cu",
     "engine.cu",
     "checkpoint.cpp",

@@ -367,6 +367,28 @@ int pumitally_get_weight_windows_at_points_device(pumitally_engine *e, const dou
   });
 }
 
+int pumitally_set_source(pumitally_engine *e, const double *strength, const double *bias, int64_t n, int32_t ngroups,
+                         int32_t per_volume) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_source(strength, bias, n, ngroups, per_volume); });
+}
+int32_t pumitally_get_source_groups(const pumitally_engine *e) {
+  return (e && e->impl) ? e->impl->source_groups() : 0;
+}
+int pumitally_get_source_strength(pumitally_engine *e, double *total) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_source_strength(total); });
+}
+int pumitally_sample_source(pumitally_engine *e, uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem,
+                            int32_t *group, double *weight, int32_t place) {
+  return guarded(e, [&](ptb::Engine &g) { return g.sample_source(seed, first, n, xyz, elem, group, weight, place); });
+}
+int pumitally_sample_source_device(pumitally_engine *e, uint64_t seed, int64_t first, int64_t n, double *d_xyz,
+                                   int32_t *d_elem, int32_t *d_group, double *d_weight, int32_t place, void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.sample_source_device(seed, first, n, d_xyz, d_elem, d_group, d_weight, place,
+                                  static_cast<cudaStream_t>(stream));
+  });
+}
+
 int pumitally_reset_tally(pumitally_engine *e) {
   return guarded(e, [&](ptb::Engine &g) { return g.reset_tally(); });
 }

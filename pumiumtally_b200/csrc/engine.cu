@@ -199,6 +199,8 @@ Engine::~Engine() {
   free_stats();
   free_regions();
   free_weight_windows();
+  free_source();
+  cudaFree(d_src_verts_);
   cudaFree(d_batch_div_); cudaFree(d_stats_red_);
   if (compute_) cudaStreamDestroy(compute_);
   if (copy_) cudaStreamDestroy(copy_);
@@ -1762,7 +1764,7 @@ int64_t Engine::debug_order(int32_t *out, int64_t n) {
 // FinalizeTallies (PumiTallyImpl.cpp:411-416).  With the collision estimator every array of the track-length tally is
 // followed by its collision twin, the same name prefixed "collision_".  With batch statistics and at least one batch
 // folded, the "_mean" / "_rel_err" arrays (batch_arrays) of both tallies follow all of these, and with weight windows
-// their bounds (ww_arrays) come last.
+// their bounds (ww_arrays) follow, then the face currents and, with a mesh source, its strengths (source_arrays).
 int Engine::write_tally_results() {
   VtkArrays coll;
   if (collision_ && (synchronize() || gather_shares() || scored_arrays(flux_len(), "collision_", coll, nullptr))) return 1;
@@ -1771,6 +1773,7 @@ int Engine::write_tally_results() {
     return 1;
   if (ww_groups_ > 0 && ww_arrays(coll)) return 1;
   if (currents_ && current_arrays(coll)) return 1;
+  if (src_groups_ > 0 && source_arrays(coll)) return 1;
   if (multi_results()) return write_scored_results(coll);
   const size_t E = size_t(mesh_.ntets);
   std::vector<double> nf(E * size_t(nbins_)), vol(E);
@@ -3379,6 +3382,183 @@ int Engine::ww_arrays(VtkArrays &a) {
       a.named.emplace_back(name + suffix, a.data.back().data());
       a.ncomp.push_back(1);
     }
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------ mesh source
+
+void Engine::free_source() {
+  cudaFree(d_src_cdf_);
+  cudaFree(d_src_bias_);
+  d_src_cdf_ = d_src_bias_ = nullptr;
+  src_groups_ = 0;
+  src_total_ = src_strength_ = 0.0;
+  src_last_ = -1;
+  std::vector<double>().swap(src_given_);
+}
+
+SourceTable Engine::source_table() const {
+  SourceTable S;
+  S.cdf = d_src_cdf_;
+  S.bias = d_src_bias_;
+  S.verts = d_src_verts_;
+  S.E = mesh_.ntets;
+  S.K = int64_t(src_groups_) * mesh_.ntets;
+  S.klast = src_last_;
+  S.total = src_total_;
+  S.ratio = src_total_ / src_strength_;
+  return S;
+}
+
+int Engine::set_source(const double *strength, const double *bias, int64_t n, int32_t ngroups, int32_t per_volume) {
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (!strength && ngroups == 0) {
+    if (synchronize()) return 1;  // a device sampling call may still read the table
+    free_source();
+    return 0;
+  }
+  const int64_t E = mesh_.ntets;
+  const char *why = ngroups < 1                 ? "ngroups must be >= 1 (0 with strength == NULL removes the source)"
+                    : !strength                 ? "null strength array"
+                    : E < 1                     ? "the mesh has no elements"
+                    : n != int64_t(ngroups) * E ? "n must be ngroups * num_elements"
+                                                : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_source refused: %s\n", why);
+    return 1;
+  }
+  std::vector<double> vol(static_cast<size_t>(E)), cdf(static_cast<size_t>(n));
+  for (int64_t i = 0; i < E; ++i) vol[size_t(mesh_.orig_of_internal[size_t(i)])] = mesh_.volume[size_t(i)];
+  double T = 0.0, Q = 0.0;
+  int64_t klast = -1, bad = -1;
+  why = source_build(strength, bias, vol.data(), E, ngroups, per_volume != 0, cdf.data(), &T, &Q, &klast, &bad);
+  if (why) {
+    if (bad >= 0)
+      fprintf(stderr, "[pumitally] ERROR: set_source refused: %s (group %lld, element %lld: strength %g, bias %g)\n",
+              why, (long long)(bad / E), (long long)(bad % E), strength[bad], bias ? bias[bad] : 1.0);
+    else
+      fprintf(stderr, "[pumitally] ERROR: set_source refused: %s (T = %g, Q = %g)\n", why, T, Q);
+    return 1;
+  }
+  if (synchronize()) return 1;
+  if (!d_src_verts_) {  // each element's four vertices, caller's numbering and local order: 96 B per element
+    std::vector<double> v(size_t(12) * size_t(E));
+    for (int64_t i = 0; i < E; ++i) {
+      double *o = &v[size_t(12) * size_t(mesh_.orig_of_internal[size_t(i)])];
+      for (int q = 0; q < 4; ++q)
+        for (int a = 0; a < 3; ++a) o[3 * q + a] = mesh_.coords[3 * size_t(mesh_.t2v[4 * size_t(i) + q]) + a];
+    }
+    double *d = nullptr;
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d), v.size() * sizeof(double));
+    if (e == cudaSuccess) e = cudaMemcpy(d, v.data(), v.size() * sizeof(double), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      cudaFree(d);
+      fprintf(stderr, "[pumitally] ERROR: set_source: no device memory for the element vertices (%zu bytes: %s)\n",
+              v.size() * sizeof(double), cudaGetErrorString(e));
+      return 1;
+    }
+    d_src_verts_ = d;
+  }
+  double *d_cdf = nullptr, *d_bias = nullptr;
+  const size_t bytes = size_t(n) * sizeof(double);
+  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d_cdf), bytes);
+  if (e == cudaSuccess) e = cudaMemcpy(d_cdf, cdf.data(), bytes, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && bias) e = cudaMalloc(reinterpret_cast<void **>(&d_bias), bytes);
+  if (e == cudaSuccess && bias) e = cudaMemcpy(d_bias, bias, bytes, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(d_cdf);
+    cudaFree(d_bias);
+    fprintf(stderr, "[pumitally] ERROR: set_source: no device memory for the source (%zu bytes: %s)\n",
+            (bias ? 2 : 1) * bytes, cudaGetErrorString(e));
+    return 1;
+  }
+  free_source();
+  d_src_cdf_ = d_cdf;
+  d_src_bias_ = d_bias;
+  src_groups_ = ngroups;
+  src_total_ = T;
+  src_strength_ = Q;
+  src_last_ = klast;
+  src_given_.assign(strength, strength + n);
+  return 0;
+}
+
+int Engine::get_source_strength(double *total) {
+  if (src_groups_ == 0 || !total) {
+    fprintf(stderr, "[pumitally] ERROR: get_source_strength refused: %s\n",
+            src_groups_ == 0 ? "no source is set (set_source)" : "null output");
+    return 1;
+  }
+  *total = src_strength_;
+  return 0;
+}
+
+bool Engine::source_refused(int64_t first, int64_t n, int32_t place) {
+  const char *why = src_groups_ == 0                 ? "no source is set (set_source)"
+                    : first < 0                      ? "first must be >= 0"
+                    : n < 0                          ? "n must be >= 0"
+                    : n > INT64_MAX - first          ? "first + n overflows"
+                    : (place && n != int64_t(n_))    ? "with place, n must be num_particles"
+                                                     : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: sample_source refused: %s\n", why);
+  return why != nullptr;
+}
+
+int Engine::sample_source(uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem, int32_t *group,
+                          double *weight, int32_t place) {
+  if (source_refused(first, n, place)) return 1;
+  if (n == 0 || !(place || xyz || elem || group || weight)) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  const int64_t chunk = std::min<int64_t>(chunk_, n);
+  if (ensure_query_buffers(size_t(chunk), size_t(chunk))) return 1;
+  if (place && (ensure_element_maps() || follow_last_stream(compute_))) return 1;  // writes the particle state
+  const SourceTable S = source_table();
+  for (int64_t b = 0; b < n; b += chunk) {
+    const int64_t cnt = std::min(chunk, n - b);
+    PTB_CUDA_OK(launch_source_sample(S, seed, uint64_t(first + b), cnt, xyz ? d_qxyz_ : nullptr,
+                                     elem ? d_qelem_ : nullptr, group ? d_qint_ : nullptr, weight ? d_qout_ : nullptr,
+                                     place ? d_state_ + b : nullptr, d_internal_of_orig_, compute_));
+    if (xyz)
+      PTB_CUDA_OK(cudaMemcpyAsync(xyz + 3 * b, d_qxyz_, size_t(cnt) * 3 * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+    if (elem)
+      PTB_CUDA_OK(cudaMemcpyAsync(elem + b, d_qelem_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+    if (group)
+      PTB_CUDA_OK(cudaMemcpyAsync(group + b, d_qint_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+    if (weight)
+      PTB_CUDA_OK(cudaMemcpyAsync(weight + b, d_qout_, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+  }
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  if (place) {  // the initial placement, as set_state_device makes it
+    initialized_ = true;
+    mirror_valid_ = false;
+    pos_mirror_valid_ = false;
+  }
+  return 0;
+}
+
+int Engine::sample_source_device(uint64_t seed, int64_t first, int64_t n, double *d_xyz, int32_t *d_elem,
+                                 int32_t *d_group, double *d_weight, int32_t place, cudaStream_t stream) {
+  if (source_refused(first, n, place)) return 1;
+  if (n == 0 || !(place || d_xyz || d_elem || d_group || d_weight)) return 0;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (place && (ensure_element_maps() || follow_last_stream(stream))) return 1;  // writes the particle state
+  PTB_CUDA_OK(launch_source_sample(source_table(), seed, uint64_t(first), n, d_xyz, d_elem, d_group, d_weight,
+                                   place ? d_state_ : nullptr, d_internal_of_orig_, stream));
+  if (place) {
+    initialized_ = true;
+    mirror_valid_ = false;
+    pos_mirror_valid_ = false;
+  }
+  return 0;
+}
+
+int Engine::source_arrays(VtkArrays &a) {
+  const size_t E = size_t(mesh_.ntets), G = size_t(src_groups_);
+  for (size_t g = 0; g < G; ++g) {
+    a.data.emplace_back(src_given_.begin() + g * E, src_given_.begin() + (g + 1) * E);
+    a.named.emplace_back(G == 1 ? std::string("source") : "source_g" + std::to_string(g), a.data.back().data());
+    a.ncomp.push_back(1);
   }
   return 0;
 }

@@ -16,6 +16,7 @@
 #include "batch_stats.cuh"
 #include "checkpoint.hpp"
 #include "host_stage.hpp"
+#include "source_sample.cuh"
 #include "tet_mesh.hpp"
 #include "walk_kernels.hpp"
 
@@ -180,6 +181,22 @@ class Engine {
   int weight_windows_at_points(const double *xyz, int64_t npts, const int32_t *groups, double *lower, double *upper);
   int weight_windows_at_points_device(const double *d_xyz, int64_t npts, const int32_t *d_groups, double *d_lower,
                                       double *d_upper, cudaStream_t stream);
+  // Mesh source (source_sample.cuh): strength [group][element] in the caller's numbering (n == ngroups * E), times
+  // each element's volume with per_volume, times bias [same layout] when bias != nullptr, sampled by a CDF over the
+  // entries.  Not tally state (no reset, set_*, end_batch, comm_init or checkpoint touches it).  A negative or
+  // non-finite strength or bias, a zero bias where the strength is > 0, or a zero or non-finite total is refused and
+  // changes nothing; strength == nullptr with ngroups == 0 removes the source.
+  int set_source(const double *strength, const double *bias, int64_t n, int32_t ngroups, int32_t per_volume);
+  int32_t source_groups() const { return src_groups_; }
+  int get_source_strength(double *total);  // Q: the sum of the unbiased strengths (times the volumes with per_volume)
+  // Samples first .. first + n - 1 of `seed`: AoS xyz, element (caller's numbering), group and birth weight, each
+  // optional.  place != 0 (n == num_particles) makes sample j particle j's position and parent element, without a walk,
+  // as the initial placement.  Without place nothing in the engine changes.  The host call works through chunk-sized
+  // device buffers and synchronises; the device call is enqueued behind the last work on the particle state.
+  int sample_source(uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem, int32_t *group,
+                    double *weight, int32_t place);
+  int sample_source_device(uint64_t seed, int64_t first, int64_t n, double *d_xyz, int32_t *d_elem, int32_t *d_group,
+                           double *d_weight, int32_t place, cudaStream_t stream);
   // n == E: time bin 0, bin 0, score 0; n == ntime * nbins * nscores * E: everything, [time][bin][score][element]
   int get_flux(double *out, int64_t n);
   // Device-side accessors, caller's element numbering, enqueued on `stream` (no synchronisation).
@@ -368,6 +385,18 @@ class Engine {
   bool ww_lookup_refused(const char *what, bool particles, int64_t n);  // with a message
   // the "ww_lower" / "ww_upper" arrays (with several groups "_g<g>" after each name), caller's numbering
   int ww_arrays(VtkArrays &a);
+  // ---- mesh source (source_kernels.cu) ----
+  int32_t src_groups_ = 0;                 // 0: no source
+  double *d_src_cdf_ = nullptr;            // [ngroups * E] C[k], caller's numbering
+  double *d_src_bias_ = nullptr;           // [ngroups * E] b[k], nullptr without bias
+  double *d_src_verts_ = nullptr;          // [E][4][3] vertices in the caller's numbering and local order (first use)
+  double src_total_ = 0.0, src_strength_ = 0.0;  // T and Q
+  int64_t src_last_ = -1;                  // the last entry with p > 0
+  std::vector<double> src_given_;          // the strengths as the caller gave them (VTK "source")
+  void free_source();
+  SourceTable source_table() const;
+  bool source_refused(int64_t first, int64_t n, int32_t place);  // with a message
+  int source_arrays(VtkArrays &a);  // "source" (with several groups "source_g<g>"), caller's numbering
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
     void *d = nullptr;    // device copy

@@ -197,4 +197,12 @@ cudaError_t launch_ww_points(const LocateParams &p, const double *xyz, int64_t n
                              const double2 *table, int32_t ngroups, int64_t E, double *lower, double *upper,
                              cudaStream_t stream);
 
+// source_kernels.cu.  Mesh source (source_sample.cuh): sample first + j for j < n, with xyz [3n], elem (caller's
+// numbering), group and weight each optional; state != nullptr also places sample j as particle j (parent element
+// internal_of_orig[elem]), without a walk.
+struct SourceTable;
+cudaError_t launch_source_sample(const SourceTable &S, uint64_t seed, uint64_t first, int64_t n, double *xyz,
+                                 int32_t *elem, int32_t *group, double *weight, ParticleState *state,
+                                 const int32_t *internal_of_orig, cudaStream_t stream);
+
 }  // namespace ptb

@@ -99,6 +99,13 @@ C_API = {
     "pumitally_get_weight_windows_at_points": (C.c_int, [C.c_void_p, _dp, C.c_int64, _ip, _dp, _dp]),
     "pumitally_get_weight_windows_at_points_device": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pumitally_set_source": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_int32, C.c_int32]),
+    "pumitally_get_source_groups": (C.c_int32, [C.c_void_p]),
+    "pumitally_get_source_strength": (C.c_int, [C.c_void_p, _dp]),
+    "pumitally_sample_source": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int64, C.c_int64, _dp, _ip, _ip, _dp, C.c_int32]),
+    "pumitally_sample_source_device": (
+        C.c_int, [C.c_void_p, C.c_uint64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                  C.c_int32, C.c_void_p]),
     "pumitally_write_tally_results": (C.c_int, [C.c_void_p]),
     "pumitally_destroy": (None, [C.c_void_p]),
     "pumitally_create_from_arrays": (C.c_void_p, [_dp, C.c_int64, _ip, C.c_int64, C.c_int32, C.c_int32]),
@@ -794,6 +801,65 @@ class PumiTally:
                                                                  hi.data_ptr(), stream):
             raise RuntimeError("get_weight_windows_at_points_device failed")
         return lo, hi
+
+    # ---- mesh source ---------------------------------------------------------------
+    def set_source(self, strength, bias=None, per_volume=False):
+        """Set the source: strength [ngroups, num_elements] (caller's numbering; one group may be given as
+        [num_elements]), times each element's volume with per_volume, sampled in proportion to strength * bias when a
+        bias of the same layout is given.  None as strength removes the source.  A refusal changes nothing."""
+        if strength is None:
+            rc = self._L.pumitally_set_source(self._h, None, None, 0, 0, 0)
+        else:
+            q = _host_f64(strength, "strength")
+            b = None if bias is None else _host_f64(bias, "bias")
+            if q.size % max(self.num_elements, 1) or (b is not None and b.size != q.size):
+                raise TypeError("strength (and bias) must hold ngroups * num_elements values")
+            rc = self._L.pumitally_set_source(self._h, q.ctypes.data_as(_dp), None if b is None else b.ctypes.data_as(_dp),
+                                              q.size, q.size // max(self.num_elements, 1), int(bool(per_volume)))
+        if rc:
+            raise ValueError("set_source failed")
+
+    @property
+    def source_groups(self) -> int:
+        """Number of energy groups of the source, 0 without one."""
+        return int(self._L.pumitally_get_source_groups(self._h))
+
+    @property
+    def source_strength(self) -> float:
+        """Q: the total unbiased strength (times the volumes with per_volume), by which the caller normalises."""
+        q = C.c_double()
+        if self._L.pumitally_get_source_strength(self._h, C.byref(q)):
+            raise RuntimeError("get_source_strength failed")
+        return q.value
+
+    def sample_source(self, n, seed, first=0, place=False):
+        """Samples first .. first + n - 1 of ``seed``: (xyz [n, 3], elem [n] (caller's numbering), group [n],
+        weight [n]).  place=True (n == num_particles) also makes sample j particle j's position and parent element."""
+        n = int(n)
+        xyz, w = np.empty((n, 3)), np.empty(n)
+        elem, group = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        if self._L.pumitally_sample_source(self._h, int(seed) & ((1 << 64) - 1), int(first), n, xyz.ctypes.data_as(_dp),
+                                           elem.ctypes.data_as(_ip), group.ctypes.data_as(_ip), w.ctypes.data_as(_dp),
+                                           int(bool(place))):
+            raise RuntimeError("sample_source failed")
+        return xyz, elem, group, w
+
+    def sample_source_device(self, n, seed, first=0, place=False, stream=None, device=None):
+        """sample_source() into CUDA tensors (float64 [n, 3], int32 [n], int32 [n], float64 [n]), enqueued on
+        ``stream`` (default: the current torch stream)."""
+        import torch
+
+        n = int(n)
+        dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        xyz, w = torch.empty((n, 3), dtype=torch.float64, device=dev), torch.empty(n, dtype=torch.float64, device=dev)
+        elem, group = (torch.empty(n, dtype=torch.int32, device=dev) for _ in range(2))
+        if stream is None:
+            stream = torch.cuda.current_stream(dev).cuda_stream
+        if self._L.pumitally_sample_source_device(self._h, int(seed) & ((1 << 64) - 1), int(first), n, xyz.data_ptr(),
+                                                  elem.data_ptr(), group.data_ptr(), w.data_ptr(), int(bool(place)),
+                                                  stream):
+            raise RuntimeError("sample_source_device failed")
+        return xyz, elem, group, w
 
     def WriteTallyResults(self, filename=None):
         if filename is not None:
