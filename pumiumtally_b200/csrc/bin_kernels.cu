@@ -58,7 +58,8 @@ __global__ void bin_count_kernel(SeedGrid g, const double *__restrict__ origin, 
   pcell[i] = c;
 }
 
-// exclusive scan of count[0..n) in three small kernels (n <= 2^24)
+// exclusive scan of count[0..n) in three small kernels (tested up to n = 1024 x 1024 x 17 = 17 825 792, the
+// grid choose_seed_grid builds for a 1000 x 1000 x 15.63 slab: 17 408 scan blocks, 17 tiles of block sums)
 __global__ void scan_block_kernel(unsigned int *__restrict__ data, unsigned int *__restrict__ sums, int n) {
   __shared__ unsigned int warp_tot[8];
   const int base = blockIdx.x * kScanBlock + threadIdx.x * 4;
@@ -87,7 +88,7 @@ __global__ void scan_block_kernel(unsigned int *__restrict__ data, unsigned int 
 }
 
 __global__ void scan_sums_kernel(unsigned int *__restrict__ sums, int nb, unsigned int *__restrict__ total) {
-  // single block: serial over tiles of 1024 block sums (nb <= 16384)
+  // single block: serial over tiles of 1024 block sums, carrying the running total from tile to tile (any nb)
   __shared__ unsigned int carry;
   __shared__ unsigned int warp_tot[32];
   if (threadIdx.x == 0) carry = 0;

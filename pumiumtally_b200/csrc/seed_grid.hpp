@@ -11,7 +11,9 @@
 
 namespace ptb {
 
-// Roughly one grid cell per `tets_per_cell` tets, cubic cells, at most 2^24 cells.
+// Roughly one grid cell per `tets_per_cell` tets, cubic cells, at most 1024 per axis.  The target is at most 2^24
+// cells, but rounding each axis up can exceed it: a cube at the cap gets 257^3 = 16 974 593 cells, a 1000 x 1000 x
+// 15.63 slab 1024 x 1024 x 17 = 17 825 792 (the binning tests run both).
 // cell_tet is left null; the caller fills the table by localising the seed points.
 inline SeedGrid choose_seed_grid(const HostMesh &m, double tets_per_cell = 4.0) {
   SeedGrid g{};

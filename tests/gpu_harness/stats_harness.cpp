@@ -85,4 +85,9 @@ int ptb_test_ww_generate(const double *mean, const double *m2, const double *vol
                                      reinterpret_cast<double2 *>(table), static_cast<cudaStream_t>(stream)));
 }
 
+int ptb_test_leakage(const double *cur, int64_t E, int32_t R, const uint32_t *hull, int64_t nhull, double *out,
+                     void *stream) {
+  return int(ptb::launch_leakage(cur, E, R, hull, nhull, out, static_cast<cudaStream_t>(stream)));
+}
+
 }  // extern "C"

@@ -2,8 +2,9 @@
 through a test-only C wrapper of their launchers (tests/gpu_harness/stats_harness.cpp), at the lengths, offsets and
 rank shares that the engine only reaches on several GPUs: odd lengths, shares that start at an odd double (the scalar
 fold and merge), shares that start inside a score record or hold only padding, region plans of several levels, and
-weight-window groups up to the engine's limit.  Every result must equal an exactly rounded host reference bit for
-bit, and every device buffer carries canaries on both sides that must come back untouched."""
+weight-window groups up to the engine's limit; and the leakage sums over hull lists of up to 100 003 slots.  Every
+result must equal an exactly rounded host reference bit for bit (the leakage: one in the documented order), and every
+device buffer carries canaries on both sides that must come back untouched."""
 import ctypes as C
 import functools
 import json
@@ -149,19 +150,24 @@ def assert_bits(got, want, label):
 # ---------------------------------------------------------------------------------------------------------------------
 # Harness
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def harness(tmp_path_factory):
+def build_harness(tmp_path_factory, name):
+    """tests/gpu_harness/<name>.cpp compiled against libpumitally.so; returns the path of the shared library"""
     from pumiumtally_b200 import build as pbuild
 
     lib = pbuild.build_library()
     cuda = os.path.dirname(os.path.dirname(pbuild._nvcc()))
-    so = str(tmp_path_factory.mktemp("stats_harness") / "libstats_harness.so")
+    so = str(tmp_path_factory.mktemp(name) / f"lib{name}.so")
     subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-O1", "-fPIC", "-shared",
                            "-I", os.path.join(ROOT, "pumiumtally_b200", "csrc"), "-I", os.path.join(ROOT, "include"),
-                           "-I", os.path.join(cuda, "include"), os.path.join(HERE, "gpu_harness", "stats_harness.cpp"),
+                           "-I", os.path.join(cuda, "include"), os.path.join(HERE, "gpu_harness", f"{name}.cpp"),
                            "-o", so, "-L", os.path.dirname(lib), "-lpumitally", "-Wl,-rpath," + os.path.dirname(lib),
                            "-L", os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + os.path.join(cuda, "lib64")])
-    return _load_harness(so)
+    return so
+
+
+@pytest.fixture(scope="module")
+def harness(tmp_path_factory):
+    return _load_harness(build_harness(tmp_path_factory, "stats_harness"))
 
 
 def _load_harness(so):
@@ -173,6 +179,7 @@ def _load_harness(so):
     L.ptb_test_batch_merge.argtypes = [p, p, p, p, i64, f64, f64, p]
     L.ptb_test_region_sums.argtypes = [p, i64, i32, i32, i32, i64, i64, p, p, C.POINTER(C.c_int), p]
     L.ptb_test_ww_generate.argtypes = [p, p, p, i64, i32, i64, i32, f64, f64, f64, f64, p, p, p]
+    L.ptb_test_leakage.argtypes = [p, i64, i32, p, i64, p, p]
     return L
 
 
@@ -1048,3 +1055,120 @@ def test_ww_generate_edges(harness, E):
         seen.append(pm[4])
     if E > 1:  # inf: the infinite r counts; r_k: the element at the limit does; one ulp below r_k: it does not
         assert seen[0] == 8.0 and seen[1] == phi_k and seen[2] < phi_k, seen
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Leakage (stats_kernels.cu, leakage_kernel): the documented order of the hull sums
+# ---------------------------------------------------------------------------------------------------------------------
+LEAK_BLOCK = 256  # kLeakBlock
+LEAK_NHULL = [0, 1, 255, 256, 257, 511, 1027, 100_003]
+LEAK_CASES = [(E, nh) for E in (1, 1000, 300_007) for nh in LEAK_NHULL if nh <= 4 * E]
+CANARY = np.array([0x7ff5a5a5c3c3e1e1], dtype=np.uint64).view(np.float64)[0]  # a signalling NaN
+
+
+def leakage_ref(cur, hull, threads=LEAK_BLOCK):
+    """out[r] of launch_leakage over cur [R, 4E] in the documented order: thread k of array r's block adds
+    cur[r, hull[k + threads j]] for j = 0, 1, ... left to right, starting from +0.0; then part[t] += part[t + h] for
+    h = threads / 2, ..., 1."""
+    J = -(-len(hull) // threads)
+    idx = np.zeros(J * threads, dtype=np.int64)
+    idx[:len(hull)] = hull
+    with np.errstate(invalid="ignore"):
+        vals = np.where(np.arange(J * threads) < len(hull), cur[:, idx], 0.0)  # +0.0 + x is x (and never -0.0)
+        part = np.zeros((len(cur), threads))
+        for j in range(J):
+            part = part + vals[:, j * threads:(j + 1) * threads]
+        h = threads // 2
+        while h:
+            part[:, :h] = part[:, :h] + part[:, h:2 * h]
+            h //= 2
+    return part[:, 0]
+
+
+def kuhn_hull_slots(n):
+    """the hull slots 4 e + f, ascending, of kuhn_box(n, n, n) as ensure_face_maps lists them: face f of a tet is the
+    one opposite its vertex f, and a face no other tet shares lies on the hull"""
+    from pumiumtally_b200.mesh import kuhn_box
+
+    _, t2v = kuhn_box(n, n, n)
+    faces = np.sort(np.stack([np.delete(t2v, f, axis=1) for f in range(4)], axis=1).reshape(-1, 3), axis=1)
+    _, inv, cnt = np.unique(faces, axis=0, return_inverse=True, return_counts=True)
+    return len(t2v), np.flatnonzero(cnt[inv.reshape(-1)] == 1).astype(np.uint32)
+
+
+def _leak_case(E, R, nhull, order, seed=0):
+    """(cur [R, 4E] with signalling-NaN canaries in every slot that is not a hull slot, hull): data of mixed magnitudes
+    (1e-8 to 1e8) and signs; with R > 3, arrays 1, 2 and 3 hold a NaN, +inf with -inf, and only -0.0"""
+    rng = np.random.default_rng([E, R, nhull, order == "shuffled", seed])
+    if order == "kuhn":
+        E, hull = kuhn_hull_slots(E)
+        nhull = len(hull)
+    else:
+        hull = np.sort(rng.choice(4 * E, nhull, replace=False)).astype(np.uint32)
+        if order == "shuffled":
+            hull = rng.permutation(hull)
+    cur = np.full((R, 4 * E), CANARY)
+    cur[:, hull] = np.where(rng.random((R, nhull)) < 0.5, -1.0, 1.0) * 10.0 ** rng.uniform(-8, 8, (R, nhull))
+    if R > 3 and nhull >= 2:
+        cur[1, hull[rng.integers(nhull)]] = np.nan
+        a, b = rng.choice(nhull, 2, replace=False)
+        cur[2, hull[a]], cur[2, hull[b]] = np.inf, -np.inf
+        cur[3, hull] = -0.0
+    return E, cur, hull
+
+
+def assert_leak(got, want, label):
+    """bit for bit, except that a NaN is only a NaN (the device's NaN of inf - inf is not the host's)"""
+    nan = np.isnan(want)
+    assert np.array_equal(np.isnan(got), nan), f"{label}: NaN at {np.flatnonzero(np.isnan(got))}, want {nan}"
+    assert_bits(got[~nan], want[~nan], label)
+
+
+def test_leakage_reference_tells_the_order_apart():
+    """The documented order differs, on many arrays, from numpy's pairwise sum, from a sequential sum and from the
+    same scheme with 128 threads; on the special arrays it gives NaN, NaN and +0.0."""
+    E, cur, hull = _leak_case(300_007, 40, 100_003, "shuffled")
+    want = leakage_ref(cur, hull)
+    normal = np.r_[0, 4:40]
+    vals = cur[normal][:, hull]
+    others = {"np.sum": vals.sum(axis=1), "sequential": np.cumsum(vals, axis=1)[:, -1],
+              "128 threads": leakage_ref(cur, hull, threads=128)[normal]}
+    for name, o in others.items():
+        assert (o != want[normal]).sum() >= len(normal) // 2, name
+    assert np.isnan(want[1]) and np.isnan(want[2]) and want[3] == 0.0 and not np.signbit(want[3])
+    exact = [math.fsum(v) for v in vals]  # and it is a sum: each term goes through at most J + 8 additions
+    h = -(-len(hull) // LEAK_BLOCK) + 8
+    bound = h * U / (1 - h * U) * np.abs(vals).sum(axis=1)
+    assert (np.abs(want[normal] - exact) <= bound).all()
+
+
+@gpu
+@pytest.mark.parametrize("order", ["ascending", "shuffled"])
+@pytest.mark.parametrize("R", [1, 3, 40])
+@pytest.mark.parametrize("E, nhull", LEAK_CASES, ids=[f"e{E}-h{nh}" for E, nh in LEAK_CASES])
+def test_leakage_is_exact(harness, E, nhull, R, order):
+    _leakage_run(harness, E, R, nhull, order)
+
+
+@gpu
+@pytest.mark.parametrize("R", [1, 3, 40])
+def test_leakage_of_a_kuhn_box_hull(harness, R):
+    _leakage_run(harness, 20, R, 0, "kuhn")
+
+
+def _leakage_run(harness, E, R, nhull, order):
+    E, cur, hull = _leak_case(E, R, nhull, order)
+    label = f"E {E} R {R} nhull {len(hull)} {order}"
+    gc, gh = Guarded(cur.reshape(-1), 1, seed=1), Guarded(hull, 1, seed=2)
+    out = Guarded(np.full(R, np.nan), seed=3)
+    assert harness.ptb_test_leakage(gc.ptr(), E, R, gh.ptr(), len(hull), out.ptr(), _stream()) == 0
+    want = leakage_ref(cur, hull)
+    assert_leak(out.values(), want, label)
+    out.assert_unchanged_outside(0, R, label + " out")
+    for g in (gc, gh):
+        g.assert_unchanged_outside(0, 0, label + " read-only input")
+    if not len(hull):
+        assert (out.values().view(np.int64) == 0).all(), label  # nothing to add: +0.0
+    if R > 3 and len(hull) >= 2:
+        got = out.values()
+        assert np.isnan(got[1]) and np.isnan(got[2]) and got[3] == 0.0 and not np.signbit(got[3]), label
