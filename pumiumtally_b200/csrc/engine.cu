@@ -17,6 +17,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <stdexcept>
+#include <type_traits>
 
 #include "host_stage.hpp"
 #include "seed_grid.hpp"
@@ -193,9 +194,9 @@ Engine::~Engine() {
   cudaFree(d_pcell_); cudaFree(d_order_); cudaFree(d_cell_count_); cudaFree(d_cell_sums_);
   cudaFree(d_work_count_);
   cudaFree(d_cand_off_); cudaFree(d_cand_);
-  cudaFree(d_qxyz_); cudaFree(d_qout_); cudaFree(d_qint_); cudaFree(d_qelem_);
+  cudaFree(d_arena_);
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
-  cudaFree(d_coll_counts_); cudaFree(d_coll_buf_);
+  cudaFree(d_coll_counts_);
   free_stats();
   free_regions();
   free_weight_windows();
@@ -1896,6 +1897,40 @@ namespace {
 double mesh_extent(const HostMesh &m) {
   return std::max({m.bbox_hi[0] - m.bbox_lo[0], m.bbox_hi[1] - m.bbox_lo[1], m.bbox_hi[2] - m.bbox_lo[2]});
 }
+
+constexpr int64_t kPointsPerLaunch = int64_t(1) << 30;
+
+// Every slice of the arena starts 256-byte aligned, as a cudaMalloc of its own would.
+size_t arena_slice(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+// One host array of a staged call (Engine::staged), `per` T per item; nullptr is absent, and then absent on the device
+// too.  A const T is an input, uploaded before each chunk's enqueue; any other T is an output, copied back after it.
+template <class T>
+struct Staged {
+  T *h;
+  size_t per;
+  std::remove_const_t<T> *d = nullptr;  // its slice of the arena
+  size_t bytes(size_t items) const { return h ? arena_slice(items * per * sizeof(T)) : 0; }
+  void carve(char *&next, size_t items) {
+    d = h ? reinterpret_cast<std::remove_const_t<T> *>(next) : nullptr;
+    next += bytes(items);
+  }
+  cudaError_t upload(size_t first, size_t count, cudaStream_t s) const {
+    if constexpr (std::is_const_v<T>)
+      if (h) return cudaMemcpyAsync(d, h + first * per, count * per * sizeof(T), cudaMemcpyHostToDevice, s);
+    return cudaSuccess;
+  }
+  cudaError_t copy_back(size_t first, size_t count, cudaStream_t s) const {
+    if constexpr (!std::is_const_v<T>)
+      if (h) return cudaMemcpyAsync(h + first * per, d, count * per * sizeof(T), cudaMemcpyDeviceToHost, s);
+    return cudaSuccess;
+  }
+};
+
+template <class T>
+Staged<T> stage(T *h, size_t per = 1) {
+  return {h, per};
+}
 }  // namespace
 
 LocateParams Engine::locate_params() const {
@@ -1928,54 +1963,62 @@ int Engine::ensure_candidates() {
   return 0;
 }
 
-int Engine::ensure_query_buffers(size_t pts, size_t out_doubles) {
-  if (pts > q_cap_) {
-    cudaFree(d_qxyz_); cudaFree(d_qint_); cudaFree(d_qelem_);
-    d_qxyz_ = nullptr; d_qint_ = d_qelem_ = nullptr;
-    q_cap_ = 0;
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qxyz_), 3 * pts * sizeof(double)));
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qint_), pts * sizeof(int32_t)));
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qelem_), pts * sizeof(int32_t)));
-    q_cap_ = pts;
-  }
-  if (out_doubles > q_out_cap_) {
-    cudaFree(d_qout_);
-    d_qout_ = nullptr;
-    q_out_cap_ = 0;
-    PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_qout_), out_doubles * sizeof(double)));
-    q_out_cap_ = out_doubles;
-  }
+int Engine::ensure_arena(size_t bytes) {
+  if (bytes <= arena_bytes_) return 0;
+  cudaFree(d_arena_);
+  d_arena_ = nullptr;
+  arena_bytes_ = 0;
+  PTB_CUDA_OK(cudaMalloc(&d_arena_, bytes));
+  arena_bytes_ = bytes;
   return 0;
 }
 
-int Engine::locate_points(const double *xyz, int64_t npts, int32_t *out_elem) {
-  if (npts < 0 || (npts > 0 && (!xyz || !out_elem))) return 1;
-  if (npts == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const int64_t chunk = std::min<int64_t>(chunk_, npts);
-  if (ensure_element_maps() || ensure_candidates() || ensure_query_buffers(size_t(chunk), 0)) return 1;
-  const LocateParams p = locate_params();
-  for (int64_t b = 0; b < npts; b += chunk) {
-    const int64_t cnt = std::min(chunk, npts - b);
-    PTB_CUDA_OK(cudaMemcpyAsync(d_qxyz_, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
-    PTB_CUDA_OK(launch_locate(p, d_qxyz_, cnt, nullptr, d_qelem_, d_orig_of_internal_, compute_));
-    PTB_CUDA_OK(cudaMemcpyAsync(out_elem + b, d_qelem_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+template <class Setup, class Enqueue, class... A>
+int Engine::staged(int64_t n, Setup &&setup, Enqueue &&enqueue, A... a) {
+  const int64_t chunk = std::min<int64_t>(chunk_, n);
+  const size_t items = n > 0 ? size_t(chunk) : 0;
+  if (int rc = setup((a.bytes(items) + ... + size_t(0)))) return std::max(rc, 0);
+  char *next = static_cast<char *>(d_arena_);
+  (a.carve(next, items), ...);
+  for (int64_t b = 0; b < n; b += chunk) {
+    const int64_t cnt = std::min(chunk, n - b);
+    cudaError_t e = cudaSuccess;
+    const auto ok = [&e](cudaError_t r) { return (e = r) == cudaSuccess; };  // the first failure ends the chunk
+    (void)((ok(a.upload(size_t(b), size_t(cnt), compute_)) && ...) && ok(enqueue(b, cnt, a.d...)) &&
+           (ok(a.copy_back(size_t(b), size_t(cnt), compute_)) && ...));
+    PTB_CUDA_OK(e);
   }
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   return 0;
 }
 
+int Engine::locate_setup(const double *xyz, int64_t npts, const int32_t *elem, size_t arena) {
+  if (npts < 0 || (npts > 0 && (!xyz || !elem))) return 1;
+  if (npts == 0) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  return ensure_element_maps() || ensure_candidates() || ensure_arena(arena);
+}
+
+cudaError_t Engine::enqueue_locate(const double *xyz, int64_t npts, int32_t *elem, cudaStream_t stream) {
+  const LocateParams p = locate_params();
+  for (int64_t b = 0; b < npts; b += kPointsPerLaunch)
+    if (cudaError_t e = launch_locate(p, xyz + 3 * b, std::min(kPointsPerLaunch, npts - b), nullptr, elem + b,
+                                      d_orig_of_internal_, stream))
+      return e;
+  return cudaSuccess;
+}
+
+int Engine::locate_points(const double *xyz, int64_t npts, int32_t *out_elem) {
+  return staged(
+      npts, [&](size_t arena) { return locate_setup(xyz, npts, out_elem, arena); },
+      [&](int64_t, int64_t cnt, const double *x, int32_t *e) { return enqueue_locate(x, cnt, e, compute_); },
+      stage(xyz, 3), stage(out_elem));
+}
+
 // The mesh tables a query reads never change after construction, so it needs no ordering against moves.
 int Engine::locate_points_device(const double *d_xyz, int64_t npts, int32_t *d_elem, cudaStream_t stream) {
-  if (npts < 0 || (npts > 0 && (!d_xyz || !d_elem))) return 1;
-  if (npts == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  if (ensure_element_maps() || ensure_candidates()) return 1;
-  const LocateParams p = locate_params();
-  const int64_t step = int64_t(1) << 30;  // points per launch
-  for (int64_t b = 0; b < npts; b += step)
-    PTB_CUDA_OK(launch_locate(p, d_xyz + 3 * b, std::min(step, npts - b), nullptr, d_elem + b,
-                              d_orig_of_internal_, stream));
+  if (int rc = locate_setup(d_xyz, npts, d_elem, 0)) return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_locate(d_xyz, npts, d_elem, stream));
   return 0;
 }
 
@@ -2030,18 +2073,28 @@ int Engine::evaluate_points(const double *xyz, int64_t npts, double *out, int64_
   const int64_t rows = n == npts ? 1 : R;
   // the results of a chunk are at most 256 MB of device memory
   const int64_t chunk = std::min<int64_t>(std::min<int64_t>(chunk_, std::max<int64_t>(1024, (int64_t(1) << 25) / rows)), npts);
-  if (ensure_element_maps() || ensure_candidates() || ensure_query_buffers(size_t(chunk), size_t(rows * chunk))) return 1;
+  // arena slices: points, internal and caller's element ids, results [rows][cnt]
+  const size_t c = size_t(chunk), xyz_bytes = arena_slice(3 * c * sizeof(double));
+  const size_t id_bytes = arena_slice(c * sizeof(int32_t));
+  if (ensure_element_maps() || ensure_candidates() ||
+      ensure_arena(xyz_bytes + 2 * id_bytes + size_t(rows) * c * sizeof(double)))
+    return 1;
+  char *arena = static_cast<char *>(d_arena_);
+  double *qxyz = reinterpret_cast<double *>(arena);
+  int32_t *qint = reinterpret_cast<int32_t *>(arena + xyz_bytes);
+  int32_t *qelem = reinterpret_cast<int32_t *>(arena + xyz_bytes + id_bytes);
+  double *qout = reinterpret_cast<double *>(arena + xyz_bytes + 2 * id_bytes);
   const LocateParams p = locate_params();
   for (int64_t b = 0; b < npts; b += chunk) {
     const int64_t cnt = std::min(chunk, npts - b);
-    PTB_CUDA_OK(cudaMemcpyAsync(d_qxyz_, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
-    PTB_CUDA_OK(launch_locate(p, d_qxyz_, cnt, d_qint_, out_elem ? d_qelem_ : nullptr, d_orig_of_internal_, compute_));
-    PTB_CUDA_OK(launch_evaluate(d_qxyz_, d_qint_, cnt, d_eval_vals_, moments_ ? d_eval_grads_ : nullptr, d_eval_cen_,
-                                mesh_.ntets, int32_t(rows), d_qout_, cnt, compute_));
-    PTB_CUDA_OK(cudaMemcpy2DAsync(out + b, size_t(npts) * sizeof(double), d_qout_, size_t(cnt) * sizeof(double),
+    PTB_CUDA_OK(cudaMemcpyAsync(qxyz, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
+    PTB_CUDA_OK(launch_locate(p, qxyz, cnt, qint, out_elem ? qelem : nullptr, d_orig_of_internal_, compute_));
+    PTB_CUDA_OK(launch_evaluate(qxyz, qint, cnt, d_eval_vals_, moments_ ? d_eval_grads_ : nullptr, d_eval_cen_,
+                                mesh_.ntets, int32_t(rows), qout, cnt, compute_));
+    PTB_CUDA_OK(cudaMemcpy2DAsync(out + b, size_t(npts) * sizeof(double), qout, size_t(cnt) * sizeof(double),
                                   size_t(cnt) * sizeof(double), size_t(rows), cudaMemcpyDeviceToHost, compute_));
     if (out_elem)
-      PTB_CUDA_OK(cudaMemcpyAsync(out_elem + b, d_qelem_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+      PTB_CUDA_OK(cudaMemcpyAsync(out_elem + b, qelem, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
   }
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   return 0;
@@ -2074,136 +2127,91 @@ bool Engine::collision_refused(const double *responses, const double *times) con
   return why != nullptr;
 }
 
-int Engine::ensure_collision_buffer(size_t bytes) {
-  if (bytes <= coll_buf_bytes_) return 0;
-  cudaFree(d_coll_buf_);
-  d_coll_buf_ = nullptr;
-  coll_buf_bytes_ = 0;
-  PTB_CUDA_OK(cudaMalloc(&d_coll_buf_, bytes));
-  coll_buf_bytes_ = bytes;
+int Engine::collide_located_setup(const double *xyz, int64_t n, const double *w, const double *r, const double *t,
+                                  size_t arena) {
+  if (collision_refused(r, t) || n < 0 || (n > 0 && (!xyz || !w))) return 1;
+  if (n == 0) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_candidates() || ensure_arena(arena)) return 1;
+  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on, as with a move
+  tallied_ = true;
   return 0;
 }
 
-namespace {
-// The chunk-sized event arrays of a host-pointer collision call in one device buffer: xyz [3c] (located calls only),
-// weights [c], responses [nscores c], times [c], bins [c], collided [c] (at-particles calls only).  Per event that is
-// 24 + 8 + 8 nscores + 8 + 4 (+ 1) bytes.
-struct EventBuffers {
-  double *xyz, *w, *r, *t;
-  int32_t *bins;
-  int8_t *collided;
-  static size_t bytes(size_t c, size_t nscores) { return c * (24 + 8 + 8 * nscores + 8 + 4 + 1); }
-  EventBuffers(void *base, size_t c, size_t nscores) {
-    xyz = static_cast<double *>(base);
-    w = xyz + 3 * c;
-    r = w + c;
-    t = r + nscores * c;
-    bins = reinterpret_cast<int32_t *>(t + c);
-    collided = reinterpret_cast<int8_t *>(bins + c);
-  }
-};
-
-cudaError_t upload(void *dst, const void *src, size_t bytes, cudaStream_t s) {
-  return src ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+cudaError_t Engine::enqueue_collide_located(const double *xyz, int64_t n, const double *w, const double *r,
+                                            const int32_t *bins, const double *t, cudaStream_t stream) {
+  const LocateParams l = locate_params();
+  const CollisionParams p = collision_params();
+  const size_t S = size_t(nscores_);
+  for (int64_t b = 0; b < n; b += kPointsPerLaunch)
+    if (cudaError_t e = launch_collide_located(l, p, xyz + 3 * b, std::min(kPointsPerLaunch, n - b), w + b,
+                                               r ? r + S * size_t(b) : nullptr, bins ? bins + b : nullptr,
+                                               ntime_ > 0 ? t + b : nullptr, d_coll_counts_, stream))
+      return e;
+  return cudaSuccess;
 }
-}  // namespace
 
 int Engine::tally_collisions(const double *xyz, int64_t nevents, const double *weights, const double *responses,
                              const int32_t *bins, const double *times) {
-  if (collision_refused(responses, times) || nevents < 0 || (nevents > 0 && (!xyz || !weights))) return 1;
-  if (nevents == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const int64_t chunk = std::min<int64_t>(chunk_, nevents);
-  const size_t S = size_t(nscores_);
-  if (ensure_candidates() || ensure_collision_buffer(EventBuffers::bytes(size_t(chunk), S))) return 1;
-  const EventBuffers d(d_coll_buf_, size_t(chunk), S);
-  const LocateParams l = locate_params();
-  const CollisionParams p = collision_params();
-  const double *t = ntime_ > 0 ? times : nullptr;
-  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on, as with a move
-  tallied_ = true;
-  for (int64_t b = 0; b < nevents; b += chunk) {
-    const size_t cnt = size_t(std::min(chunk, nevents - b));
-    PTB_CUDA_OK(upload(d.xyz, xyz + 3 * b, 3 * cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.w, weights + b, cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.r, responses ? responses + S * size_t(b) : nullptr, S * cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.t, t ? t + b : nullptr, cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.bins, bins ? bins + b : nullptr, cnt * sizeof(int32_t), compute_));
-    PTB_CUDA_OK(launch_collide_located(l, p, d.xyz, int64_t(cnt), d.w, responses ? d.r : nullptr, bins ? d.bins : nullptr,
-                                       d.t, d_coll_counts_, compute_));
-  }
-  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
-  return 0;
+  return staged(
+      nevents, [&](size_t arena) { return collide_located_setup(xyz, nevents, weights, responses, times, arena); },
+      [&](int64_t, int64_t cnt, const double *x, const double *w, const double *r, const double *t, const int32_t *bn) {
+        return enqueue_collide_located(x, cnt, w, r, bn, t, compute_);
+      },
+      // times are read only while time bins are set, so only then do they travel
+      stage(xyz, 3), stage(weights), stage(responses, size_t(nscores_)), stage(ntime_ > 0 ? times : nullptr),
+      stage(bins));
 }
 
 // The mesh tables location reads never change after construction, so located events need no ordering against moves.
 int Engine::tally_collisions_device(const double *d_xyz, int64_t nevents, const double *d_weights,
                                     const double *d_responses, const int32_t *d_bins, const double *d_times,
                                     cudaStream_t stream) {
-  if (collision_refused(d_responses, d_times) || nevents < 0 || (nevents > 0 && (!d_xyz || !d_weights))) return 1;
-  if (nevents == 0) return 0;
+  if (int rc = collide_located_setup(d_xyz, nevents, d_weights, d_responses, d_times, 0)) return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_collide_located(d_xyz, nevents, d_weights, d_responses, d_bins, d_times, stream));
+  return 0;
+}
+
+int Engine::collide_particles_setup(const int8_t *collided, const double *w, const double *r, const double *t,
+                                    int32_t n, size_t arena, cudaStream_t stream) {
+  if (collision_refused(r, t)) return 1;
+  if (n != n_ || (n > 0 && (!collided || !w))) {
+    fprintf(stderr, "[pumitally] ERROR: collision events at the particles: n must be num_particles (%d)\n", n_);
+    return 1;
+  }
+  if (n == 0) return -1;
   PTB_CUDA_OK(cudaSetDevice(device_));
-  if (ensure_candidates()) return 1;
-  const LocateParams l = locate_params();
-  const CollisionParams p = collision_params();
-  const size_t S = size_t(nscores_);
+  if (ensure_arena(arena) || follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
   tallied_ = true;
-  const int64_t step = int64_t(1) << 30;  // events per launch
-  for (int64_t b = 0; b < nevents; b += step)
-    PTB_CUDA_OK(launch_collide_located(l, p, d_xyz + 3 * b, std::min(step, nevents - b), d_weights + b,
-                                       d_responses ? d_responses + S * size_t(b) : nullptr, d_bins ? d_bins + b : nullptr,
-                                       ntime_ > 0 ? d_times + b : nullptr, d_coll_counts_, stream));
   return 0;
+}
+
+cudaError_t Engine::enqueue_collide_particles(int32_t first, int32_t n, const int8_t *collided, const double *w,
+                                              const double *r, const int32_t *bins, const double *t,
+                                              cudaStream_t stream) {
+  return launch_collide_particles(d_state_ + first, collided, n, collision_params(), w, r, bins,
+                                  ntime_ > 0 ? t : nullptr, d_coll_counts_, stream);
 }
 
 int Engine::tally_collisions_at_particles(const int8_t *collided, const double *weights, const double *responses,
                                           const int32_t *bins, const double *times, int32_t n) {
-  if (collision_refused(responses, times)) return 1;
-  if (n != n_ || (n > 0 && (!collided || !weights))) {
-    fprintf(stderr, "[pumitally] ERROR: collision events at the particles: n must be num_particles (%d)\n", n_);
-    return 1;
-  }
-  if (n == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const int32_t chunk = std::min(chunk_, n);
-  const size_t S = size_t(nscores_);
-  if (ensure_collision_buffer(EventBuffers::bytes(size_t(chunk), S))) return 1;
-  const EventBuffers d(d_coll_buf_, size_t(chunk), S);
-  const CollisionParams p = collision_params();
-  const double *t = ntime_ > 0 ? times : nullptr;
-  if (follow_last_stream(compute_)) return 1;  // reads the particle state the last move wrote
-  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
-  tallied_ = true;
-  for (int32_t b = 0; b < n; b += chunk) {
-    const size_t cnt = size_t(std::min(chunk, n - b));
-    PTB_CUDA_OK(upload(d.collided, collided + b, cnt, compute_));
-    PTB_CUDA_OK(upload(d.w, weights + b, cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.r, responses ? responses + S * size_t(b) : nullptr, S * cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.t, t ? t + b : nullptr, cnt * sizeof(double), compute_));
-    PTB_CUDA_OK(upload(d.bins, bins ? bins + b : nullptr, cnt * sizeof(int32_t), compute_));
-    PTB_CUDA_OK(launch_collide_particles(d_state_ + b, d.collided, int32_t(cnt), p, d.w, responses ? d.r : nullptr,
-                                         bins ? d.bins : nullptr, d.t, d_coll_counts_, compute_));
-  }
-  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
-  return 0;
+  return staged(
+      n, [&](size_t arena) { return collide_particles_setup(collided, weights, responses, times, n, arena, compute_); },
+      [&](int64_t b, int64_t cnt, const int8_t *c, const double *w, const double *r, const double *t,
+          const int32_t *bn) {
+        return enqueue_collide_particles(int32_t(b), int32_t(cnt), c, w, r, bn, t, compute_);
+      },
+      stage(collided), stage(weights), stage(responses, size_t(nscores_)), stage(ntime_ > 0 ? times : nullptr),
+      stage(bins));
 }
 
 int Engine::tally_collisions_at_particles_device(const int8_t *d_collided, const double *d_weights,
                                                  const double *d_responses, const int32_t *d_bins,
                                                  const double *d_times, int32_t n, cudaStream_t stream) {
-  if (collision_refused(d_responses, d_times)) return 1;
-  if (n != n_ || (n > 0 && (!d_collided || !d_weights))) {
-    fprintf(stderr, "[pumitally] ERROR: collision events at the particles: n must be num_particles (%d)\n", n_);
-    return 1;
-  }
-  if (n == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  if (follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
-  flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;
-  tallied_ = true;
-  PTB_CUDA_OK(launch_collide_particles(d_state_, d_collided, n, collision_params(), d_weights, d_responses, d_bins,
-                                       ntime_ > 0 ? d_times : nullptr, d_coll_counts_, stream));
+  if (int rc = collide_particles_setup(d_collided, d_weights, d_responses, d_times, n, 0, stream))
+    return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_collide_particles(0, n, d_collided, d_weights, d_responses, d_bins, d_times, stream));
   return 0;
 }
 
@@ -3295,79 +3303,71 @@ int Engine::generate_weight_windows(int32_t tally, int32_t score, int32_t time_b
   return 0;
 }
 
-bool Engine::ww_lookup_refused(const char *what, bool particles, int64_t n) {
-  const char *why = !particles ? (n < 0 ? "npts must be >= 0" : nullptr)
-                    : n != n_  ? "n must be num_particles"
-                    : !initialized_ ? "called before CopyInitialPosition"
-                                    : nullptr;
-  if (why) fprintf(stderr, "[pumitally] ERROR: weight windows %s refused: %s\n", what, why);
-  return why != nullptr;
+int Engine::ww_particles_setup(int32_t n, const double *lower, const double *upper, size_t arena,
+                               cudaStream_t stream) {
+  const char *why = n != n_ ? "n must be num_particles" : !initialized_ ? "called before CopyInitialPosition" : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: weight windows at the particles refused: %s\n", why);
+  if (why || (n > 0 && (!lower || !upper))) return 1;
+  if (n == 0) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  return ensure_arena(arena) || follow_last_stream(stream);  // reads the particle state the last move wrote
+}
+
+cudaError_t Engine::enqueue_ww_particles(int32_t first, int32_t n, const int32_t *groups, double *lower,
+                                         double *upper, cudaStream_t stream) {
+  return launch_ww_particles(d_state_ + first, n, groups, d_ww_, ww_groups_, mesh_.ntets, lower, upper, stream);
 }
 
 int Engine::weight_windows_at_particles(const int32_t *groups, double *lower, double *upper, int32_t n) {
-  if (ww_lookup_refused("at the particles", true, n) || (n > 0 && (!lower || !upper))) return 1;
-  if (n == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const int32_t chunk = std::min(chunk_, n);
-  if (ensure_query_buffers(size_t(chunk), 2 * size_t(chunk))) return 1;
-  if (follow_last_stream(compute_)) return 1;  // reads the particle state the last move wrote
-  for (int32_t b = 0; b < n; b += chunk) {
-    const int32_t cnt = std::min(chunk, n - b);
-    if (groups)
-      PTB_CUDA_OK(cudaMemcpyAsync(d_qint_, groups + b, size_t(cnt) * sizeof(int32_t), cudaMemcpyHostToDevice, compute_));
-    PTB_CUDA_OK(launch_ww_particles(d_state_ + b, cnt, groups ? d_qint_ : nullptr, d_ww_, ww_groups_, mesh_.ntets,
-                                    d_qout_, d_qout_ + cnt, compute_));
-    PTB_CUDA_OK(cudaMemcpyAsync(lower + b, d_qout_, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
-    PTB_CUDA_OK(cudaMemcpyAsync(upper + b, d_qout_ + cnt, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
-  }
-  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
-  return 0;
+  return staged(
+      n, [&](size_t arena) { return ww_particles_setup(n, lower, upper, arena, compute_); },
+      [&](int64_t b, int64_t cnt, const int32_t *g, double *lo, double *up) {
+        return enqueue_ww_particles(int32_t(b), int32_t(cnt), g, lo, up, compute_);
+      },
+      stage(groups), stage(lower), stage(upper));
 }
 
 int Engine::weight_windows_at_particles_device(const int32_t *d_groups, double *d_lower, double *d_upper, int32_t n,
                                                cudaStream_t stream) {
-  if (ww_lookup_refused("at the particles", true, n) || (n > 0 && (!d_lower || !d_upper))) return 1;
-  if (n == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  if (follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
-  PTB_CUDA_OK(launch_ww_particles(d_state_, n, d_groups, d_ww_, ww_groups_, mesh_.ntets, d_lower, d_upper, stream));
+  if (int rc = ww_particles_setup(n, d_lower, d_upper, 0, stream)) return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_ww_particles(0, n, d_groups, d_lower, d_upper, stream));
   return 0;
+}
+
+int Engine::ww_points_setup(const double *xyz, int64_t npts, const double *lower, const double *upper, size_t arena) {
+  if (npts < 0) fprintf(stderr, "[pumitally] ERROR: weight windows at points refused: npts must be >= 0\n");
+  if (npts < 0 || (npts > 0 && (!xyz || !lower || !upper))) return 1;
+  if (npts == 0) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  return ensure_candidates() || ensure_arena(arena);
+}
+
+cudaError_t Engine::enqueue_ww_points(const double *xyz, int64_t npts, const int32_t *groups, double *lower,
+                                      double *upper, cudaStream_t stream) {
+  const LocateParams p = locate_params();
+  for (int64_t b = 0; b < npts; b += kPointsPerLaunch)
+    if (cudaError_t e = launch_ww_points(p, xyz + 3 * b, std::min(kPointsPerLaunch, npts - b),
+                                         groups ? groups + b : nullptr, d_ww_, ww_groups_, mesh_.ntets, lower + b,
+                                         upper + b, stream))
+      return e;
+  return cudaSuccess;
 }
 
 int Engine::weight_windows_at_points(const double *xyz, int64_t npts, const int32_t *groups, double *lower,
                                      double *upper) {
-  if (ww_lookup_refused("at points", false, npts) || (npts > 0 && (!xyz || !lower || !upper))) return 1;
-  if (npts == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const int64_t chunk = std::min<int64_t>(chunk_, npts);
-  if (ensure_candidates() || ensure_query_buffers(size_t(chunk), 2 * size_t(chunk))) return 1;
-  const LocateParams p = locate_params();
-  for (int64_t b = 0; b < npts; b += chunk) {
-    const int64_t cnt = std::min(chunk, npts - b);
-    PTB_CUDA_OK(cudaMemcpyAsync(d_qxyz_, xyz + 3 * b, size_t(cnt) * 3 * sizeof(double), cudaMemcpyHostToDevice, compute_));
-    if (groups)
-      PTB_CUDA_OK(cudaMemcpyAsync(d_qint_, groups + b, size_t(cnt) * sizeof(int32_t), cudaMemcpyHostToDevice, compute_));
-    PTB_CUDA_OK(launch_ww_points(p, d_qxyz_, cnt, groups ? d_qint_ : nullptr, d_ww_, ww_groups_, mesh_.ntets, d_qout_,
-                                 d_qout_ + cnt, compute_));
-    PTB_CUDA_OK(cudaMemcpyAsync(lower + b, d_qout_, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
-    PTB_CUDA_OK(cudaMemcpyAsync(upper + b, d_qout_ + cnt, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
-  }
-  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
-  return 0;
+  return staged(
+      npts, [&](size_t arena) { return ww_points_setup(xyz, npts, lower, upper, arena); },
+      [&](int64_t, int64_t cnt, const double *x, const int32_t *g, double *lo, double *up) {
+        return enqueue_ww_points(x, cnt, g, lo, up, compute_);
+      },
+      stage(xyz, 3), stage(groups), stage(lower), stage(upper));
 }
 
 // The mesh tables location reads never change after construction, so a point lookup needs no ordering against moves.
 int Engine::weight_windows_at_points_device(const double *d_xyz, int64_t npts, const int32_t *d_groups, double *d_lower,
                                             double *d_upper, cudaStream_t stream) {
-  if (ww_lookup_refused("at points", false, npts) || (npts > 0 && (!d_xyz || !d_lower || !d_upper))) return 1;
-  if (npts == 0) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  if (ensure_candidates()) return 1;
-  const LocateParams p = locate_params();
-  const int64_t step = int64_t(1) << 30;  // points per launch
-  for (int64_t b = 0; b < npts; b += step)
-    PTB_CUDA_OK(launch_ww_points(p, d_xyz + 3 * b, std::min(step, npts - b), d_groups ? d_groups + b : nullptr, d_ww_,
-                                 ww_groups_, mesh_.ntets, d_lower + b, d_upper + b, stream));
+  if (int rc = ww_points_setup(d_xyz, npts, d_lower, d_upper, 0)) return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_ww_points(d_xyz, npts, d_groups, d_lower, d_upper, stream));
   return 0;
 }
 
@@ -3494,42 +3494,22 @@ int Engine::get_source_strength(double *total) {
   return 0;
 }
 
-bool Engine::source_refused(int64_t first, int64_t n, int32_t place) {
+int Engine::source_setup(int64_t first, int64_t n, bool outputs, int32_t place, size_t arena, cudaStream_t stream) {
   const char *why = src_groups_ == 0                 ? "no source is set (set_source)"
                     : first < 0                      ? "first must be >= 0"
                     : n < 0                          ? "n must be >= 0"
                     : n > INT64_MAX - first          ? "first + n overflows"
                     : (place && n != int64_t(n_))    ? "with place, n must be num_particles"
                                                      : nullptr;
-  if (why) fprintf(stderr, "[pumitally] ERROR: sample_source refused: %s\n", why);
-  return why != nullptr;
-}
-
-int Engine::sample_source(uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem, int32_t *group,
-                          double *weight, int32_t place) {
-  if (source_refused(first, n, place)) return 1;
-  if (n == 0 || !(place || xyz || elem || group || weight)) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  const int64_t chunk = std::min<int64_t>(chunk_, n);
-  if (ensure_query_buffers(size_t(chunk), size_t(chunk))) return 1;
-  if (place && (ensure_element_maps() || follow_last_stream(compute_))) return 1;  // writes the particle state
-  const SourceTable S = source_table();
-  for (int64_t b = 0; b < n; b += chunk) {
-    const int64_t cnt = std::min(chunk, n - b);
-    PTB_CUDA_OK(launch_source_sample(S, seed, uint64_t(first + b), cnt, xyz ? d_qxyz_ : nullptr,
-                                     elem ? d_qelem_ : nullptr, group ? d_qint_ : nullptr, weight ? d_qout_ : nullptr,
-                                     place ? d_state_ + b : nullptr, d_internal_of_orig_, compute_));
-    if (xyz)
-      PTB_CUDA_OK(cudaMemcpyAsync(xyz + 3 * b, d_qxyz_, size_t(cnt) * 3 * sizeof(double), cudaMemcpyDeviceToHost, compute_));
-    if (elem)
-      PTB_CUDA_OK(cudaMemcpyAsync(elem + b, d_qelem_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
-    if (group)
-      PTB_CUDA_OK(cudaMemcpyAsync(group + b, d_qint_, size_t(cnt) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
-    if (weight)
-      PTB_CUDA_OK(cudaMemcpyAsync(weight + b, d_qout_, size_t(cnt) * sizeof(double), cudaMemcpyDeviceToHost, compute_));
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: sample_source refused: %s\n", why);
+    return 1;
   }
-  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  if (n == 0 || !(place || outputs)) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_arena(arena)) return 1;
   if (place) {  // the initial placement, as set_state_device makes it
+    if (ensure_element_maps() || follow_last_stream(stream)) return 1;  // writes the particle state
     initialized_ = true;
     mirror_valid_ = false;
     pos_mirror_valid_ = false;
@@ -3537,19 +3517,26 @@ int Engine::sample_source(uint64_t seed, int64_t first, int64_t n, double *xyz, 
   return 0;
 }
 
+cudaError_t Engine::enqueue_source(uint64_t seed, int64_t first, int64_t b, int64_t n, double *xyz, int32_t *elem,
+                                   int32_t *group, double *weight, bool place, cudaStream_t stream) {
+  return launch_source_sample(source_table(), seed, uint64_t(first + b), n, xyz, elem, group, weight,
+                              place ? d_state_ + b : nullptr, d_internal_of_orig_, stream);
+}
+
+int Engine::sample_source(uint64_t seed, int64_t first, int64_t n, double *xyz, int32_t *elem, int32_t *group,
+                          double *weight, int32_t place) {
+  return staged(
+      n, [&](size_t arena) { return source_setup(first, n, xyz || elem || group || weight, place, arena, compute_); },
+      [&](int64_t b, int64_t cnt, double *x, int32_t *e, int32_t *g, double *w) {
+        return enqueue_source(seed, first, b, cnt, x, e, g, w, place, compute_);
+      },
+      stage(xyz, 3), stage(elem), stage(group), stage(weight));
+}
+
 int Engine::sample_source_device(uint64_t seed, int64_t first, int64_t n, double *d_xyz, int32_t *d_elem,
                                  int32_t *d_group, double *d_weight, int32_t place, cudaStream_t stream) {
-  if (source_refused(first, n, place)) return 1;
-  if (n == 0 || !(place || d_xyz || d_elem || d_group || d_weight)) return 0;
-  PTB_CUDA_OK(cudaSetDevice(device_));
-  if (place && (ensure_element_maps() || follow_last_stream(stream))) return 1;  // writes the particle state
-  PTB_CUDA_OK(launch_source_sample(source_table(), seed, uint64_t(first), n, d_xyz, d_elem, d_group, d_weight,
-                                   place ? d_state_ : nullptr, d_internal_of_orig_, stream));
-  if (place) {
-    initialized_ = true;
-    mirror_valid_ = false;
-    pos_mirror_valid_ = false;
-  }
+  if (int rc = source_setup(first, n, d_xyz || d_elem || d_group || d_weight, place, 0, stream)) return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_source(seed, first, 0, n, d_xyz, d_elem, d_group, d_weight, place, stream));
   return 0;
 }
 

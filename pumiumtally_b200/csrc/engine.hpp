@@ -292,11 +292,17 @@ class Engine {
   int32_t *d_cand_ = nullptr;
   size_t cand_entries_ = 0;
   bool candidates_ready_ = false;
-  // chunk-sized buffers of the host-pointer queries: points, internal and caller's element ids, results
-  size_t q_cap_ = 0, q_out_cap_ = 0;
-  double *d_qxyz_ = nullptr, *d_qout_ = nullptr;
-  int32_t *d_qint_ = nullptr, *d_qelem_ = nullptr;
-  int ensure_query_buffers(size_t pts, size_t out_doubles);
+  // The query, event and sampling calls: each has a setup its host and device forms share (refusal, device, lazy tables,
+  // `arena` bytes for the host form, stream order, flags; 1 refused or failed, -1 nothing to enqueue, 0 go on) and an
+  // enqueue of its kernels from device pointers, which the host form runs through staged().
+  int locate_setup(const double *xyz, int64_t npts, const int32_t *elem, size_t arena);
+  cudaError_t enqueue_locate(const double *xyz, int64_t npts, int32_t *elem, cudaStream_t stream);
+  // n items in chunks of min(chunk_, n) through the arena (Staged arrays, engine.cu): setup(arena bytes), then per chunk
+  // the uploads, enqueue(first item, count, device arrays...) and the copies back on compute_; one sync at the end
+  template <class Setup, class Enqueue, class... A> int staged(int64_t n, Setup &&setup, Enqueue &&enqueue, A... a);
+  void *d_arena_ = nullptr;  // grow-only device scratch of the host forms, carved into 256-byte aligned slices
+  size_t arena_bytes_ = 0;
+  int ensure_arena(size_t bytes);
   // evaluation table, internal element order: vals [R][E] normalised results, with moments grads [R][E][3] (the
   // normalised gradient) and cen [E][3] (vertex-average centroids); valid until the next move, reset, exchange or change
   // of the source normalisation or of the configuration
@@ -318,9 +324,14 @@ class Engine {
   bool collision_refused(const double *responses, const double *times) const;  // with a message
   int follow_last_stream(cudaStream_t stream);  // order work on the particle state behind the last such work
   unsigned long long *d_coll_counts_ = nullptr;  // [3] events tallied, outside the mesh, rejected since the last reset
-  void *d_coll_buf_ = nullptr;                   // chunk-sized event arrays of the host-pointer calls
-  size_t coll_buf_bytes_ = 0;
-  int ensure_collision_buffer(size_t bytes);
+  int collide_located_setup(const double *xyz, int64_t n, const double *w, const double *r, const double *t,
+                            size_t arena);
+  cudaError_t enqueue_collide_located(const double *xyz, int64_t n, const double *w, const double *r,
+                                      const int32_t *bins, const double *t, cudaStream_t stream);
+  int collide_particles_setup(const int8_t *collided, const double *w, const double *r, const double *t, int32_t n,
+                              size_t arena, cudaStream_t stream);
+  cudaError_t enqueue_collide_particles(int32_t first, int32_t n, const int8_t *collided, const double *w,
+                                        const double *r, const int32_t *bins, const double *t, cudaStream_t stream);
   // ---- batch statistics (stats_kernels.cu) ----
   bool batch_stats_ = false;
   int64_t batches_ = 0;                            // batches folded
@@ -382,7 +393,12 @@ class Engine {
   double2 *d_ww_ = nullptr;   // [ww_groups_][internal element] (lower, upper), (-1, -1) where there is none
   void free_weight_windows();
   int alloc_weight_windows(int32_t ngroups, double2 **out);  // 16 ngroups E bytes; nothing changes when it fails
-  bool ww_lookup_refused(const char *what, bool particles, int64_t n);  // with a message
+  int ww_particles_setup(int32_t n, const double *lower, const double *upper, size_t arena, cudaStream_t stream);
+  cudaError_t enqueue_ww_particles(int32_t first, int32_t n, const int32_t *groups, double *lower, double *upper,
+                                   cudaStream_t stream);
+  int ww_points_setup(const double *xyz, int64_t npts, const double *lower, const double *upper, size_t arena);
+  cudaError_t enqueue_ww_points(const double *xyz, int64_t npts, const int32_t *groups, double *lower, double *upper,
+                                cudaStream_t stream);
   // the "ww_lower" / "ww_upper" arrays (with several groups "_g<g>" after each name), caller's numbering
   int ww_arrays(VtkArrays &a);
   // ---- mesh source (source_kernels.cu) ----
@@ -395,7 +411,10 @@ class Engine {
   std::vector<double> src_given_;          // the strengths as the caller gave them (VTK "source")
   void free_source();
   SourceTable source_table() const;
-  bool source_refused(int64_t first, int64_t n, int32_t place);  // with a message
+  int source_setup(int64_t first, int64_t n, bool outputs, int32_t place, size_t arena, cudaStream_t stream);
+  // samples first + b .. first + b + n - 1, with place into particles b .. b + n - 1
+  cudaError_t enqueue_source(uint64_t seed, int64_t first, int64_t b, int64_t n, double *xyz, int32_t *elem,
+                             int32_t *group, double *weight, bool place, cudaStream_t stream);
   int source_arrays(VtkArrays &a);  // "source" (with several groups "source_g<g>"), caller's numbering
   // per-particle side arrays of a host-pointer move on their way to the device (upload_aux)
   struct AuxUpload {
