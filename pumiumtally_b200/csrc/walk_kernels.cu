@@ -271,7 +271,9 @@ cudaError_t launch_product(const KernelParamsCU<NS, TM, CU> &p, int variant, int
     case kVariantPersistRefill8:
       return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, NS, TM, MO, CU>(p, n, stream);
     case kVariantPersistGatherL1:
-      return launch_persist<128, kFetchPolicyL1, 6, 8, 1, 40, NS, TM, MO, CU>(p, n, stream);
+      // five blocks: six do not fit the cooperative fetch's rows next to the L1 (the timed walk, which keeps the per-lane
+      // fetch, runs at the same occupancy as the others)
+      return launch_persist<128, kFetchCoopL1, 5, 8, 1, 40, NS, TM, MO, CU>(p, n, stream);
     case kVariantPacked:
       if (!p.rows) return cudaErrorInvalidValue;
       return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, NS, TM, MO, CU>(p, n, stream);

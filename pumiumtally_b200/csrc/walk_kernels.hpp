@@ -26,7 +26,7 @@ enum WalkVariant : int {
   kVariantPersistRefill8Occ8 = 9,    // 8 compiled for 8 resident blocks (64 registers) -- re-test after entry-face elision
   kVariantPersistBulkOcc7 = 13,      // 6 compiled for 7 resident blocks
   kVariantPersistGather = 15,        // 8 on spatially binned particles (order[] from launch_bin_particles)
-  kVariantPersistGatherL1 = 16,      // 15 with L1-allocating tet loads (default, mesh >> L2)
+  kVariantPersistGatherL1 = 16,      // 15 with the cooperative L1-allocating record fetch, 5 blocks/SM (default, mesh >> L2)
   kVariantPersistGatherPlain = 17,   // 15 with plain tet loads (no L2 policy)
   kVariantEdge = 20,        // compact layout + edge-function exit test (walk_compact.cuh), streaming order
   kVariantEdgeGather = 21,  // 20 on spatially binned particles

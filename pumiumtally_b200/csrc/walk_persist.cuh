@@ -189,15 +189,17 @@ __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedR
 //   2  as 1, plus the L2::128B prefetch size (first sector miss pulls the whole line)
 //   3  one cp.async.bulk of 128 B per lane into a shared-memory row (policies as 1)
 //   (4 was a cooperative quad-load + shared-memory transpose: slower, removed)
-//   5  as 1 but the tet loads allocate in L1 (worth it once particles are processed in
-//      spatial order and neighbouring lanes/warps revisit the same records)
+//   5  cooperative line fetch (coop_plane_step): the warp copies the records of its active lanes into
+//      per-warp shared-memory rows, eight lanes per record, so one 128-bit load touches 4 lines instead of 32;
+//      L1-allocating, evict_last in L2 (the binned kernel, variant 16)
+//   11 as 1 but the tet loads allocate in L1, each lane fetching its own record
 //   6  compact layout + edge-function exit test (walk_compact.cuh): one 32-byte TetLinks sector and
 //      one 32-byte vertex per crossing, both L2-resident; degenerate rays finish on the plane records
-//   7, 8  as 1 and 5 with the warp-aggregated tally of walk_core.cuh (experiment)
-//   9, 10 as 1 and 5 with the lean crossing step (plane_step_lean: the three record loads issued as one
+//   7, 8  as 1 and 11 with the warp-aggregated tally of walk_core.cuh (experiment)
+//   9, 10 as 1 and 11 with the lean crossing step (plane_step_lean: the three record loads issued as one
 //         block, payload decoded once, ray target re-read at the end of the ray instead of held in registers)
-enum : int { kFetchPlain = 0, kFetchPolicy = 1, kFetchPolicy128 = 2, kFetchBulk = 3, kFetchPolicyL1 = 5, kFetchEdge = 6,
-             kFetchPolicyAgg = 7, kFetchPolicyL1Agg = 8, kFetchLean = 9, kFetchLeanL1 = 10 };
+enum : int { kFetchPlain = 0, kFetchPolicy = 1, kFetchPolicy128 = 2, kFetchBulk = 3, kFetchCoopL1 = 5, kFetchEdge = 6,
+             kFetchPolicyAgg = 7, kFetchPolicyL1Agg = 8, kFetchLean = 9, kFetchLeanL1 = 10, kFetchPolicyL1 = 11 };
 
 __device__ __forceinline__ uint64_t l2_policy_keep() {
   uint64_t p;
@@ -336,6 +338,31 @@ __device__ __forceinline__ void target_out(const Ray &r, double *tgt) {
   }
 }
 
+// The rest of a crossing once the record's faces are in registers: q holds the three faces other than the entry
+// face, in face order (all but the fourth on a ray's first tet, r.entry < 0), q3 the fourth face of a first tet.
+template <bool AGG, int NS, bool TM, bool MO, bool CU>
+__device__ __forceinline__ void plane_exit(const WalkParams &P, Ray &r, Counters &c, const double (&q)[3][4],
+                                           const double (&q3)[4], double *tgt, const int32_t *id, const ScoreLane *sl) {
+  ExitScan sc;
+  const int en = r.entry;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int fk = k + ((en >= 0 && k >= en) ? 1 : 0);
+    int32_t nb, bk;
+    face_payload(q[k][0], q[k][1], q[k][2], q[k][3], r.e, fk, nb, bk);
+    scan_face(sc, q[k][0], q[k][1], q[k][2], q[k][3], nb, bk, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
+  }
+  if (en < 0) {
+    int32_t nb, bk;
+    face_payload(q3[0], q3[1], q3[2], q3[3], r.e, 3, nb, bk);
+    scan_face(sc, q3[0], q3[1], q3[2], q3[3], nb, bk, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz);
+  }
+  const double texit = exit_parameter(sc);
+  const int my_i = target_in(P, r, texit, sc.nbr, tgt, id);
+  advance<false, AGG, NS, TM, MO, CU>(P, my_i, r, texit, sc.nbr, sc.back, c, true, sl);
+  target_out(r, tgt);
+}
+
 // One crossing on the plane records.  Entry-face elision: after a crossing the face the ray came
 // in through is known (r.entry) and can never be the exit, so only the other three 32-byte
 // sectors of the record are fetched; the first tet of a ray needs all four.  tgt, id: the lane's slots.
@@ -371,6 +398,77 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, Ray &r, Counters
   advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM, MO, CU>(P, my_i, r, texit, sc.nbr,
                                                                                       sc.back, c, true, sl);
   target_out(r, tgt);
+}
+
+// ---- cooperative record fetch (kFetchCoopL1) ------------------------------------------------
+// A lane's own record load touches a line no other lane of the warp asks for, so a warp-wide 128-bit load
+// costs 32 line lookups in L1TEX and up to 32 L2 requests, and each record line is asked for six times per
+// crossing.  Here the warp fetches the records of its active lanes together: lanes 8j..8j+7 copy the eight
+// 16-byte pieces of one record (cp.async, L1-allocating, evict_last in L2) into a per-warp shared-memory row,
+// so every copy instruction touches 4 lines and asks each of them once.  The pieces of the entry face are not
+// copied and the others are packed into three 32-byte slots, so each lane reads back exactly the faces
+// plane_step() would have loaded; the fourth face of a ray's first tet comes with the lane's own load.
+constexpr int kCoopRowBytes = 96;
+
+// Shared-memory address of 16-byte chunk p (0..5) of row m.  Rows are packed at 96 bytes; rows 4..7 of every
+// eight are rotated by one chunk so that eight consecutive rows read at the same chunk land in eight different
+// 16-byte bank groups (a quarter-warp phase of ld.shared.v2.f64 is then conflict-free).
+__device__ __forceinline__ uint32_t coop_chunk(uint32_t rows, int m, int p) {
+  const int pr = p + ((m >> 2) & 1);
+  return rows + (uint32_t)(kCoopRowBytes * m + 16 * (pr == 6 ? 0 : pr));
+}
+
+__device__ __forceinline__ void cp_async_16_l1(uint32_t dst, const void *src, uint64_t pol) {
+  asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol)
+               : "memory");
+}
+
+// Per-warp shared memory of the cooperative fetch: 32 rows, then 32 (element, entry face) slots, both by rank.
+constexpr int kCoopWarpBytes = 32 * kCoopRowBytes + 32 * 8;
+
+// One crossing for every active lane of the warp (act: the active mask; every lane of the warp calls it).
+// rows: shared-memory address of the warp's kCoopWarpBytes.
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+__device__ __forceinline__ void coop_plane_step(const WalkParams &P, Ray &r, Counters &c, unsigned act, uint32_t rows,
+                                                double *tgt, const int32_t *id, const ScoreLane *sl = nullptr) {
+  const int lane = threadIdx.x & 31;
+  const bool on = (act >> lane) & 1u;
+  const int n = __popc(act);
+  const int rank = __popc(act & ((1u << lane) - 1u));  // idle lanes leave no gap between the rows
+  const int en = r.entry;
+  const uint64_t pol = l2_policy_keep_now();
+  double q[3][4], q3[4] = {0.0, 0.0, 0.0, 0.0};
+  if (on) {
+    asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(rows + 32 * kCoopRowBytes + 8 * rank), "r"(r.e), "r"(en)
+                 : "memory");
+    if (en < 0) load_face<kFetchPolicyL1>(P.tets[r.e].d + 12, pol, q3[0], q3[1], q3[2], q3[3]);
+  }
+  __syncwarp();
+  const int piece = lane & 7, f = piece >> 1;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (4 * j >= n) break;
+    const int m = 4 * j + (lane >> 3);
+    if (m < n) {
+      int32_t e, sen;
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(e), "=r"(sen) : "r"(rows + 32 * kCoopRowBytes + 8 * m)
+                   : "memory");
+      const int skip = sen < 0 ? 3 : sen;  // the entry face, or on a first tet the fourth (the owner loads it)
+      if (f != skip)
+        cp_async_16_l1(coop_chunk(rows, m, 2 * (f - (f > skip ? 1 : 0)) + (piece & 1)), P.tets[e].d + 2 * piece, pol);
+    }
+  }
+  // (this also waits for gather copies of a particle stage still in flight: issued before, they rarely land later)
+  asm volatile("cp.async.wait_all;" ::: "memory");
+  __syncwarp();
+  if (!on) return;
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    asm volatile("ld.shared.v2.f64 {%0,%1}, [%4];\n\t"
+                 "ld.shared.v2.f64 {%2,%3}, [%5];"
+                 : "=d"(q[k][0]), "=d"(q[k][1]), "=d"(q[k][2]), "=d"(q[k][3])
+                 : "r"(coop_chunk(rows, rank, 2 * k)), "r"(coop_chunk(rows, rank, 2 * k + 1)));
+  plane_exit<false, NS, TM, MO, CU>(P, r, c, q, q3, tgt, id, sl);
 }
 
 // Lean crossing step.  The compiler can sink the third record load of plane_step() below the arithmetic on

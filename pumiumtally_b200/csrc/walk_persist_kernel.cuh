@@ -13,6 +13,10 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
   __shared__ ParticleStage stages[WARPS][2];
   __shared__ __align__(8) unsigned long long bars[WARPS][3];
   __shared__ __align__(128) unsigned char rows[kRows ? WARPS : 1][kRows ? 32 * kRowBytes : 16];
+  // The timed walk keeps the per-lane L1 fetch in the binned kernel: with the cooperative one it ran 19 % slower (DESIGN
+  // section 4.1, item 6).
+  constexpr bool kCoop = FETCH == kFetchCoopL1 && !TM;
+  __shared__ __align__(16) unsigned char coop_rows[kCoop ? WARPS : 1][kCoop ? kCoopWarpBytes : 16];
   constexpr bool kEdge = FETCH == kFetchEdge;
   // each lane's ray target (plane_step, edge_persist_step) and particle id (plane_step); the whole-record
   // and lean steps keep their own
@@ -242,7 +246,11 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
       mbar_wait(bar_row, row_parity);
       row_parity ^= 1u;
     }
-    if (r.stage != kStageDone) {
+    if constexpr (kCoop) {  // warp-collective: the idle lanes help fetch the active lanes' records
+      const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
+      coop_plane_step<NS, TM, MO, CU>(P, r, c, ~idle, smem_u32(&coop_rows[warp][0]), tgt, &lane_ids[threadIdx.x],
+                                      NS > 0 ? &sl : nullptr);
+    } else if (r.stage != kStageDone) {
       if constexpr (FETCH == kFetchEdge) {
         edge_persist_step(P, my_i, r, g, c, l2_policy_keep_now(), tgt);
       } else if constexpr (kRows) {
@@ -259,8 +267,9 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
         plane_step_lean<FETCH>(P, my_i, r, c, l2_policy_keep_now());
       } else {
         const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-        plane_step<FETCH, NS, TM, MO, CU>(P, r, c, FETCH != kFetchPlain ? l2_policy_keep_now() : 0, tgt,
-                                      &lane_ids[kTargetSlot ? threadIdx.x : 0], NS > 0 ? &sl : nullptr);
+        plane_step<FETCH == kFetchCoopL1 ? kFetchPolicyL1 : FETCH, NS, TM, MO, CU>(
+            P, r, c, FETCH != kFetchPlain ? l2_policy_keep_now() : 0, tgt, &lane_ids[kTargetSlot ? threadIdx.x : 0],
+            NS > 0 ? &sl : nullptr);
       }
     }
   }
