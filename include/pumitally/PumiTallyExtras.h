@@ -143,6 +143,27 @@ inline int GetRegionBatchResults(const PumiTally &tally, int32_t which, int32_t 
   return pumitally_get_region_batch_results(engine_of(tally), which, kind, out, n);
 }
 
+// Region currents (see pumitally_set_region_currents in pumitally_c.h): with regions set and face currents on, the
+// partial and net current of every ordered pair of adjacent regions (-1: no region, -2: outside the mesh).
+// GetRegionCurrentPairs: the pairs (n = pair count); GetRegionCurrentAreas: each pair's face area.
+// GetRegionCurrentResults: which 0 partial, 1 net; kind 0 value, 1 batch mean, 2 standard error, 3 relative error;
+// n = ntime * nbins * pair count, [time][bin][pair].
+inline int SetRegionCurrents(const PumiTally &tally, int32_t on) {
+  return pumitally_set_region_currents(engine_of(tally), on);
+}
+inline int64_t GetRegionCurrentPairCount(const PumiTally &tally) {
+  return pumitally_get_region_current_pair_count(engine_of(tally));
+}
+inline int GetRegionCurrentPairs(const PumiTally &tally, int32_t *from, int32_t *to, int64_t n) {
+  return pumitally_get_region_current_pairs(engine_of(tally), from, to, n);
+}
+inline int GetRegionCurrentAreas(const PumiTally &tally, double *out, int64_t n) {
+  return pumitally_get_region_current_areas(engine_of(tally), out, n);
+}
+inline int GetRegionCurrentResults(const PumiTally &tally, int32_t which, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_region_current_results(engine_of(tally), which, kind, out, n);
+}
+
 // Checkpoints (see pumitally_save_checkpoint in pumitally_c.h): SaveCheckpoint writes the tally state and the batch
 // statistics to a file atomically; LoadCheckpoint restores them into an engine set up with the same configuration;
 // MergeCheckpoint adds another run's folded batches.  No particle state is saved: after LoadCheckpoint, call

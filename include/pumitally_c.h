@@ -494,6 +494,42 @@ int pumitally_get_region_volumes(pumitally_engine *e, double *out, int64_t n);
 int pumitally_get_region_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
 int pumitally_get_region_batch_results(pumitally_engine *e, int32_t tally, int32_t kind, double *out, int64_t n);
 
+/* ---- additive: region currents (partial and net currents between adjacent regions and out through the hull) ----
+ * pumitally_set_region_currents(e, 1), while regions are set and face currents are on, also reports, per time bin and
+ * score bin, the partial current of every ordered pair of adjacent regions (the weight crossing from region A into
+ * region B) and its net current.  Region ids are the caller's; -1 (elements in no region) is a region of its own and
+ * -2 stands for outside the mesh.  The pairs come from the face-current slots (see pumitally_set_face_currents): an
+ * interior face between element e in region A and element n in region B != A adds the weight entering n through it to
+ * pair A -> B and the weight entering e to B -> A; a face with A == B belongs to no pair; a hull face of an element in
+ * A adds the weight leaving through it to A -> -2.  The pair list holds every pair with at least one face, in
+ * ascending (from, to) order as signed integers; it depends on the mesh and the region map only.  The partial current
+ * of pair p is the sum of its faces' currents, formed on the device in the order of the region sums (so the same tally
+ * gives the same bits); net[p] = partial[p] - partial[B -> A], the second term 0 when that pair does not exist (always
+ * for to == -2).  The partials of the pairs into -2 add up to pumitally_get_leakage (up to summation order).
+ * The call is refused, changing nothing, without regions, with face currents off, after pumitally_comm_init, when 4 * E
+ * exceeds INT32_MAX, or for `on` other than 0 or 1.  Like every pumitally_set_* call it resets the tally and discards
+ * the folded batches.  pumitally_set_regions(e, NULL, 0) and pumitally_set_face_currents(e, 0) switch region currents
+ * off; pumitally_set_regions with a new map keeps them on with the new map's pairs (or fails, changing nothing).
+ * pumitally_get_region_current_pair_count(e): P, 0 while region currents are off.
+ * pumitally_get_region_current_pairs(e, from, to, n == P): the pair list.
+ * pumitally_get_region_current_areas(e, out, n == P): the summed area of each pair's faces (fp64, summed in the order of
+ * the partials), to divide by for a current per area such as a wall loading.
+ * pumitally_get_region_current_results(e, which, kind, out, n): which 0 partial, 1 net; kind 0 the open tally divided
+ * by the per-source divisor, 1 the batch mean, 2 its standard error, 3 its relative error.  Layout [time][bin][pair],
+ * n == ntime * nbins * P.  Kind 0 reads the tally pumitally_get_region_results reads (collective after
+ * pumitally_reduce_tally_to_owners); kinds 1-3 are refused as pumitally_get_batch_results refuses them and are not
+ * collective.  While batch statistics are on, pumitally_end_batch forms every partial and net current of the batch next
+ * to the region sums, before the exchange, and folds them with them: the error of a partial includes the covariances
+ * of its faces, and the error of a net current the covariance of its two partials (a flight through a slab scores
+ * both).  Checkpoints carry these statistics in their region sections; a checkpoint saved with the other setting is
+ * refused. */
+int pumitally_set_region_currents(pumitally_engine *e, int32_t on);
+int32_t pumitally_get_region_currents(const pumitally_engine *e);
+int64_t pumitally_get_region_current_pair_count(const pumitally_engine *e);
+int pumitally_get_region_current_pairs(pumitally_engine *e, int32_t *from, int32_t *to, int64_t n);
+int pumitally_get_region_current_areas(pumitally_engine *e, double *out, int64_t n);
+int pumitally_get_region_current_results(pumitally_engine *e, int32_t which, int32_t kind, double *out, int64_t n);
+
 /* ---- additive: checkpoints (save the tally state to a file, restart from it, merge independent runs) ----
  * A checkpoint holds the engine's tally state: the open batch (the raw tally, the first-track weight, the collision
  * counters, the pumitally_get_stats counts and the move counters), included only when something was moved, collided

@@ -11,6 +11,7 @@
 #endif
 #include <algorithm>
 #include <cstdint>
+#include <utility>
 #include <vector>
 
 namespace ptb {
@@ -86,16 +87,8 @@ struct RegionPlan {
   std::vector<RegionLevel> levels;
 };
 
-// The plan of region_of_internal[e] in [-1, nregions) for e < E (-1: in no region).
-inline RegionPlan build_region_plan(const int32_t *region_of_internal, int64_t E, int32_t nregions) {
-  RegionPlan p;
-  std::vector<int64_t> n(size_t(nregions), 0), off(size_t(nregions) + 1, 0);
-  for (int64_t e = 0; e < E; ++e)
-    if (region_of_internal[e] >= 0) ++n[size_t(region_of_internal[e])];
-  for (size_t g = 0; g < n.size(); ++g) off[g + 1] = off[g] + n[g];
-  p.elems.resize(size_t(off.back()));
-  for (int64_t e = 0; e < E; ++e)  // ascending id within each region
-    if (region_of_internal[e] >= 0) p.elems[size_t(off[size_t(region_of_internal[e])]++)] = int32_t(e);
+// Cuts p.elems, already grouped (group g holds n[g] consecutive inputs, in group order), into the plan's levels.
+inline void cut_region_levels(std::vector<int64_t> n, RegionPlan &p) {
   for (bool done = false; !done;) {
     RegionLevel l{int64_t(p.starts.size()), 0, 0};
     done = true;
@@ -110,6 +103,19 @@ inline RegionPlan build_region_plan(const int32_t *region_of_internal, int64_t E
     p.starts.push_back(int32_t(l.inputs));
     p.levels.push_back(l);
   }
+}
+
+// The plan of region_of_internal[e] in [-1, nregions) for e < E (-1: in no region).
+inline RegionPlan build_region_plan(const int32_t *region_of_internal, int64_t E, int32_t nregions) {
+  RegionPlan p;
+  std::vector<int64_t> n(size_t(nregions), 0), off(size_t(nregions) + 1, 0);
+  for (int64_t e = 0; e < E; ++e)
+    if (region_of_internal[e] >= 0) ++n[size_t(region_of_internal[e])];
+  for (size_t g = 0; g < n.size(); ++g) off[g + 1] = off[g] + n[g];
+  p.elems.resize(size_t(off.back()));
+  for (int64_t e = 0; e < E; ++e)  // ascending id within each region
+    if (region_of_internal[e] >= 0) p.elems[size_t(off[size_t(region_of_internal[e])]++)] = int32_t(e);
+  cut_region_levels(std::move(n), p);
   return p;
 }
 
@@ -138,6 +144,89 @@ inline std::vector<double> region_sums_host(const RegionPlan &p, const double *v
     in.swap(out);
   }
   return in;
+}
+
+// ---- region currents (engine.cu, set_region_currents / get_region_current_results / end_batch) ----
+// The face-current slots (walk_core.cuh, CurrentParams) grouped by ordered pair of regions.  Slot 4 n + b holds the
+// weight entering element n through its face b; a hull slot 4 e + f holds the weight leaving e through f.  With reg()
+// the region of an element, -1 for none and kOutside for outside the mesh: the interior slot 4 n + b, across from
+// element e, belongs to pair reg(e) -> reg(n) when the two differ (and to no pair when they are equal); the hull slot
+// 4 e + f belongs to pair reg(e) -> kOutside.  The pairs with at least one slot are listed in ascending (from, to)
+// order as signed integers.  A pair's partial current is the sum of its slots in the RegionPlan order (its slots
+// ascending, in chunks of kRegionChunk, level by level), its net current that minus the partial of the reverse pair.
+constexpr int32_t kOutside = -2;
+
+struct RegionCurrentPlan {
+  RegionPlan sums;                 // elems: the slots, ascending pair, then ascending slot
+  std::vector<int64_t> first;      // [P + 1] pair p's slots are sums.elems[first[p], first[p + 1])
+  std::vector<int32_t> from, to;   // [P] the pairs
+  std::vector<int32_t> rev;        // [P] the pair to -> from, -1 when there is none (always for to == kOutside)
+  std::vector<double> area;        // [P] the pair's slot areas summed in the plan's order
+};
+
+// The area of face f (opposite local vertex f) of element e, from its three other vertices a, b, c in local order:
+// |(b - a) x (c - a)| / 2, every operation rounded separately.
+inline double face_area(const double *coords, const int32_t *t2v, int64_t e, int f) {
+  const double *v[3];
+  for (int q = 0, j = 0; q < 4; ++q)
+    if (q != f) v[j++] = coords + 3 * int64_t(t2v[4 * e + q]);
+  const double u0 = v[1][0] - v[0][0], u1 = v[1][1] - v[0][1], u2 = v[1][2] - v[0][2];
+  const double w0 = v[2][0] - v[0][0], w1 = v[2][1] - v[0][1], w2 = v[2][2] - v[0][2];
+  const double x = u1 * w2 - u2 * w1, y = u2 * w0 - u0 * w2, z = u0 * w1 - u1 * w0;
+  const double s = x * x + y * y;
+  return sqrt(s + z * z) * 0.5;
+}
+
+// The plan of region_of_internal[e] in [-1, nregions) for e < E, with t2t [4E] the neighbour across each face (-1 on
+// the hull) and slot_area [4E] the area of each slot's face.  Needs 4E <= INT32_MAX (slot ids are int32).
+inline RegionCurrentPlan build_region_current_plan(const int32_t *region_of_internal, const int32_t *t2t, int64_t E,
+                                                   const double *slot_area) {
+  RegionCurrentPlan p;
+  // (pair key, slot) of every slot in a pair; the key orders (from, to) as signed integers
+  auto key = [](int32_t a, int32_t b) { return int64_t(a) * (int64_t(1) << 32) + int64_t(uint32_t(b) ^ 0x80000000u); };
+  std::vector<std::pair<int64_t, int32_t>> ks;
+  for (int64_t e = 0; e < E; ++e)
+    for (int f = 0; f < 4; ++f) {
+      const int32_t nb = t2t[4 * e + f], a = region_of_internal[e];
+      if (nb < 0) {
+        ks.emplace_back(key(a, kOutside), int32_t(4 * e + f));
+        continue;
+      }
+      const int32_t b = region_of_internal[nb];
+      if (a == b) continue;
+      int back = 0;
+      for (int q = 0; q < 4; ++q)
+        if (t2t[4 * int64_t(nb) + q] == int32_t(e)) back = q;
+      ks.emplace_back(key(a, b), int32_t(4 * int64_t(nb) + back));  // e -> nb enters nb through its face back
+    }
+  std::sort(ks.begin(), ks.end());
+  std::vector<int64_t> n;
+  p.sums.elems.resize(ks.size());
+  for (size_t i = 0; i < ks.size(); ++i) {
+    if (i == 0 || ks[i].first != ks[i - 1].first) {
+      n.push_back(0);
+      p.from.push_back(int32_t(ks[i].first >> 32));
+      p.to.push_back(int32_t(uint32_t(ks[i].first) ^ 0x80000000u));
+    }
+    ++n.back();
+    p.sums.elems[i] = ks[i].second;
+  }
+  p.first.assign(1, 0);
+  for (int64_t m : n) p.first.push_back(p.first.back() + m);
+  cut_region_levels(std::move(n), p.sums);
+  const size_t P = p.from.size();
+  p.rev.assign(P, -1);
+  for (size_t q = 0; q < P; ++q) {
+    const int32_t a = p.to[q], b = p.from[q];  // the reverse pair, found by binary search in the sorted list
+    size_t lo = 0, hi = P;
+    while (lo < hi) {
+      const size_t m = (lo + hi) / 2;
+      if (key(p.from[m], p.to[m]) < key(a, b)) lo = m + 1; else hi = m;
+    }
+    if (lo < P && p.from[lo] == a && p.to[lo] == b) p.rev[q] = int32_t(lo);
+  }
+  p.area = region_sums_host(p.sums, slot_area);
+  return p;
 }
 
 }  // namespace ptb

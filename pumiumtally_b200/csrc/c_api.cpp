@@ -318,6 +318,28 @@ int pumitally_get_region_batch_results(pumitally_engine *e, int32_t tally, int32
   return guarded(e, [&](ptb::Engine &g) { return g.get_region_batch_results(tally, kind, out, n); });
 }
 
+int pumitally_set_region_currents(pumitally_engine *e, int32_t on) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_region_currents(on); });
+}
+int32_t pumitally_get_region_currents(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "region_currents")) : 0;
+}
+int64_t pumitally_get_region_current_pair_count(const pumitally_engine *e) {
+  return e ? pumitally_get_option(e, "region_current_pairs") : 0;
+}
+int pumitally_get_region_current_pairs(pumitally_engine *e, int32_t *from, int32_t *to, int64_t n) {
+  if (n > 0 && (!from || !to)) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_region_current_pairs(from, to, n); });
+}
+int pumitally_get_region_current_areas(pumitally_engine *e, double *out, int64_t n) {
+  if (n > 0 && !out) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_region_current_areas(out, n); });
+}
+int pumitally_get_region_current_results(pumitally_engine *e, int32_t which, int32_t kind, double *out, int64_t n) {
+  if (n > 0 && !out) return 1;
+  return guarded(e, [&](ptb::Engine &g) { return g.get_region_current_results(which, kind, out, n); });
+}
+
 int pumitally_save_checkpoint(pumitally_engine *e, const char *path) {
   if (!path) return 1;
   return guarded(e, [&](ptb::Engine &g) { return g.save_checkpoint(path); });

@@ -199,6 +199,7 @@ Engine::~Engine() {
   cudaFree(d_coll_counts_);
   free_stats();
   free_regions();
+  free_region_currents();
   free_weight_windows();
   free_source();
   cudaFree(d_src_verts_);
@@ -1213,7 +1214,9 @@ int Engine::set_face_currents(int32_t on) {
     fprintf(stderr, "[pumitally] ERROR: set_face_currents after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores_, ntime_, moments_, collision_, on != 0);
+  if (resize_flux(nbins_, nscores_, ntime_, moments_, collision_, on != 0)) return 1;
+  if (!on) free_region_currents();  // (their statistics went with the batches resize_flux discarded)
+  return 0;
 }
 
 int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents) {
@@ -1631,6 +1634,8 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "batch_statistics") return batch_stats_ ? 1 : 0;
   if (name == "batches") return batches_;  // batches folded into the statistics
   if (name == "regions") return nregions_;
+  if (name == "region_currents") return rc_on() ? 1 : 0;
+  if (name == "region_current_pairs") return region_current_pair_count();
   // collision events since the last reset: tallied, located outside the mesh, rejected (non-finite inputs)
   if (name == "collisions" || name == "collisions_outside" || name == "collisions_rejected") {
     unsigned long long c[3] = {0, 0, 0};
@@ -2308,6 +2313,7 @@ int Engine::end_batch() {
     const size_t RL = region_len();
     double *sums = d_region_stats_;
     if (region_sums(d_flux_, int64_t(collision_ ? 2 : 1) * result_arrays(), sums)) return 1;
+    if (rc_on() && region_current_sums(d_flux_ + current_base(), sums + rc_base())) return 1;
     if (sharded() && nccl_allreduce_sum_f64(nccl_comm_, sums, sums, RL, compute_)) return 1;
     PTB_CUDA_OK(launch_batch_fold(sums, sums + RL, sums + 2 * RL, int64_t(RL), d_batch_div_, nb, compute_));
   }
@@ -2635,6 +2641,7 @@ void Engine::free_regions() {
   region_scratch_ = 0;
   region_levels_.clear();
   region_volume_.clear();
+  region_of_internal_.clear();
   nregions_ = 0;
 }
 
@@ -2663,8 +2670,16 @@ int Engine::set_regions(const int32_t *region_of_element, int64_t n, int32_t nre
   std::vector<double> vol;
   int32_t *elems = nullptr, *starts = nullptr, *ident = nullptr;
   double *dvol = nullptr;
+  RegionCurrentPlan rc;  // with region currents on, the new map's pair plan
+  int32_t *rc_dev[4] = {nullptr, nullptr, nullptr, nullptr};
+  double *rc_ones = nullptr;
+  auto release_rc = [&] {
+    for (int32_t *d : rc_dev) cudaFree(d);
+    cudaFree(rc_ones);
+  };
+  std::vector<int32_t> region_of_internal;
   if (!remove) {
-    std::vector<int32_t> region_of_internal(static_cast<size_t>(E));
+    region_of_internal.resize(static_cast<size_t>(E));
     for (int64_t i = 0; i < E; ++i) region_of_internal[size_t(i)] = region_of_element[mesh_.orig_of_internal[size_t(i)]];
     plan = build_region_plan(region_of_internal.data(), E, nregions);
     vol = region_sums_host(plan, mesh_.volume.data());
@@ -2681,21 +2696,29 @@ int Engine::set_regions(const int32_t *region_of_element, int64_t n, int32_t nre
       fprintf(stderr, "[pumitally] ERROR: no device memory for the regions (%s)\n", cudaGetErrorString(err));
       return 1;
     }
+    if (rc_on() && build_region_currents(region_of_internal.data(), &rc, rc_dev, &rc_ones)) {
+      cudaFree(elems); cudaFree(starts); cudaFree(ident); cudaFree(dvol);
+      return 1;
+    }
   }
   if (batch_stats_ && alloc_stats(reported_len())) {  // discards the folded batches (element and region)
     cudaFree(elems); cudaFree(starts); cudaFree(ident); cudaFree(dvol);
+    release_rc();
     return 1;
   }
   free_regions();
+  free_region_currents();  // removed, or replaced by the new map's plan below
   region_hash_ = remove ? 0 : ckpt::hash64(region_of_element, size_t(E) * sizeof(int32_t), uint64_t(nregions));
   if (!remove) {
     nregions_ = nregions;
+    region_of_internal_ = std::move(region_of_internal);
     region_levels_ = plan.levels;
     region_volume_ = std::move(vol);
     d_region_elems_ = elems;
     d_region_starts_ = starts;
     d_region_ident_ = ident;
     d_region_volume_ = dvol;
+    if (!rc.from.empty()) install_region_currents(std::move(rc), rc_dev, rc_ones);
   }
   return reset_tally();
 }
@@ -2704,8 +2727,10 @@ int Engine::ensure_region_work() {
   const int64_t A = 2 * int64_t(result_arrays());  // (both tallies)
   RegionPlan p;
   p.levels = region_levels_;
-  const int64_t scratch = region_scratch_len(p, A, nscores_);
-  const size_t need = size_t(scratch) + size_t(A) * size_t(nregions_) * size_t(nscores_);
+  // the region sums of both tallies, or the region currents' partials and nets, whichever needs more
+  const int64_t R = result_arrays(), P = region_current_pair_count();
+  const int64_t scratch = std::max(region_scratch_len(p, A, nscores_), region_scratch_len(rc_plan_.sums, R, 1));
+  const size_t need = size_t(scratch) + std::max(size_t(A) * size_t(nregions_) * size_t(nscores_), 2 * size_t(R * P));
   if (d_region_work_ && scratch == region_scratch_ && need <= region_work_len_) return 0;
   cudaFree(d_region_work_);
   d_region_work_ = nullptr;
@@ -2807,6 +2832,156 @@ int Engine::get_region_batch_results(int32_t tally, int32_t kind, double *out, i
   cudaFree(d_out);
   if (e != cudaSuccess) {
     fprintf(stderr, "[pumitally] CUDA error %s reading the region statistics\n", cudaGetErrorString(e));
+    return 1;
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------ region currents
+
+void Engine::free_region_currents() {
+  cudaFree(d_rc_slots_);
+  cudaFree(d_rc_starts_);
+  cudaFree(d_rc_rev_);
+  cudaFree(d_rc_ident_);
+  cudaFree(d_rc_ones_);
+  d_rc_slots_ = d_rc_starts_ = d_rc_rev_ = d_rc_ident_ = nullptr;
+  d_rc_ones_ = nullptr;
+  rc_plan_ = RegionCurrentPlan();
+}
+
+int Engine::build_region_currents(const int32_t *region_of_internal, RegionCurrentPlan *plan, int32_t *dev[4],
+                                  double **ones) {
+  const int64_t E = mesh_.ntets;
+  std::vector<double> area(size_t(4 * E));
+  for (int64_t e = 0; e < E; ++e)
+    for (int f = 0; f < 4; ++f) area[size_t(4 * e + f)] = face_area(mesh_.coords.data(), mesh_.t2v.data(), e, f);
+  *plan = build_region_current_plan(region_of_internal, mesh_.t2t.data(), E, area.data());
+  const size_t P = plan->from.size();
+  std::vector<int32_t> id(P);
+  for (size_t q = 0; q < P; ++q) id[q] = int32_t(q);
+  const std::vector<double> one(P, 1.0);
+  auto up = [](auto **d, const auto &h) {
+    const size_t bytes = std::max<size_t>(h.size(), 1) * sizeof(h[0]);
+    return cudaMalloc(reinterpret_cast<void **>(d), bytes) == cudaSuccess &&
+           cudaMemcpy(*d, h.data(), h.size() * sizeof(h[0]), cudaMemcpyHostToDevice) == cudaSuccess;
+  };
+  if (!up(&dev[0], plan->sums.elems) || !up(&dev[1], plan->sums.starts) || !up(&dev[2], plan->rev) ||
+      !up(&dev[3], id) || !up(ones, one)) {
+    const cudaError_t err = cudaGetLastError();
+    for (int i = 0; i < 4; ++i) cudaFree(dev[i]);
+    cudaFree(*ones);
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the region currents (%s)\n", cudaGetErrorString(err));
+    return 1;
+  }
+  return 0;
+}
+
+void Engine::install_region_currents(RegionCurrentPlan &&plan, int32_t *dev[4], double *ones) {
+  rc_plan_ = std::move(plan);
+  d_rc_slots_ = dev[0];
+  d_rc_starts_ = dev[1];
+  d_rc_rev_ = dev[2];
+  d_rc_ident_ = dev[3];
+  d_rc_ones_ = ones;
+}
+
+int Engine::set_region_currents(int32_t on) {
+  const int64_t E = mesh_.ntets;
+  const char *why = (on != 0 && on != 1)               ? "on must be 0 or 1"
+                    : nccl_comm_                        ? "after comm_init (the batch statistics are sized by then)"
+                    : (on && nregions_ == 0)            ? "no regions are set (set_regions)"
+                    : (on && !currents_)                ? "face currents are off (set_face_currents)"
+                    : (on && 4 * E > INT32_MAX)         ? "4 * number of elements exceeds INT32_MAX"
+                                                        : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_region_currents: %s\n", why);
+    return 1;
+  }
+  if (synchronize()) return 1;
+  RegionCurrentPlan plan;
+  int32_t *dev[4] = {nullptr, nullptr, nullptr, nullptr};
+  double *ones = nullptr;
+  if (on) {
+    if (build_region_currents(region_of_internal_.data(), &plan, dev, &ones)) return 1;
+  }
+  if (batch_stats_ && alloc_stats(reported_len())) {  // discards the folded batches (element and region)
+    for (int32_t *d : dev) cudaFree(d);
+    cudaFree(ones);
+    return 1;
+  }
+  free_region_currents();
+  if (on) install_region_currents(std::move(plan), dev, ones);
+  return reset_tally();
+}
+
+int Engine::get_region_current_pairs(int32_t *from, int32_t *to, int64_t n) {
+  const int64_t P = region_current_pair_count();
+  if (!rc_on() || n != P || !from || !to) {
+    fprintf(stderr, "[pumitally] ERROR: get_region_current_pairs: %s\n",
+            rc_on() ? "n must be the pair count" : "region currents are off (set_region_currents)");
+    return 1;
+  }
+  std::memcpy(from, rc_plan_.from.data(), size_t(P) * sizeof(int32_t));
+  std::memcpy(to, rc_plan_.to.data(), size_t(P) * sizeof(int32_t));
+  return 0;
+}
+
+int Engine::get_region_current_areas(double *out, int64_t n) {
+  if (!rc_on() || n != region_current_pair_count() || !out) {
+    fprintf(stderr, "[pumitally] ERROR: get_region_current_areas: %s\n",
+            rc_on() ? "n must be the pair count" : "region currents are off (set_region_currents)");
+    return 1;
+  }
+  std::memcpy(out, rc_plan_.area.data(), size_t(n) * sizeof(double));
+  return 0;
+}
+
+int Engine::region_current_sums(const double *cur, double *out) {
+  const int64_t R = result_arrays(), P = region_current_pair_count();
+  PTB_CUDA_OK(launch_region_sums(cur, 4 * mesh_.ntets, 1, 1, R, d_rc_slots_, d_rc_starts_, rc_plan_.sums.levels.data(),
+                                 int(rc_plan_.sums.levels.size()), d_region_work_, region_scratch_, out, compute_));
+  PTB_CUDA_OK(launch_region_net(out, d_rc_rev_, P, R, out + R * P, compute_));
+  return 0;
+}
+
+int Engine::get_region_current_results(int32_t which, int32_t kind, double *out, int64_t n) {
+  const int64_t R = result_arrays(), P = region_current_pair_count();
+  const char *why = !rc_on()                            ? "region currents are off (set_region_currents)"
+                    : (which != 0 && which != 1)        ? "which must be 0 (partial) or 1 (net)"
+                    : (kind < 0 || kind > 3)            ? "kind must be 0 (value), 1 (batch mean), 2 (standard "
+                                                          "error) or 3 (relative error)"
+                    : (n != R * P || !out)              ? "n must be ntime * nbins * the pair count"
+                                                        : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: get_region_current_results: %s\n", why);
+    return 1;
+  }
+  if (kind > 0 && batch_refused(0, kind - 1)) return 1;
+  if (synchronize()) return 1;
+  if (kind == 0) {  // the open tally's currents, read where get_region_results reads the tally
+    double div = 1.0;
+    if (gather_shares() || !per_source_divisor(&div) || ensure_region_work()) return 1;
+    double *d_out = d_region_work_ + region_scratch_;
+    if (region_current_sums(flux_view() + current_base(), d_out)) return 1;
+    PTB_CUDA_OK(cudaMemcpyAsync(out, d_out + size_t(which) * size_t(R * P), size_t(n) * sizeof(double),
+                                cudaMemcpyDeviceToHost, compute_));
+    PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+    for (int64_t i = 0; i < n; ++i) out[i] /= div;
+    return 0;
+  }
+  if (ensure_region_stats()) return 1;
+  const size_t RL = region_len(), base = rc_base() + size_t(which) * size_t(R * P);
+  double *d_out = nullptr;
+  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d_out), std::max<size_t>(size_t(n), 1) * sizeof(double));
+  if (e == cudaSuccess)
+    e = launch_batch_readout(d_region_stats_ + RL + base, d_region_stats_ + 2 * RL + base, d_rc_ones_, d_rc_ident_,
+                             d_out, P, int32_t(R), 1, 1, double(batches_), kind - 1, compute_);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, size_t(n) * sizeof(double), cudaMemcpyDeviceToHost, compute_);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
+  cudaFree(d_out);
+  if (e != cudaSuccess) {
+    fprintf(stderr, "[pumitally] CUDA error %s reading the region-current statistics\n", cudaGetErrorString(e));
     return 1;
   }
   return 0;
@@ -3018,16 +3193,25 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     return refuse(std::string("the checkpoint differs from this engine in: ") + field);
   const size_t RL = batch_stats_ && nregions_ ? region_len() : 0;
   // the lengths this engine would have with face currents on or off (the fingerprint does not hold the setting)
-  auto lengths_match = [&](bool currents) {
+  auto lengths_match = [&](bool currents, size_t region_len) {
     const size_t rep = reported_len_for(currents);
     const size_t SL = !batch_stats_ ? 0 : sharded() ? (rep + size_t(nranks_) - 1) / size_t(nranks_) : rep;
-    return h.stats_len == SL && h.region_len == RL && (!h.open || h.open_len == rep) && (batch_stats_ || h.batches == 0);
+    return h.stats_len == SL && h.region_len == region_len && (!h.open || h.open_len == rep) &&
+           (batch_stats_ || h.batches == 0);
   };
-  if (!lengths_match(currents_))
-    return refuse(lengths_match(!currents_)
+  // Region currents add 2 ntime nbins P region results (P >= 1: every mesh has a hull), and need face currents.  Saved
+  // with them on, a file has face currents on and a region length above rc_base() by a multiple of 2 ntime nbins.
+  const size_t RCA = 2 * size_t(result_arrays());
+  const bool rc_differ = RL && (rc_on() ? lengths_match(true, rc_base())
+                                        : h.region_len > RL && (h.region_len - RL) % RCA == 0 &&
+                                              lengths_match(true, h.region_len));
+  if (!lengths_match(currents_, RL))
+    return refuse(lengths_match(!currents_, RL)
                       ? std::string("the face currents differ: the checkpoint was saved with them ") +
                             (currents_ ? "off" : "on") + " (set_face_currents)"
-                      : std::string("the declared lengths do not match this engine's configuration"));
+                  : rc_differ ? std::string("the region currents differ: the checkpoint was saved with them ") +
+                                    (rc_on() ? "off" : "on") + " (set_region_currents)"
+                              : std::string("the declared lengths do not match this engine's configuration"));
   const size_t SL = batch_stats_ ? stats_len() : 0;
   if (merge && h.open)
     return refuse("the checkpoint holds an open batch, which a merge would drop (save at a batch end)");

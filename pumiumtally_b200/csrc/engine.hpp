@@ -151,6 +151,18 @@ class Engine {
   int get_region_results(int32_t tally, int32_t kind, double *out, int64_t n);
   // kinds 0-2 of get_batch_results for the region sums, folded by end_batch while regions are set; not collective
   int get_region_batch_results(int32_t tally, int32_t kind, double *out, int64_t n);
+  // Region currents (batch_stats.cuh, RegionCurrentPlan): on == 1 (regions set, face currents on, 4E <= INT32_MAX) also
+  // reports the partial and net current of every ordered pair of adjacent regions (-1: no region, -2: outside the
+  // mesh), summed from the face-current slots, with batch statistics folded next to the region sums.  Resets the
+  // tally, discards the folded batches; before comm_init.  Anything else is refused and changes nothing.
+  int set_region_currents(int32_t on);
+  int32_t region_currents() const { return rc_on() ? 1 : 0; }
+  int64_t region_current_pair_count() const { return int64_t(rc_plan_.from.size()); }
+  int get_region_current_pairs(int32_t *from, int32_t *to, int64_t n);
+  int get_region_current_areas(double *out, int64_t n);
+  // which 0 partial, 1 net; kind 0 the open tally / the per-source divisor (collective as get_region_results), 1 batch
+  // mean, 2 standard error, 3 relative error (not collective).  n == ntime * nbins * P, [time][bin][pair].
+  int get_region_current_results(int32_t which, int32_t kind, double *out, int64_t n);
   // Checkpoints (checkpoint.hpp): the tally state -- the open batch, if anything was tallied since the last reset, and
   // the batch statistics (element and region) -- with a fingerprint of the configuration.  No particle state: after a
   // load the caller places the particles (CopyInitialPosition) before the next move.  Save changes nothing in the
@@ -355,6 +367,7 @@ class Engine {
   int32_t nregions_ = 0;                           // 0: no regions
   std::vector<RegionLevel> region_levels_;         // of the plan set_regions built
   std::vector<double> region_volume_;              // [nregions_], summed in the plan's order
+  std::vector<int32_t> region_of_internal_;        // [E] the map set_regions took, internal order (the pair plan's)
   int32_t *d_region_elems_ = nullptr, *d_region_starts_ = nullptr;  // the plan's elems and starts
   int32_t *d_region_ident_ = nullptr;              // [nregions_] 0, 1, ...: the readout's order map
   double *d_region_volume_ = nullptr;              // [nregions_]
@@ -362,8 +375,13 @@ class Engine {
   int64_t region_scratch_ = 0;                     // doubles of that scratch
   size_t region_work_len_ = 0;                     // doubles at d_region_work_
   double *d_region_stats_ = nullptr;               // [3 * region_len()]: the batch's sums, running mean, M2
-  // region results of every reported tally: [tally][time][bin][region][score]
-  size_t region_len() const { return (collision_ ? 2 : 1) * size_t(result_arrays()) * size_t(nregions_) * size_t(nscores_); }
+  // region results of every reported tally: [tally][time][bin][region][score], then with region currents the partials
+  // and the nets [time][bin][pair] from rc_base()
+  size_t rc_base() const { return (collision_ ? 2 : 1) * size_t(result_arrays()) * size_t(nregions_) * size_t(nscores_); }
+  size_t region_len_for(bool rcur) const {
+    return rc_base() + (rcur ? 2 * size_t(result_arrays()) * rc_plan_.from.size() : 0);
+  }
+  size_t region_len() const { return region_len_for(rc_on()); }
   void free_regions();
   int ensure_region_work();   // d_region_work_ for the current layout
   int ensure_region_stats();  // d_region_stats_ (zeroed when allocated: it is freed whenever the batches are discarded)
@@ -371,6 +389,18 @@ class Engine {
   int region_sums(const double *flux, int64_t narrays, double *out);
   bool region_refused(int32_t tally, int32_t kind, int32_t max_kind, int64_t n) const;  // with a message
   uint64_t region_hash_ = 0;                       // of the map set_regions took (caller's numbering), 0 without
+  // ---- region currents (stats_kernels.cu, launch_region_sums / launch_region_net) ----
+  RegionCurrentPlan rc_plan_;                      // empty while region currents are off
+  int32_t *d_rc_slots_ = nullptr, *d_rc_starts_ = nullptr, *d_rc_rev_ = nullptr;  // the plan's slots, starts and rev
+  int32_t *d_rc_ident_ = nullptr;                  // [P] 0, 1, ...: the readout's order map
+  double *d_rc_ones_ = nullptr;                    // [P] 1.0: the readout's volumes
+  bool rc_on() const { return !rc_plan_.from.empty(); }
+  void free_region_currents();
+  // the plan of region_of_internal on the device into *fresh (nothing changes in the engine), with a message on failure
+  int build_region_currents(const int32_t *region_of_internal, RegionCurrentPlan *plan, int32_t *dev[4], double **ones);
+  void install_region_currents(RegionCurrentPlan &&plan, int32_t *dev[4], double *ones);
+  // partials then nets of the R current arrays at cur (R * 4E doubles) into out[2 R P], on compute_
+  int region_current_sums(const double *cur, double *out);
   // ---- checkpoints (checkpoint.hpp) ----
   bool tallied_ = false;  // a move, collision or localisation since the last reset: a checkpoint holds the open batch
   bool mesh_hashed_ = false;

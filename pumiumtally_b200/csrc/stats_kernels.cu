@@ -183,6 +183,17 @@ __global__ void region_level_kernel(const double *__restrict__ src, const int32_
   out[u * nscores + k] = acc[0];
 }
 
+// Region currents (batch_stats.cuh, RegionCurrentPlan): thread per (array a, pair p) of the partials [a][P],
+// net[a * P + p] = partial[a * P + p] - partial[a * P + rev[p]] (0 for rev[p] < 0).
+__global__ void region_net_kernel(const double *__restrict__ partial, const int32_t *__restrict__ rev, int64_t P,
+                                  int64_t narrays, double *__restrict__ net) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= P * narrays) return;
+  const int64_t a = t / P, p = t - a * P;
+  const int32_t r = __ldg(rev + p);
+  net[t] = partial[t] - (r < 0 ? 0.0 : partial[a * P + r]);
+}
+
 unsigned grid_for(int64_t work, int block) {
   int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -274,6 +285,14 @@ cudaError_t launch_region_sums(const double *flux, int64_t array_len, int32_t st
     src = dst;
   }
   return cudaSuccess;
+}
+
+cudaError_t launch_region_net(const double *partial, const int32_t *rev, int64_t P, int64_t narrays, double *net,
+                              cudaStream_t stream) {
+  const int64_t n = P * narrays;
+  if (n <= 0) return cudaSuccess;
+  region_net_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(partial, rev, P, narrays, net);
+  return cudaGetLastError();
 }
 
 }  // namespace ptb

@@ -170,6 +170,10 @@ struct RegionLevel;
 cudaError_t launch_region_sums(const double *flux, int64_t array_len, int32_t stride, int32_t nscores, int64_t narrays,
                                const int32_t *elems, const int32_t *starts, const RegionLevel *levels, int nlevels,
                                double *scratch, int64_t scratch_len, double *out, cudaStream_t stream);
+// Region currents (batch_stats.cuh, RegionCurrentPlan): net[a * P + p] = partial[a * P + p] - partial[a * P + rev[p]]
+// (the second term 0 for rev[p] < 0), for the narrays arrays of P partial currents that launch_region_sums formed.
+cudaError_t launch_region_net(const double *partial, const int32_t *rev, int64_t P, int64_t narrays, double *net,
+                              cudaStream_t stream);
 // Face currents (walk_core.cuh, CurrentParams) of R arrays [r][E][4] (internal order), opp [4E] as the engine keeps it
 // (4 * neighbour + back, kNoFace on the hull).  out[(r * E + caller's id of e) * 4 + f] is, for direction 0 (outgoing) the
 // slot of the neighbour across f (interior) or of (e, f) itself (hull), for direction 1 (incoming) the slot (e, f)

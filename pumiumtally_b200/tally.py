@@ -85,6 +85,12 @@ C_API = {
     "pumitally_get_region_volumes": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pumitally_get_region_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
     "pumitally_get_region_batch_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
+    "pumitally_set_region_currents": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_get_region_currents": (C.c_int32, [C.c_void_p]),
+    "pumitally_get_region_current_pair_count": (C.c_int64, [C.c_void_p]),
+    "pumitally_get_region_current_pairs": (C.c_int, [C.c_void_p, _ip, _ip, C.c_int64]),
+    "pumitally_get_region_current_areas": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pumitally_get_region_current_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
     "pumitally_save_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
     "pumitally_load_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
     "pumitally_merge_checkpoint": (C.c_int, [C.c_void_p, C.c_char_p]),
@@ -682,6 +688,44 @@ class PumiTally:
         """kind 0 mean, 1 standard error (both / region volume), 2 relative error of the region sums over the
         batches: [ntime, nbins, nscores, nregions]."""
         return self._region_call(self._L.pumitally_get_region_batch_results, tally, kind, "get_region_batch_results")
+
+    # ---- region currents -----------------------------------------------------------
+    def set_region_currents(self, on: bool):
+        """True (regions set, face currents on) also reports the partial and net current of every ordered pair of
+        adjacent regions, -1 for elements in no region and -2 for outside the mesh; False stops it.  Resets the
+        tally and discards the folded batches."""
+        if self._L.pumitally_set_region_currents(self._h, int(on)):
+            raise ValueError("set_region_currents failed")
+
+    @property
+    def region_currents(self) -> bool:
+        return bool(self._L.pumitally_get_region_currents(self._h))
+
+    def region_current_pairs(self):
+        """(from, to): the int32 region ids of every pair, in ascending (from, to) order (empty while region currents
+        are off)."""
+        n = int(self._L.pumitally_get_region_current_pair_count(self._h))
+        a, b = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        if n and self._L.pumitally_get_region_current_pairs(self._h, a.ctypes.data_as(_ip), b.ctypes.data_as(_ip), n):
+            raise RuntimeError("get_region_current_pairs failed")
+        return a, b
+
+    def region_current_areas(self):
+        """The summed face area of every pair."""
+        out = np.empty(int(self._L.pumitally_get_region_current_pair_count(self._h)))
+        if self._L.pumitally_get_region_current_areas(self._h, out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError("get_region_current_areas failed")
+        return out
+
+    def region_current_results(self, which=0, kind=0):
+        """which 0 partial, 1 net current; kind 0 the open tally / per-source divisor, 1 batch mean, 2 standard
+        error, 3 relative error: [ntime, nbins, npairs]."""
+        P = int(self._L.pumitally_get_region_current_pair_count(self._h))
+        out = np.empty((max(self.time_bins, 1), self.score_bins, P))
+        if self._L.pumitally_get_region_current_results(self._h, int(which), int(kind), out.ctypes.data_as(_dp),
+                                                        out.size):
+            raise RuntimeError(f"get_region_current_results({which}, {kind}) failed")
+        return out
 
     # ---- checkpoints -------------------------------------------------------------
     def save_checkpoint(self, path):
