@@ -78,6 +78,15 @@ inline int GetLeakage(const PumiTally &tally, int32_t kind, double *out, int64_t
   return pumitally_get_leakage(engine_of(tally), kind, out, n);
 }
 
+// Cosine bins of the face currents (see pumitally_set_current_cosine_bins in pumitally_c.h): edges mu_0 < ... < mu_C
+// in [0, 1] split every crossing by the cosine between its flight and the face normal.  The current results gain a
+// cosine axis after the score-bin axis: GetFaceCurrentResults n = ntime * nbins * C * E * 4, GetLeakage n = ntime *
+// nbins * C, GetRegionCurrentResults n = ntime * nbins * C * P.  (nullptr, 0) removes them.
+inline int SetCurrentCosineBins(const PumiTally &tally, const double *edges, int32_t nedges) {
+  return pumitally_set_current_cosine_bins(engine_of(tally), edges, nedges);
+}
+inline int32_t GetCurrentCosineBins(const PumiTally &tally) { return pumitally_get_current_cosine_bins(engine_of(tally)); }
+
 // Point queries (see pumitally_locate_points in pumitally_c.h): the element containing each of npts points (AoS xyz),
 // -1 outside the mesh; and every normalised result at the points, [time][bin][score][point], n = npts or
 // ntime * nbins * nscores * npts (the linear reconstruction with moments, NaN outside).  out_elem may be nullptr.

@@ -423,6 +423,27 @@ int32_t pumitally_get_face_currents(const pumitally_engine *e);
 int pumitally_get_face_current_results(pumitally_engine *e, int32_t direction, int32_t kind, double *out, int64_t n);
 int pumitally_get_leakage(pumitally_engine *e, int32_t kind, double *out, int64_t n);
 
+/* ---- additive: cosine bins of the face currents ----
+ * pumitally_set_current_cosine_bins(e, edges, nedges) sets edges mu_0 < mu_1 < ... < mu_C in [0, 1], C = nedges - 1
+ * between 1 and 64, finite and strictly increasing; (NULL, 0) removes them; anything else is refused and changes
+ * nothing.  Each crossing of the face currents then also goes to the bin of its cosine mu = min(bden * (1 / |u|), 1):
+ * bden is n . u of the face the walk leaves through (n the stored unit normal, u = destination - origin of the flight)
+ * and 1 / |u| is formed once per flight.  mu lies in (0, 1], measured against the face normal that points the way the
+ * particle travels, and the same mu goes to the neighbour's incoming slot or the hull's outgoing one.  Against a face
+ * with a fixed normal (OpenMC's MuSurfaceFilter), an outgoing partial current holds the crossings at +mu and an
+ * incoming one those at -mu.  Bin k holds mu_k <= mu < mu_k+1 and mu == mu_C goes to the last bin; a crossing with mu
+ * outside [mu_0, mu_C] adds nothing to any current, leakage included.  While bins are set and face currents are on:
+ *   pumitally_get_face_current_results takes n = ntime * nbins * C * E * 4, [time][bin][cosine][element][face];
+ *   pumitally_get_leakage takes n = ntime * nbins * C, [time][bin][cosine];
+ *   pumitally_get_region_current_results takes n = ntime * nbins * C * P, [time][bin][cosine][pair];
+ * with the same kinds.  A net current per cosine bin is the difference of the two partials in that bin, and summed over
+ * the bins of edges that cover [0, 1] every result is the result without bins.  The call may come before or after
+ * pumitally_set_face_currents; nothing changes while face currents are off.  It resets the tally and discards the
+ * folded batches; refused after pumitally_comm_init.  pumitally_get_current_cosine_bins (or the option
+ * "current_cosine_bins") returns C, 0 without bins.  A checkpoint saved with other cosine bins is refused. */
+int pumitally_set_current_cosine_bins(pumitally_engine *e, const double *edges, int32_t nedges);
+int32_t pumitally_get_current_cosine_bins(const pumitally_engine *e);
+
 /* ---- additive: batch statistics (mean, standard and relative errors over batches, on the device) ----
  * A Monte Carlo tally is reported as mean +- standard error over batches.  pumitally_set_batch_statistics(e, 1) keeps,
  * for every reported result (the track-length tally and, with the estimator on, the collision tally: every time bin,

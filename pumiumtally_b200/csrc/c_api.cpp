@@ -283,6 +283,12 @@ int pumitally_get_face_current_results(pumitally_engine *e, int32_t direction, i
 int pumitally_get_leakage(pumitally_engine *e, int32_t kind, double *out, int64_t n) {
   return guarded(e, [&](ptb::Engine &g) { return g.get_leakage(kind, out, n); });
 }
+int pumitally_set_current_cosine_bins(pumitally_engine *e, const double *edges, int32_t nedges) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_current_cosine_bins(edges, nedges); });
+}
+int32_t pumitally_get_current_cosine_bins(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "current_cosine_bins")) : 0;
+}
 
 int pumitally_set_batch_statistics(pumitally_engine *e, int32_t on) {
   return guarded(e, [&](ptb::Engine &g) { return g.set_batch_statistics(on); });

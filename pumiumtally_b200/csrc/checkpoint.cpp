@@ -13,6 +13,7 @@ namespace {
 constexpr char kMagic[8] = {'P', 'T', 'B', 'C', 'K', 'P', 'T', '\0'};
 constexpr uint32_t kEndianMarker = 0x01020304u;
 constexpr uint32_t kMaxEdges = 1025;          // kMaxTimeBins + 1 (walk_core.cuh)
+constexpr uint32_t kMaxMuEdges = 65;          // kMaxCosineBins + 1 (walk_core.cuh)
 constexpr uint64_t kMaxLen = uint64_t(1) << 56;  // doubles: beyond any device memory, and no overflow below
 constexpr size_t kSectionHead = 16;           // id (u32), byte length (u64), CRC-32 (u32)
 
@@ -59,9 +60,13 @@ void put_header(std::vector<uint8_t> &b, const Header &h, const Fingerprint &f) 
   put_le(b, f.share, 8);
   put_le(b, uint32_t(f.edges.size()), 4);
   for (double e : f.edges) put_le(b, bits_of(e), 8);
+  if (!f.mu_edges.empty()) {  // version 2 only
+    put_le(b, uint32_t(f.mu_edges.size()), 4);
+    for (double e : f.mu_edges) put_le(b, bits_of(e), 8);
+  }
 }
 
-void get_header(const uint8_t *p, Header *h, Fingerprint *f) {
+void get_header(const uint8_t *p, Header *h, Fingerprint *f, bool cosines) {
   h->batches = int64_t(get_le(p, 8));
   h->open = uint32_t(get_le(p + 8, 4));
   h->open_len = get_le(p + 16, 8);
@@ -88,6 +93,13 @@ void get_header(const uint8_t *p, Header *h, Fingerprint *f) {
   p += 36;
   f->edges.resize(ne);
   for (uint32_t j = 0; j < ne; ++j) f->edges[j] = double_of(get_le(p + 8 * j, 8));
+  f->mu_edges.clear();
+  if (cosines) {
+    p += 8 * size_t(ne);
+    const uint32_t nm = uint32_t(get_le(p, 4));
+    f->mu_edges.resize(nm);
+    for (uint32_t j = 0; j < nm; ++j) f->mu_edges[j] = double_of(get_le(p + 4 + 8 * j, 8));
+  }
 }
 
 uint64_t rotl(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
@@ -135,6 +147,9 @@ const char *fingerprint_mismatch(const Fingerprint &a, const Fingerprint &b, boo
   if (a.edges.size() != b.edges.size()) return "number of time bins";
   for (size_t j = 0; j < a.edges.size(); ++j)
     if (bits_of(a.edges[j]) != bits_of(b.edges[j])) return "time-bin edges";
+  if (a.mu_edges.size() != b.mu_edges.size()) return "number of current cosine bins (set_current_cosine_bins)";
+  for (size_t j = 0; j < a.mu_edges.size(); ++j)
+    if (bits_of(a.mu_edges[j]) != bits_of(b.mu_edges[j])) return "current cosine-bin edges (set_current_cosine_bins)";
   if (a.moments != b.moments) return "moment order";
   if (a.collision != b.collision) return "collision estimator";
   if (a.batch_stats != b.batch_stats) return "batch statistics on/off";
@@ -207,7 +222,7 @@ bool Writer::put(const void *p, size_t n) {
 
 bool Writer::begin(const Header &h, const Fingerprint &f) {
   std::vector<uint8_t> b(kMagic, kMagic + 8);
-  put_le(b, kVersion, 4);
+  put_le(b, f.mu_edges.empty() ? kVersion : kVersionCosines, 4);
   put_le(b, kEndianMarker, 4);
   put_header(b, h, f);
   put_le(b, crc32(b.data(), b.size()), 4);
@@ -261,10 +276,12 @@ bool Reader::begin(Header *h, Fingerprint *f) {
     err_ = "not a checkpoint file (wrong magic)";
     return false;
   }
-  if (get_le(b.data() + 8, 4) != kVersion) {
-    err_ = "unsupported format version " + std::to_string(get_le(b.data() + 8, 4));
+  const uint64_t version = get_le(b.data() + 8, 4);
+  if (version != kVersion && version != kVersionCosines) {
+    err_ = "unsupported format version " + std::to_string(version);
     return false;
   }
+  const bool cosines = version == kVersionCosines;
   if (get_le(b.data() + 12, 4) != kEndianMarker) {
     err_ = "wrong endianness marker";
     return false;
@@ -277,11 +294,22 @@ bool Reader::begin(Header *h, Fingerprint *f) {
   const size_t fixed = b.size();
   b.resize(fixed + 8 * size_t(ne) + 4);
   if (!get(b.data() + fixed, b.size() - fixed)) return false;
+  if (cosines) {  // the last 4 bytes read are the cosine-edge count, not the CRC
+    const uint32_t nm = uint32_t(get_le(b.data() + b.size() - 4, 4));
+    if (nm < 2 || nm > kMaxMuEdges) {
+      err_ = "corrupt version 2 header (cosine-bin edge count)";
+      return false;
+    }
+    const size_t at = b.size();
+    b.resize(at + 8 * size_t(nm) + 4);
+    if (!get(b.data() + at, b.size() - at)) return false;
+  }
   if (crc32(b.data(), b.size() - 4) != uint32_t(get_le(b.data() + b.size() - 4, 4))) {
-    err_ = "corrupt header or fingerprint (CRC mismatch)";
+    err_ = cosines ? "corrupt version 2 header or fingerprint (CRC mismatch)"
+                   : "corrupt header or fingerprint (CRC mismatch)";
     return false;
   }
-  get_header(b.data() + 16, h, f);
+  get_header(b.data() + 16, h, f, cosines);
   if (h->open > 1 || (!h->open && h->open_len) || h->batches < 0 || h->open_len > kMaxLen ||
       h->stats_len > kMaxLen || h->region_len > kMaxLen) {
     err_ = "corrupt header (declared lengths)";

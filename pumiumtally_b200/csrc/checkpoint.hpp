@@ -6,7 +6,7 @@
 //   magic "PTBCKPT\0" (8 B), format version (u32), endianness marker 0x01020304 (u32),
 //   the fixed header (Header: batches, open flag, declared lengths),
 //   the fingerprint (Fingerprint: every value the layout and meaning of the arrays depend on; the time-bin edges last,
-//     preceded by their count),
+//     preceded by their count; in a version-2 file, the current cosine-bin edges after them, preceded by their count),
 //   the CRC-32 of everything before it (u32),
 //   then one section per present array, in the order of SectionId: id (u32), byte length (u64), CRC-32 of the payload
 //   (u32), payload.
@@ -23,7 +23,10 @@
 namespace ptb {
 namespace ckpt {
 
+// Version 1: no cosine bins.  A file whose fingerprint holds cosine-bin edges is written as version 2, which a build
+// that does not know them refuses instead of misreading; every other file keeps version 1's bytes.
 constexpr uint32_t kVersion = 1;
+constexpr uint32_t kVersionCosines = 2;
 
 // 64-bit hash of a byte string (not cryptographic: it tells configurations apart, it does not authenticate them).
 // Chainable: hash64(b, nb, hash64(a, na)) hashes a then b.
@@ -46,6 +49,7 @@ struct Fingerprint {
   int32_t rank = 0, nranks = 1;
   uint64_t share = 0;
   std::vector<double> edges;  // time-bin edges (empty: no time filter), compared bit for bit
+  std::vector<double> mu_edges;  // cosine-bin edges of the face currents (empty: none), compared bit for bit
 };
 
 // The name of the first field in which `file` differs from `engine`, nullptr when they agree.  ignore_norm_value:

@@ -159,6 +159,7 @@ Engine::~Engine() {
     if (u->ev) cudaEventDestroy(u->ev);
   }
   cudaFree(d_edges_);
+  cudaFree(d_mu_edges_);
   cudaFree(d_face_opp_);
   cudaFree(d_hull_slots_);
   if (ev_copy0_) cudaEventDestroy(ev_copy0_);
@@ -352,13 +353,13 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
   if (follow_last_stream(stream)) return 1;
   if (d_dest) flux_global_valid_ = flux_owned_only_ = eval_valid_ = false;  // the local tally moves on; the last exchange no longer describes it
   const int64_t slice = int64_t(nbins_) * int64_t(bin_len());  // time filter: from one time bin of an array to the next
-  // face currents: [time][bin][element][4] after the tallies; a binned move's unmatched particles cross into the scratch
-  // array after the unreported flux array
-  const int64_t E4 = 4 * int64_t(mesh_.ntets), cur_slice = int64_t(nbins_) * E4;
+  // face currents: [time][bin][cosine][element][4] after the tallies; a binned move's unmatched particles cross into the
+  // scratch array after the unreported flux array (every cosine bin into it)
+  const int64_t E4 = 4 * int64_t(mesh_.ntets), cur_bin = int64_t(ncos()) * E4, cur_slice = int64_t(nbins_) * cur_bin;
   double *cur = currents_ ? d_flux_ + current_base() : nullptr;
   if (!(t.bins && d_dest))
     return launch_range_into(d_flux_, d_origin, d_dest, d_flying, d_weights, begin, end, stream, t, slice, move_variant_,
-                             move_tag_, cur, cur_slice);
+                             move_tag_, cur, cur_slice, E4);
   // Score filter: particles are independent and a particle that does not fly is not touched, so the range
   // is walked once per bin with the flying flags masked down to that bin's particles and the tally pointed
   // at that bin's flux array -- the walk kernels themselves are the unfiltered ones.  One more pass (array
@@ -375,8 +376,8 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
     // the unreported array follows every reported one (with a time filter, all time bins of a bin-b pass go to it)
     if (launch_range_into(d_flux_ + (b < nbins_ ? size_t(b) * bin_len() : reported_len()), d_origin, d_dest, d_mask_,
                           d_weights, begin, end, stream, t, b < nbins_ ? slice : 0, variant, tag,
-                          cur ? (b < nbins_ ? cur + b * E4 : d_flux_ + reported_len() + bin_len()) : nullptr,
-                          b < nbins_ ? cur_slice : 0))
+                          cur ? (b < nbins_ ? cur + b * cur_bin : d_flux_ + reported_len() + bin_len()) : nullptr,
+                          b < nbins_ ? cur_slice : 0, b < nbins_ ? E4 : 0))
       return 1;
   }
   return 0;
@@ -385,7 +386,7 @@ int Engine::launch_range(const double *d_origin, const double *d_dest, const int
 int Engine::launch_range_into(double *d_flux, const double *d_origin, const double *d_dest, const int8_t *d_flying,
                               const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream,
                               const MoveTally &t, int64_t slice, int variant, int tag, double *d_cur,
-                              int64_t cur_slice) {
+                              int64_t cur_slice, int64_t mu_stride) {
   if (d_dest && d_weights && initial_weight_pending_)  // first tracks of the batch: their total weight
     PTB_CUDA_OK(launch_sum_flying_weights(d_flying, d_weights, begin, end, d_initial_weight_, stream));
   CurrentWalkParams tp{};
@@ -395,7 +396,7 @@ int Engine::launch_range_into(double *d_flux, const double *d_origin, const doub
   const bool scored = scored_move(t) && d_dest;
   if (scored) tp.sc = ScoreParams{t.responses, nscores_, stride_};
   if (timed_walk) tp.tm = TimeParams{d_edges_, t.times, t.speeds, ntime_, slice};
-  if (scored && currents_) tp.cu = CurrentParams{d_cur, cur_slice};
+  if (scored && currents_) tp.cu = CurrentParams{d_cur, cur_slice, d_mu_edges_, nmu_, mu_stride};
   p.tets = d_tets_;
   p.links = d_links_;
   p.verts = d_verts_;
@@ -1141,7 +1142,7 @@ int Engine::set_score_bins(int32_t nbins) {
     fprintf(stderr, "[pumitally] ERROR: set_score_bins after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins, nscores_, ntime_, moments_, collision_, currents_);
+  return resize_flux(nbins, nscores_, ntime_, moments_, collision_, currents_, nmu_);
 }
 
 // Scores (walk_core.cuh, ScoreParams): the flux array becomes [bin][element][score_stride(nscores)].
@@ -1151,7 +1152,7 @@ int Engine::set_scores(int32_t nscores) {
     fprintf(stderr, "[pumitally] ERROR: set_scores after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores, ntime_, moments_, collision_, currents_);
+  return resize_flux(nbins_, nscores, ntime_, moments_, collision_, currents_, nmu_);
 }
 
 // Time filter (walk_core.cuh, TimeParams): the flux array becomes [time][bin][element][stride], the edges live on
@@ -1162,7 +1163,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (!edges && nedges == 0) {  // no time filter
-    if (resize_flux(nbins_, nscores_, 0, moments_, collision_, currents_)) return 1;
+    if (resize_flux(nbins_, nscores_, 0, moments_, collision_, currents_, nmu_)) return 1;
     cudaFree(d_edges_);
     d_edges_ = nullptr;
     return 0;
@@ -1177,7 +1178,7 @@ int Engine::set_time_bins(const double *edges, int32_t nedges) {
     return 1;
   }
   if (cudaMemcpy(ne, edges, size_t(nedges) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
-      resize_flux(nbins_, nscores_, nedges - 1, moments_, collision_, currents_)) {
+      resize_flux(nbins_, nscores_, nedges - 1, moments_, collision_, currents_, nmu_)) {
     cudaGetLastError();
     cudaFree(ne);
     return 1;
@@ -1194,7 +1195,7 @@ int Engine::set_moments(int32_t order) {
     fprintf(stderr, "[pumitally] ERROR: set_moments after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores_, ntime_, order, collision_, currents_);
+  return resize_flux(nbins_, nscores_, ntime_, order, collision_, currents_, nmu_);
 }
 
 // Collision estimator (walk_core.cuh, collision_event): a second tally of the same layout after the track-length one.
@@ -1204,7 +1205,7 @@ int Engine::set_collision_estimator(int32_t on) {
     fprintf(stderr, "[pumitally] ERROR: set_collision_estimator after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  return resize_flux(nbins_, nscores_, ntime_, moments_, on != 0, currents_);
+  return resize_flux(nbins_, nscores_, ntime_, moments_, on != 0, currents_, nmu_);
 }
 
 // Face currents (walk_core.cuh, CurrentParams): the current slots and the leakage slots after both tallies.
@@ -1214,19 +1215,58 @@ int Engine::set_face_currents(int32_t on) {
     fprintf(stderr, "[pumitally] ERROR: set_face_currents after comm_init (the exchange buffers are sized by then)\n");
     return 1;
   }
-  if (resize_flux(nbins_, nscores_, ntime_, moments_, collision_, on != 0)) return 1;
+  if (resize_flux(nbins_, nscores_, ntime_, moments_, collision_, on != 0, nmu_)) return 1;
   if (!on) free_region_currents();  // (their statistics went with the batches resize_flux discarded)
   return 0;
 }
 
-int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents) {
+// Cosine bins (walk_core.cuh, CurrentParams, MU): the current block becomes [time][bin][cosine][element][4], with
+// [time][bin][cosine] leakage slots, and the edges live on the device.  Nothing changes unless the edges are valid and
+// the new arrays can be allocated.  Region currents keep their pair plan; their lengths follow cur_arrays().
+int Engine::set_current_cosine_bins(const double *edges, int32_t nedges) {
+  const char *why = nccl_comm_ ? "after comm_init (the exchange buffers are sized by then)"
+                    : (!edges && nedges == 0) ? nullptr
+                    : (!edges || nedges < 2 || nedges - 1 > kMaxCosineBins)
+                        ? "nedges must be 2..65 (1..64 cosine bins), or edges NULL with nedges 0"
+                        : nullptr;
+  for (int32_t j = 0; !why && edges && j < nedges; ++j)
+    if (!std::isfinite(edges[j]) || edges[j] < 0.0 || edges[j] > 1.0 || (j > 0 && !(edges[j] > edges[j - 1])))
+      why = "the edges must be finite, in [0, 1] and strictly increasing";
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_current_cosine_bins: %s\n", why);
+    return 1;
+  }
+  const int32_t nmu = edges ? nedges - 1 : 0;
+  double *ne = nullptr;
+  if (nmu > 0) {
+    PTB_CUDA_OK(cudaSetDevice(device_));
+    if (cudaMalloc(reinterpret_cast<void **>(&ne), size_t(nedges) * sizeof(double)) != cudaSuccess ||
+        cudaMemcpy(ne, edges, size_t(nedges) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaGetLastError();
+      cudaFree(ne);
+      return 1;
+    }
+  }
+  if (resize_flux(nbins_, nscores_, ntime_, moments_, collision_, currents_, nmu)) {
+    cudaFree(ne);
+    return 1;
+  }
+  cudaFree(d_mu_edges_);
+  d_mu_edges_ = ne;
+  mu_edges_.assign(edges, edges + (nmu > 0 ? nedges : 0));
+  return 0;
+}
+
+int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents,
+                        int32_t nmu) {
   if (synchronize()) return 1;
   const size_t E = size_t(mesh_.ntets), stride = size_t(score_stride(nscores)) * (moments ? kMomentSlots : 1);
-  // [time][bin][element][stride], the collision tally of the same layout, with face currents [time][bin][element][4]
-  // and [time][bin] leakage slots, then the unreported array of the particles no bin matches (and its currents)
+  // [time][bin][element][stride], the collision tally of the same layout, with face currents
+  // [time][bin][cosine][element][4] and [time][bin][cosine] leakage slots, then the unreported array of the particles no
+  // bin matches (and its currents, every cosine bin in one)
   const size_t arrays = size_t(ntime > 0 ? ntime : 1) * size_t(nbins);
   const size_t tally = arrays * (collision ? 2 : 1);
-  const size_t reported = tally * E * stride + (currents ? arrays * (4 * E + 1) : 0);
+  const size_t reported = tally * E * stride + (currents ? arrays * size_t(nmu > 0 ? nmu : 1) * (4 * E + 1) : 0);
   const size_t len = reported + (nbins > 1 ? E * stride + (currents ? 4 * E : 0) : 0) + kFluxPad;
   double *nf = nullptr;
   const cudaError_t err = cudaMalloc(reinterpret_cast<void **>(&nf), len * sizeof(double));
@@ -1250,6 +1290,7 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
   moments_ = moments;
   collision_ = collision;
   currents_ = currents;
+  nmu_ = nmu;
   if (nbins > 1 && !d_mask_) PTB_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&d_mask_), std::max<size_t>(size_t(n_), 16)));
   return reset_tally();  // a new set of arrays starts from zero
 }
@@ -1631,6 +1672,7 @@ int64_t Engine::get_option(const std::string &name) const {
   if (name == "locate_candidates") return int64_t(cand_entries_);  // entries of the point-location candidate lists
   if (name == "collision_estimator") return collision_ ? 1 : 0;
   if (name == "face_currents") return currents_ ? 1 : 0;
+  if (name == "current_cosine_bins") return nmu_;
   if (name == "batch_statistics") return batch_stats_ ? 1 : 0;
   if (name == "batches") return batches_;  // batches folded into the statistics
   if (name == "regions") return nregions_;
@@ -2515,17 +2557,17 @@ int Engine::ensure_face_maps() {
 
 int Engine::leakage_sums(const double *cur, double *out) {
   if (ensure_face_maps()) return 1;
-  PTB_CUDA_OK(launch_leakage(cur, mesh_.ntets, result_arrays(), d_hull_slots_, nhull_, out, compute_));
+  PTB_CUDA_OK(launch_leakage(cur, mesh_.ntets, cur_arrays(), d_hull_slots_, nhull_, out, compute_));
   return 0;
 }
 
 int Engine::get_face_current_results(int32_t direction, int32_t kind, double *out, int64_t n) {
-  const int64_t E = mesh_.ntets, R = result_arrays();
+  const int64_t E = mesh_.ntets, R = cur_arrays();
   const char *why = !currents_                               ? "face currents are off (set_face_currents)"
                     : (direction != 0 && direction != 1)     ? "direction must be 0 (outgoing) or 1 (incoming)"
                     : (kind < 0 || kind > 3)                 ? "kind must be 0 (value), 1 (batch mean), 2 (standard "
                                                                "error) or 3 (relative error)"
-                    : (n != R * E * 4 || !out)               ? "n must be ntime * nbins * E * 4"
+                    : (n != R * E * 4 || !out)               ? "n must be ntime * nbins * cosine bins * E * 4"
                                                              : nullptr;
   if (why) {
     fprintf(stderr, "[pumitally] ERROR: get_face_current_results: %s\n", why);
@@ -2562,11 +2604,11 @@ int Engine::get_face_current_results(int32_t direction, int32_t kind, double *ou
 // The open tally's leakage is summed from its hull slots (its leakage slots fill only at end_batch); the batch kinds
 // read the folded leakage slots.
 int Engine::get_leakage(int32_t kind, double *out, int64_t n) {
-  const int64_t R = result_arrays();
+  const int64_t R = cur_arrays();
   const char *why = !currents_                 ? "face currents are off (set_face_currents)"
                     : (kind < 0 || kind > 3)   ? "kind must be 0 (value), 1 (batch mean), 2 (standard error) or 3 "
                                                  "(relative error)"
-                    : (n != R || !out)         ? "n must be ntime * nbins"
+                    : (n != R || !out)         ? "n must be ntime * nbins * cosine bins"
                                                : nullptr;
   if (why) {
     fprintf(stderr, "[pumitally] ERROR: get_leakage: %s\n", why);
@@ -2605,24 +2647,36 @@ int Engine::get_leakage(int32_t kind, double *out, int64_t n) {
   return 0;
 }
 
+// With C > 1 cosine bins, also current_out_mu<k> and current_in_mu<k>: cosine bin k summed over time and score bins.
 int Engine::current_arrays(VtkArrays &a) {
-  const size_t E = size_t(mesh_.ntets), R = size_t(result_arrays());
+  const size_t E = size_t(mesh_.ntets), R = size_t(cur_arrays()), C = ncos();
   for (int32_t dir = 0; dir < 2; ++dir) {
     std::vector<double> all(R * E * 4);
     if (get_face_current_results(dir, 0, all.data(), int64_t(all.size()))) return 1;
-    for (size_t r = 1; r < R; ++r)
-      for (size_t i = 0; i < E * 4; ++i) all[i] += all[r * E * 4 + i];
-    all.resize(E * 4);
+    // per cosine bin k: the sum over the arrays r with r % C == k, into all[k * 4E ..]; then their sum into sum
+    for (size_t r = C; r < R; ++r)
+      for (size_t i = 0; i < E * 4; ++i) all[(r % C) * E * 4 + i] += all[r * E * 4 + i];
+    all.resize(C * E * 4);
     // component k is the face opposite vertex k of the cell as written, which swaps vertices 2 and 3 of a negatively
     // oriented tet
-    for (size_t i = 0; i < E; ++i)
-      if (vtk_cell_flipped(mesh_, mesh_.t2v.data() + 4 * i)) {
-        double *c = all.data() + 4 * size_t(mesh_.orig_of_internal[i]);
-        std::swap(c[2], c[3]);
-      }
-    a.data.push_back(std::move(all));
-    a.named.emplace_back(dir == 0 ? "current_out" : "current_in", a.data.back().data());
+    for (size_t k = 0; k < C; ++k)
+      for (size_t i = 0; i < E; ++i)
+        if (vtk_cell_flipped(mesh_, mesh_.t2v.data() + 4 * i)) {
+          double *c = all.data() + k * E * 4 + 4 * size_t(mesh_.orig_of_internal[i]);
+          std::swap(c[2], c[3]);
+        }
+    std::vector<double> sum(all.begin(), all.begin() + std::ptrdiff_t(E * 4));
+    for (size_t k = 1; k < C; ++k)
+      for (size_t i = 0; i < E * 4; ++i) sum[i] += all[k * E * 4 + i];
+    const char *name = dir == 0 ? "current_out" : "current_in";
+    a.data.push_back(std::move(sum));
+    a.named.emplace_back(name, a.data.back().data());
     a.ncomp.push_back(4);
+    for (size_t k = 0; C > 1 && k < C; ++k) {
+      a.data.emplace_back(all.begin() + std::ptrdiff_t(k * E * 4), all.begin() + std::ptrdiff_t((k + 1) * E * 4));
+      a.named.emplace_back(std::string(name) + "_mu" + std::to_string(k), a.data.back().data());
+      a.ncomp.push_back(4);
+    }
   }
   return 0;
 }
@@ -2728,7 +2782,7 @@ int Engine::ensure_region_work() {
   RegionPlan p;
   p.levels = region_levels_;
   // the region sums of both tallies, or the region currents' partials and nets, whichever needs more
-  const int64_t R = result_arrays(), P = region_current_pair_count();
+  const int64_t R = cur_arrays(), P = region_current_pair_count();
   const int64_t scratch = std::max(region_scratch_len(p, A, nscores_), region_scratch_len(rc_plan_.sums, R, 1));
   const size_t need = size_t(scratch) + std::max(size_t(A) * size_t(nregions_) * size_t(nscores_), 2 * size_t(R * P));
   if (d_region_work_ && scratch == region_scratch_ && need <= region_work_len_) return 0;
@@ -2938,7 +2992,7 @@ int Engine::get_region_current_areas(double *out, int64_t n) {
 }
 
 int Engine::region_current_sums(const double *cur, double *out) {
-  const int64_t R = result_arrays(), P = region_current_pair_count();
+  const int64_t R = cur_arrays(), P = region_current_pair_count();
   PTB_CUDA_OK(launch_region_sums(cur, 4 * mesh_.ntets, 1, 1, R, d_rc_slots_, d_rc_starts_, rc_plan_.sums.levels.data(),
                                  int(rc_plan_.sums.levels.size()), d_region_work_, region_scratch_, out, compute_));
   PTB_CUDA_OK(launch_region_net(out, d_rc_rev_, P, R, out + R * P, compute_));
@@ -2946,12 +3000,12 @@ int Engine::region_current_sums(const double *cur, double *out) {
 }
 
 int Engine::get_region_current_results(int32_t which, int32_t kind, double *out, int64_t n) {
-  const int64_t R = result_arrays(), P = region_current_pair_count();
+  const int64_t R = cur_arrays(), P = region_current_pair_count();
   const char *why = !rc_on()                            ? "region currents are off (set_region_currents)"
                     : (which != 0 && which != 1)        ? "which must be 0 (partial) or 1 (net)"
                     : (kind < 0 || kind > 3)            ? "kind must be 0 (value), 1 (batch mean), 2 (standard "
                                                           "error) or 3 (relative error)"
-                    : (n != R * P || !out)              ? "n must be ntime * nbins * the pair count"
+                    : (n != R * P || !out)              ? "n must be ntime * nbins * cosine bins * the pair count"
                                                         : nullptr;
   if (why) {
     fprintf(stderr, "[pumitally] ERROR: get_region_current_results: %s\n", why);
@@ -3054,6 +3108,7 @@ ckpt::Fingerprint Engine::fingerprint() {
     if (cudaMemcpy(f.edges.data(), d_edges_, f.edges.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess)
       f.edges.assign(f.edges.size(), std::nan(""));  // (compares unequal to every file's edges)
   }
+  if (currents_) f.mu_edges = mu_edges_;  // the cosine bins shape the arrays only with face currents on
   return f;
 }
 
@@ -3201,7 +3256,7 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
   };
   // Region currents add 2 ntime nbins P region results (P >= 1: every mesh has a hull), and need face currents.  Saved
   // with them on, a file has face currents on and a region length above rc_base() by a multiple of 2 ntime nbins.
-  const size_t RCA = 2 * size_t(result_arrays());
+  const size_t RCA = 2 * size_t(cur_arrays());
   const bool rc_differ = RL && (rc_on() ? lengths_match(true, rc_base())
                                         : h.region_len > RL && (h.region_len - RL) % RCA == 0 &&
                                               lengths_match(true, h.region_len));

@@ -123,11 +123,19 @@ class Engine {
   // batches; before comm_init.  Combines with everything else and changes none of its results.
   int set_face_currents(int32_t on);
   int32_t face_currents() const { return currents_ ? 1 : 0; }
+  // Cosine bins of the face currents (walk_core.cuh, CurrentParams, MU): edges mu_0 < ... < mu_C in [0, 1] (C = nedges
+  // - 1, 1..kMaxCosineBins) split every crossing by the cosine between its flight and the face normal; the current
+  // results gain a cosine axis after the score-bin axis (C arrays where there was one).  edges == nullptr with nedges
+  // == 0 removes them.  Resets the tally, discards the folded batches; before comm_init.  Takes effect while face
+  // currents are on.
+  int set_current_cosine_bins(const double *edges, int32_t nedges);
+  int32_t current_cosine_bins() const { return nmu_; }
   // direction 0 outgoing, 1 incoming partial current of face f (opposite the caller's local vertex f) of every element;
   // kind 0 the open tally / the per-source divisor, 1 batch mean, 2 standard error, 3 relative error (neither divided
-  // by an area or volume).  n == ntime * nbins * E * 4, [time][bin][element][face] in the caller's numbering.
+  // by an area or volume).  n == ntime * nbins * C * E * 4, [time][bin][cosine][element][face] in the caller's
+  // numbering (C = 1 without cosine bins).
   int get_face_current_results(int32_t direction, int32_t kind, double *out, int64_t n);
-  // the outgoing current summed over every hull face, kinds as above; n == ntime * nbins, [time][bin]
+  // the outgoing current summed over every hull face, kinds as above; n == ntime * nbins * C, [time][bin][cosine]
   int get_leakage(int32_t kind, double *out, int64_t n);
   // Batch statistics (batch_stats.cuh): on == 1 keeps a running mean and sum of squared deviations of every reported
   // double (both tallies), folded by end_batch from the batch's results divided by its source-normalisation divisor;
@@ -161,7 +169,7 @@ class Engine {
   int get_region_current_pairs(int32_t *from, int32_t *to, int64_t n);
   int get_region_current_areas(double *out, int64_t n);
   // which 0 partial, 1 net; kind 0 the open tally / the per-source divisor (collective as get_region_results), 1 batch
-  // mean, 2 standard error, 3 relative error (not collective).  n == ntime * nbins * P, [time][bin][pair].
+  // mean, 2 standard error, 3 relative error (not collective).  n == ntime * nbins * C * P, [time][bin][cosine][pair].
   int get_region_current_results(int32_t which, int32_t kind, double *out, int64_t n);
   // Checkpoints (checkpoint.hpp): the tally state -- the open batch, if anything was tallied since the last reset, and
   // the batch statistics (element and region) -- with a fingerprint of the configuration.  No particle state: after a
@@ -253,10 +261,12 @@ class Engine {
   int move_host(const double *origin, const double *dest, int8_t *flying, const double *weights, int32_t size,
                 const MoveTally &dev, int32_t chunk);
   // slice: doubles between time bins of d_flux; variant, tag: the kernel and its auto-tuner slot (-1: none)
-  // d_cur, cur_slice: the face currents of the score bin and the doubles between their time bins (read with currents)
+  // d_cur, cur_slice: the face currents of the score bin and the doubles between their time bins (read with currents);
+  // mu_stride: the doubles between their cosine bins (0: every cosine bin into one array)
   int launch_range_into(double *d_flux, const double *d_origin, const double *d_dest, const int8_t *d_flying,
                         const double *d_weights, int32_t begin, int32_t end, cudaStream_t stream, const MoveTally &t,
-                        int64_t slice, int variant, int tag, double *d_cur = nullptr, int64_t cur_slice = 0);
+                        int64_t slice, int variant, int tag, double *d_cur = nullptr, int64_t cur_slice = 0,
+                        int64_t mu_stride = 0);
   // scored and timed moves, and every move with moments or face currents: a tallied walk kernel, never one of the
   // auto-tuner's samples
   bool scored_move(const MoveTally &t) const { return t.kind != MoveTally::kPlain || moments_ > 0 || currents_; }
@@ -272,25 +282,30 @@ class Engine {
   int32_t moments_ = 0;               // moment order (0: none, 1: linear; walk_core.cuh, moment_tally)
   bool collision_ = false;            // the collision tally follows the track-length one in d_flux_
   bool currents_ = false;             // face currents and leakage follow both tallies in d_flux_
+  int32_t nmu_ = 0;                   // cosine bins of the face currents (0: none)
   size_t flux_alloc_ = 0;             // doubles allocated at d_flux_
   // d_flux_: the track-length tally [time][bin][element][stride_] (flux_len()), with the collision estimator the
   // collision tally of the same layout, then the unreported array of a binned move's unmatched particles and padding
   size_t nslices() const { return ntime_ > 0 ? size_t(ntime_) : 1; }
   size_t flux_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * size_t(stride_); }
-  // With face currents the reported part goes on: the current slots [time][bin][element][4] (walk_core.cuh,
-  // CurrentParams) from current_base(), then one leakage slot per [time][bin], filled by end_batch.
+  // With face currents the reported part goes on: the current slots [time][bin][cosine][element][4] (walk_core.cuh,
+  // CurrentParams) from current_base(), then one leakage slot per [time][bin][cosine], filled by end_batch.  The
+  // (time, bin) arrays of the tallies stay result_arrays(); the currents have cur_arrays() = C times as many.
   size_t current_base() const { return flux_len() * (collision_ ? 2 : 1); }
-  size_t current_len() const { return nslices() * size_t(nbins_) * size_t(mesh_.ntets) * 4; }
+  size_t ncos() const { return nmu_ > 0 ? size_t(nmu_) : 1; }
+  int32_t cur_arrays() const { return result_arrays() * int32_t(ncos()); }  // [time][bin][cosine] arrays of 4E doubles
+  size_t current_len() const { return size_t(cur_arrays()) * size_t(mesh_.ntets) * 4; }
   size_t leak_base() const { return current_base() + current_len(); }
   size_t reported_len_for(bool currents) const {
-    return current_base() + (currents ? current_len() + size_t(result_arrays()) : 0);
+    return current_base() + (currents ? current_len() + size_t(cur_arrays()) : 0);
   }
   size_t reported_len() const { return reported_len_for(currents_); }  // what the exchange moves
   size_t bin_len() const { return size_t(mesh_.ntets) * size_t(stride_); }
   int32_t result_arrays() const { return int32_t(nslices()) * nbins_; }  // (time, bin) arrays of bin_len() doubles
   // results laid out [time][bin][score][element] (and read through the score-stride kernels)
   bool multi_results() const { return nscores_ > 1 || ntime_ > 0 || moments_ > 0; }
-  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents);
+  int resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t moments, bool collision, bool currents,
+                  int32_t nmu);
   // base: doubles from d_flux_ (or the exchanged array) to the tally read, 0 (track length) or flux_len() (collision)
   // [time][bin][score][element][3]; src != nullptr: the records at src + base, gradients not divided by a source divisor
   int copy_moments(std::vector<double> &out, bool gradient, size_t base = 0, const double *src = nullptr);
@@ -376,10 +391,10 @@ class Engine {
   size_t region_work_len_ = 0;                     // doubles at d_region_work_
   double *d_region_stats_ = nullptr;               // [3 * region_len()]: the batch's sums, running mean, M2
   // region results of every reported tally: [tally][time][bin][region][score], then with region currents the partials
-  // and the nets [time][bin][pair] from rc_base()
+  // and the nets [time][bin][cosine][pair] from rc_base()
   size_t rc_base() const { return (collision_ ? 2 : 1) * size_t(result_arrays()) * size_t(nregions_) * size_t(nscores_); }
   size_t region_len_for(bool rcur) const {
-    return rc_base() + (rcur ? 2 * size_t(result_arrays()) * rc_plan_.from.size() : 0);
+    return rc_base() + (rcur ? 2 * size_t(cur_arrays()) * rc_plan_.from.size() : 0);
   }
   size_t region_len() const { return region_len_for(rc_on()); }
   void free_regions();
@@ -459,6 +474,8 @@ class Engine {
   AuxUpload resp_up_;                 // [N * nscores_] responses of a host-pointer scored or timed move
   AuxUpload bins_up_;                 // [N] bins of a host-pointer move
   double *d_edges_ = nullptr;         // [ntime_ + 1] time bin edges
+  double *d_mu_edges_ = nullptr;      // [nmu_ + 1] cosine bin edges
+  std::vector<double> mu_edges_;      // the same on the host (checkpoint fingerprint)
   uint64_t scored_moves_ = 0;         // scored_move() moves since the last reset (not the auto-tuner's samples)
   int8_t *d_mask_ = nullptr;          // [N] flying flags of one bin
   bool host_is_pinned(const void *p) const;

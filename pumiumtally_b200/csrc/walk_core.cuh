@@ -383,9 +383,25 @@ struct TimeLane : ScoreLane {
 // crossing costs one more reduction and no fetch, since the neighbour and `back` are already decoded.  With a time
 // filter the crossing goes to the bin that holds its time (time_tally's bin after the segment: a crossing exactly on
 // an edge stays in the bin below).
+//
+// Cosine bins (MU): a crossing also goes to the bin of its cosine mu = fmin(bden * inv, 1.0), one rounded product and
+// a clamp (crossing_cosine).  bden is the exit scan's n.u of the face the walk leaves through: the normal exactly as the
+// record stores it, payload byte included, and the products summed as scan_face() sums them.  inv = 1.0 / len, one
+// rounded division formed once per flight when the tally phase starts, where len = sqrt(ux * ux + uy * uy + uz * uz) is
+// the length start_tally_to() forms for the weights (nvcc may contract that sum of squares into fmas; the host build,
+// compiled without contraction, rounds each operation as written).  The face is an exit face, so mu lies in (0, 1], measured against the normal that points the way the particle travels; the same mu goes
+// to whichever slot the crossing adds to (the neighbour's incoming slot or the hull's outgoing one).  Against a face
+// with a fixed normal, an outgoing partial current holds the crossings at +mu and an incoming one those at -mu.  Bin k
+// holds edges[k] <= mu < edges[k + 1], and mu == edges[nmu] goes to the last bin (OpenMC's MuFilter rule); a crossing
+// with mu outside [edges[0], edges[nmu]] adds nothing.
+constexpr int kMaxCosineBins = 64;
+
 struct CurrentParams {
-  double *cur;    // [E][4] of time bin 0 of the score bin
-  int64_t slice;  // doubles from time bin j to j + 1 of cur (0: every time bin into one array)
+  double *cur;            // [E][4] of time bin 0 of the score bin (and cosine bin 0)
+  int64_t slice;          // doubles from time bin j to j + 1 of cur (0: every time bin into one array)
+  const double *edges;    // MU: [nmu + 1] cosine-bin edges in [0, 1], strictly increasing
+  int32_t nmu;            // MU: cosine bins, 1..kMaxCosineBins
+  int64_t mu_stride;      // MU: doubles from cosine bin k to k + 1 of cur (0: every cosine bin into one array)
 };
 
 // Parameters of a launch with face currents: the timed ones, unchanged, followed by the currents.
@@ -487,6 +503,28 @@ PTB_HD void time_start(const TimedWalkParams &T, const TimeLane *tl, double t0, 
   *tl->bin = j;
 }
 
+// Time bin of t: the number of edges <= t, minus one (-1 before T_0, nt at or after T_nt): a time on an edge belongs
+// to the bin above it, as a track that starts there does (time_start).
+PTB_HD int time_bin(const double *ed, int nt, double t) {
+  int lo = 0, hi = nt + 1;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (PTB_LDG(ed + mid) <= t) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo - 1;
+}
+
+// MU: the cosine of a crossing whose exit face has n.u == bden, for a flight with 1 / |u| == inv.
+PTB_HD double crossing_cosine(double bden, double inv) { return fmin(bden * inv, 1.0); }
+
+// MU: the cosine bin of mu, -1 outside the edges.  time_bin() over edges[0..nmu - 1] gives the bin whose lower edge is
+// the last one <= mu; mu == edges[nmu] stays in the last bin.
+PTB_HD int cosine_bin(const CurrentParams &cu, double mu) {
+  const int k = time_bin(cu.edges, cu.nmu - 1, mu);
+  return (k >= 0 && mu <= PTB_LDG(cu.edges + cu.nmu)) ? k : -1;
+}
+
 // Timed walk, one crossing: the segment [tcur, tnew] (ray parameters) of element e.  While the exit time lies
 // beyond the current bin's upper edge, the segment is cut at the edge's ray parameter and the bins are walked
 // forward (time only increases along a ray).  A flight that ends exactly on an edge stays in the bin below.
@@ -533,11 +571,13 @@ PTB_UNROLL
 // MO: moment walk (NS > 0); responses may be nullptr here too (every r[i,k] 1), for the plain and binned moves.
 // CU: face currents (NS > 0; P is a CurrentWalkParams): w goes to the lane's kCurrentSlot, 0 for a bad track; responses may
 // be nullptr as with MO.
-template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+// MU: cosine bins (CU): 1 / |u| (1.0 / len, 0 for a bad track) goes to the slot after kCurrentSlot.
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 PTB_HD void start_tally_to(const WalkParams &P, Ray &r, double x, double y, double z, double tx, double ty,
                            double tz, double w, Counters &c, bool writer, int i = 0,
                            const ScoreLane *sl = nullptr) {
   static_assert(!CU || NS > 0, "face currents run on the tallied walk");
+  static_assert(!MU || CU, "cosine bins split the face currents");
   if constexpr (NS == 0) {
     if (!all_finite(tx, ty, tz) || !all_finite(w, 0.0, 0.0)) {
       tx = x; ty = y; tz = z;
@@ -577,15 +617,16 @@ PTB_UNROLL
     if constexpr (TM)
       time_start<NS>(static_cast<const TimedWalkParams &>(P), static_cast<const TimeLane *>(sl), t0, len / v, bad);
     if constexpr (CU) sl->wl[kCurrentSlot<NS, TM> * sl->step] = bad ? 0.0 : w;
+    if constexpr (MU) sl->wl[(kCurrentSlot<NS, TM> + 1) * sl->step] = bad ? 0.0 : 1.0 / len;
   }
   r.stage = kStageTally;
   if (writer) c.tracks++;
 }
 
-template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 PTB_HD void start_tally(const WalkParams &P, int i, Ray &r, double x, double y, double z,
                         Counters &c, bool writer, const ScoreLane *sl = nullptr) {
-  start_tally_to<NS, TM, MO, CU>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
+  start_tally_to<NS, TM, MO, CU, MU>(P, r, x, y, z, PTB_LDG(P.dest + 3 * (size_t)i), PTB_LDG(P.dest + 3 * (size_t)i + 1),
                      PTB_LDG(P.dest + 3 * (size_t)i + 2), PTB_LDG(P.weights + i), c, writer, i, sl);
 }
 
@@ -616,7 +657,7 @@ PTB_HD void start_reloc(const WalkParams &P, Ray &r, double x, double y, double 
 }
 
 // K1/K2/K3 of the reference folded into the prologue: pick the walk target.
-template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool writer,
                            const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -637,14 +678,14 @@ PTB_HD void begin_particle(const WalkParams &P, int i, Ray &r, Counters &c, bool
       return;
     }
   }
-  if (P.dest) start_tally<NS, TM, MO, CU>(P, i, r, x, y, z, c, writer, sl);
+  if (P.dest) start_tally<NS, TM, MO, CU, MU>(P, i, r, x, y, z, c, writer, sl);
 }
 
 // The current ray ended (target reached, hull hit, or iteration limit).
 // kReloadTarget: the caller does not keep Ray::tx,ty,tz alive in registers (the compact-layout
 // kernel); the target is read back from the caller's array, where it came from: dest[] in the
 // tally phase, origin[] in phase 1.  Same values, six registers fewer in the crossing loop.
-template <bool kReloadTarget = false, int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <bool kReloadTarget = false, int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tnew, Counters &c,
                     bool writer, const ScoreLane *sl = nullptr) {
   // crossings of the ray that just ended: tally contributions in the tally phase, relocation crossings
@@ -674,7 +715,7 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
     x = fma(tnew, r.ux, r.ox) + P.cx; y = fma(tnew, r.uy, r.oy) + P.cy; z = fma(tnew, r.uz, r.oz) + P.cz;
   }
   if (r.stage != kStageTally && P.dest) {
-    start_tally<NS, TM, MO, CU>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
+    start_tally<NS, TM, MO, CU, MU>(P, i, r, x, y, z, c, writer, sl);  // phase 2 starts where phase 1 ended
   } else {
     if (writer) {
       store_state(P.state + i, x, y, z, r.e);
@@ -689,12 +730,21 @@ PTB_HD void end_ray(const WalkParams &P, int i, Ray &r, bool reached, double tne
 // MO: moment walk (NS > 0): each of those reductions comes with the three of its first moment (moment_tally).
 // CU: face currents (NS > 0): a crossing of the tally phase -- not the end of a flight, not a face the iteration limit
 // stopped the walk at -- adds w to the slot of the face (CurrentParams).
+// MU: cosine bins (CU): bden is the exit scan's n.u of that face, and the crossing goes to the slot of its cosine bin
+// (cosine_bin), or nowhere outside the edges.  Without MU, bden is not read.
 template <bool kReloadTarget = false, bool kAggregateTally = false, int NS = 0, bool TM = false, bool MO = false,
-          bool CU = false>
+          bool CU = false, bool MU = false>
 PTB_HD void advance(const WalkParams &P, int i, Ray &r, double texit, int32_t next, int32_t back,
-                    Counters &c, bool writer, const ScoreLane *sl = nullptr) {
+                    Counters &c, bool writer, const ScoreLane *sl = nullptr, double bden = 0.0) {
   const bool reached = !(texit < 1.0);  // last_exit == -1: destination inside this tet
   const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
+  // MU: the crossing's cosine bin (-1: none) waits in the lane's second MU slot while the flux is tallied, so that
+  // neither bden nor the bin is held in registers across it.  It is found for every step, relocation and the end of a
+  // flight included, and read only for a crossing of the tally phase (where the 1 / |u| slot is the flight's own): a
+  // guard on the tally phase here made ptxas spill 8 B more in the timed walks of variants 8 and 24.
+  if constexpr (MU)
+    sl->wl[(kCurrentSlot<NS, TM> + 2) * sl->step] = cosine_bin(static_cast<const CurrentWalkParams &>(P).cu,
+        crossing_cosine(bden, sl->wl[(kCurrentSlot<NS, TM> + 1) * sl->step]));
   if constexpr (TM) {
     if (r.stage == kStageTally && writer)
       time_tally<NS, MO>(static_cast<const TimedWalkParams &>(P), r.e, r.tcur, tnew, static_cast<const TimeLane *>(sl), &r);
@@ -727,13 +777,20 @@ PTB_UNROLL
       int j = 0;
       if constexpr (TM) j = *static_cast<const TimeLane *>(sl)->bin;
       const double w = sl->wl[kCurrentSlot<NS, TM> * sl->step];
-      if (!TM || (j >= 0 && j < Q.tm.nt))
+      if constexpr (MU) {
+        const int kmu = (int)sl->wl[(kCurrentSlot<NS, TM> + 2) * sl->step];
+        if ((!TM || (j >= 0 && j < Q.tm.nt)) && kmu >= 0)
+          PTB_TALLY_ADD(Q.cu.cur + (size_t)j * (size_t)Q.cu.slice + (size_t)kmu * (size_t)Q.cu.mu_stride +
+                            (size_t)(hull ? r.e : next) * 4 + back,
+                        w);
+      } else if (!TM || (j >= 0 && j < Q.tm.nt)) {
         PTB_TALLY_ADD(Q.cu.cur + (size_t)j * (size_t)Q.cu.slice + (size_t)(hull ? r.e : next) * 4 + back, w);
+      }
     }
   }
   if (reached || hull || over) {
     if (over && !reached && !hull && writer && r.stage != kStageSeed) c.lost++;
-    end_ray<kReloadTarget, NS, TM, MO, CU>(P, i, r, reached, tnew, c, writer, sl);
+    end_ray<kReloadTarget, NS, TM, MO, CU, MU>(P, i, r, reached, tnew, c, writer, sl);
   } else {
     r.e = next;  // UpdateCurrentElement (Impl.cpp:247-253)
     r.entry = back;
@@ -850,18 +907,6 @@ constexpr int kEventTallied = 0;
 constexpr int kEventOutside = 1;   // located outside the mesh
 constexpr int kEventRejected = 2;  // non-finite coordinate, weight * response or time
 constexpr int kEventSkipped = 3;   // bin outside [0, nbins), or time before T_0 or at or after T_nt
-
-// Time bin of t: the number of edges <= t, minus one (-1 before T_0, nt at or after T_nt): a time on an edge belongs
-// to the bin above it, as a track that starts there does (time_start).
-PTB_HD int time_bin(const double *ed, int nt, double t) {
-  int lo = 0, hi = nt + 1;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (PTB_LDG(ed + mid) <= t) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo - 1;
-}
 
 // One event in element e (internal id, -1: outside the mesh) at (x, y, z) (caller's coordinates) with weight w,
 // responses resp[0..nscores) (nullptr: every response 1), score bin `bin` and time t (read only with time bins).

@@ -34,16 +34,17 @@ namespace {
 // TM: timed walk (NS > 0); the lanes' time slots sit next to the scores.
 // MO: moment walk (NS > 0; walk_core.cuh, moment_tally).
 // CU: face currents (NS > 0; walk_core.cuh, CurrentParams); the lane's weight slot follows the others.
-template <int NS, bool TM, bool MO = false, bool CU = false>
+// MU: cosine bins (CU); the lane's 1 / |u| slot follows the weight.
+template <int NS, bool TM, bool MO = false, bool CU = false, bool MU = false>
 __device__ __forceinline__ void ldg_walk(const KernelParamsCU<NS, TM, CU> &P) {
   const int i = P.begin + blockIdx.x * blockDim.x + threadIdx.x;
-  __shared__ double score_wl[kLaneSlots<NS, TM, CU>][NS > 0 ? 256 : 1];
+  __shared__ double score_wl[kLaneSlots<NS, TM, CU, MU>][NS > 0 ? 256 : 1];
   __shared__ int32_t time_bin[TM ? 256 : 1];
   const auto sl = walk_lane<NS, 256, TM>(P, &score_wl[0][0], &time_bin[0]);
   Counters c;
   Ray r;
   r.stage = kStageDone;
-  if (i < P.end) begin_particle<NS, TM, MO, CU>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
+  if (i < P.end) begin_particle<NS, TM, MO, CU, MU>(P, i, r, c, true, NS > 0 ? &sl : nullptr);
   while (r.stage != kStageDone) {
     const double *rec = P.tets[r.e].d;
     double raw[16];
@@ -52,7 +53,8 @@ __device__ __forceinline__ void ldg_walk(const KernelParamsCU<NS, TM, CU> &P) {
       load_face_256(rec + 4 * f, raw[4 * f], raw[4 * f + 1], raw[4 * f + 2], raw[4 * f + 3]);
     ExitScan sc;
     scan_record(raw, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
-    advance<false, false, NS, TM, MO, CU>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr);
+    advance<false, false, NS, TM, MO, CU, MU>(P, i, r, exit_parameter(sc), sc.nbr, sc.back, c, true, NS > 0 ? &sl : nullptr,
+                                              sc.bden);
   }
   flush_counters(P, c);
 }
@@ -84,6 +86,20 @@ __global__ void __launch_bounds__(256, 4) walk_ldg_moments_current_kernel(const 
 }
 __global__ void __launch_bounds__(256, 4) walk_ldg_timed_moments_current_kernel(const CurrentWalkParams P) {
   ldg_walk<kMaxScores, true, true, true>(P);
+}
+
+// And with cosine bins.
+__global__ void __launch_bounds__(256, 4) walk_ldg_current_mu_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, false, false, true, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_timed_current_mu_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, true, false, true, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_moments_current_mu_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, false, true, true, true>(P);
+}
+__global__ void __launch_bounds__(256, 4) walk_ldg_timed_moments_current_mu_kernel(const CurrentWalkParams P) {
+  ldg_walk<kMaxScores, true, true, true, true>(P);
 }
 
 // ------------------------------------------------------------ small kernels
@@ -253,10 +269,10 @@ __global__ void sum_flying_weights_kernel(const int8_t *flying, const double *we
 }
 
 // The product kernels of one instantiation of the walk: NS scores (0: the plain tally), TM the time filter, MO the
-// moments, CU the face currents.  ldg is its thread-per-particle kernel, handed in because each instantiation has its
+// moments, CU the face currents, MU their cosine bins.  ldg is its thread-per-particle kernel, handed in because each instantiation has its
 // own launch bounds.  Every other variant is refused, except that the plain walk hands it to the experiments when they
 // are linked in.
-template <int NS, bool TM, bool MO, bool CU = false>
+template <int NS, bool TM, bool MO, bool CU = false, bool MU = false>
 cudaError_t launch_product(const KernelParamsCU<NS, TM, CU> &p, int variant, int block, cudaStream_t stream,
                            void (*ldg)(KernelParamsCU<NS, TM, CU>)) {
   const long long n = (long long)p.end - p.begin;
@@ -269,14 +285,14 @@ cudaError_t launch_product(const KernelParamsCU<NS, TM, CU> &p, int variant, int
       return cudaGetLastError();
     }
     case kVariantPersistRefill8:
-      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, NS, TM, MO, CU>(p, n, stream);
+      return launch_persist<128, kFetchPolicy, 7, 8, 0, -1, NS, TM, MO, CU, MU>(p, n, stream);
     case kVariantPersistGatherL1:
       // five blocks: six do not fit the cooperative fetch's rows next to the L1 (the timed walk, which keeps the per-lane
       // fetch, runs at the same occupancy as the others)
-      return launch_persist<128, kFetchCoopL1, 5, 8, 1, 40, NS, TM, MO, CU>(p, n, stream);
+      return launch_persist<128, kFetchCoopL1, 5, 8, 1, 40, NS, TM, MO, CU, MU>(p, n, stream);
     case kVariantPacked:
       if (!p.rows) return cudaErrorInvalidValue;
-      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, NS, TM, MO, CU>(p, n, stream);
+      return launch_persist<128, kFetchPolicy, 7, 8, 2, -1, NS, TM, MO, CU, MU>(p, n, stream);
     default:
 #ifdef PTB_EXPERIMENTS
       if constexpr (NS == 0) return launch_walk_experiment(p, variant, block, stream);
@@ -300,6 +316,18 @@ cudaError_t launch_walk_tallied(const CurrentWalkParams &p, bool timed, bool mom
   if (timed && (p.tm.nt < 1 || p.tm.nt > kMaxTimeBins || p.tm.slice < 0 || !p.tm.edges || !p.tm.times || !p.tm.speeds))
     return cudaErrorInvalidValue;
   if (currents && (!p.cu.cur || p.cu.slice < 0)) return cudaErrorInvalidValue;
+  if (currents && p.cu.nmu > 0) {
+    if (p.cu.nmu > kMaxCosineBins || !p.cu.edges || p.cu.mu_stride < 0) return cudaErrorInvalidValue;
+    if (timed)
+      return moments ? launch_product<kMaxScores, true, true, true, true>(p, variant, block, stream,
+                                                                          walk_ldg_timed_moments_current_mu_kernel)
+                     : launch_product<kMaxScores, true, false, true, true>(p, variant, block, stream,
+                                                                           walk_ldg_timed_current_mu_kernel);
+    return moments ? launch_product<kMaxScores, false, true, true, true>(p, variant, block, stream,
+                                                                         walk_ldg_moments_current_mu_kernel)
+                   : launch_product<kMaxScores, false, false, true, true>(p, variant, block, stream,
+                                                                          walk_ldg_current_mu_kernel);
+  }
   if (currents) {
     if (timed)
       return moments ? launch_product<kMaxScores, true, true, true>(p, variant, block, stream,

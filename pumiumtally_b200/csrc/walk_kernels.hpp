@@ -63,7 +63,8 @@ bool walk_variant_available(int variant);  // compiled into this library?
 // moments: the moment walk (walk_core.cuh, moment_tally): p.sc.stride is kMomentSlots * score_stride(nscores), and
 // p.sc.responses may be nullptr when p.sc.nscores == 1 (every response 1: the plain and binned moves).
 // currents: face currents (walk_core.cuh, CurrentParams) into p.cu.cur ([E][4] per time bin, p.cu.slice apart); p.cu is
-// read only then, and p.sc.responses may be nullptr when p.sc.nscores == 1 here too.
+// read only then, and p.sc.responses may be nullptr when p.sc.nscores == 1 here too.  p.cu.nmu > 0 (currents only):
+// cosine bins, the MU kernels; cosine bin k of the currents is at p.cu.cur + k * p.cu.mu_stride.
 cudaError_t launch_walk_tallied(const CurrentWalkParams &p, bool timed, bool moments, bool currents, int variant,
                                 int block, cudaStream_t stream);
 // blocks per SM the occupancy calculator gave the last persistent walk kernel launched (0: none yet)

@@ -136,7 +136,7 @@ __device__ __forceinline__ void stage_load(const WalkParams &P, int chunk, Parti
 }
 
 // begin_particle() reading the staged copy instead of global memory (i: the slot's particle index)
-template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const ParticleStage *st, int s,
                                                  Ray &r, Counters &c, int i = 0, const ScoreLane *sl = nullptr) {
   r.stage = kStageDone;
@@ -156,12 +156,12 @@ __device__ __forceinline__ void begin_from_stage(const WalkParams &P, const Part
     }
   }
   if (P.dest)
-    start_tally_to<NS, TM, MO, CU>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c, true, i,
-                                   sl);
+    start_tally_to<NS, TM, MO, CU, MU>(P, r, x, y, z, st->dest[3 * s], st->dest[3 * s + 1], st->dest[3 * s + 2], st->w[s], c,
+                                       true, i, sl);
 }
 
 // begin_particle() for a packed row (only flying particles have rows).  Returns the particle id.
-template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedRow *row, Ray &r, Counters &c,
                                               const ScoreLane *sl = nullptr) {
   const int id = row->id;
@@ -178,7 +178,7 @@ __device__ __forceinline__ int begin_from_row(const WalkParams &P, const PackedR
     return id;
   }
   r.e = (int32_t)(el & kIdMask);
-  start_tally_to<NS, TM, MO, CU>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
+  start_tally_to<NS, TM, MO, CU, MU>(P, r, ox, oy, oz, row->dx, row->dy, row->dz, row->w, c, true, id, sl);
   return id;
 }
 
@@ -340,7 +340,7 @@ __device__ __forceinline__ void target_out(const Ray &r, double *tgt) {
 
 // The rest of a crossing once the record's faces are in registers: q holds the three faces other than the entry
 // face, in face order (all but the fourth on a ray's first tet, r.entry < 0), q3 the fourth face of a first tet.
-template <bool AGG, int NS, bool TM, bool MO, bool CU>
+template <bool AGG, int NS, bool TM, bool MO, bool CU, bool MU = false>
 __device__ __forceinline__ void plane_exit(const WalkParams &P, Ray &r, Counters &c, const double (&q)[3][4],
                                            const double (&q3)[4], double *tgt, const int32_t *id, const ScoreLane *sl) {
   ExitScan sc;
@@ -359,14 +359,14 @@ __device__ __forceinline__ void plane_exit(const WalkParams &P, Ray &r, Counters
   }
   const double texit = exit_parameter(sc);
   const int my_i = target_in(P, r, texit, sc.nbr, tgt, id);
-  advance<false, AGG, NS, TM, MO, CU>(P, my_i, r, texit, sc.nbr, sc.back, c, true, sl);
+  advance<false, AGG, NS, TM, MO, CU, MU>(P, my_i, r, texit, sc.nbr, sc.back, c, true, sl, sc.bden);
   target_out(r, tgt);
 }
 
 // One crossing on the plane records.  Entry-face elision: after a crossing the face the ray came
 // in through is known (r.entry) and can never be the exit, so only the other three 32-byte
 // sectors of the record are fetched; the first tet of a ray needs all four.  tgt, id: the lane's slots.
-template <int FETCH, int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <int FETCH, int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 __device__ __forceinline__ void plane_step(const WalkParams &P, Ray &r, Counters &c, uint64_t pol, double *tgt,
                                            const int32_t *id, const ScoreLane *sl = nullptr) {
   ExitScan sc;
@@ -395,8 +395,8 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, Ray &r, Counters
   }
   const double texit = exit_parameter(sc);
   const int my_i = target_in(P, r, texit, sc.nbr, tgt, id);
-  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM, MO, CU>(P, my_i, r, texit, sc.nbr,
-                                                                                      sc.back, c, true, sl);
+  advance<false, FETCH == kFetchPolicyAgg || FETCH == kFetchPolicyL1Agg, NS, TM, MO, CU, MU>(P, my_i, r, texit, sc.nbr,
+                                                                                          sc.back, c, true, sl, sc.bden);
   target_out(r, tgt);
 }
 
@@ -428,7 +428,7 @@ constexpr int kCoopWarpBytes = 32 * kCoopRowBytes + 32 * 8;
 
 // One crossing for every active lane of the warp (act: the active mask; every lane of the warp calls it).
 // rows: shared-memory address of the warp's kCoopWarpBytes.
-template <int NS = 0, bool TM = false, bool MO = false, bool CU = false>
+template <int NS = 0, bool TM = false, bool MO = false, bool CU = false, bool MU = false>
 __device__ __forceinline__ void coop_plane_step(const WalkParams &P, Ray &r, Counters &c, unsigned act, uint32_t rows,
                                                 double *tgt, const int32_t *id, const ScoreLane *sl = nullptr) {
   const int lane = threadIdx.x & 31;
@@ -468,7 +468,7 @@ __device__ __forceinline__ void coop_plane_step(const WalkParams &P, Ray &r, Cou
                  "ld.shared.v2.f64 {%2,%3}, [%5];"
                  : "=d"(q[k][0]), "=d"(q[k][1]), "=d"(q[k][2]), "=d"(q[k][3])
                  : "r"(coop_chunk(rows, rank, 2 * k)), "r"(coop_chunk(rows, rank, 2 * k + 1)));
-  plane_exit<false, NS, TM, MO, CU>(P, r, c, q, q3, tgt, id, sl);
+  plane_exit<false, NS, TM, MO, CU, MU>(P, r, c, q, q3, tgt, id, sl);
 }
 
 // Lean crossing step.  The compiler can sink the third record load of plane_step() below the arithmetic on
@@ -694,9 +694,10 @@ using KernelParams = std::conditional_t<TM, TimedWalkParams, std::conditional_t<
 template <int NS, bool TM, bool CU>
 using KernelParamsCU = std::conditional_t<CU, CurrentWalkParams, KernelParams<NS, TM>>;
 
-// Shared-memory rows of score_wl: the scores, for the timed walk its three time slots, with currents the weight.
-template <int NS, bool TM, bool CU = false>
-constexpr int kLaneSlots = NS > 0 ? NS + (TM ? 3 : 0) + (CU ? 1 : 0) : 1;
+// Shared-memory rows of score_wl: the scores, for the timed walk its three time slots, with currents the weight, with
+// cosine bins 1 / |u| and the cosine of the crossing in flight (MU: 2 KB more per block of 128 lanes).
+template <int NS, bool TM, bool CU = false, bool MU = false>
+constexpr int kLaneSlots = NS > 0 ? NS + (TM ? 3 : 0) + (CU ? 1 : 0) + (MU ? 2 : 0) : 1;
 
 // The lane's ScoreLane, built where it is used from the parameters and the thread index, so that nothing of
 // it stays live in registers across the crossing loop.  wl0: slot 0 of lane 0; STEP lanes per score.
@@ -727,17 +728,30 @@ __device__ __forceinline__ std::conditional_t<TM, TimeLane, ScoreLane> walk_lane
 #define PTB_PERSIST_NAME walk_persist_kernel
 #define PTB_PERSIST_PARAMS KernelParams<NS, TM>
 #define PTB_PERSIST_CU false
-#include "walk_persist_kernel.cuh"  // (no include guard: it is meant to be included twice)
+#define PTB_PERSIST_MU false
+#include "walk_persist_kernel.cuh"  // (no include guard: it is meant to be included three times)
 #undef PTB_PERSIST_NAME
 #undef PTB_PERSIST_PARAMS
 #undef PTB_PERSIST_CU
+#undef PTB_PERSIST_MU
 #define PTB_PERSIST_NAME walk_persist_current_kernel
 #define PTB_PERSIST_PARAMS CurrentWalkParams
 #define PTB_PERSIST_CU true
-#include "walk_persist_kernel.cuh"  // (no include guard: it is meant to be included twice)
+#define PTB_PERSIST_MU false
+#include "walk_persist_kernel.cuh"
 #undef PTB_PERSIST_NAME
 #undef PTB_PERSIST_PARAMS
 #undef PTB_PERSIST_CU
+#undef PTB_PERSIST_MU
+#define PTB_PERSIST_NAME walk_persist_current_mu_kernel
+#define PTB_PERSIST_PARAMS CurrentWalkParams
+#define PTB_PERSIST_CU true
+#define PTB_PERSIST_MU true
+#include "walk_persist_kernel.cuh"
+#undef PTB_PERSIST_NAME
+#undef PTB_PERSIST_PARAMS
+#undef PTB_PERSIST_CU
+#undef PTB_PERSIST_MU
 
 // Blocks per SM of the last persistent launch (diagnostics: engine option "walk_blocks_per_sm").
 inline int &last_persist_occupancy() {
@@ -746,10 +760,11 @@ inline int &last_persist_occupancy() {
 }
 
 template <int BLOCK, int FETCH, int MINB, int REFILL_T = 1, int GATHER = 0, int CARVE = -1, int NS = 0, bool TM = false,
-          bool MO = false, bool CU = false>
+          bool MO = false, bool CU = false, bool MU = false>
 cudaError_t launch_persist(const KernelParamsCU<NS, TM, CU> &p, long long n, cudaStream_t stream) {
   constexpr auto kernel = [] {
-    if constexpr (CU) return walk_persist_current_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>;
+    if constexpr (MU) return walk_persist_current_mu_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>;
+    else if constexpr (CU) return walk_persist_current_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>;
     else return walk_persist_kernel<BLOCK, FETCH, MINB, REFILL_T, GATHER, NS, TM, MO>;
   }();
   static int sms = 0, occ = 0;

@@ -1,10 +1,12 @@
-// The persistent walk kernel, included twice by walk_persist.cuh: as walk_persist_kernel (PTB_PERSIST_CU false, the
-// parameters KernelParams<NS, TM>) and as walk_persist_current_kernel (true, CurrentWalkParams: the walks with face
-// currents).  The face-current kernels get a name of their own so that their instantiations stay apart from the
-// others, and the text is shared, not wrapped, so that the others compile to exactly the code they had before.
+// The persistent walk kernel, included three times by walk_persist.cuh: as walk_persist_kernel (PTB_PERSIST_CU false, the
+// parameters KernelParams<NS, TM>), as walk_persist_current_kernel (true, CurrentWalkParams: the walks with face
+// currents) and as walk_persist_current_mu_kernel (PTB_PERSIST_MU true as well: face currents with cosine bins).  The
+// face-current kernels get names of their own so that their instantiations stay apart from the others, and the text
+// is shared, not wrapped, so that the others compile to exactly the code they had before.
 template <int BLOCK, int FETCH, int MINB, int REFILL_T, int STAGING, int NS = 0, bool TM = false, bool MO = false>
 __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIST_PARAMS P) {
   constexpr bool CU = PTB_PERSIST_CU;
+  constexpr bool MU = PTB_PERSIST_MU;
   constexpr bool GATHER = STAGING == 1;
   constexpr bool PACKED = STAGING == 2;
   constexpr int WARPS = BLOCK / 32;
@@ -29,7 +31,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
   static_assert(NS == 0 || (!kEdge && !kRows), "scored walks run on the plane records");
   static_assert(!TM || NS > 0, "the timed walk is a scored walk");
   static_assert(!CU || NS > 0, "face currents run on the tallied walk");
-  __shared__ double score_wl[kLaneSlots<NS, TM, CU>][NS > 0 ? BLOCK : 1];  // scored walk: ScoreLane::wl of each lane
+  __shared__ double score_wl[kLaneSlots<NS, TM, CU, MU>][NS > 0 ? BLOCK : 1];  // scored walk: ScoreLane::wl of each lane
   __shared__ int32_t time_bin[TM ? BLOCK : 1];                          // timed walk: TimeLane::bin of each lane
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t bar0 = smem_u32(&bars[warp][0]);
@@ -186,12 +188,12 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
         if (r.stage == kStageDone && slot < s.cur_count) {
           if constexpr (PACKED) {
             const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-            my_i = begin_from_row<NS, TM, MO, CU>(P, reinterpret_cast<const PackedRow *>(&stages[warp][s.cur]) + slot, r,
-                                              c, NS > 0 ? &sl : nullptr);
+            my_i = begin_from_row<NS, TM, MO, CU, MU>(P, reinterpret_cast<const PackedRow *>(&stages[warp][s.cur]) + slot,
+                                                      r, c, NS > 0 ? &sl : nullptr);
           } else {
             my_i = GATHER ? stages[warp][s.cur].id[slot] : P.begin + s.chunk_cur * kChunk + slot;
             const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-            begin_from_stage<NS, TM, MO, CU>(P, &stages[warp][s.cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
+            begin_from_stage<NS, TM, MO, CU, MU>(P, &stages[warp][s.cur], slot, r, c, my_i, NS > 0 ? &sl : nullptr);
           }
           if constexpr (FETCH == kFetchEdge) g.dv = 0;
           if constexpr (kTargetSlot) {
@@ -248,8 +250,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
     }
     if constexpr (kCoop) {  // warp-collective: the idle lanes help fetch the active lanes' records
       const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-      coop_plane_step<NS, TM, MO, CU>(P, r, c, ~idle, smem_u32(&coop_rows[warp][0]), tgt, &lane_ids[threadIdx.x],
-                                      NS > 0 ? &sl : nullptr);
+      coop_plane_step<NS, TM, MO, CU, MU>(P, r, c, ~idle, smem_u32(&coop_rows[warp][0]), tgt, &lane_ids[threadIdx.x],
+                                          NS > 0 ? &sl : nullptr);
     } else if (r.stage != kStageDone) {
       if constexpr (FETCH == kFetchEdge) {
         edge_persist_step(P, my_i, r, g, c, l2_policy_keep_now(), tgt);
@@ -267,7 +269,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
         plane_step_lean<FETCH>(P, my_i, r, c, l2_policy_keep_now());
       } else {
         const auto sl = walk_lane<NS, BLOCK, TM>(P, &score_wl[0][0], &time_bin[0]);
-        plane_step<FETCH == kFetchCoopL1 ? kFetchPolicyL1 : FETCH, NS, TM, MO, CU>(
+        plane_step<FETCH == kFetchCoopL1 ? kFetchPolicyL1 : FETCH, NS, TM, MO, CU, MU>(
             P, r, c, FETCH != kFetchPlain ? l2_policy_keep_now() : 0, tgt, &lane_ids[kTargetSlot ? threadIdx.x : 0],
             NS > 0 ? &sl : nullptr);
       }

@@ -69,6 +69,8 @@ C_API = {
     "pumitally_get_face_currents": (C.c_int32, [C.c_void_p]),
     "pumitally_get_face_current_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
     "pumitally_get_leakage": (C.c_int, [C.c_void_p, C.c_int32, _dp, C.c_int64]),
+    "pumitally_set_current_cosine_bins": (C.c_int, [C.c_void_p, _dp, C.c_int32]),
+    "pumitally_get_current_cosine_bins": (C.c_int32, [C.c_void_p]),
     "pumitally_tally_collisions": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, _dp, _ip, _dp]),
     "pumitally_tally_collisions_device": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -493,19 +495,41 @@ class PumiTally:
     def face_currents(self) -> bool:
         return bool(self._L.pumitally_get_face_currents(self._h))
 
+    def set_current_cosine_bins(self, edges):
+        """Cosine bins of the face currents: edges mu_0 < ... < mu_C in [0, 1] (2..65 of them; resets the tally and
+        discards the folded batches).  Every crossing also goes to the bin of the cosine between its flight and the
+        face normal that points the way it travels; face_current_results, leakage and region_current_results gain an
+        axis of C cosine bins after the score-bin axis.  ``None`` removes them."""
+        if edges is None:
+            rc = self._L.pumitally_set_current_cosine_bins(self._h, None, 0)
+        else:
+            e = np.ascontiguousarray(edges, dtype=np.float64).reshape(-1)
+            rc = self._L.pumitally_set_current_cosine_bins(self._h, e.ctypes.data_as(_dp), int(e.size))
+        if rc:
+            raise ValueError("set_current_cosine_bins failed")
+
+    @property
+    def current_cosine_bins(self) -> int:
+        """Number of cosine bins of the face currents, 0 without them."""
+        return int(self._L.pumitally_get_current_cosine_bins(self._h))
+
+    def _cosine_axis(self):
+        C = self.current_cosine_bins
+        return (C,) if C > 0 else ()
+
     def face_current_results(self, direction=0, kind=0):
-        """Partial currents [ntime, nbins, num_elements, 4] in the caller's numbering, face f opposite local vertex f:
-        direction 0 outgoing, 1 incoming; kind 0 the open tally / the per-source divisor, 1 batch mean, 2 standard
-        error, 3 relative error."""
-        out = np.empty((max(self.time_bins, 1), self.score_bins, self.num_elements, 4))
+        """Partial currents [ntime, nbins, (C,) num_elements, 4] in the caller's numbering, face f opposite local
+        vertex f (the cosine axis only while cosine bins are set): direction 0 outgoing, 1 incoming; kind 0 the open
+        tally / the per-source divisor, 1 batch mean, 2 standard error, 3 relative error."""
+        out = np.empty((max(self.time_bins, 1), self.score_bins) + self._cosine_axis() + (self.num_elements, 4))
         if self._L.pumitally_get_face_current_results(self._h, int(direction), int(kind), out.ctypes.data_as(_dp),
                                                       out.size):
             raise RuntimeError("get_face_current_results failed")
         return out
 
     def leakage(self, kind=0):
-        """The outgoing current summed over the hull faces, [ntime, nbins]; kinds as face_current_results."""
-        out = np.empty((max(self.time_bins, 1), self.score_bins))
+        """The outgoing current summed over the hull faces, [ntime, nbins, (C)]; kinds as face_current_results."""
+        out = np.empty((max(self.time_bins, 1), self.score_bins) + self._cosine_axis())
         if self._L.pumitally_get_leakage(self._h, int(kind), out.ctypes.data_as(_dp), out.size):
             raise RuntimeError("get_leakage failed")
         return out
@@ -719,9 +743,9 @@ class PumiTally:
 
     def region_current_results(self, which=0, kind=0):
         """which 0 partial, 1 net current; kind 0 the open tally / per-source divisor, 1 batch mean, 2 standard
-        error, 3 relative error: [ntime, nbins, npairs]."""
+        error, 3 relative error: [ntime, nbins, (C,) npairs] (the cosine axis only while cosine bins are set)."""
         P = int(self._L.pumitally_get_region_current_pair_count(self._h))
-        out = np.empty((max(self.time_bins, 1), self.score_bins, P))
+        out = np.empty((max(self.time_bins, 1), self.score_bins) + self._cosine_axis() + (P,))
         if self._L.pumitally_get_region_current_results(self._h, int(which), int(kind), out.ctypes.data_as(_dp),
                                                         out.size):
             raise RuntimeError(f"get_region_current_results({which}, {kind}) failed")
