@@ -117,6 +117,33 @@ inline int TallyCollisionsAtParticles(const PumiTally &tally, const int8_t *coll
   return pumitally_tally_collisions_at_particles(engine_of(tally), collided, weights, responses, bins, times, size);
 }
 
+// Point detectors (see pumitally_set_point_detectors in pumitally_c.h): next-event estimates of the flux at fixed
+// points.  SetDetectorCrossSections takes Sigma_t [bin][element] (n = nbins * E).  TallyDetectors scores events at
+// arbitrary points (located as LocatePoints does), TallyDetectorsAtParticles at the particles' positions after the last
+// move, for every i with flagged[i] != 0 (size = num_particles).  pdf [event][detector] may be nullptr (isotropic).
+// GetDetectorResults: kind 0 the open tally per source, 1 batch mean, 2 standard error, 3 relative error.
+inline int SetPointDetectors(const PumiTally &tally, const double *xyz, int32_t ndet, const double *r0) {
+  return pumitally_set_point_detectors(engine_of(tally), xyz, ndet, r0);
+}
+inline int SetDetectorCrossSections(const PumiTally &tally, const double *sigma_t, int64_t n) {
+  return pumitally_set_detector_cross_sections(engine_of(tally), sigma_t, n);
+}
+inline int TallyDetectors(const PumiTally &tally, const double *xyz, int64_t nevents, const double *weights,
+                          const double *pdf = nullptr, const double *responses = nullptr, const int32_t *bins = nullptr,
+                          const double *times = nullptr, const double *speeds = nullptr) {
+  return pumitally_tally_detectors(engine_of(tally), xyz, nevents, weights, pdf, responses, bins, times, speeds);
+}
+inline int TallyDetectorsAtParticles(const PumiTally &tally, const int8_t *flagged, const double *weights, int32_t size,
+                                     const double *pdf = nullptr, const double *responses = nullptr,
+                                     const int32_t *bins = nullptr, const double *times = nullptr,
+                                     const double *speeds = nullptr) {
+  return pumitally_tally_detectors_at_particles(engine_of(tally), flagged, weights, pdf, responses, bins, times, speeds,
+                                                size);
+}
+inline int GetDetectorResults(const PumiTally &tally, int32_t kind, double *out, int64_t n) {
+  return pumitally_get_detector_results(engine_of(tally), kind, out, n);
+}
+
 // Batch statistics (see pumitally_set_batch_statistics in pumitally_c.h): EndBatch folds the batch's per-source results
 // into a running mean and variance on the device and starts the next batch.  GetBatchResults: tally 0 track length, 1
 // collision; kind 0 mean, 1 standard error, 2 relative error, 3 gradient of the mean (n as pumitally_get_normalized_flux

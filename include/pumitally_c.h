@@ -399,6 +399,73 @@ int pumitally_tally_collisions_at_particles_device(pumitally_engine *e, const in
                                                    void *stream);
 int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *out, int64_t n);
 
+/* ---- additive: point detectors (next-event flux estimates at fixed points; MCNP's F5 tally) ----
+ * pumitally_set_point_detectors(e, xyz, ndet, r0) sets D = ndet detectors, 1 <= D <= 256, at the AoS positions
+ * xyz[3D], each located at set time as pumitally_locate_points locates it, with exclusion radii r0[D] (finite, >= 0;
+ * required).  (NULL, 0, NULL) removes them.  Refused, changing nothing: a position outside the mesh or non-finite, a bad
+ * r0, D out of range.  The call resets the tally, discards the folded batches, combines with the other pumitally_set_*
+ * calls in any order and is refused after pumitally_comm_init.  pumitally_get_point_detectors and the read-only option
+ * "point_detectors" return D.
+ * pumitally_set_detector_cross_sections(e, sigma_t, n): the total cross sections Sigma_t[bin][element] in the caller's
+ * numbering, n == nbins * num_elements, finite and >= 0 (or nothing changes); the score bin is the energy group.  The
+ * call resets nothing and may come at any time; a later pumitally_set_score_bins that changes nbins drops the table.
+ * Detector calls are refused while there is no table.
+ * Scoring: event i (position x, element, weight w, responses r[k], score bin b, with time bins a time t and a speed v)
+ * and detector d at x_d form one ray.  R = |x_d - x|; p = pdf[i * D + d], the angular density toward the detector per
+ * steradian (pdf NULL: isotropic, 1 / (4 pi)).  If R >= r0_d and R > 0 the ray is traced through the mesh and scores
+ * s_k = w r[k] p exp(-tau) / R^2, tau the sum over the tets it crosses of Sigma_t[b][tet] times the length inside.  If
+ * R < r0_d nothing is traced and s_k = w r[k] p 3 g(Sigma_t[b][e_i] r0_d) / r0_d^2, g(x) = (1 - exp(-x)) / x (1 at 0):
+ * the mean of exp(-Sigma r) / r^2 over the ball.  The arrival time t + R / v goes into the time bin that holds it (an
+ * edge belongs to the bin above).  Results are laid out [time][bin][score][detector].
+ * Ray outcomes: traced (the walk reaches the tet that contains the detector); shadowed (the ray leaves the mesh through
+ * the hull first and scores 0: outside the mesh counts as a void of zero importance, which is exact for rays that stay
+ * inside the mesh; re-entry across a concave part of the hull is NOT followed); lost (stopped by the option
+ * "max_iters"; scores 0).
+ * Event outcomes, checked in this order and shared by all the event's rays: rejected (a non-finite coordinate, weight *
+ * response, time or pdf value, a negative pdf value, a speed not > 0 with time bins, or R == 0 at a detector with
+ * r0_d == 0); outside (a located event outside the mesh).  Then per ray, skipped (a bin outside [0, nbins) or an
+ * arrival time outside [T_0, T_n): not traced, not counted).  With a pdf every ray reads the event's D values, and with
+ * a detector of r0 == 0 every ray compares the event with the D positions.  A multigroup scattering matrix, whose outgoing group depends on the direction, is handled by the
+ * caller passing one event per outgoing group g' with bin g' and pdf p(g -> g', mu_d).
+ * pumitally_tally_detectors: nevents events at AoS points xyz[3 * nevents], each located as pumitally_locate_points
+ * locates it; host calls work through device buffers of the option "chunk" events.  The _device variant takes device
+ * arrays and is enqueued on `stream`.  pumitally_tally_detectors_at_particles: an event for every particle i with
+ * flagged[i] != 0, at its stored position in its parent element (n must be num_particles); the _device variant is
+ * enqueued behind the last move.  pdf may be NULL; responses may be NULL only with one score; bins may be NULL (bin 0);
+ * times and speeds are required while time bins are set and ignored otherwise.
+ * pumitally_get_detector_results(e, kind, out, n), n == ntime * nbins * nscores * D: kind 0 the open tally divided by
+ * the per-source divisor (the sum over ranks after a batch-end exchange), 1 the batch mean, 2 its standard error, 3 its
+ * relative error (kinds 1-3 need batch statistics, kinds 2-3 two batches).  end_batch folds the detector tally (summed
+ * over the ranks) on every rank.
+ * Read-only counters since the last pumitally_reset_tally: "detector_rays" (traced), "detector_rays_shadowed",
+ * "detector_rays_lost", "detector_inside_r0" (rays inside an exclusion radius), "detector_crossings" (interior faces
+ * the traced, shadowed and lost rays crossed), "detector_events_outside" (once per event) and
+ * "detector_events_rejected" (once per event).  The four ray counters add up to D times the events neither rejected
+ * nor outside, less the skipped rays.
+ * A detector call changes no particle, flying flag, track-length or collision result, element statistic or kernel
+ * choice; like a collision call it opens the batch a checkpoint then holds.  Checkpoints hold the open detector tally
+ * and counters, and its batch mean and M2 (merged by Chan's update); the fingerprint holds D, the positions and r0 bit
+ * for bit and the CRC-32 of the cross-section table as uploaded, so a file of other detectors or another table is
+ * refused with a message that names them.  A file with detectors is written as format version 3; every other file
+ * keeps its version and bytes. */
+int pumitally_set_point_detectors(pumitally_engine *e, const double *xyz, int32_t ndet, const double *r0);
+int32_t pumitally_get_point_detectors(const pumitally_engine *e);
+int pumitally_set_detector_cross_sections(pumitally_engine *e, const double *sigma_t, int64_t n);
+int pumitally_tally_detectors(pumitally_engine *e, const double *xyz, int64_t nevents, const double *weights,
+                              const double *pdf, const double *responses, const int32_t *bins, const double *times,
+                              const double *speeds);
+int pumitally_tally_detectors_device(pumitally_engine *e, const double *d_xyz, int64_t nevents, const double *d_weights,
+                                     const double *d_pdf, const double *d_responses, const int32_t *d_bins,
+                                     const double *d_times, const double *d_speeds, void *stream);
+int pumitally_tally_detectors_at_particles(pumitally_engine *e, const int8_t *flagged, const double *weights,
+                                           const double *pdf, const double *responses, const int32_t *bins,
+                                           const double *times, const double *speeds, int32_t n);
+int pumitally_tally_detectors_at_particles_device(pumitally_engine *e, const int8_t *d_flagged, const double *d_weights,
+                                                  const double *d_pdf, const double *d_responses, const int32_t *d_bins,
+                                                  const double *d_times, const double *d_speeds, int32_t n,
+                                                  void *stream);
+int pumitally_get_detector_results(pumitally_engine *e, int32_t kind, double *out, int64_t n);
+
 /* ---- additive: face currents (the weight crossing every element face, and the leakage through the hull) ----
  * pumitally_set_face_currents(e, 1) makes every move -- plain, binned, scored and timed, host and device pointers --
  * also tally, for each face a track crosses in the tally phase of a move, the particle's weight (weights[i], no

@@ -23,6 +23,7 @@ SOURCES = [
     "walk_kernels.cu",
     "bin_kernels.cu",
     "locate_kernels.cu",
+    "detector_kernels.cu",
     "stats_kernels.cu",
     "ww_kernels.cu",
     "source_kernels.cu",

@@ -271,6 +271,50 @@ int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *o
   return guarded(e, [&](ptb::Engine &g) { return g.get_collision_results(kind, out, n); });
 }
 
+int pumitally_set_point_detectors(pumitally_engine *e, const double *xyz, int32_t ndet, const double *r0) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_point_detectors(xyz, ndet, r0); });
+}
+int32_t pumitally_get_point_detectors(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "point_detectors")) : 0;
+}
+int pumitally_set_detector_cross_sections(pumitally_engine *e, const double *sigma_t, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_detector_cross_sections(sigma_t, n); });
+}
+int pumitally_tally_detectors(pumitally_engine *e, const double *xyz, int64_t nevents, const double *weights,
+                              const double *pdf, const double *responses, const int32_t *bins, const double *times,
+                              const double *speeds) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_detectors(xyz, nevents, weights, pdf, responses, bins, times, speeds);
+  });
+}
+int pumitally_tally_detectors_device(pumitally_engine *e, const double *d_xyz, int64_t nevents, const double *d_weights,
+                                     const double *d_pdf, const double *d_responses, const int32_t *d_bins,
+                                     const double *d_times, const double *d_speeds, void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_detectors_device(d_xyz, nevents, d_weights, d_pdf, d_responses, d_bins, d_times, d_speeds,
+                                    static_cast<cudaStream_t>(stream));
+  });
+}
+int pumitally_tally_detectors_at_particles(pumitally_engine *e, const int8_t *flagged, const double *weights,
+                                           const double *pdf, const double *responses, const int32_t *bins,
+                                           const double *times, const double *speeds, int32_t n) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_detectors_at_particles(flagged, weights, pdf, responses, bins, times, speeds, n);
+  });
+}
+int pumitally_tally_detectors_at_particles_device(pumitally_engine *e, const int8_t *d_flagged, const double *d_weights,
+                                                  const double *d_pdf, const double *d_responses, const int32_t *d_bins,
+                                                  const double *d_times, const double *d_speeds, int32_t n,
+                                                  void *stream) {
+  return guarded(e, [&](ptb::Engine &g) {
+    return g.tally_detectors_at_particles_device(d_flagged, d_weights, d_pdf, d_responses, d_bins, d_times, d_speeds, n,
+                                                 static_cast<cudaStream_t>(stream));
+  });
+}
+int pumitally_get_detector_results(pumitally_engine *e, int32_t kind, double *out, int64_t n) {
+  return guarded(e, [&](ptb::Engine &g) { return g.get_detector_results(kind, out, n); });
+}
+
 int pumitally_set_face_currents(pumitally_engine *e, int32_t on) {
   return guarded(e, [&](ptb::Engine &g) { return g.set_face_currents(on); });
 }

@@ -14,6 +14,7 @@ constexpr char kMagic[8] = {'P', 'T', 'B', 'C', 'K', 'P', 'T', '\0'};
 constexpr uint32_t kEndianMarker = 0x01020304u;
 constexpr uint32_t kMaxEdges = 1025;          // kMaxTimeBins + 1 (walk_core.cuh)
 constexpr uint32_t kMaxMuEdges = 65;          // kMaxCosineBins + 1 (walk_core.cuh)
+constexpr uint32_t kMaxDetectors = 256;       // kMaxDetectors (walk_core.cuh)
 constexpr uint64_t kMaxLen = uint64_t(1) << 56;  // doubles: beyond any device memory, and no overflow below
 constexpr size_t kSectionHead = 16;           // id (u32), byte length (u64), CRC-32 (u32)
 
@@ -60,13 +61,20 @@ void put_header(std::vector<uint8_t> &b, const Header &h, const Fingerprint &f) 
   put_le(b, f.share, 8);
   put_le(b, uint32_t(f.edges.size()), 4);
   for (double e : f.edges) put_le(b, bits_of(e), 8);
-  if (!f.mu_edges.empty()) {  // version 2 only
+  if (!f.mu_edges.empty() || !f.det_r0.empty()) {  // versions 2 and 3
     put_le(b, uint32_t(f.mu_edges.size()), 4);
     for (double e : f.mu_edges) put_le(b, bits_of(e), 8);
   }
+  if (!f.det_r0.empty()) {  // version 3 only
+    put_le(b, uint32_t(f.det_r0.size()), 4);
+    for (double e : f.det_xyz) put_le(b, bits_of(e), 8);
+    for (double e : f.det_r0) put_le(b, bits_of(e), 8);
+    put_le(b, f.sigma_crc, 4);
+    put_le(b, h.det_len, 8);
+  }
 }
 
-void get_header(const uint8_t *p, Header *h, Fingerprint *f, bool cosines) {
+void get_header(const uint8_t *p, Header *h, Fingerprint *f, bool cosines, bool detectors) {
   h->batches = int64_t(get_le(p, 8));
   h->open = uint32_t(get_le(p + 8, 4));
   h->open_len = get_le(p + 16, 8);
@@ -94,11 +102,28 @@ void get_header(const uint8_t *p, Header *h, Fingerprint *f, bool cosines) {
   f->edges.resize(ne);
   for (uint32_t j = 0; j < ne; ++j) f->edges[j] = double_of(get_le(p + 8 * j, 8));
   f->mu_edges.clear();
-  if (cosines) {
+  f->det_xyz.clear();
+  f->det_r0.clear();
+  f->sigma_crc = 0;
+  h->det_len = 0;
+  if (cosines || detectors) {
     p += 8 * size_t(ne);
     const uint32_t nm = uint32_t(get_le(p, 4));
     f->mu_edges.resize(nm);
     for (uint32_t j = 0; j < nm; ++j) f->mu_edges[j] = double_of(get_le(p + 4 + 8 * j, 8));
+    p += 4 + 8 * size_t(nm);
+  }
+  if (detectors) {
+    const uint32_t nd = uint32_t(get_le(p, 4));
+    p += 4;
+    f->det_xyz.resize(3 * size_t(nd));
+    f->det_r0.resize(nd);
+    for (size_t j = 0; j < 3 * size_t(nd); ++j) f->det_xyz[j] = double_of(get_le(p + 8 * j, 8));
+    p += 24 * size_t(nd);
+    for (size_t j = 0; j < nd; ++j) f->det_r0[j] = double_of(get_le(p + 8 * j, 8));
+    p += 8 * size_t(nd);
+    f->sigma_crc = uint32_t(get_le(p, 4));
+    h->det_len = get_le(p + 4, 8);
   }
 }
 
@@ -161,6 +186,12 @@ const char *fingerprint_mismatch(const Fingerprint &a, const Fingerprint &b, boo
   if (a.rank != b.rank) return "rank";
   if (a.nranks != b.nranks) return "number of ranks";
   if (a.share != b.share) return "rank share";
+  if (a.det_r0.size() != b.det_r0.size()) return "number of point detectors (set_point_detectors)";
+  for (size_t j = 0; j < a.det_xyz.size(); ++j)
+    if (bits_of(a.det_xyz[j]) != bits_of(b.det_xyz[j])) return "point-detector positions (set_point_detectors)";
+  for (size_t j = 0; j < a.det_r0.size(); ++j)
+    if (bits_of(a.det_r0[j]) != bits_of(b.det_r0[j])) return "point-detector exclusion radii (set_point_detectors)";
+  if (a.sigma_crc != b.sigma_crc) return "detector cross-section table (set_detector_cross_sections)";
   return nullptr;
 }
 
@@ -206,6 +237,14 @@ std::vector<std::pair<uint32_t, uint64_t>> sections_of(const Header &h) {
     s.emplace_back(kRegionMean, 8 * h.region_len);
     s.emplace_back(kRegionM2, 8 * h.region_len);
   }
+  if (h.det_len && h.open) {
+    s.emplace_back(kDetOpen, 8 * h.det_len);
+    s.emplace_back(kDetCounts, 8 * kDetCountWords);
+  }
+  if (h.det_len && h.stats_len) {
+    s.emplace_back(kDetMean, 8 * h.det_len);
+    s.emplace_back(kDetM2, 8 * h.det_len);
+  }
   return s;
 }
 
@@ -222,7 +261,7 @@ bool Writer::put(const void *p, size_t n) {
 
 bool Writer::begin(const Header &h, const Fingerprint &f) {
   std::vector<uint8_t> b(kMagic, kMagic + 8);
-  put_le(b, f.mu_edges.empty() ? kVersion : kVersionCosines, 4);
+  put_le(b, !f.det_r0.empty() ? kVersionDetectors : f.mu_edges.empty() ? kVersion : kVersionCosines, 4);
   put_le(b, kEndianMarker, 4);
   put_header(b, h, f);
   put_le(b, crc32(b.data(), b.size()), 4);
@@ -277,11 +316,11 @@ bool Reader::begin(Header *h, Fingerprint *f) {
     return false;
   }
   const uint64_t version = get_le(b.data() + 8, 4);
-  if (version != kVersion && version != kVersionCosines) {
+  if (version != kVersion && version != kVersionCosines && version != kVersionDetectors) {
     err_ = "unsupported format version " + std::to_string(version);
     return false;
   }
-  const bool cosines = version == kVersionCosines;
+  const bool cosines = version == kVersionCosines, detectors = version == kVersionDetectors;
   if (get_le(b.data() + 12, 4) != kEndianMarker) {
     err_ = "wrong endianness marker";
     return false;
@@ -304,14 +343,33 @@ bool Reader::begin(Header *h, Fingerprint *f) {
     b.resize(at + 8 * size_t(nm) + 4);
     if (!get(b.data() + at, b.size() - at)) return false;
   }
+  if (detectors) {  // the last 4 bytes read are the cosine-edge count (0 or 2..65), then come the detectors
+    const uint32_t nm = uint32_t(get_le(b.data() + b.size() - 4, 4));
+    if (nm == 1 || nm > kMaxMuEdges) {
+      err_ = "corrupt version 3 header (cosine-bin edge count)";
+      return false;
+    }
+    size_t at = b.size();
+    b.resize(at + 8 * size_t(nm) + 4);
+    if (!get(b.data() + at, b.size() - at)) return false;
+    const uint32_t nd = uint32_t(get_le(b.data() + b.size() - 4, 4));
+    if (nd < 1 || nd > kMaxDetectors) {
+      err_ = "corrupt version 3 header (detector count)";
+      return false;
+    }
+    at = b.size();
+    b.resize(at + 32 * size_t(nd) + 4 + 8 + 4);
+    if (!get(b.data() + at, b.size() - at)) return false;
+  }
   if (crc32(b.data(), b.size() - 4) != uint32_t(get_le(b.data() + b.size() - 4, 4))) {
     err_ = cosines ? "corrupt version 2 header or fingerprint (CRC mismatch)"
-                   : "corrupt header or fingerprint (CRC mismatch)";
+           : detectors ? "corrupt version 3 header or fingerprint (CRC mismatch)"
+                       : "corrupt header or fingerprint (CRC mismatch)";
     return false;
   }
-  get_header(b.data() + 16, h, f, cosines);
+  get_header(b.data() + 16, h, f, cosines, detectors);
   if (h->open > 1 || (!h->open && h->open_len) || h->batches < 0 || h->open_len > kMaxLen ||
-      h->stats_len > kMaxLen || h->region_len > kMaxLen) {
+      h->stats_len > kMaxLen || h->region_len > kMaxLen || h->det_len > kMaxLen || (detectors && !h->det_len)) {
     err_ = "corrupt header (declared lengths)";
     return false;
   }

@@ -27,6 +27,10 @@ namespace ckpt {
 // that does not know them refuses instead of misreading; every other file keeps version 1's bytes.
 constexpr uint32_t kVersion = 1;
 constexpr uint32_t kVersionCosines = 2;
+// Version 3: point detectors.  After the time-bin edges come the cosine-bin edges (count, possibly 0), the detectors
+// (count D, positions [3D], exclusion radii [D]), the CRC-32 of the cross-section table and det_len (u64).  Only a file
+// whose fingerprint holds detectors is written as version 3.
+constexpr uint32_t kVersionDetectors = 3;
 
 // 64-bit hash of a byte string (not cryptographic: it tells configurations apart, it does not authenticate them).
 // Chainable: hash64(b, nb, hash64(a, na)) hashes a then b.
@@ -50,6 +54,8 @@ struct Fingerprint {
   uint64_t share = 0;
   std::vector<double> edges;  // time-bin edges (empty: no time filter), compared bit for bit
   std::vector<double> mu_edges;  // cosine-bin edges of the face currents (empty: none), compared bit for bit
+  std::vector<double> det_xyz, det_r0;  // point detectors (empty: none), compared bit for bit
+  uint32_t sigma_crc = 0;               // CRC-32 of the detector cross-section table as uploaded (0: no table)
 };
 
 // The name of the first field in which `file` differs from `engine`, nullptr when they agree.  ignore_norm_value:
@@ -62,6 +68,7 @@ struct Header {
   uint64_t open_len = 0;    // doubles of the open tally (0 without one)
   uint64_t stats_len = 0;   // doubles of each of kMean and kM2 (0 without statistics)
   uint64_t region_len = 0;  // doubles of each of kRegionMean and kRegionM2 (0 without region statistics)
+  uint64_t det_len = 0;     // doubles of the detector tally (version 3 only; 0 without detectors)
 };
 
 enum SectionId : uint32_t {
@@ -71,7 +78,12 @@ enum SectionId : uint32_t {
   kM2 = 4,            // sums of squared deviations [stats_len]
   kRegionMean = 5,    // [region_len]
   kRegionM2 = 6,      // [region_len]
+  kDetOpen = 7,       // the open detector tally [det_len] (with kOpenTally)
+  kDetCounts = 8,     // kDetCountWords 64-bit detector counters (with kOpenTally)
+  kDetMean = 9,       // [det_len] (with kMean)
+  kDetM2 = 10,        // [det_len] (with kMean)
 };
+constexpr size_t kDetCountWords = 7;
 
 // The small state of the open batch, as 64-bit words in this order.
 struct OpenScalars {

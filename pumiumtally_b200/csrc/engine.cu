@@ -85,6 +85,8 @@ Engine::Engine(HostMesh &&mesh, int32_t num_particles, int device)
   dev_alloc(&d_stats_, 1, "stats");
   dev_alloc(&d_coll_counts_, 3, "collision counters");
   cuda_or_throw(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)), "memset");
+  dev_alloc(&d_det_counts_, kDetCounters, "detector counters");
+  cuda_or_throw(cudaMemset(d_det_counts_, 0, kDetCounters * sizeof(unsigned long long)), "memset");
   dev_alloc(&d_initial_weight_, 1, "initial weight");
   cuda_or_throw(cudaMemset(d_initial_weight_, 0, sizeof(double)), "memset");
   dev_alloc(&d_batch_div_, 2, "batch divisor");
@@ -198,6 +200,8 @@ Engine::~Engine() {
   cudaFree(d_arena_);
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
   cudaFree(d_coll_counts_);
+  cudaFree(d_det_counts_);
+  cudaFree(d_det_); cudaFree(d_det_pos_); cudaFree(d_det_r0_); cudaFree(d_sigma_);
   free_stats();
   free_regions();
   free_region_currents();
@@ -1276,9 +1280,21 @@ int Engine::resize_flux(int32_t nbins, int32_t nscores, int32_t ntime, int32_t m
             cudaGetErrorString(err));
     return 1;
   }
-  if (batch_stats_ && alloc_stats(reported)) {  // statistics of the new layout, no batch folded yet
+  double *nd = nullptr;  // the detector tally [time][bin][score][detector] of the new layout
+  const int det_rc = ndet_ > 0 ? alloc_detectors(arrays * size_t(nscores) * size_t(ndet_), batch_stats_, &nd) : 0;
+  if (det_rc || (batch_stats_ && alloc_stats(reported))) {  // statistics of the new layout, no batch folded yet
     cudaFree(nf);
+    cudaFree(nd);
     return 1;
+  }
+  if (ndet_ > 0) {
+    cudaFree(d_det_);
+    d_det_ = nd;
+  }
+  if (nbins != sigma_bins_) {  // a table of another number of groups no longer applies
+    cudaFree(d_sigma_);
+    d_sigma_ = nullptr;
+    sigma_bins_ = 0;
   }
   cudaFree(d_flux_);
   d_flux_ = nf;
@@ -1611,6 +1627,9 @@ int Engine::reset_tally() {
   scored_moves_ = 0;
   PTB_CUDA_OK(cudaMemset(d_stats_, 0, sizeof(DeviceStats)));
   PTB_CUDA_OK(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)));
+  PTB_CUDA_OK(cudaMemset(d_det_counts_, 0, kDetCounters * sizeof(unsigned long long)));
+  if (ndet_ > 0) PTB_CUDA_OK(cudaMemset(d_det_, 0, 2 * det_len() * sizeof(double)));
+  det_global_valid_ = false;
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = tallied_ = false;
   kernel_ms_ = 0.0;
   h2d_bytes_ = 0.0;
@@ -1688,6 +1707,21 @@ int64_t Engine::get_option(const std::string &name) const {
     }
     return int64_t(c[name == "collisions" ? 0 : name == "collisions_outside" ? 1 : 2]);
   }
+  if (name == "point_detectors") return ndet_;
+  // detector rays and events since the last reset (kDetCount* in walk_kernels.hpp)
+  static const char *const kDetNames[kDetCounters] = {"detector_rays", "detector_rays_shadowed", "detector_rays_lost",
+                                                      "detector_inside_r0", "detector_crossings",
+                                                      "detector_events_outside", "detector_events_rejected"};
+  for (int c = 0; c < kDetCounters; ++c)
+    if (name == kDetNames[c]) {
+      unsigned long long v[kDetCounters] = {};
+      if (cudaSetDevice(device_) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+          cudaMemcpy(v, d_det_counts_, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) {
+        cudaGetLastError();
+        return -1;
+      }
+      return int64_t(v[c]);
+    }
   if (name == "walk_blocks_per_sm") return walk_blocks_per_sm();  // occupancy of the last persistent walk kernel launched
   if (name == "die_split") return die_split_ ? 1 : 0;
   if (name == "l2_partition0_sms") return die0_sms_;  // SMs in the L2 partition of SM 0 (0: no map found)
@@ -2262,6 +2296,270 @@ int Engine::tally_collisions_at_particles_device(const int8_t *d_collided, const
   return 0;
 }
 
+// ------------------------------------------------------------------ point detectors
+
+// d_det_: [open][exchanged sum], then with batch statistics [mean][M2], each L doubles.
+int Engine::alloc_detectors(size_t L, bool stats, double **out) {
+  *out = nullptr;
+  const size_t bytes = std::max<size_t>((stats ? 4 : 2) * L, 1) * sizeof(double);
+  if (cudaMalloc(reinterpret_cast<void **>(out), bytes) != cudaSuccess || cudaMemset(*out, 0, bytes) != cudaSuccess) {
+    const cudaError_t err = cudaGetLastError();
+    cudaFree(*out);
+    *out = nullptr;
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the detector tally of %zu results (%s)\n", L,
+            cudaGetErrorString(err));
+    return 1;
+  }
+  return 0;
+}
+
+int Engine::set_point_detectors(const double *xyz, int32_t ndet, const double *r0) {
+  const bool remove = !xyz && !r0 && ndet == 0;
+  const char *why = nccl_comm_ ? "after comm_init (the exchange buffers are sized by then)"
+                    : remove   ? nullptr
+                    : (!xyz || !r0 || ndet < 1 || ndet > kMaxDetectors)
+                        ? "ndet must be 1..256 with positions and radii, or (NULL, 0, NULL)"
+                        : nullptr;
+  for (int32_t d = 0; !why && !remove && d < ndet; ++d)
+    if (!std::isfinite(r0[d]) || r0[d] < 0.0) why = "every exclusion radius must be finite and >= 0";
+  std::vector<int32_t> elem(size_t(std::max(ndet, 0)), -1);
+  if (!why && !remove) {
+    if (synchronize() || ensure_candidates() || ensure_arena(arena_slice(3 * size_t(ndet) * sizeof(double)) +
+                                                             arena_slice(size_t(ndet) * sizeof(int32_t))))
+      return 1;
+    double *dx = static_cast<double *>(d_arena_);
+    int32_t *de = reinterpret_cast<int32_t *>(static_cast<char *>(d_arena_) + arena_slice(3 * size_t(ndet) * sizeof(double)));
+    PTB_CUDA_OK(cudaMemcpy(dx, xyz, 3 * size_t(ndet) * sizeof(double), cudaMemcpyHostToDevice));
+    PTB_CUDA_OK(launch_locate(locate_params(), dx, ndet, de, nullptr, nullptr, compute_));
+    PTB_CUDA_OK(cudaMemcpyAsync(elem.data(), de, size_t(ndet) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
+    PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+    for (int32_t d = 0; d < ndet; ++d)
+      if (elem[size_t(d)] < 0) why = "every detector must lie inside the mesh, with finite coordinates";
+  }
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_point_detectors: %s\n", why);
+    return 1;
+  }
+  if (synchronize()) return 1;
+  double *nd = nullptr, *npos = nullptr, *nr0 = nullptr;
+  if (!remove) {
+    if (alloc_detectors(nslices() * size_t(nbins_) * size_t(nscores_) * size_t(ndet), batch_stats_, &nd)) return 1;
+    if (cudaMalloc(reinterpret_cast<void **>(&npos), 3 * size_t(ndet) * sizeof(double)) != cudaSuccess ||
+        cudaMalloc(reinterpret_cast<void **>(&nr0), size_t(ndet) * sizeof(double)) != cudaSuccess ||
+        cudaMemcpy(npos, xyz, 3 * size_t(ndet) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(nr0, r0, size_t(ndet) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaGetLastError();
+      cudaFree(nd);
+      cudaFree(npos);
+      cudaFree(nr0);
+      fprintf(stderr, "[pumitally] ERROR: set_point_detectors: no device memory for the detectors\n");
+      return 1;
+    }
+  }
+  if (batch_stats_ && alloc_stats(reported_len())) {  // discards the folded batches, as every set_* call does
+    cudaFree(nd);
+    cudaFree(npos);
+    cudaFree(nr0);
+    return 1;
+  }
+  cudaFree(d_det_);
+  cudaFree(d_det_pos_);
+  cudaFree(d_det_r0_);
+  d_det_ = nd;
+  d_det_pos_ = npos;
+  d_det_r0_ = nr0;
+  ndet_ = remove ? 0 : ndet;
+  det_xyz_.assign(xyz, xyz + 3 * size_t(ndet_));
+  det_r0_.assign(r0, r0 + size_t(ndet_));
+  det_elem_ = remove ? std::vector<int32_t>() : elem;
+  return reset_tally();
+}
+
+int Engine::set_detector_cross_sections(const double *sigma_t, int64_t n) {
+  const int64_t E = mesh_.ntets;
+  const char *why = !sigma_t || n != int64_t(nbins_) * E ? "n must be nbins * num_elements" : nullptr;
+  for (int64_t i = 0; !why && i < n; ++i)
+    if (!std::isfinite(sigma_t[i]) || sigma_t[i] < 0.0) why = "every cross section must be finite and >= 0";
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_detector_cross_sections: %s\n", why);
+    return 1;
+  }
+  std::vector<double> internal(static_cast<size_t>(n));  // [bin][internal element]
+  for (int64_t b = 0; b < nbins_; ++b)
+    for (int64_t i = 0; i < E; ++i) internal[size_t(b * E + i)] = sigma_t[b * E + mesh_.orig_of_internal[size_t(i)]];
+  if (synchronize()) return 1;
+  double *ns = nullptr;
+  if (cudaMalloc(reinterpret_cast<void **>(&ns), size_t(n) * sizeof(double)) != cudaSuccess ||
+      cudaMemcpy(ns, internal.data(), size_t(n) * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(ns);
+    fprintf(stderr, "[pumitally] ERROR: set_detector_cross_sections: no device memory for the table\n");
+    return 1;
+  }
+  cudaFree(d_sigma_);
+  d_sigma_ = ns;
+  sigma_bins_ = nbins_;
+  sigma_crc_ = ckpt::crc32(internal.data(), internal.size() * sizeof(double));
+  return 0;
+}
+
+DetectorParams Engine::detector_params() const {
+  DetectorParams p{};
+  p.tally = d_det_;
+  p.sigma = d_sigma_;
+  p.pos = d_det_pos_;
+  p.r0 = d_det_r0_;
+  p.edges = d_edges_;
+  p.nt = ntime_;
+  p.nbins = nbins_;
+  p.nscores = nscores_;
+  p.ndet = ndet_;
+  p.zero_r0 = std::count(det_r0_.begin(), det_r0_.end(), 0.0) > 0 ? 1 : 0;
+  p.E = mesh_.ntets;
+  return p;
+}
+
+bool Engine::detector_refused(const double *responses, const double *times, const double *speeds) const {
+  const char *why = ndet_ == 0                       ? "no point detectors are set (set_point_detectors)"
+                    : !d_sigma_                      ? "no cross-section table is set (set_detector_cross_sections)"
+                    : (!responses && nscores_ > 1)   ? "responses are required with several scores"
+                    : ((!times || !speeds) && ntime_ > 0) ? "times and speeds are required while time bins are set"
+                                                     : nullptr;
+  if (why) fprintf(stderr, "[pumitally] ERROR: detector events refused: %s\n", why);
+  return why != nullptr;
+}
+
+int Engine::detect_located_setup(const double *xyz, int64_t n, const double *w, const double *r, const double *t,
+                                 const double *v, size_t arena) {
+  if (detector_refused(r, t, v) || n < 0 || (n > 0 && (!xyz || !w))) return 1;
+  if (n == 0) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_candidates() || ensure_arena(arena)) return 1;
+  det_global_valid_ = false;
+  tallied_ = true;  // a checkpoint now holds the open batch, the detector tally with it
+  return 0;
+}
+
+cudaError_t Engine::enqueue_detect_located(const double *xyz, int64_t n, const double *w, const double *pdf,
+                                           const double *r, const int32_t *bins, const double *t, const double *v,
+                                           cudaStream_t stream) {
+  const LocateParams l = locate_params();
+  const DetectorParams p = detector_params();
+  const size_t S = size_t(nscores_), D = size_t(ndet_);
+  const int64_t per = std::max<int64_t>(1, kPointsPerLaunch / ndet_);  // rays per launch stay below 2^30
+  for (int64_t b = 0; b < n; b += per)
+    if (cudaError_t e = launch_detect_located(l, p, xyz + 3 * b, std::min(per, n - b), w + b,
+                                              pdf ? pdf + D * size_t(b) : nullptr, r ? r + S * size_t(b) : nullptr,
+                                              bins ? bins + b : nullptr, ntime_ > 0 ? t + b : nullptr,
+                                              ntime_ > 0 ? v + b : nullptr, d_det_counts_, stream))
+      return e;
+  return cudaSuccess;
+}
+
+int Engine::tally_detectors(const double *xyz, int64_t nevents, const double *weights, const double *pdf,
+                            const double *responses, const int32_t *bins, const double *times, const double *speeds) {
+  return staged(
+      nevents,
+      [&](size_t arena) { return detect_located_setup(xyz, nevents, weights, responses, times, speeds, arena); },
+      [&](int64_t, int64_t cnt, const double *x, const double *w, const double *p, const double *r, const double *t,
+          const double *v, const int32_t *bn) { return enqueue_detect_located(x, cnt, w, p, r, bn, t, v, compute_); },
+      // times and speeds are read only while time bins are set, so only then do they travel
+      stage(xyz, 3), stage(weights), stage(pdf, size_t(ndet_)), stage(responses, size_t(nscores_)),
+      stage(ntime_ > 0 ? times : nullptr), stage(ntime_ > 0 ? speeds : nullptr), stage(bins));
+}
+
+int Engine::tally_detectors_device(const double *d_xyz, int64_t nevents, const double *d_weights, const double *d_pdf,
+                                   const double *d_responses, const int32_t *d_bins, const double *d_times,
+                                   const double *d_speeds, cudaStream_t stream) {
+  if (int rc = detect_located_setup(d_xyz, nevents, d_weights, d_responses, d_times, d_speeds, 0))
+    return std::max(rc, 0);
+  PTB_CUDA_OK(enqueue_detect_located(d_xyz, nevents, d_weights, d_pdf, d_responses, d_bins, d_times, d_speeds, stream));
+  return 0;
+}
+
+int Engine::detect_particles_setup(const int8_t *flagged, const double *w, const double *r, const double *t,
+                                   const double *v, int32_t n, size_t arena, cudaStream_t stream) {
+  if (detector_refused(r, t, v)) return 1;
+  if (n != n_ || (n > 0 && (!flagged || !w))) {
+    fprintf(stderr, "[pumitally] ERROR: detector events at the particles: n must be num_particles (%d)\n", n_);
+    return 1;
+  }
+  if (n == 0) return -1;
+  PTB_CUDA_OK(cudaSetDevice(device_));
+  if (ensure_arena(arena) || follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
+  det_global_valid_ = false;
+  tallied_ = true;
+  return 0;
+}
+
+int Engine::tally_detectors_at_particles(const int8_t *flagged, const double *weights, const double *pdf,
+                                         const double *responses, const int32_t *bins, const double *times,
+                                         const double *speeds, int32_t n) {
+  WalkParams wp{};
+  wp.tets = d_tets_;
+  wp.max_iters = locate_params().max_iters;
+  wp.cx = mesh_.center[0]; wp.cy = mesh_.center[1]; wp.cz = mesh_.center[2];
+  return staged(
+      n, [&](size_t arena) { return detect_particles_setup(flagged, weights, responses, times, speeds, n, arena, compute_); },
+      [&](int64_t b, int64_t cnt, const int8_t *c, const double *w, const double *p, const double *r, const double *t,
+          const double *v, const int32_t *bn) {
+        return launch_detect_particles(wp, detector_params(), d_state_ + b, c, int32_t(cnt), w, p, r, bn,
+                                       ntime_ > 0 ? t : nullptr, ntime_ > 0 ? v : nullptr, d_det_counts_, compute_);
+      },
+      stage(flagged), stage(weights), stage(pdf, size_t(ndet_)), stage(responses, size_t(nscores_)),
+      stage(ntime_ > 0 ? times : nullptr), stage(ntime_ > 0 ? speeds : nullptr), stage(bins));
+}
+
+int Engine::tally_detectors_at_particles_device(const int8_t *d_flagged, const double *d_weights, const double *d_pdf,
+                                                const double *d_responses, const int32_t *d_bins, const double *d_times,
+                                                const double *d_speeds, int32_t n, cudaStream_t stream) {
+  if (int rc = detect_particles_setup(d_flagged, d_weights, d_responses, d_times, d_speeds, n, 0, stream))
+    return std::max(rc, 0);
+  WalkParams wp{};
+  wp.tets = d_tets_;
+  wp.max_iters = locate_params().max_iters;
+  wp.cx = mesh_.center[0]; wp.cy = mesh_.center[1]; wp.cz = mesh_.center[2];
+  PTB_CUDA_OK(launch_detect_particles(wp, detector_params(), d_state_, d_flagged, n, d_weights, d_pdf, d_responses,
+                                      d_bins, ntime_ > 0 ? d_times : nullptr, ntime_ > 0 ? d_speeds : nullptr,
+                                      d_det_counts_, stream));
+  return 0;
+}
+
+int Engine::exchange_detectors() {
+  if (ndet_ == 0 || !sharded()) return 0;
+  const size_t L = det_len();
+  if (nccl_allreduce_sum_f64(nccl_comm_, d_det_, d_det_ + L, L, compute_)) return 1;
+  PTB_CUDA_OK(cudaStreamSynchronize(compute_));
+  det_global_valid_ = true;
+  return 0;
+}
+
+int Engine::get_detector_results(int32_t kind, double *out, int64_t n) {
+  const size_t L = det_len();
+  const char *why = ndet_ == 0                ? "no point detectors are set (set_point_detectors)"
+                    : (kind < 0 || kind > 3)  ? "kind must be 0 (value), 1 (batch mean), 2 (standard error) or 3 "
+                                                "(relative error)"
+                    : (n != int64_t(L) || !out) ? "n must be ntime * nbins * nscores * ndet"
+                                              : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: get_detector_results: %s\n", why);
+    return 1;
+  }
+  if (kind > 0 && batch_refused(0, kind - 1)) return 1;
+  if (synchronize()) return 1;
+  if (kind == 0) {
+    double div = 1.0;
+    if (!per_source_divisor(&div)) return 1;
+    PTB_CUDA_OK(cudaMemcpy(out, d_det_ + (det_global_valid_ ? L : 0), L * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < L; ++i) out[i] /= div;
+    return 0;
+  }
+  std::vector<double> m(2 * L);
+  PTB_CUDA_OK(cudaMemcpy(m.data(), d_det_ + 2 * L, 2 * L * sizeof(double), cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < L; ++i) out[i] = batch_readout(m[i], m[L + i], double(batches_), 1.0, kind - 1);
+  return 0;
+}
+
 // ------------------------------------------------------------------ batch statistics
 
 int Engine::alloc_stats(size_t len) {
@@ -2298,10 +2596,19 @@ int Engine::set_batch_statistics(int32_t on) {
     return 1;
   }
   if (synchronize()) return 1;
+  double *nd = nullptr;
+  if (ndet_ > 0 && alloc_detectors(det_len(), on != 0, &nd)) return 1;
   if (on) {
-    if (alloc_stats(reported_len())) return 1;  // (a second call with 1 discards the folded batches)
+    if (alloc_stats(reported_len())) {  // (a second call with 1 discards the folded batches)
+      cudaFree(nd);
+      return 1;
+    }
   } else {
     free_stats();
+  }
+  if (ndet_ > 0) {
+    cudaFree(d_det_);
+    d_det_ = nd;
   }
   batch_stats_ = on != 0;
   return reset_tally();
@@ -2358,6 +2665,13 @@ int Engine::end_batch() {
     if (rc_on() && region_current_sums(d_flux_ + current_base(), sums + rc_base())) return 1;
     if (sharded() && nccl_allreduce_sum_f64(nccl_comm_, sums, sums, RL, compute_)) return 1;
     PTB_CUDA_OK(launch_batch_fold(sums, sums + RL, sums + 2 * RL, int64_t(RL), d_batch_div_, nb, compute_));
+  }
+  if (ndet_ > 0) {  // the detector tally summed over the ranks, folded the same on every rank
+    const size_t DL = det_len();
+    if (batches_ == 0) PTB_CUDA_OK(cudaMemsetAsync(d_det_ + 2 * DL, 0, 2 * DL * sizeof(double), compute_));
+    if (sharded() && nccl_allreduce_sum_f64(nccl_comm_, d_det_, d_det_ + DL, DL, compute_)) return 1;
+    PTB_CUDA_OK(launch_batch_fold(d_det_ + (sharded() ? DL : 0), d_det_ + 2 * DL, d_det_ + 3 * DL, int64_t(DL),
+                                  d_batch_div_, nb, compute_));
   }
   if (sharded()) {
     const size_t lo = size_t(rank_) * share_;  // the last share ends in padding (or a binned move's unreported array)
@@ -3109,6 +3423,9 @@ ckpt::Fingerprint Engine::fingerprint() {
       f.edges.assign(f.edges.size(), std::nan(""));  // (compares unequal to every file's edges)
   }
   if (currents_) f.mu_edges = mu_edges_;  // the cosine bins shape the arrays only with face currents on
+  f.det_xyz = det_xyz_;
+  f.det_r0 = det_r0_;
+  f.sigma_crc = ndet_ > 0 && d_sigma_ ? sigma_crc_ : 0;
   return f;
 }
 
@@ -3126,7 +3443,9 @@ int Engine::save_checkpoint(const std::string &path) {
   h.open_len = tallied_ ? reported_len() : 0;
   h.stats_len = batch_stats_ ? stats_len() : 0;
   h.region_len = RL;
-  std::vector<uint8_t> scalars;
+  const size_t DL = det_len();
+  h.det_len = DL;
+  std::vector<uint8_t> scalars, det_counts;
   if (tallied_) {
     ckpt::OpenScalars s;
     DeviceStats ds;
@@ -3144,6 +3463,12 @@ int Engine::save_checkpoint(const std::string &path) {
     s.moves = moves_;
     s.scored_moves = scored_moves_;
     scalars = ckpt::pack_open_scalars(s);
+    if (DL) {
+      unsigned long long dc[kDetCounters];
+      PTB_CUDA_OK(cudaMemcpy(dc, d_det_counts_, sizeof(dc), cudaMemcpyDeviceToHost));
+      det_counts.resize(sizeof(dc));
+      std::memcpy(det_counts.data(), dc, sizeof(dc));  // (little-endian hosts only, as the rest of the engine)
+    }
   }
   // the arrays of the sections, in file order (nullptr: zeros -- region statistics before the first end_batch)
   struct Src { uint32_t id; const double *d; const uint8_t *host; uint64_t bytes; };
@@ -3159,6 +3484,14 @@ int Engine::save_checkpoint(const std::string &path) {
   if (RL) {
     src.push_back({ckpt::kRegionMean, d_region_stats_ ? d_region_stats_ + RL : nullptr, nullptr, 8 * RL});
     src.push_back({ckpt::kRegionM2, d_region_stats_ ? d_region_stats_ + 2 * RL : nullptr, nullptr, 8 * RL});
+  }
+  if (DL && h.open) {
+    src.push_back({ckpt::kDetOpen, d_det_, nullptr, 8 * DL});
+    src.push_back({ckpt::kDetCounts, nullptr, det_counts.data(), det_counts.size()});
+  }
+  if (DL && h.stats_len) {  // (zeros before the first end_batch: the fold starts from zeros then too)
+    src.push_back({ckpt::kDetMean, batches_ > 0 ? d_det_ + 2 * DL : nullptr, nullptr, 8 * DL});
+    src.push_back({ckpt::kDetM2, batches_ > 0 ? d_det_ + 3 * DL : nullptr, nullptr, 8 * DL});
   }
   uint64_t largest = 0;
   for (const Src &s : src) largest = std::max(largest, s.bytes);
@@ -3252,7 +3585,7 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     const size_t rep = reported_len_for(currents);
     const size_t SL = !batch_stats_ ? 0 : sharded() ? (rep + size_t(nranks_) - 1) / size_t(nranks_) : rep;
     return h.stats_len == SL && h.region_len == region_len && (!h.open || h.open_len == rep) &&
-           (batch_stats_ || h.batches == 0);
+           (batch_stats_ || h.batches == 0) && h.det_len == det_len();
   };
   // Region currents add 2 ntime nbins P region results (P >= 1: every mesh has a hull), and need face currents.  Saved
   // with them on, a file has face currents on and a region length above rc_base() by a multiple of 2 ntime nbins.
@@ -3272,8 +3605,10 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     return refuse("the checkpoint holds an open batch, which a merge would drop (save at a batch end)");
   // new buffers: the open tally (whole allocation, zero past the reported part), the statistics, the region statistics
   // (load: the engine's [sums][mean][M2] layout; merge: [mean][M2] scratch)
-  double *nflux = nullptr, *nmean = nullptr, *nm2 = nullptr, *nreg = nullptr;
+  double *nflux = nullptr, *nmean = nullptr, *nm2 = nullptr, *nreg = nullptr, *ndet = nullptr;
+  const size_t DL = det_len();
   auto release = [&] {
+    cudaFree(ndet);
     cudaFree(nflux);
     cudaFree(nmean);
     cudaFree(nm2);
@@ -3286,11 +3621,11 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
   };
   const size_t reg_off = merge ? 0 : RL;  // where the region means go in nreg
   if ((!merge && h.open && !alloc(&nflux, flux_alloc_)) || (SL && (!alloc(&nmean, SL) || !alloc(&nm2, SL))) ||
-      (RL && !alloc(&nreg, (merge ? 2 : 3) * RL))) {
+      (RL && !alloc(&nreg, (merge ? 2 : 3) * RL)) || (DL && alloc_detectors(DL, batch_stats_, &ndet))) {
     release();
     return refuse("no device memory for a second copy of the checkpoint's arrays");
   }
-  std::vector<uint8_t> scalars(8 * ckpt::kOpenScalarWords);
+  std::vector<uint8_t> scalars(8 * ckpt::kOpenScalarWords), det_counts(8 * ckpt::kDetCountWords);
   struct Dst { uint32_t id; double *d; uint64_t bytes; };
   std::vector<Dst> dst;
   if (h.open) {
@@ -3305,6 +3640,14 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     dst.push_back({ckpt::kRegionMean, nreg + reg_off, 8 * RL});
     dst.push_back({ckpt::kRegionM2, nreg + reg_off + RL, 8 * RL});
   }
+  if (DL && h.open) {  // [open] of the new detector buffer; the counters arrive on the host
+    dst.push_back({ckpt::kDetOpen, ndet, 8 * DL});
+    dst.push_back({ckpt::kDetCounts, nullptr, det_counts.size()});
+  }
+  if (DL && SL) {  // [mean][M2] of the new detector buffer
+    dst.push_back({ckpt::kDetMean, ndet + 2 * DL, 8 * DL});
+    dst.push_back({ckpt::kDetM2, ndet + 3 * DL, 8 * DL});
+  }
   uint64_t largest = 0;
   for (const Dst &d : dst) largest = std::max(largest, d.bytes);
   bool ok = true;
@@ -3318,7 +3661,8 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     for (const Dst &d : dst) {
       if (!ok) break;
       if (!d.d) {
-        ok = r.section(d.id, d.bytes, buf.bytes, [&](size_t) -> void * { return scalars.data(); },
+        uint8_t *host = d.id == ckpt::kDetCounts ? det_counts.data() : scalars.data();
+        ok = r.section(d.id, d.bytes, buf.bytes, [&](size_t) -> void * { return host; },
                        [](size_t, uint64_t, const void *, size_t) { return true; });
       } else {
         // chunk k is read into the buffer whose last copy (chunk k - 2, or a chunk of the section before) has finished;
@@ -3365,6 +3709,12 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
       if (e == cudaSuccess && RL)
         e = launch_batch_merge(nreg, nreg + RL, d_region_stats_ + RL, d_region_stats_ + 2 * RL, int64_t(RL), na, nb,
                                compute_);
+      if (e == cudaSuccess && DL) {
+        if (batches_ == 0) e = cudaMemsetAsync(d_det_ + 2 * DL, 0, 2 * DL * sizeof(double), compute_);
+        if (e == cudaSuccess)
+          e = launch_batch_merge(ndet + 2 * DL, ndet + 3 * DL, d_det_ + 2 * DL, d_det_ + 3 * DL, int64_t(DL), na, nb,
+                                 compute_);
+      }
       if (e == cudaSuccess) e = cudaStreamSynchronize(compute_);
       release();
       PTB_CUDA_OK(e);
@@ -3393,6 +3743,15 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     cudaFree(d_region_stats_);
     d_region_stats_ = nreg;
     nreg = nullptr;
+  }
+  if (DL) {
+    cudaFree(d_det_);
+    d_det_ = ndet;
+    ndet = nullptr;
+    det_global_valid_ = false;
+    unsigned long long dc[kDetCounters] = {};
+    if (h.open) std::memcpy(dc, det_counts.data(), sizeof(dc));
+    PTB_CUDA_OK(cudaMemcpy(d_det_counts_, dc, sizeof(dc), cudaMemcpyHostToDevice));
   }
   batches_ = h.batches;
   DeviceStats ds{sc.segments, sc.tracks, sc.relocations, sc.lost, sc.fallbacks};
@@ -3857,6 +4216,7 @@ int Engine::allreduce_tally() {
   PTB_CUDA_OK(cudaEventRecord(ev_ar0_, compute_));
   if (nccl_allreduce_sum_f64(nccl_comm_, d_flux_, d_flux_global_, reported_len(), compute_)) return 1;
   PTB_CUDA_OK(cudaEventRecord(ev_ar1_, compute_));
+  if (exchange_detectors()) return 1;
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   float ms = 0.f;
   if (cudaEventElapsedTime(&ms, ev_ar0_, ev_ar1_) == cudaSuccess) allreduce_ms_ = ms;
@@ -3873,6 +4233,7 @@ int Engine::reduce_tally_to_owners() {
   PTB_CUDA_OK(cudaEventRecord(ev_ar0_, compute_));
   if (nccl_reduce_scatter_sum_f64(nccl_comm_, d_flux_, d_flux_global_ + size_t(rank_) * share_, share_, compute_)) return 1;
   PTB_CUDA_OK(cudaEventRecord(ev_ar1_, compute_));
+  if (exchange_detectors()) return 1;
   PTB_CUDA_OK(cudaStreamSynchronize(compute_));
   float ms = 0.f;
   if (cudaEventElapsedTime(&ms, ev_ar0_, ev_ar1_) == cudaSuccess) allreduce_ms_ = ms;

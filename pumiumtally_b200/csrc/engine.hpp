@@ -137,6 +137,34 @@ class Engine {
   int get_face_current_results(int32_t direction, int32_t kind, double *out, int64_t n);
   // the outgoing current summed over every hull face, kinds as above; n == ntime * nbins * C, [time][bin][cosine]
   int get_leakage(int32_t kind, double *out, int64_t n);
+  // Point detectors (walk_core.cuh, detector_event): D = ndet detectors at xyz[3D] (AoS, each inside the mesh) with
+  // exclusion radii r0[D] (finite, >= 0), 1 <= D <= kMaxDetectors; xyz == r0 == nullptr with ndet == 0 removes them.
+  // Resets the tally, discards the folded batches; before comm_init.  Anything else is refused and changes nothing.
+  int set_point_detectors(const double *xyz, int32_t ndet, const double *r0);
+  int32_t point_detectors() const { return ndet_; }
+  // Sigma_t [bin][element] in the caller's numbering, n == nbins * E, finite and >= 0; kept until set_score_bins changes
+  // nbins.  Resets nothing.  Detector calls are refused without it.
+  int set_detector_cross_sections(const double *sigma_t, int64_t n);
+  // Next-event estimates of every (event, detector) ray into [time][bin][score][detector].  pdf[i * D + d] is the
+  // angular density toward detector d per steradian (nullptr: 1 / (4 pi)); responses may be nullptr with one score, bins
+  // nullptr (bin 0); times and speeds are required while time bins are set.  tally_detectors: events at nevents points,
+  // located as locate_points does; host calls work through chunk-sized buffers.  tally_detectors_at_particles: the
+  // particles i with flagged[i] != 0, at their stored positions and elements (n == num_particles).  Neither touches the
+  // particles, any other tally or the move statistics.
+  int tally_detectors(const double *xyz, int64_t nevents, const double *weights, const double *pdf,
+                      const double *responses, const int32_t *bins, const double *times, const double *speeds);
+  int tally_detectors_device(const double *d_xyz, int64_t nevents, const double *d_weights, const double *d_pdf,
+                             const double *d_responses, const int32_t *d_bins, const double *d_times,
+                             const double *d_speeds, cudaStream_t stream);  // enqueue only
+  int tally_detectors_at_particles(const int8_t *flagged, const double *weights, const double *pdf,
+                                   const double *responses, const int32_t *bins, const double *times,
+                                   const double *speeds, int32_t n);
+  int tally_detectors_at_particles_device(const int8_t *d_flagged, const double *d_weights, const double *d_pdf,
+                                          const double *d_responses, const int32_t *d_bins, const double *d_times,
+                                          const double *d_speeds, int32_t n, cudaStream_t stream);
+  // kind 0 the open tally / the per-source divisor (the sum over ranks after an exchange), 1 batch mean, 2 standard
+  // error, 3 relative error; n == ntime * nbins * nscores * D, [time][bin][score][detector].
+  int get_detector_results(int32_t kind, double *out, int64_t n);
   // Batch statistics (batch_stats.cuh): on == 1 keeps a running mean and sum of squared deviations of every reported
   // double (both tallies), folded by end_batch from the batch's results divided by its source-normalisation divisor;
   // 0 frees them.  Resets the tally; before comm_init.  Any later set_* call discards the folded batches.
@@ -359,6 +387,30 @@ class Engine {
                               size_t arena, cudaStream_t stream);
   cudaError_t enqueue_collide_particles(int32_t first, int32_t n, const int8_t *collided, const double *w,
                                         const double *r, const int32_t *bins, const double *t, cudaStream_t stream);
+  // ---- point detectors (detector_kernels.cu) ----
+  int32_t ndet_ = 0;                               // 0: no detectors
+  std::vector<double> det_xyz_, det_r0_;           // as set_point_detectors took them
+  std::vector<int32_t> det_elem_;                  // internal element of each detector
+  double *d_det_pos_ = nullptr, *d_det_r0_ = nullptr;
+  double *d_sigma_ = nullptr;                      // [nbins][E] internal order; nullptr: no table
+  int32_t sigma_bins_ = 0;                         // nbins of the table
+  uint32_t sigma_crc_ = 0;                         // CRC-32 of the table as uploaded
+  // [2 * det_len()]: the open tally and the sum over ranks of the last exchange; then, with batch statistics,
+  // [2 * det_len()]: the batch mean and M2
+  double *d_det_ = nullptr;
+  bool det_global_valid_ = false;                  // the second block holds the exchanged sum of the first
+  unsigned long long *d_det_counts_ = nullptr;     // [kDetCounters] since the last reset
+  size_t det_len() const { return nslices() * size_t(nbins_) * size_t(nscores_) * size_t(ndet_); }
+  int alloc_detectors(size_t len, bool stats, double **out);  // len doubles per block, zeroed; nothing changes on failure
+  DetectorParams detector_params() const;
+  bool detector_refused(const double *responses, const double *times, const double *speeds) const;  // with a message
+  int detect_located_setup(const double *xyz, int64_t n, const double *w, const double *r, const double *t,
+                           const double *v, size_t arena);
+  cudaError_t enqueue_detect_located(const double *xyz, int64_t n, const double *w, const double *pdf, const double *r,
+                                     const int32_t *bins, const double *t, const double *v, cudaStream_t stream);
+  int detect_particles_setup(const int8_t *flagged, const double *w, const double *r, const double *t, const double *v,
+                             int32_t n, size_t arena, cudaStream_t stream);
+  int exchange_detectors();  // the detector block summed over the ranks into its second block (collective)
   // ---- batch statistics (stats_kernels.cu) ----
   bool batch_stats_ = false;
   int64_t batches_ = 0;                            // batches folded

@@ -945,4 +945,120 @@ PTB_UNROLL
   return kEventTallied;
 }
 
+// ---- point detectors: next-event estimates of the flux at fixed points ------------------------------------------------
+// Event i at x in element e and detector d at x_d form one ray.  Its score is w * r[k] * p * exp(-tau) / R^2, R = |x_d -
+// x| and tau the line integral of Sigma_t from x to x_d over the mesh (detector_ray).  Inside the exclusion radius r0
+// (R < r0) nothing is traced and the ray scores the mean of exp(-Sigma r) / r^2 over the ball instead, with Sigma the
+// event element's: w * r[k] * p * 3 g(Sigma r0) / r0^2, g(x) = -expm1(-x) / x.
+constexpr int kRayTraced = 0;    // the walk reached the tet that contains the detector
+constexpr int kRayShadowed = 1;  // the ray left the mesh through the hull first: it scores 0
+constexpr int kRayLost = 2;      // stopped by the iteration limit: it scores 0
+constexpr int kRayInsideR0 = 3;  // R < r0: the ball formula, no walk
+// the outcomes of detector_event that are not one of the four above
+constexpr int kDetOutside = 4;   // the event lies outside the mesh (counted once per event)
+constexpr int kDetRejected = 5;  // a non-finite coordinate, w * r[k], time or pdf value, a negative pdf value, a speed
+                                 // not > 0, or R == 0 at a detector with r0 == 0 (counted once per event)
+constexpr int kDetSkipped = 6;   // bin outside [0, nbins), or arrival time outside [T_0, T_nt): not traced, not counted
+
+constexpr int kMaxDetectors = 256;
+
+struct DetectorParams {
+  double *tally;          // [time][bin][score][D]
+  const double *sigma;    // [nbins][E] Sigma_t in internal element order
+  const double *pos;      // [3D] detector positions (caller's coordinates)
+  const double *r0;       // [D] exclusion radii
+  const double *edges;    // [nt + 1] time bin edges (nt > 0)
+  int32_t nt;             // time bins (0: times and speeds are not read)
+  int32_t nbins, nscores, ndet;
+  int32_t zero_r0;        // some detector has r0 == 0 (an event exactly on it is rejected)
+  int64_t E;
+};
+
+// tau / R of the straight line from (x, y, z) in element e to (tx, ty, tz): the sum over the tets the walk crosses of
+// sig[tet] times the ray parameter spent in it.  The loop is locate_point's (record, scan_record, exit_parameter), the
+// step rule advance()'s.  Returns kRayTraced, kRayShadowed or kRayLost; crossings += the interior faces crossed.
+template <class Fetch>
+PTB_HD int detector_ray(const WalkParams &P, const double *sig, int32_t e, double x, double y, double z, double tx,
+                        double ty, double tz, double &tau_over_r, uint32_t &crossings, Fetch &&fetch) {
+  Ray r;
+  set_ray(P, r, x, y, z, tx, ty, tz);
+  r.e = e;
+  double s = 0.0;
+  for (;;) {
+    double rec[16];
+    fetch(r.e, rec);
+    ExitScan sc;
+    scan_record(rec, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
+    const double texit = exit_parameter(sc);
+    const bool reached = !(texit < 1.0);
+    const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
+    s += PTB_LDG(sig + r.e) * (tnew - r.tcur);
+    tau_over_r = s;
+    if (reached) return kRayTraced;
+    if (sc.nbr < 0) return kRayShadowed;  // graveyard outside the hull: re-entry across a concave notch is not followed
+    if (++r.iters >= P.max_iters) return kRayLost;
+    ++crossings;
+    r.e = sc.nbr;
+    r.tcur = tnew;
+  }
+}
+
+// g(x) = (1 - exp(-x)) / x, 1 at x = 0, through expm1 so that small x keeps its digits
+PTB_HD double ball_g(double x) { return x > 0.0 ? -expm1(-x) / x : 1.0; }
+
+// Event (x, y, z) in element e (internal id, -1 outside) with weight w, responses resp (nullptr: 1), score bin `bin`,
+// time t and speed v (read only with time bins), and pdf[0..D) the event's angular densities toward the detectors (per
+// steradian; nullptr: 1 / (4 pi)).  Every ray of an event checks the whole event, pdf row and R == 0 == r0 at every
+// detector included (kDetRejected), before whether it lies in the mesh (kDetOutside): rejection takes precedence, and
+// all the rays of an event share its outcome, which the kernels count once per event.  On a scoring outcome (traced,
+// inside r0) val[k] = the score of score k and *slot = its [time][bin][0][d] index (score k at slot + k D).
+// Shadowed and lost rays return val 0.  crossings += the interior faces the walk crossed.
+template <class Fetch>
+PTB_HD int detector_event(const WalkParams &W, const DetectorParams &P, int d, int32_t e, double x, double y, double z,
+                          double w, const double *resp, int32_t bin, double t, double v, const double *pdf,
+                          double *val, int64_t *slot, uint32_t &crossings, Fetch &&fetch) {
+  bool bad = !all_finite(x, y, z) || (P.nt > 0 && (!all_finite(t, 0.0, 0.0) || !(v > 0.0)));
+PTB_UNROLL
+  for (int k = 0; k < kMaxScores; ++k)
+    if (k < P.nscores) {
+      val[k] = w * (resp ? PTB_LDG(resp + k) : 1.0);
+      bad = bad || !all_finite(val[k], 0.0, 0.0);
+    }
+  if (pdf)
+    for (int q = 0; q < P.ndet; ++q) {
+      const double p = PTB_LDG(pdf + q);
+      bad = bad || !all_finite(p, 0.0, 0.0) || p < 0.0;
+    }
+  if (P.zero_r0 && !bad)
+    for (int q = 0; q < P.ndet; ++q) {
+      const double ax = PTB_LDG(P.pos + 3 * q) - x, ay = PTB_LDG(P.pos + 3 * q + 1) - y, az = PTB_LDG(P.pos + 3 * q + 2) - z;
+      bad = bad || (PTB_LDG(P.r0 + q) == 0.0 && sqrt(ax * ax + ay * ay + az * az) == 0.0);
+    }
+  if (bad) return kDetRejected;
+  if (e < 0) return kDetOutside;
+  const double pd = pdf ? PTB_LDG(pdf + d) : 0.25 / M_PI;
+  const double dx = PTB_LDG(P.pos + 3 * d), dy = PTB_LDG(P.pos + 3 * d + 1), dz = PTB_LDG(P.pos + 3 * d + 2);
+  const double ux = dx - x, uy = dy - y, uz = dz - z;
+  const double R = sqrt(ux * ux + uy * uy + uz * uz);
+  const double r0 = PTB_LDG(P.r0 + d);
+  const int j = P.nt > 0 ? time_bin(P.edges, P.nt, t + R / v) : 0;
+  if (bin < 0 || bin >= P.nbins || j < 0 || (P.nt > 0 && j >= P.nt)) return kDetSkipped;
+  const double *sig = P.sigma + (size_t)bin * (size_t)P.E;
+  double f;
+  int outcome;
+  if (R < r0) {
+    f = pd * 3.0 * ball_g(PTB_LDG(sig + e) * r0) / (r0 * r0);
+    outcome = kRayInsideR0;
+  } else {
+    double tr = 0.0;
+    outcome = detector_ray(W, sig, e, x, y, z, dx, dy, dz, tr, crossings, fetch);
+    f = outcome == kRayTraced ? pd * exp(-(tr * R)) / (R * R) : 0.0;
+  }
+PTB_UNROLL
+  for (int k = 0; k < kMaxScores; ++k)
+    if (k < P.nscores) val[k] *= f;
+  *slot = ((int64_t)j * P.nbins + bin) * (int64_t)P.nscores * P.ndet + d;
+  return outcome;
+}
+
 }  // namespace ptb

@@ -144,6 +144,23 @@ cudaError_t launch_collide_particles(const ParticleState *state, const int8_t *c
                                      const CollisionParams &c, const double *w, const double *resp, const int32_t *bins,
                                      const double *times, unsigned long long *counts, cudaStream_t stream);
 
+// detector_kernels.cu.  Point detectors (walk_core.cuh, detector_event), thread per (event, detector) ray, q = d n + i.
+// Located: event i at xyz[3i..], located as launch_locate does (n < 2^39 / D).  Particles: event i at particle i's stored
+// position and element, for every i < n with flagged[i] != 0.  w[i], pdf[i D + d] (nullptr: 1 / (4 pi)), resp[i nscores
+// + k] (nullptr: every response 1), bins[i] (nullptr: bin 0), times[i] and speeds[i] (read only when p.nt > 0).  The
+// scores go to p.tally, the outcomes to counts[kDetCounters].  Up to kDetSmemSlots slots are aggregated in shared memory.
+constexpr int kDetCountTraced = 0, kDetCountShadowed = 1, kDetCountLost = 2, kDetCountInsideR0 = 3,
+              kDetCountCrossings = 4, kDetCountOutside = 5, kDetCountRejected = 6, kDetCounters = 7;
+constexpr int64_t kDetSmemSlots = 2048;
+cudaError_t launch_detect_located(const LocateParams &l, const DetectorParams &p, const double *xyz, int64_t n,
+                                  const double *w, const double *pdf, const double *resp, const int32_t *bins,
+                                  const double *times, const double *speeds, unsigned long long *counts,
+                                  cudaStream_t stream);
+cudaError_t launch_detect_particles(const WalkParams &wp, const DetectorParams &p, const ParticleState *state,
+                                    const int8_t *flagged, int32_t n, const double *w, const double *pdf,
+                                    const double *resp, const int32_t *bins, const double *times, const double *speeds,
+                                    unsigned long long *counts, cudaStream_t stream);
+
 // stats_kernels.cu.  Batch statistics (batch_stats.cuh).  fold: (mean[i], m2[i]) <- welford_fold(x[i] / *divisor, nb)
 // for i < n, nb the number of batches including this one; the divisor is read on the device.
 cudaError_t launch_batch_fold(const double *x, double *mean, double *m2, int64_t n, const double *divisor, double nb,

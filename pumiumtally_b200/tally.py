@@ -78,6 +78,18 @@ C_API = {
     "pumitally_tally_collisions_at_particles_device": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "pumitally_get_collision_results": (C.c_int, [C.c_void_p, C.c_int32, _dp, C.c_int64]),
+    "pumitally_set_point_detectors": (C.c_int, [C.c_void_p, _dp, C.c_int32, _dp]),
+    "pumitally_get_point_detectors": (C.c_int32, [C.c_void_p]),
+    "pumitally_set_detector_cross_sections": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pumitally_tally_detectors": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, _dp, _dp, _ip, _dp, _dp]),
+    "pumitally_tally_detectors_device": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                  C.c_void_p, C.c_void_p]),
+    "pumitally_tally_detectors_at_particles": (C.c_int, [C.c_void_p, _bp, _dp, _dp, _dp, _ip, _dp, _dp, C.c_int32]),
+    "pumitally_tally_detectors_at_particles_device": (
+        C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                  C.c_int32, C.c_void_p]),
+    "pumitally_get_detector_results": (C.c_int, [C.c_void_p, C.c_int32, _dp, C.c_int64]),
     "pumitally_set_batch_statistics": (C.c_int, [C.c_void_p, C.c_int32]),
     "pumitally_end_batch": (C.c_int, [C.c_void_p]),
     "pumitally_get_batch_results": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_int64]),
@@ -545,12 +557,13 @@ class PumiTally:
     def collision_estimator(self) -> bool:
         return bool(self._L.pumitally_get_collision_estimator(self._h))
 
-    def _event_args(self, n, weights, responses, bins, times):
-        """Host event arrays as contiguous numpy arrays (None stays None), checked against n events."""
+    def _event_args(self, n, weights, responses, bins, times, pdf=None, speeds=None):
+        """Host event arrays as contiguous numpy arrays (None stays None), checked against n events: (arrays, pointers
+        to weights, responses, bins, times, pdf [n, point_detectors] and speeds)."""
         w = _host_f64(weights, "weights")
         if w.size != n:
             raise TypeError("weights must hold one value per event")
-        r = t = b = None
+        r = t = b = p = v = None
         if responses is not None:
             r = _host_f64(responses, "responses")
             if r.size != n * self.scores:
@@ -563,14 +576,22 @@ class PumiTally:
             b = np.ascontiguousarray(bins, dtype=np.int32).reshape(-1)
             if b.size != n:
                 raise TypeError("bins must hold one value per event")
-        ptr = lambda a, p: None if a is None else a.ctypes.data_as(p)  # noqa: E731
-        return (w, r, b, t), (ptr(w, _dp), ptr(r, _dp), ptr(b, _ip), ptr(t, _dp))
+        if pdf is not None:
+            p = _host_f64(pdf, "pdf")
+            if p.size != n * self.point_detectors:
+                raise TypeError(f"pdf must hold {self.point_detectors} values per event")
+        if speeds is not None:
+            v = _host_f64(speeds, "speeds")
+            if v.size != n:
+                raise TypeError("speeds must hold one value per event")
+        ptr = lambda a, q: None if a is None else a.ctypes.data_as(q)  # noqa: E731
+        return (w, r, b, t, p, v), (ptr(w, _dp), ptr(r, _dp), ptr(b, _ip), ptr(t, _dp), ptr(p, _dp), ptr(v, _dp))
 
     def tally_collisions(self, points, weights, responses=None, bins=None, times=None):
         """Collision events at ``points`` [n, 3], each located as locate() does: event i adds weights[i] *
         responses[i, k] to score k of its element, bin bins[i] and the time bin of times[i]."""
         p, n = self._points(points)
-        _keep, (w, r, b, t) = self._event_args(n, weights, responses, bins, times)
+        _keep, (w, r, b, t, _, _) = self._event_args(n, weights, responses, bins, times)
         if self._L.pumitally_tally_collisions(self._h, p.ctypes.data_as(_dp), n, w, r, b, t):
             raise RuntimeError("tally_collisions failed")
 
@@ -582,13 +603,16 @@ class PumiTally:
             raise TypeError(f"{what} must be a contiguous {dtype} CUDA tensor of {numel} values")
         return x.data_ptr()
 
-    def _device_event_args(self, n, weights, responses, bins, times, stream, device):
+    def _device_event_args(self, n, weights, responses, bins, times, stream, device, pdf=None, speeds=None):
+        """Device pointers of weights, responses, bins, times, pdf [n, point_detectors] and speeds, and the stream."""
         import torch
 
         args = (self._tensor_ptr(weights, torch.float64, n, "weights"),
                 self._tensor_ptr(responses, torch.float64, n * self.scores, "responses"),
                 self._tensor_ptr(bins, torch.int32, n, "bins"),
-                self._tensor_ptr(times, torch.float64, n, "times"))
+                self._tensor_ptr(times, torch.float64, n, "times"),
+                self._tensor_ptr(pdf, torch.float64, n * self.point_detectors, "pdf"),
+                self._tensor_ptr(speeds, torch.float64, n, "speeds"))
         if stream is None:
             stream = torch.cuda.current_stream(device).cuda_stream
         return args, stream
@@ -601,14 +625,14 @@ class PumiTally:
         if not (points.is_cuda and points.dtype == torch.float64 and points.is_contiguous() and points.numel() % 3 == 0):
             raise TypeError("points must be a contiguous float64 CUDA tensor of shape [n, 3]")
         n = points.numel() // 3
-        (w, r, b, t), stream = self._device_event_args(n, weights, responses, bins, times, stream, points.device)
+        (w, r, b, t, _, _), stream = self._device_event_args(n, weights, responses, bins, times, stream, points.device)
         if self._L.pumitally_tally_collisions_device(self._h, points.data_ptr(), n, w, r, b, t, stream):
             raise RuntimeError("tally_collisions_device failed")
 
     def tally_collisions_at_particles(self, collided, weights, responses=None, bins=None, times=None):
         """Collision events at the stored positions of the particles i with collided[i] != 0, in their elements."""
         c = np.ascontiguousarray(collided, dtype=np.int8).reshape(-1)
-        _keep, (w, r, b, t) = self._event_args(c.size, weights, responses, bins, times)
+        _keep, (w, r, b, t, _, _) = self._event_args(c.size, weights, responses, bins, times)
         if self._L.pumitally_tally_collisions_at_particles(self._h, c.ctypes.data_as(_bp), w, r, b, t, c.size):
             raise RuntimeError("tally_collisions_at_particles failed")
 
@@ -619,7 +643,8 @@ class PumiTally:
 
         n = self.num_particles
         c = self._tensor_ptr(collided, torch.int8, n, "collided")
-        (w, r, b, t), stream = self._device_event_args(n, weights, responses, bins, times, stream, collided.device)
+        (w, r, b, t, _, _), stream = self._device_event_args(n, weights, responses, bins, times, stream,
+                                                             collided.device)
         if self._L.pumitally_tally_collisions_at_particles_device(self._h, c, w, r, b, t, n, stream):
             raise RuntimeError("tally_collisions_at_particles_device failed")
 
@@ -631,6 +656,83 @@ class PumiTally:
         out = np.empty(shape)
         if self._L.pumitally_get_collision_results(self._h, int(kind), out.ctypes.data_as(_dp), out.size):
             raise RuntimeError(f"get_collision_results({kind}) failed")
+        return out
+
+    # ---- point detectors -----------------------------------------------------------
+    def set_point_detectors(self, points, r0):
+        """Next-event (point-detector) estimates at ``points`` [D, 3] (1 <= D <= 256, inside the mesh) with exclusion
+        radii ``r0`` [D] (finite, >= 0).  ``points`` None removes them.  Resets the tally and discards the folded
+        batches."""
+        if points is None:
+            rc = self._L.pumitally_set_point_detectors(self._h, None, 0, None)
+        else:
+            p = _host_f64(points, "points")
+            r = _host_f64(r0, "r0")
+            if p.size % 3 or r.size != p.size // 3:
+                raise TypeError("points must be [D, 3] and r0 [D]")
+            rc = self._L.pumitally_set_point_detectors(self._h, p.ctypes.data_as(_dp), p.size // 3, r.ctypes.data_as(_dp))
+        if rc:
+            raise ValueError("set_point_detectors failed")
+
+    @property
+    def point_detectors(self) -> int:
+        """Number of point detectors D, 0 without."""
+        return int(self._L.pumitally_get_point_detectors(self._h))
+
+    def set_detector_cross_sections(self, sigma):
+        """Sigma_t [nbins, num_elements] (caller's numbering, finite, >= 0) the detector rays are attenuated by; the
+        score bin is the energy group."""
+        s = _host_f64(sigma, "sigma")
+        if self._L.pumitally_set_detector_cross_sections(self._h, s.ctypes.data_as(_dp), s.size):
+            raise ValueError("set_detector_cross_sections failed")
+
+    def tally_detectors(self, points, weights, pdf=None, responses=None, bins=None, times=None, speeds=None):
+        """Events at ``points`` [n, 3], each located as locate() does, scored at every detector: pdf [n, D] per
+        steradian (None: isotropic), responses [n, nscores], bins [n], and with time bins times and speeds [n]."""
+        p, n = self._points(points)
+        _keep, (w, r, b, t, q, v) = self._event_args(n, weights, responses, bins, times, pdf, speeds)
+        if self._L.pumitally_tally_detectors(self._h, p.ctypes.data_as(_dp), n, w, q, r, b, t, v):
+            raise RuntimeError("tally_detectors failed")
+
+    def tally_detectors_device(self, points, weights, pdf=None, responses=None, bins=None, times=None, speeds=None,
+                               stream=None):
+        """tally_detectors() on CUDA tensors; enqueued on ``stream`` (default: the current torch stream)."""
+        import torch
+
+        if not (points.is_cuda and points.dtype == torch.float64 and points.is_contiguous() and points.numel() % 3 == 0):
+            raise TypeError("points must be a contiguous float64 CUDA tensor of shape [n, 3]")
+        n = points.numel() // 3
+        (w, r, b, t, q, v), stream = self._device_event_args(n, weights, responses, bins, times, stream, points.device,
+                                                             pdf, speeds)
+        if self._L.pumitally_tally_detectors_device(self._h, points.data_ptr(), n, w, q, r, b, t, v, stream):
+            raise RuntimeError("tally_detectors_device failed")
+
+    def tally_detectors_at_particles(self, flagged, weights, pdf=None, responses=None, bins=None, times=None,
+                                     speeds=None):
+        """Events at the stored positions of the particles i with flagged[i] != 0, in their elements."""
+        c = np.ascontiguousarray(flagged, dtype=np.int8).reshape(-1)
+        _keep, (w, r, b, t, q, v) = self._event_args(c.size, weights, responses, bins, times, pdf, speeds)
+        if self._L.pumitally_tally_detectors_at_particles(self._h, c.ctypes.data_as(_bp), w, q, r, b, t, v, c.size):
+            raise RuntimeError("tally_detectors_at_particles failed")
+
+    def tally_detectors_at_particles_device(self, flagged, weights, pdf=None, responses=None, bins=None, times=None,
+                                            speeds=None, stream=None):
+        """tally_detectors_at_particles() on CUDA tensors (flagged int8 [num_particles]); enqueued on ``stream``."""
+        import torch
+
+        n = self.num_particles
+        c = self._tensor_ptr(flagged, torch.int8, n, "flagged")
+        (w, r, b, t, q, v), stream = self._device_event_args(n, weights, responses, bins, times, stream,
+                                                             flagged.device, pdf, speeds)
+        if self._L.pumitally_tally_detectors_at_particles_device(self._h, c, w, q, r, b, t, v, n, stream):
+            raise RuntimeError("tally_detectors_at_particles_device failed")
+
+    def detector_results(self, kind=0):
+        """kind 0 the open tally / per-source divisor, 1 batch mean, 2 standard error, 3 relative error:
+        [ntime, nbins, nscores, D]."""
+        out = np.empty((max(self.time_bins, 1), self.score_bins, self.scores, self.point_detectors))
+        if self._L.pumitally_get_detector_results(self._h, int(kind), out.ctypes.data_as(_dp), out.size):
+            raise RuntimeError(f"get_detector_results({kind}) failed")
         return out
 
     # ---- batch statistics ----------------------------------------------------------

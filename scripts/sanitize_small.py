@@ -76,3 +76,27 @@ for step in range(2):
 np.testing.assert_allclose(e.flux_bins, want, rtol=1e-9, atol=1e-12)
 np.testing.assert_array_equal(e.elem_ids, orc.elem_ids)
 print("score bins ok", flush=True)
+
+# point detectors: located and at-particles calls, host and device, with the shared-memory slots (few) and the warp
+# aggregation (more slots than fit)
+for nbins, D, edges in ((1, 2, None), (3, 50, np.linspace(0.0, 16.0, 17))):
+    e = PumiTally.from_arrays(coords, t2v, wl.n)
+    e.set_option("chunk", 1024)
+    e.set_score_bins(nbins)
+    if edges is not None:
+        e.set_time_bins(edges)
+    rng = np.random.default_rng(D)
+    det = rng.uniform(0.5, 3.5, size=(D, 3))
+    e.set_point_detectors(det, np.full(D, 0.2))
+    e.set_detector_cross_sections(np.full((nbins, len(t2v)), 0.3))
+    e.CopyInitialPosition(wl.initial_positions().reshape(-1).copy())
+    pts = rng.uniform(-0.5, 5.5, size=(wl.n, 3))
+    kw = {} if edges is None else {"times": rng.uniform(0, 16, wl.n), "speeds": np.full(wl.n, 2.0)}
+    kw["bins"] = rng.integers(0, nbins, wl.n).astype(np.int32)
+    e.tally_detectors(pts, np.ones(wl.n), **kw)
+    e.tally_detectors_at_particles(np.ones(wl.n, dtype=np.int8), np.ones(wl.n), **kw)
+    dev = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in kw.items()}
+    e.tally_detectors_device(torch.from_numpy(pts).cuda(), torch.ones(wl.n, dtype=torch.float64, device="cuda"), **dev)
+    torch.cuda.synchronize()
+    assert np.isfinite(e.detector_results(0)).all()
+    print("detectors", nbins, D, "ok", flush=True)
