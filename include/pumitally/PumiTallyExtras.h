@@ -125,6 +125,12 @@ inline int TallyCollisionsAtParticles(const PumiTally &tally, const int8_t *coll
 inline int SetPointDetectors(const PumiTally &tally, const double *xyz, int32_t ndet, const double *r0) {
   return pumitally_set_point_detectors(engine_of(tally), xyz, ndet, r0);
 }
+// Detector void (see pumitally_set_detector_void in pumitally_c.h): on == 1 lets detector rays cross the space outside
+// the mesh as a void, so detectors and events may lie outside it and rays re-enter across concave parts of the hull.
+inline int SetDetectorVoid(const PumiTally &tally, bool on) {
+  return pumitally_set_detector_void(engine_of(tally), on ? 1 : 0);
+}
+inline bool GetDetectorVoid(const PumiTally &tally) { return pumitally_get_detector_void(engine_of(tally)) != 0; }
 inline int SetDetectorCrossSections(const PumiTally &tally, const double *sigma_t, int64_t n) {
   return pumitally_set_detector_cross_sections(engine_of(tally), sigma_t, n);
 }

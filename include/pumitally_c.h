@@ -419,8 +419,8 @@ int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *o
  * edge belongs to the bin above).  Results are laid out [time][bin][score][detector].
  * Ray outcomes: traced (the walk reaches the tet that contains the detector); shadowed (the ray leaves the mesh through
  * the hull first and scores 0: outside the mesh counts as a void of zero importance, which is exact for rays that stay
- * inside the mesh; re-entry across a concave part of the hull is NOT followed); lost (stopped by the option
- * "max_iters"; scores 0).
+ * inside the mesh; with the detector void off, re-entry across a concave part of the hull is NOT followed: see
+ * pumitally_set_detector_void below for the mode that follows it); lost (stopped by the option "max_iters"; scores 0).
  * Event outcomes, checked in this order and shared by all the event's rays: rejected (a non-finite coordinate, weight *
  * response, time or pdf value, a negative pdf value, a speed not > 0 with time bins, or R == 0 at a detector with
  * r0_d == 0); outside (a located event outside the mesh).  Then per ray, skipped (a bin outside [0, nbins) or an
@@ -450,6 +450,35 @@ int pumitally_get_collision_results(pumitally_engine *e, int32_t kind, double *o
  * keeps its version and bytes. */
 int pumitally_set_point_detectors(pumitally_engine *e, const double *xyz, int32_t ndet, const double *r0);
 int32_t pumitally_get_point_detectors(const pumitally_engine *e);
+
+/* ---- additive: the detector void (point-detector rays through the space outside the mesh) ----
+ * pumitally_set_detector_void(e, on), on 0 or 1 (default 0), treats the space outside the mesh as a void (Sigma_t = 0)
+ * that the detector rays cross.  pumitally_get_detector_void and the read-only option "detector_void" return the mode.
+ * The call may come before or after pumitally_set_point_detectors and is refused after pumitally_comm_init.  Setting the
+ * mode the engine has changes nothing; switching resets the tally and discards the folded batches.  Switching off while
+ * a detector lies outside the mesh is refused and changes nothing.  Anything but 0 or 1 is refused.
+ * With the mode on:
+ * - tau is the sum over the tets of Sigma_t[b][tet] times the length of the segment event -> detector inside the tet,
+ *   over the whole segment; its parts outside the mesh add 0.  A ray that leaves through the hull is followed to where
+ *   it enters the mesh again (across a notch, a gap or a cavity), so no ray is shadowed.
+ * - Detector positions may be any finite point: inside the mesh, in a notch or cavity, or outside the bounding box.
+ *   They are still located, so a detector inside keeps its element.
+ * - A located event outside the mesh (pumitally_tally_detectors) is traced from where it is and is not counted as
+ *   outside ("detector_events_outside" stays 0).  Inside r0 such an event scores the ball
+ *   formula with Sigma = 0: s_k = w r[k] p 3 / r0_d^2.
+ * - Ray outcomes are traced, lost and inside r0; the four ray counters add up to D times the events not rejected, less
+ *   the skipped rays.  Every entry into the mesh counts as one iteration against "max_iters", so every ray is bounded.
+ * - The read-only counter "detector_hull_entries" counts the rays' entries into the mesh through the hull: the first
+ *   entry of an outside event's ray and every re-entry after a hull exit (0 with the mode off; pumitally_reset_tally
+ *   zeroes it).  On a convex hull a ray that has left the mesh cannot come back, so only outside events enter.
+ * The entry search runs over lists of hull tets per seed-grid cell, built and uploaded at the mode's first detector
+ * call ("detector_hull_candidates" returns their length).  With the mode off every result, counter, refusal and
+ * checkpoint byte is what it was without the call.  A checkpoint of an engine with detectors and the mode on is written
+ * as format version 4 (version 3's header, and the hull-entry counter with the others); the fingerprint holds the mode
+ * while detectors are set, and a load or merge across the two settings is refused with a message that names the
+ * detector void. */
+int pumitally_set_detector_void(pumitally_engine *e, int32_t on);
+int32_t pumitally_get_detector_void(const pumitally_engine *e);
 int pumitally_set_detector_cross_sections(pumitally_engine *e, const double *sigma_t, int64_t n);
 int pumitally_tally_detectors(pumitally_engine *e, const double *xyz, int64_t nevents, const double *weights,
                               const double *pdf, const double *responses, const int32_t *bins, const double *times,

@@ -277,6 +277,12 @@ int pumitally_set_point_detectors(pumitally_engine *e, const double *xyz, int32_
 int32_t pumitally_get_point_detectors(const pumitally_engine *e) {
   return e ? int32_t(pumitally_get_option(e, "point_detectors")) : 0;
 }
+int pumitally_set_detector_void(pumitally_engine *e, int32_t on) {
+  return guarded(e, [&](ptb::Engine &g) { return g.set_detector_void(on); });
+}
+int32_t pumitally_get_detector_void(const pumitally_engine *e) {
+  return e ? int32_t(pumitally_get_option(e, "detector_void")) : 0;
+}
 int pumitally_set_detector_cross_sections(pumitally_engine *e, const double *sigma_t, int64_t n) {
   return guarded(e, [&](ptb::Engine &g) { return g.set_detector_cross_sections(sigma_t, n); });
 }

@@ -192,6 +192,7 @@ const char *fingerprint_mismatch(const Fingerprint &a, const Fingerprint &b, boo
   for (size_t j = 0; j < a.det_r0.size(); ++j)
     if (bits_of(a.det_r0[j]) != bits_of(b.det_r0[j])) return "point-detector exclusion radii (set_point_detectors)";
   if (a.sigma_crc != b.sigma_crc) return "detector cross-section table (set_detector_cross_sections)";
+  if (a.det_void != b.det_void) return "detector void (set_detector_void)";
   return nullptr;
 }
 
@@ -239,7 +240,7 @@ std::vector<std::pair<uint32_t, uint64_t>> sections_of(const Header &h) {
   }
   if (h.det_len && h.open) {
     s.emplace_back(kDetOpen, 8 * h.det_len);
-    s.emplace_back(kDetCounts, 8 * kDetCountWords);
+    s.emplace_back(kDetCounts, 8 * uint64_t(h.det_words));
   }
   if (h.det_len && h.stats_len) {
     s.emplace_back(kDetMean, 8 * h.det_len);
@@ -261,7 +262,10 @@ bool Writer::put(const void *p, size_t n) {
 
 bool Writer::begin(const Header &h, const Fingerprint &f) {
   std::vector<uint8_t> b(kMagic, kMagic + 8);
-  put_le(b, !f.det_r0.empty() ? kVersionDetectors : f.mu_edges.empty() ? kVersion : kVersionCosines, 4);
+  put_le(b, !f.det_r0.empty() ? (f.det_void ? kVersionDetectorVoid : kVersionDetectors)
+            : f.mu_edges.empty() ? kVersion
+                                 : kVersionCosines,
+         4);
   put_le(b, kEndianMarker, 4);
   put_header(b, h, f);
   put_le(b, crc32(b.data(), b.size()), 4);
@@ -316,11 +320,13 @@ bool Reader::begin(Header *h, Fingerprint *f) {
     return false;
   }
   const uint64_t version = get_le(b.data() + 8, 4);
-  if (version != kVersion && version != kVersionCosines && version != kVersionDetectors) {
+  if (version != kVersion && version != kVersionCosines && version != kVersionDetectors &&
+      version != kVersionDetectorVoid) {
     err_ = "unsupported format version " + std::to_string(version);
     return false;
   }
-  const bool cosines = version == kVersionCosines, detectors = version == kVersionDetectors;
+  const bool cosines = version == kVersionCosines, det_void = version == kVersionDetectorVoid,
+             detectors = version == kVersionDetectors || det_void;
   if (get_le(b.data() + 12, 4) != kEndianMarker) {
     err_ = "wrong endianness marker";
     return false;
@@ -363,11 +369,14 @@ bool Reader::begin(Header *h, Fingerprint *f) {
   }
   if (crc32(b.data(), b.size() - 4) != uint32_t(get_le(b.data() + b.size() - 4, 4))) {
     err_ = cosines ? "corrupt version 2 header or fingerprint (CRC mismatch)"
+           : det_void  ? "corrupt version 4 header or fingerprint (CRC mismatch)"
            : detectors ? "corrupt version 3 header or fingerprint (CRC mismatch)"
                        : "corrupt header or fingerprint (CRC mismatch)";
     return false;
   }
   get_header(b.data() + 16, h, f, cosines, detectors);
+  f->det_void = det_void ? 1 : 0;
+  h->det_words = uint32_t(det_void ? kDetCountWordsVoid : kDetCountWords);
   if (h->open > 1 || (!h->open && h->open_len) || h->batches < 0 || h->open_len > kMaxLen ||
       h->stats_len > kMaxLen || h->region_len > kMaxLen || h->det_len > kMaxLen || (detectors && !h->det_len)) {
     err_ = "corrupt header (declared lengths)";

@@ -31,6 +31,10 @@ constexpr uint32_t kVersionCosines = 2;
 // (count D, positions [3D], exclusion radii [D]), the CRC-32 of the cross-section table and det_len (u64).  Only a file
 // whose fingerprint holds detectors is written as version 3.
 constexpr uint32_t kVersionDetectors = 3;
+// Version 4: point detectors with the detector void (pumitally_set_detector_void) on.  The header is version 3's; the
+// version itself records the mode, and kDetCounts holds kDetCountWordsVoid counters (the hull entries last).  Every
+// file saved with the mode off keeps its version and bytes.
+constexpr uint32_t kVersionDetectorVoid = 4;
 
 // 64-bit hash of a byte string (not cryptographic: it tells configurations apart, it does not authenticate them).
 // Chainable: hash64(b, nb, hash64(a, na)) hashes a then b.
@@ -56,6 +60,7 @@ struct Fingerprint {
   std::vector<double> mu_edges;  // cosine-bin edges of the face currents (empty: none), compared bit for bit
   std::vector<double> det_xyz, det_r0;  // point detectors (empty: none), compared bit for bit
   uint32_t sigma_crc = 0;               // CRC-32 of the detector cross-section table as uploaded (0: no table)
+  uint32_t det_void = 0;                // the detector void is on (with detectors only: version 4)
 };
 
 // The name of the first field in which `file` differs from `engine`, nullptr when they agree.  ignore_norm_value:
@@ -68,7 +73,8 @@ struct Header {
   uint64_t open_len = 0;    // doubles of the open tally (0 without one)
   uint64_t stats_len = 0;   // doubles of each of kMean and kM2 (0 without statistics)
   uint64_t region_len = 0;  // doubles of each of kRegionMean and kRegionM2 (0 without region statistics)
-  uint64_t det_len = 0;     // doubles of the detector tally (version 3 only; 0 without detectors)
+  uint64_t det_len = 0;     // doubles of the detector tally (versions 3 and 4; 0 without detectors)
+  uint32_t det_words = 7;   // 64-bit words of kDetCounts: kDetCountWords, kDetCountWordsVoid in version 4 (not stored)
 };
 
 enum SectionId : uint32_t {
@@ -84,6 +90,7 @@ enum SectionId : uint32_t {
   kDetM2 = 10,        // [det_len] (with kMean)
 };
 constexpr size_t kDetCountWords = 7;
+constexpr size_t kDetCountWordsVoid = 8;
 
 // The small state of the open batch, as 64-bit words in this order.
 struct OpenScalars {

@@ -85,8 +85,8 @@ Engine::Engine(HostMesh &&mesh, int32_t num_particles, int device)
   dev_alloc(&d_stats_, 1, "stats");
   dev_alloc(&d_coll_counts_, 3, "collision counters");
   cuda_or_throw(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)), "memset");
-  dev_alloc(&d_det_counts_, kDetCounters, "detector counters");
-  cuda_or_throw(cudaMemset(d_det_counts_, 0, kDetCounters * sizeof(unsigned long long)), "memset");
+  dev_alloc(&d_det_counts_, kDetCountersVoid, "detector counters");
+  cuda_or_throw(cudaMemset(d_det_counts_, 0, kDetCountersVoid * sizeof(unsigned long long)), "memset");
   dev_alloc(&d_initial_weight_, 1, "initial weight");
   cuda_or_throw(cudaMemset(d_initial_weight_, 0, sizeof(double)), "memset");
   dev_alloc(&d_batch_div_, 2, "batch divisor");
@@ -197,6 +197,7 @@ Engine::~Engine() {
   cudaFree(d_pcell_); cudaFree(d_order_); cudaFree(d_cell_count_); cudaFree(d_cell_sums_);
   cudaFree(d_work_count_);
   cudaFree(d_cand_off_); cudaFree(d_cand_);
+  cudaFree(d_hull_off_); cudaFree(d_hull_tets_);
   cudaFree(d_arena_);
   cudaFree(d_eval_vals_); cudaFree(d_eval_grads_); cudaFree(d_eval_cen_);
   cudaFree(d_coll_counts_);
@@ -1627,7 +1628,7 @@ int Engine::reset_tally() {
   scored_moves_ = 0;
   PTB_CUDA_OK(cudaMemset(d_stats_, 0, sizeof(DeviceStats)));
   PTB_CUDA_OK(cudaMemset(d_coll_counts_, 0, 3 * sizeof(unsigned long long)));
-  PTB_CUDA_OK(cudaMemset(d_det_counts_, 0, kDetCounters * sizeof(unsigned long long)));
+  PTB_CUDA_OK(cudaMemset(d_det_counts_, 0, kDetCountersVoid * sizeof(unsigned long long)));
   if (ndet_ > 0) PTB_CUDA_OK(cudaMemset(d_det_, 0, 2 * det_len() * sizeof(double)));
   det_global_valid_ = false;
   flux_global_valid_ = flux_owned_only_ = eval_valid_ = tallied_ = false;
@@ -1708,13 +1709,15 @@ int64_t Engine::get_option(const std::string &name) const {
     return int64_t(c[name == "collisions" ? 0 : name == "collisions_outside" ? 1 : 2]);
   }
   if (name == "point_detectors") return ndet_;
+  if (name == "detector_void") return det_void_ ? 1 : 0;
+  if (name == "detector_hull_candidates") return int64_t(hull_entries_);  // entries of the void's hull-tet lists
   // detector rays and events since the last reset (kDetCount* in walk_kernels.hpp)
-  static const char *const kDetNames[kDetCounters] = {"detector_rays", "detector_rays_shadowed", "detector_rays_lost",
-                                                      "detector_inside_r0", "detector_crossings",
-                                                      "detector_events_outside", "detector_events_rejected"};
-  for (int c = 0; c < kDetCounters; ++c)
+  static const char *const kDetNames[kDetCountersVoid] = {
+      "detector_rays",       "detector_rays_shadowed",  "detector_rays_lost",       "detector_inside_r0",
+      "detector_crossings",  "detector_events_outside", "detector_events_rejected", "detector_hull_entries"};
+  for (int c = 0; c < kDetCountersVoid; ++c)
     if (name == kDetNames[c]) {
-      unsigned long long v[kDetCounters] = {};
+      unsigned long long v[kDetCountersVoid] = {};
       if (cudaSetDevice(device_) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
           cudaMemcpy(v, d_det_counts_, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) {
         cudaGetLastError();
@@ -2044,6 +2047,35 @@ int Engine::ensure_candidates() {
   return 0;
 }
 
+// The hull-tet lists of the detector void over the seed grid, padded as the point-location lists are.
+int Engine::ensure_hull_grid() {
+  if (hull_ready_) return 0;
+  std::vector<int64_t> off;
+  std::vector<int32_t> tets;
+  HullGrid h = hull_grid(mesh_, grid_, kLocateBand * mesh_extent(mesh_), &off, &tets);
+  int64_t *doff = nullptr;
+  int32_t *dtets = nullptr;
+  if (cudaMalloc(reinterpret_cast<void **>(&doff), off.size() * sizeof(int64_t)) != cudaSuccess ||
+      cudaMalloc(reinterpret_cast<void **>(&dtets), std::max<size_t>(tets.size(), 1) * sizeof(int32_t)) != cudaSuccess ||
+      cudaMemcpy(doff, off.data(), off.size() * sizeof(int64_t), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(dtets, tets.data(), tets.size() * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) {
+    const cudaError_t err = cudaGetLastError();
+    cudaFree(doff);
+    cudaFree(dtets);
+    fprintf(stderr, "[pumitally] ERROR: no device memory for the hull grid of the detector void (%s)\n",
+            cudaGetErrorString(err));
+    return 1;
+  }
+  h.off = doff;
+  h.tets = dtets;
+  hull_ = h;
+  d_hull_off_ = doff;
+  d_hull_tets_ = dtets;
+  hull_entries_ = tets.size();
+  hull_ready_ = true;
+  return 0;
+}
+
 int Engine::ensure_arena(size_t bytes) {
   if (bytes <= arena_bytes_) return 0;
   cudaFree(d_arena_);
@@ -2334,7 +2366,10 @@ int Engine::set_point_detectors(const double *xyz, int32_t ndet, const double *r
     PTB_CUDA_OK(cudaMemcpyAsync(elem.data(), de, size_t(ndet) * sizeof(int32_t), cudaMemcpyDeviceToHost, compute_));
     PTB_CUDA_OK(cudaStreamSynchronize(compute_));
     for (int32_t d = 0; d < ndet; ++d)
-      if (elem[size_t(d)] < 0) why = "every detector must lie inside the mesh, with finite coordinates";
+      if (!std::isfinite(xyz[3 * d]) || !std::isfinite(xyz[3 * d + 1]) || !std::isfinite(xyz[3 * d + 2]))
+        why = "every detector must have finite coordinates";
+      else if (elem[size_t(d)] < 0 && !det_void_)
+        why = "every detector must lie inside the mesh (or the detector void be on: set_detector_void)";
   }
   if (why) {
     fprintf(stderr, "[pumitally] ERROR: set_point_detectors: %s\n", why);
@@ -2372,6 +2407,24 @@ int Engine::set_point_detectors(const double *xyz, int32_t ndet, const double *r
   det_xyz_.assign(xyz, xyz + 3 * size_t(ndet_));
   det_r0_.assign(r0, r0 + size_t(ndet_));
   det_elem_ = remove ? std::vector<int32_t>() : elem;
+  return reset_tally();
+}
+
+int Engine::set_detector_void(int32_t on) {
+  const bool outside = std::count(det_elem_.begin(), det_elem_.end(), -1) > 0;
+  const char *why = nccl_comm_                  ? "after comm_init (the exchange buffers are sized by then)"
+                    : (on != 0 && on != 1)      ? "on must be 0 or 1"
+                    : (on == 0 && det_void_ && outside)
+                        ? "a point detector lies outside the mesh (move or remove it first: set_point_detectors)"
+                        : nullptr;
+  if (why) {
+    fprintf(stderr, "[pumitally] ERROR: set_detector_void: %s\n", why);
+    return 1;
+  }
+  if ((on != 0) == det_void_) return 0;
+  if (synchronize()) return 1;
+  if (batch_stats_ && alloc_stats(reported_len())) return 1;  // discards the folded batches, as every set_* call does
+  det_void_ = on != 0;
   return reset_tally();
 }
 
@@ -2434,7 +2487,7 @@ int Engine::detect_located_setup(const double *xyz, int64_t n, const double *w, 
   if (detector_refused(r, t, v) || n < 0 || (n > 0 && (!xyz || !w))) return 1;
   if (n == 0) return -1;
   PTB_CUDA_OK(cudaSetDevice(device_));
-  if (ensure_candidates() || ensure_arena(arena)) return 1;
+  if (ensure_candidates() || (det_void_ && ensure_hull_grid()) || ensure_arena(arena)) return 1;
   det_global_valid_ = false;
   tallied_ = true;  // a checkpoint now holds the open batch, the detector tally with it
   return 0;
@@ -2451,7 +2504,7 @@ cudaError_t Engine::enqueue_detect_located(const double *xyz, int64_t n, const d
     if (cudaError_t e = launch_detect_located(l, p, xyz + 3 * b, std::min(per, n - b), w + b,
                                               pdf ? pdf + D * size_t(b) : nullptr, r ? r + S * size_t(b) : nullptr,
                                               bins ? bins + b : nullptr, ntime_ > 0 ? t + b : nullptr,
-                                              ntime_ > 0 ? v + b : nullptr, d_det_counts_, stream))
+                                              ntime_ > 0 ? v + b : nullptr, d_det_counts_, stream, hull_grid_params()))
       return e;
   return cudaSuccess;
 }
@@ -2486,7 +2539,8 @@ int Engine::detect_particles_setup(const int8_t *flagged, const double *w, const
   }
   if (n == 0) return -1;
   PTB_CUDA_OK(cudaSetDevice(device_));
-  if (ensure_arena(arena) || follow_last_stream(stream)) return 1;  // reads the particle state the last move wrote
+  // reads the particle state the last move wrote
+  if ((det_void_ && ensure_hull_grid()) || ensure_arena(arena) || follow_last_stream(stream)) return 1;
   det_global_valid_ = false;
   tallied_ = true;
   return 0;
@@ -2504,7 +2558,8 @@ int Engine::tally_detectors_at_particles(const int8_t *flagged, const double *we
       [&](int64_t b, int64_t cnt, const int8_t *c, const double *w, const double *p, const double *r, const double *t,
           const double *v, const int32_t *bn) {
         return launch_detect_particles(wp, detector_params(), d_state_ + b, c, int32_t(cnt), w, p, r, bn,
-                                       ntime_ > 0 ? t : nullptr, ntime_ > 0 ? v : nullptr, d_det_counts_, compute_);
+                                       ntime_ > 0 ? t : nullptr, ntime_ > 0 ? v : nullptr, d_det_counts_, compute_,
+                                       hull_grid_params());
       },
       stage(flagged), stage(weights), stage(pdf, size_t(ndet_)), stage(responses, size_t(nscores_)),
       stage(ntime_ > 0 ? times : nullptr), stage(ntime_ > 0 ? speeds : nullptr), stage(bins));
@@ -2521,7 +2576,7 @@ int Engine::tally_detectors_at_particles_device(const int8_t *d_flagged, const d
   wp.cx = mesh_.center[0]; wp.cy = mesh_.center[1]; wp.cz = mesh_.center[2];
   PTB_CUDA_OK(launch_detect_particles(wp, detector_params(), d_state_, d_flagged, n, d_weights, d_pdf, d_responses,
                                       d_bins, ntime_ > 0 ? d_times : nullptr, ntime_ > 0 ? d_speeds : nullptr,
-                                      d_det_counts_, stream));
+                                      d_det_counts_, stream, hull_grid_params()));
   return 0;
 }
 
@@ -3426,6 +3481,7 @@ ckpt::Fingerprint Engine::fingerprint() {
   f.det_xyz = det_xyz_;
   f.det_r0 = det_r0_;
   f.sigma_crc = ndet_ > 0 && d_sigma_ ? sigma_crc_ : 0;
+  f.det_void = det_void_ && ndet_ > 0 ? 1 : 0;  // without detectors the mode shapes nothing a file holds
   return f;
 }
 
@@ -3445,6 +3501,7 @@ int Engine::save_checkpoint(const std::string &path) {
   h.region_len = RL;
   const size_t DL = det_len();
   h.det_len = DL;
+  h.det_words = uint32_t(f.det_void ? ckpt::kDetCountWordsVoid : ckpt::kDetCountWords);
   std::vector<uint8_t> scalars, det_counts;
   if (tallied_) {
     ckpt::OpenScalars s;
@@ -3464,10 +3521,10 @@ int Engine::save_checkpoint(const std::string &path) {
     s.scored_moves = scored_moves_;
     scalars = ckpt::pack_open_scalars(s);
     if (DL) {
-      unsigned long long dc[kDetCounters];
+      unsigned long long dc[kDetCountersVoid];  // the hull entries (the last) only with the detector void on
       PTB_CUDA_OK(cudaMemcpy(dc, d_det_counts_, sizeof(dc), cudaMemcpyDeviceToHost));
-      det_counts.resize(sizeof(dc));
-      std::memcpy(det_counts.data(), dc, sizeof(dc));  // (little-endian hosts only, as the rest of the engine)
+      det_counts.resize(8 * size_t(h.det_words));
+      std::memcpy(det_counts.data(), dc, det_counts.size());  // (little-endian hosts only, as the rest of the engine)
     }
   }
   // the arrays of the sections, in file order (nullptr: zeros -- region statistics before the first end_batch)
@@ -3625,7 +3682,7 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     release();
     return refuse("no device memory for a second copy of the checkpoint's arrays");
   }
-  std::vector<uint8_t> scalars(8 * ckpt::kOpenScalarWords), det_counts(8 * ckpt::kDetCountWords);
+  std::vector<uint8_t> scalars(8 * ckpt::kOpenScalarWords), det_counts(8 * size_t(h.det_words));
   struct Dst { uint32_t id; double *d; uint64_t bytes; };
   std::vector<Dst> dst;
   if (h.open) {
@@ -3749,8 +3806,8 @@ int Engine::read_checkpoint(const std::string &path, bool merge) {
     d_det_ = ndet;
     ndet = nullptr;
     det_global_valid_ = false;
-    unsigned long long dc[kDetCounters] = {};
-    if (h.open) std::memcpy(dc, det_counts.data(), sizeof(dc));
+    unsigned long long dc[kDetCountersVoid] = {};
+    if (h.open) std::memcpy(dc, det_counts.data(), det_counts.size());
     PTB_CUDA_OK(cudaMemcpy(d_det_counts_, dc, sizeof(dc), cudaMemcpyHostToDevice));
   }
   batches_ = h.batches;

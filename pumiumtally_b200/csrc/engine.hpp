@@ -137,11 +137,18 @@ class Engine {
   int get_face_current_results(int32_t direction, int32_t kind, double *out, int64_t n);
   // the outgoing current summed over every hull face, kinds as above; n == ntime * nbins * C, [time][bin][cosine]
   int get_leakage(int32_t kind, double *out, int64_t n);
-  // Point detectors (walk_core.cuh, detector_event): D = ndet detectors at xyz[3D] (AoS, each inside the mesh) with
+  // Point detectors (walk_core.cuh, detector_event): D = ndet detectors at xyz[3D] (AoS, each inside the mesh, or
+// anywhere finite with the detector void on) with
   // exclusion radii r0[D] (finite, >= 0), 1 <= D <= kMaxDetectors; xyz == r0 == nullptr with ndet == 0 removes them.
   // Resets the tally, discards the folded batches; before comm_init.  Anything else is refused and changes nothing.
   int set_point_detectors(const double *xyz, int32_t ndet, const double *r0);
   int32_t point_detectors() const { return ndet_; }
+  // Detector void (walk_core.cuh, detector_ray): on == 1 treats the space outside the mesh as a void the rays cross, so
+  // detectors may lie anywhere, events outside the mesh are traced and rays re-enter across concave parts of the hull.
+  // Setting the current mode changes nothing; switching resets the tally and discards the folded batches; switching
+  // off while a detector lies outside the mesh is refused; before comm_init.
+  int set_detector_void(int32_t on);
+  int32_t detector_void() const { return det_void_ ? 1 : 0; }
   // Sigma_t [bin][element] in the caller's numbering, n == nbins * E, finite and >= 0; kept until set_score_bins changes
   // nbins.  Resets nothing.  Detector calls are refused without it.
   int set_detector_cross_sections(const double *sigma_t, int64_t n);
@@ -399,7 +406,16 @@ class Engine {
   // [2 * det_len()]: the batch mean and M2
   double *d_det_ = nullptr;
   bool det_global_valid_ = false;                  // the second block holds the exchanged sum of the first
-  unsigned long long *d_det_counts_ = nullptr;     // [kDetCounters] since the last reset
+  unsigned long long *d_det_counts_ = nullptr;     // [kDetCountersVoid] since the last reset
+  bool det_void_ = false;                          // the detector void (set_detector_void)
+  // the hull grid of the detector void: hull-tet lists of the seed-grid cells, uploaded at the mode's first use
+  HullGrid hull_{};
+  int64_t *d_hull_off_ = nullptr;
+  int32_t *d_hull_tets_ = nullptr;
+  size_t hull_entries_ = 0;                        // entries of the hull-tet lists
+  bool hull_ready_ = false;
+  int ensure_hull_grid();
+  const HullGrid *hull_grid_params() const { return det_void_ ? &hull_ : nullptr; }  // nullptr: the mode is off
   size_t det_len() const { return nslices() * size_t(nbins_) * size_t(nscores_) * size_t(ndet_); }
   int alloc_detectors(size_t len, bool stats, double **out);  // len doubles per block, zeroed; nothing changes on failure
   DetectorParams detector_params() const;

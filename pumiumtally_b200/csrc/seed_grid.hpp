@@ -64,8 +64,9 @@ inline std::vector<int32_t> morton_cell_ranks(const SeedGrid &g) {
 // Candidate tets of every grid cell for point location on a non-convex hull (locate_point in walk_core.cuh): CSR
 // lists, off[c] .. off[c + 1] of `tets` hold the internal ids of the tets whose bounding box, widened by `pad`,
 // overlaps cell c (closed intervals).  A tet that contains a point of the cell is therefore in the cell's list.
+// keep (optional, [ntets]): only the tets e with keep[e] != 0 are listed (the hull tets of the detector void).
 inline void cell_candidates(const HostMesh &m, const SeedGrid &g, double pad, std::vector<int64_t> *off,
-                            std::vector<int32_t> *tets) {
+                            std::vector<int32_t> *tets, const uint8_t *keep = nullptr) {
   const int64_t ncell = int64_t(g.nx) * g.ny * g.nz;
   const int n[3] = {g.nx, g.ny, g.nz};
   const double lo[3] = {g.x0, g.y0, g.z0};
@@ -88,6 +89,7 @@ inline void cell_candidates(const HostMesh &m, const SeedGrid &g, double pad, st
   };
   off->assign(size_t(ncell) + 1, 0);
   for (int64_t e = 0; e < m.ntets; ++e) {
+    if (keep && !keep[e]) continue;
     int a[3], b[3];
     range(e, a, b);
     for (int z = a[2]; z <= b[2]; ++z)
@@ -98,12 +100,39 @@ inline void cell_candidates(const HostMesh &m, const SeedGrid &g, double pad, st
   tets->resize(size_t((*off)[size_t(ncell)]));
   std::vector<int64_t> cur(off->begin(), off->end() - 1);
   for (int64_t e = 0; e < m.ntets; ++e) {
+    if (keep && !keep[e]) continue;
     int a[3], b[3];
     range(e, a, b);
     for (int z = a[2]; z <= b[2]; ++z)
       for (int y = a[1]; y <= b[1]; ++y)
         for (int x = a[0]; x <= b[0]; ++x) (*tets)[size_t(cur[size_t((int64_t(z) * g.ny + y) * g.nx + x)]++)] = int32_t(e);
   }
+}
+
+// keep[e] = 1 for the hull tets (a face on the hull), the candidates of the detector void's entry search
+// (walk_core.cuh, hull_entry).
+inline std::vector<uint8_t> hull_tets(const HostMesh &m) {
+  std::vector<uint8_t> keep(size_t(m.ntets), 0);
+  for (int64_t e = 0; e < m.ntets; ++e)
+    for (int f = 0; f < 4; ++f) keep[size_t(e)] |= m.t2t[size_t(4 * e + f)] < 0 ? 1 : 0;
+  return keep;
+}
+
+// The hull grid of the detector void over the seed grid g, for a mesh centred at m.center: the CSR lists of hull tets
+// (pad as the point-location lists use) are returned in off and tets; the grid's device pointers are the caller's.
+inline HullGrid hull_grid(const HostMesh &m, const SeedGrid &g, double pad, std::vector<int64_t> *off,
+                          std::vector<int32_t> *tets) {
+  const std::vector<uint8_t> keep = hull_tets(m);
+  cell_candidates(m, g, pad, off, tets, keep.data());
+  HullGrid h{};
+  h.g = g;
+  h.g.cell_tet = nullptr;
+  h.g.cell_rank = nullptr;
+  h.ox = g.x0 - m.center[0];
+  h.oy = g.y0 - m.center[1];
+  h.oz = g.z0 - m.center[2];
+  h.convex = m.hull_convex ? 1 : 0;
+  return h;
 }
 
 }  // namespace ptb

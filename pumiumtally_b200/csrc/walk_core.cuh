@@ -974,32 +974,170 @@ struct DetectorParams {
   int64_t E;
 };
 
+// ---- detector void: the space outside the mesh is a void the rays cross (pumitally_set_detector_void) -------------
+// With the void on, a ray that leaves the mesh through the hull is not shadowed: hull_entry() finds the first tet it
+// enters again, and a ray from an event outside the mesh starts there.  The candidates are the hull tets (a tet with a
+// face on the hull) of every seed-grid cell, CSR lists built by cell_candidates() (seed_grid.hpp) with a hull filter.
+struct HullGrid {
+  SeedGrid g;           // the seed grid's geometry (h, inv_h, nx, ny, nz); cell_tet is not read
+  double ox, oy, oz;    // the grid's low corner (x0, y0, z0) in mesh-centred coordinates, as the rays' origins are
+  const int64_t *off;   // [ncell + 1] hull-tet list of each cell
+  const int32_t *tets;  // internal tet ids
+  int32_t convex;       // HostMesh::hull_convex: a ray that has left the mesh cannot come back
+};
+
+// Entry parameter of the ray into the record's tet: the largest num / den over the faces the ray enters through (den <
+// -tol, with num and den as scan_face forms them), -inf when there is none, +inf when a face parallel to the ray within
+// tol has the ray outside its plane (num < 0).
+PTB_HD double entry_parameter(const double (&r)[16], const Ray &ray) {
+  const double tol = kParallelTol * (fabs(ray.ux) + fabs(ray.uy) + fabs(ray.uz));
+  double tin = -__builtin_huge_val();
+PTB_UNROLL
+  for (int f = 0; f < 4; ++f) {
+    const double nx = r[4 * f], ny = r[4 * f + 1], nz = r[4 * f + 2];
+    const double den = nx * ray.ux + ny * ray.uy + nz * ray.uz;
+    const double num = r[4 * f + 3] - (nx * ray.ox + ny * ray.oy + nz * ray.oz);
+    if (den < -tol) tin = fmax(tin, num / den);
+    else if (!(den > tol) && num < 0.0) tin = __builtin_huge_val();
+  }
+  return tin;
+}
+
+// The first tet the ray enters at or after tcur.  [tcur, 1] is clipped to the grid's box and the cells along it are
+// visited in order (Amanatides-Woo).  Every candidate of a cell is clipped against its record's four planes: [tin,
+// tout], tout from scan_record and exit_parameter exactly as the walk forms its exit, tin from entry_parameter.  A
+// candidate with tout > tcur and tin <= tout enters at max(tin, tcur); the smallest wins, ties to the first found, and
+// the search stops once it lies within the cell being visited.  Returns the tet (-1: the ray enters no tet before t =
+// 1) and *tenter.  The walk then leaves the tet at its own exit parameter, which is this tout > tcur, through the same
+// planes: it stays monotone and watertight.  A cell missed by rounding at a cell boundary is covered by the lists'
+// padding (kLocateBand * extent, Engine::ensure_hull_grid).  fetch(e, r) loads record e.
+template <class Fetch>
+PTB_HD int32_t hull_entry(const HullGrid &H, const Ray &ray, double tcur, double *tenter, Fetch &&fetch) {
+  const SeedGrid &g = H.g;
+  const double inf = __builtin_huge_val();
+  // position in cell units: f + t df
+  const double fx = (ray.ox - H.ox) * g.inv_h, fy = (ray.oy - H.oy) * g.inv_h, fz = (ray.oz - H.oz) * g.inv_h;
+  const double dfx = ray.ux * g.inv_h, dfy = ray.uy * g.inv_h, dfz = ray.uz * g.inv_h;
+  double t0 = tcur, t1 = 1.0;
+  auto clip = [&](double f, double df, int n) {
+    if (df == 0.0) {
+      if (!(f >= 0.0 && f <= (double)n)) t1 = -inf;
+    } else {
+      const double a = -f / df, b = ((double)n - f) / df;
+      t0 = fmax(t0, fmin(a, b));
+      t1 = fmin(t1, fmax(a, b));
+    }
+  };
+  clip(fx, dfx, g.nx);
+  clip(fy, dfy, g.ny);
+  clip(fz, dfz, g.nz);
+  if (!(t0 <= t1)) return -1;
+  auto cell_of = [&](double f, double df, int n) { return (int)fmin(fmax(floor(f + t0 * df), 0.0), (double)(n - 1)); };
+  auto next_of = [&](int c, double f, double df) { return df == 0.0 ? inf : ((double)(c + (df > 0.0)) - f) / df; };
+  int cx = cell_of(fx, dfx, g.nx), cy = cell_of(fy, dfy, g.ny), cz = cell_of(fz, dfz, g.nz);
+  double nxt = next_of(cx, fx, dfx), nyt = next_of(cy, fy, dfy), nzt = next_of(cz, fz, dfz);
+  int32_t best = -1;
+  double bt = inf;
+  for (;;) {
+    const double tfar = fmin(fmin(nxt, nyt), fmin(nzt, t1));
+    const int64_t cell = ((int64_t)cz * g.ny + cy) * g.nx + cx;
+    const int64_t a = PTB_LDG(H.off + cell), b = PTB_LDG(H.off + cell + 1);
+    for (int64_t k = a; k < b; ++k) {
+      const int32_t t = PTB_LDG(H.tets + k);
+      double rec[16];
+      fetch(t, rec);
+      ExitScan sc;
+      scan_record(rec, t, ray.ox, ray.oy, ray.oz, ray.ux, ray.uy, ray.uz, sc);
+      const double tout = exit_parameter(sc), tin = entry_parameter(rec, ray);
+      const double te = fmax(tin, tcur);
+      if (tout > tcur && tin <= tout && te < bt) {
+        bt = te;
+        best = t;
+      }
+    }
+    if (bt <= tfar || !(tfar < t1)) break;
+    if (nxt <= nyt && nxt <= nzt) {
+      cx += dfx > 0.0 ? 1 : -1;
+      if (cx < 0 || cx >= g.nx) break;
+      nxt = next_of(cx, fx, dfx);
+    } else if (nyt <= nzt) {
+      cy += dfy > 0.0 ? 1 : -1;
+      if (cy < 0 || cy >= g.ny) break;
+      nyt = next_of(cy, fy, dfy);
+    } else {
+      cz += dfz > 0.0 ? 1 : -1;
+      if (cz < 0 || cz >= g.nz) break;
+      nzt = next_of(cz, fz, dfz);
+    }
+  }
+  if (!(bt < 1.0)) return -1;
+  *tenter = bt;
+  return best;
+}
+
 // tau / R of the straight line from (x, y, z) in element e to (tx, ty, tz): the sum over the tets the walk crosses of
 // sig[tet] times the ray parameter spent in it.  The loop is locate_point's (record, scan_record, exit_parameter), the
 // step rule advance()'s.  Returns kRayTraced, kRayShadowed or kRayLost; crossings += the interior faces crossed.
-template <class Fetch>
+// VOID (the detector void, with H its hull grid): an event outside the mesh (e == -1) starts at its ray's first entry,
+// a hull exit searches for the next entry from the exit instead of shadowing the ray, and a ray that enters no tet
+// again is traced: the void adds nothing to tau.  On a convex hull a ray that has left never comes back, so only the
+// first entry is searched for.  Every entry counts one iteration against max_iters and one in *entries.
+template <bool VOID = false, class Fetch>
 PTB_HD int detector_ray(const WalkParams &P, const double *sig, int32_t e, double x, double y, double z, double tx,
-                        double ty, double tz, double &tau_over_r, uint32_t &crossings, Fetch &&fetch) {
+                        double ty, double tz, double &tau_over_r, uint32_t &crossings, Fetch &&fetch,
+                        const HullGrid *H = nullptr, uint32_t *entries = nullptr) {
   Ray r;
   set_ray(P, r, x, y, z, tx, ty, tz);
   r.e = e;
   double s = 0.0;
-  for (;;) {
-    double rec[16];
-    fetch(r.e, rec);
-    ExitScan sc;
-    scan_record(rec, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
-    const double texit = exit_parameter(sc);
-    const bool reached = !(texit < 1.0);
-    const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
-    s += PTB_LDG(sig + r.e) * (tnew - r.tcur);
-    tau_over_r = s;
-    if (reached) return kRayTraced;
-    if (sc.nbr < 0) return kRayShadowed;  // graveyard outside the hull: re-entry across a concave notch is not followed
-    if (++r.iters >= P.max_iters) return kRayLost;
-    ++crossings;
-    r.e = sc.nbr;
-    r.tcur = tnew;
+  if constexpr (VOID) {
+    // one search site, so that the search and the walk share their registers
+    tau_over_r = 0.0;
+    bool search = e < 0;
+    for (;;) {
+      if (search) {
+        r.e = hull_entry(*H, r, r.tcur, &r.tcur, fetch);
+        if (r.e < 0) return kRayTraced;  // the rest of the ray lies in the void
+        if (++r.iters >= P.max_iters) return kRayLost;
+        ++*entries;
+      }
+      double rec[16];
+      fetch(r.e, rec);
+      ExitScan sc;
+      scan_record(rec, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
+      const double texit = exit_parameter(sc);
+      const bool reached = !(texit < 1.0);
+      const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
+      s += PTB_LDG(sig + r.e) * (tnew - r.tcur);
+      tau_over_r = s;
+      if (reached) return kRayTraced;
+      search = sc.nbr < 0;  // out through the hull: on to the next entry, if the hull lets there be one
+      if (search && H->convex) return kRayTraced;
+      if (!search) {
+        if (++r.iters >= P.max_iters) return kRayLost;
+        ++crossings;
+        r.e = sc.nbr;
+      }
+      r.tcur = tnew;
+    }
+  } else {
+    for (;;) {
+      double rec[16];
+      fetch(r.e, rec);
+      ExitScan sc;
+      scan_record(rec, r.e, r.ox, r.oy, r.oz, r.ux, r.uy, r.uz, sc);
+      const double texit = exit_parameter(sc);
+      const bool reached = !(texit < 1.0);
+      const double tnew = reached ? 1.0 : fmax(texit, r.tcur);
+      s += PTB_LDG(sig + r.e) * (tnew - r.tcur);
+      tau_over_r = s;
+      if (reached) return kRayTraced;
+      if (sc.nbr < 0) return kRayShadowed;  // graveyard outside the hull: re-entry across a concave notch is not followed
+      if (++r.iters >= P.max_iters) return kRayLost;
+      ++crossings;
+      r.e = sc.nbr;
+      r.tcur = tnew;
+    }
   }
 }
 
@@ -1013,10 +1151,13 @@ PTB_HD double ball_g(double x) { return x > 0.0 ? -expm1(-x) / x : 1.0; }
 // all the rays of an event share its outcome, which the kernels count once per event.  On a scoring outcome (traced,
 // inside r0) val[k] = the score of score k and *slot = its [time][bin][0][d] index (score k at slot + k D).
 // Shadowed and lost rays return val 0.  crossings += the interior faces the walk crossed.
-template <class Fetch>
+// VOID (the detector void, detector_ray): an event outside the mesh is not kDetOutside but traced from where it is, and
+// inside r0 it takes the ball formula with Sigma = 0 (3 / r0^2); *entries += the ray's entries through the hull.
+template <bool VOID = false, class Fetch>
 PTB_HD int detector_event(const WalkParams &W, const DetectorParams &P, int d, int32_t e, double x, double y, double z,
                           double w, const double *resp, int32_t bin, double t, double v, const double *pdf,
-                          double *val, int64_t *slot, uint32_t &crossings, Fetch &&fetch) {
+                          double *val, int64_t *slot, uint32_t &crossings, Fetch &&fetch, const HullGrid *H = nullptr,
+                          uint32_t *entries = nullptr) {
   bool bad = !all_finite(x, y, z) || (P.nt > 0 && (!all_finite(t, 0.0, 0.0) || !(v > 0.0)));
 PTB_UNROLL
   for (int k = 0; k < kMaxScores; ++k)
@@ -1035,7 +1176,8 @@ PTB_UNROLL
       bad = bad || (PTB_LDG(P.r0 + q) == 0.0 && sqrt(ax * ax + ay * ay + az * az) == 0.0);
     }
   if (bad) return kDetRejected;
-  if (e < 0) return kDetOutside;
+  if constexpr (!VOID)
+    if (e < 0) return kDetOutside;
   const double pd = pdf ? PTB_LDG(pdf + d) : 0.25 / M_PI;
   const double dx = PTB_LDG(P.pos + 3 * d), dy = PTB_LDG(P.pos + 3 * d + 1), dz = PTB_LDG(P.pos + 3 * d + 2);
   const double ux = dx - x, uy = dy - y, uz = dz - z;
@@ -1047,11 +1189,11 @@ PTB_UNROLL
   double f;
   int outcome;
   if (R < r0) {
-    f = pd * 3.0 * ball_g(PTB_LDG(sig + e) * r0) / (r0 * r0);
+    f = pd * 3.0 * ball_g((VOID && e < 0 ? 0.0 : PTB_LDG(sig + e)) * r0) / (r0 * r0);
     outcome = kRayInsideR0;
   } else {
     double tr = 0.0;
-    outcome = detector_ray(W, sig, e, x, y, z, dx, dy, dz, tr, crossings, fetch);
+    outcome = detector_ray<VOID>(W, sig, e, x, y, z, dx, dy, dz, tr, crossings, fetch, H, entries);
     f = outcome == kRayTraced ? pd * exp(-(tr * R)) / (R * R) : 0.0;
   }
 PTB_UNROLL

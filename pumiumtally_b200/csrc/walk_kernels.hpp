@@ -149,17 +149,20 @@ cudaError_t launch_collide_particles(const ParticleState *state, const int8_t *c
 // position and element, for every i < n with flagged[i] != 0.  w[i], pdf[i D + d] (nullptr: 1 / (4 pi)), resp[i nscores
 // + k] (nullptr: every response 1), bins[i] (nullptr: bin 0), times[i] and speeds[i] (read only when p.nt > 0).  The
 // scores go to p.tally, the outcomes to counts[kDetCounters].  Up to kDetSmemSlots slots are aggregated in shared memory.
+// hull != nullptr: the detector void (walk_core.cuh, detector_ray) with that hull grid, its own kernels, which also
+// count the hull entries in counts[kDetCountHullEntries] (counts then holds kDetCountersVoid).
 constexpr int kDetCountTraced = 0, kDetCountShadowed = 1, kDetCountLost = 2, kDetCountInsideR0 = 3,
-              kDetCountCrossings = 4, kDetCountOutside = 5, kDetCountRejected = 6, kDetCounters = 7;
+              kDetCountCrossings = 4, kDetCountOutside = 5, kDetCountRejected = 6, kDetCounters = 7,
+              kDetCountHullEntries = 7, kDetCountersVoid = 8;
 constexpr int64_t kDetSmemSlots = 2048;
 cudaError_t launch_detect_located(const LocateParams &l, const DetectorParams &p, const double *xyz, int64_t n,
                                   const double *w, const double *pdf, const double *resp, const int32_t *bins,
                                   const double *times, const double *speeds, unsigned long long *counts,
-                                  cudaStream_t stream);
+                                  cudaStream_t stream, const HullGrid *hull = nullptr);
 cudaError_t launch_detect_particles(const WalkParams &wp, const DetectorParams &p, const ParticleState *state,
                                     const int8_t *flagged, int32_t n, const double *w, const double *pdf,
                                     const double *resp, const int32_t *bins, const double *times, const double *speeds,
-                                    unsigned long long *counts, cudaStream_t stream);
+                                    unsigned long long *counts, cudaStream_t stream, const HullGrid *hull = nullptr);
 
 // stats_kernels.cu.  Batch statistics (batch_stats.cuh).  fold: (mean[i], m2[i]) <- welford_fold(x[i] / *divisor, nb)
 // for i < n, nb the number of batches including this one; the divisor is read on the device.

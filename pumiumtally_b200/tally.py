@@ -81,6 +81,8 @@ C_API = {
     "pumitally_set_point_detectors": (C.c_int, [C.c_void_p, _dp, C.c_int32, _dp]),
     "pumitally_get_point_detectors": (C.c_int32, [C.c_void_p]),
     "pumitally_set_detector_cross_sections": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pumitally_set_detector_void": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pumitally_get_detector_void": (C.c_int32, [C.c_void_p]),
     "pumitally_tally_detectors": (C.c_int, [C.c_void_p, _dp, C.c_int64, _dp, _dp, _dp, _ip, _dp, _dp]),
     "pumitally_tally_detectors_device": (
         C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -660,7 +662,8 @@ class PumiTally:
 
     # ---- point detectors -----------------------------------------------------------
     def set_point_detectors(self, points, r0):
-        """Next-event (point-detector) estimates at ``points`` [D, 3] (1 <= D <= 256, inside the mesh) with exclusion
+        """Next-event (point-detector) estimates at ``points`` [D, 3] (1 <= D <= 256, inside the mesh, or anywhere
+        finite with the detector void on: set_detector_void) with exclusion
         radii ``r0`` [D] (finite, >= 0).  ``points`` None removes them.  Resets the tally and discards the folded
         batches."""
         if points is None:
@@ -678,6 +681,24 @@ class PumiTally:
     def point_detectors(self) -> int:
         """Number of point detectors D, 0 without."""
         return int(self._L.pumitally_get_point_detectors(self._h))
+
+    def set_detector_void(self, on):
+        """``on`` True treats the space outside the mesh as a void the detector rays cross: detectors may lie anywhere,
+        events outside the mesh are traced, and rays re-enter across concave parts of the hull.  Setting the current
+        mode changes nothing; switching resets the tally and discards the folded batches, and switching off while a
+        detector lies outside the mesh is refused.  Before comm_init."""
+        if self._L.pumitally_set_detector_void(self._h, int(on)):  # anything but 0 or 1 (or a bool) is refused
+            raise ValueError("set_detector_void failed")
+
+    @property
+    def detector_void(self) -> bool:
+        """Whether the space outside the mesh is a void the detector rays cross (set_detector_void)."""
+        return bool(self._L.pumitally_get_detector_void(self._h))
+
+    @property
+    def detector_hull_entries(self) -> int:
+        """Entries of detector rays into the mesh through the hull since the last reset (0 with the void off)."""
+        return int(self.get_option("detector_hull_entries"))
 
     def set_detector_cross_sections(self, sigma):
         """Sigma_t [nbins, num_elements] (caller's numbering, finite, >= 0) the detector rays are attenuated by; the

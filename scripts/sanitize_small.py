@@ -100,3 +100,30 @@ for nbins, D, edges in ((1, 2, None), (3, 50, np.linspace(0.0, 16.0, 17))):
     torch.cuda.synchronize()
     assert np.isfinite(e.detector_results(0)).all()
     print("detectors", nbins, D, "ok", flush=True)
+
+# the detector void on a non-convex mesh (an L-shaped prism): detectors in the notch and beyond the box, events inside,
+# in the notch and outside, with both aggregations
+from helpers import l_shaped_mesh  # noqa: E402
+
+lc, lt = l_shaped_mesh(8, 8, 2)
+for D in (2, 50):
+    e = PumiTally.from_arrays(lc, lt, 2048)
+    e.set_option("chunk", 1024)
+    e.set_detector_void(True)
+    if D > 2:
+        e.set_time_bins(np.linspace(0.0, 40.0, 41))
+    rng = np.random.default_rng(D)
+    det = rng.uniform([-4.0, -4.0, -1.0], [12.0, 12.0, 3.0], size=(D, 3))
+    det[0] = (6.0, 6.0, 1.0)
+    e.set_point_detectors(det, np.full(D, 0.2))
+    e.set_detector_cross_sections(np.full((1, len(lt)), 0.3))
+    pts = rng.uniform([-2.0, -2.0, -0.5], [10.0, 10.0, 2.5], size=(2048, 3))
+    kw = {} if D == 2 else {"times": rng.uniform(0, 16, 2048), "speeds": np.full(2048, 2.0)}
+    e.tally_detectors(pts, np.ones(2048), **kw)
+    dev = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in kw.items()}
+    e.tally_detectors_device(torch.from_numpy(pts).cuda(), torch.ones(2048, dtype=torch.float64, device="cuda"), **dev)
+    e.tally_detectors_at_particles(np.ones(2048, dtype=np.int8), np.ones(2048), **kw)
+    torch.cuda.synchronize()
+    assert np.isfinite(e.detector_results(0)).all() and e.detector_hull_entries > 0
+    assert e.get_option("detector_rays_shadowed") == 0 and e.get_option("detector_rays_lost") == 0
+    print("detector void", D, "ok", flush=True)
