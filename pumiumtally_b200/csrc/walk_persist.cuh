@@ -410,21 +410,21 @@ __device__ __forceinline__ void plane_step(const WalkParams &P, Ray &r, Counters
 // plane_step() would have loaded; the fourth face of a ray's first tet comes with the lane's own load.
 constexpr int kCoopRowBytes = 96;
 
-// Shared-memory address of 16-byte chunk p (0..5) of row m.  Rows are packed at 96 bytes; rows 4..7 of every
-// eight are rotated by one chunk so that eight consecutive rows read at the same chunk land in eight different
-// 16-byte bank groups (a quarter-warp phase of ld.shared.v2.f64 is then conflict-free).
+// Shared-memory address of 16-byte chunk p (0..5) of row m.  Rows are packed at 96 bytes; in rows 4..7 of every
+// eight the two chunks of each face trade places, so that eight consecutive rows read at the same chunk land in
+// eight different 16-byte bank groups (a quarter-warp phase of ld.shared.v2.f64 is then conflict-free).
 __device__ __forceinline__ uint32_t coop_chunk(uint32_t rows, int m, int p) {
-  const int pr = p + ((m >> 2) & 1);
-  return rows + (uint32_t)(kCoopRowBytes * m + 16 * (pr == 6 ? 0 : pr));
+  return rows + (uint32_t)(kCoopRowBytes * m + 16 * (p ^ ((m >> 2) & 1)));
 }
 
-__device__ __forceinline__ void cp_async_16_l1(uint32_t dst, const void *src, uint64_t pol) {
-  asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol)
-               : "memory");
-}
+// The (element, face not to copy) slots: rank m sits in group m & 3 at position m >> 2, so the slots of the
+// eight records lanes 8g..8g+7 copy are one contiguous 64-byte run.  Groups are 80 bytes apart, so the four groups
+// a 128-bit read asks for lie in different banks.  (96 would also spare the slot stores a bank conflict, but with
+// 256 bytes more per block, launch_persist's carveout for five plain blocks passes the 164 KB configuration.)
+constexpr int kCoopSlotGroupBytes = 80;
 
-// Per-warp shared memory of the cooperative fetch: 32 rows, then 32 (element, entry face) slots, both by rank.
-constexpr int kCoopWarpBytes = 32 * kCoopRowBytes + 32 * 8;
+// Per-warp shared memory of the cooperative fetch: 32 rows by rank, then the four slot groups.
+constexpr int kCoopWarpBytes = 32 * kCoopRowBytes + 4 * kCoopSlotGroupBytes;
 
 // One crossing for every active lane of the warp (act: the active mask; every lane of the warp calls it).
 // rows: shared-memory address of the warp's kCoopWarpBytes.
@@ -437,26 +437,48 @@ __device__ __forceinline__ void coop_plane_step(const WalkParams &P, Ray &r, Cou
   const int rank = __popc(act & ((1u << lane) - 1u));  // idle lanes leave no gap between the rows
   const int en = r.entry;
   const uint64_t pol = l2_policy_keep_now();
+  const uint32_t slots = rows + 32 * kCoopRowBytes;
   double q[3][4], q3[4] = {0.0, 0.0, 0.0, 0.0};
   if (on) {
-    asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(rows + 32 * kCoopRowBytes + 8 * rank), "r"(r.e), "r"(en)
+    // the face not to copy: the entry face, or on a first tet (entry -1) the fourth, which the owner loads itself
+    asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(slots + kCoopSlotGroupBytes * (rank & 3) + 8 * (rank >> 2)),
+                 "r"(r.e), "r"(en & 3)
                  : "memory");
     if (en < 0) load_face<kFetchPolicyL1>(P.tets[r.e].d + 12, pol, q3[0], q3[1], q3[2], q3[3]);
   }
   __syncwarp();
-  const int piece = lane & 7, f = piece >> 1;
+  // Lane 8g + piece copies piece `piece` (half piece & 1 of face f) of the records of ranks g, g + 4, ..., g + 28:
+  // round j is rank and row 4j + g, whose chunks trade places (coop_chunk) when j is odd.  The copies are issued
+  // under predicates, not behind branches, so the warp's copies leave back to back after the four slot reads.
+  const int g = lane >> 3, piece = lane & 7, f = piece >> 1;
+  int32_t s[16];  // (element, face not to copy) of round j in s[2j], s[2j + 1]
+  asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%16];\n\t"
+               "ld.shared.v4.b32 {%4,%5,%6,%7}, [%16+16];\n\t"
+               "ld.shared.v4.b32 {%8,%9,%10,%11}, [%16+32];\n\t"
+               "ld.shared.v4.b32 {%12,%13,%14,%15}, [%16+48];"
+               : "=r"(s[0]), "=r"(s[1]), "=r"(s[2]), "=r"(s[3]), "=r"(s[4]), "=r"(s[5]), "=r"(s[6]), "=r"(s[7]),
+                 "=r"(s[8]), "=r"(s[9]), "=r"(s[10]), "=r"(s[11]), "=r"(s[12]), "=r"(s[13]), "=r"(s[14]), "=r"(s[15])
+               : "r"(slots + kCoopSlotGroupBytes * g)
+               : "memory");
+  const char *src = reinterpret_cast<const char *>(P.tets) + 16 * piece;
+  const uint32_t dst_even = rows + kCoopRowBytes * g + 32 * f + 16 * (piece & 1);
+  const uint32_t dst_odd = rows + kCoopRowBytes * g + 32 * f + 16 * (~piece & 1);
+  const int left = n - g;  // round j copies while 4j < left
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
-    if (4 * j >= n) break;
-    const int m = 4 * j + (lane >> 3);
-    if (m < n) {
-      int32_t e, sen;
-      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(e), "=r"(sen) : "r"(rows + 32 * kCoopRowBytes + 8 * m)
-                   : "memory");
-      const int skip = sen < 0 ? 3 : sen;  // the entry face, or on a first tet the fourth (the owner loads it)
-      if (f != skip)
-        cp_async_16_l1(coop_chunk(rows, m, 2 * (f - (f > skip ? 1 : 0)) + (piece & 1)), P.tets[e].d + 2 * piece, pol);
-    }
+    // Warp-uniform: at most 28 active lanes need seven rounds.  The branch also keeps ptxas from repeating the
+    // whole fetch on the divergent path of the two __syncwarp()s around it.
+    if (j == 7 && n <= 28) break;
+    const int skip = s[2 * j + 1];
+    // the faces after the skipped one move up one 32-byte slot
+    const uint32_t dst = (j & 1 ? dst_odd : dst_even) + 4 * kCoopRowBytes * j - (f > skip ? 32u : 0u);
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 a;\n\t"
+                 "setp.gt.s32 p, %3, %4;\n\t"
+                 "setp.ne.and.s32 p, %5, %6, p;\n\t"
+                 "mad.wide.u32 a, %7, 128, %1;\n\t"
+                 "@p cp.async.ca.shared.global.L2::cache_hint [%0], [a], 16, %2;\n\t}"
+                 ::"r"(dst), "l"(src), "l"(pol), "r"(left), "r"(4 * j), "r"(f), "r"(skip), "r"(s[2 * j])
+                 : "memory");
   }
   // (this also waits for gather copies of a particle stage still in flight: issued before, they rarely land later)
   asm volatile("cp.async.wait_all;" ::: "memory");

@@ -15,8 +15,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) PTB_PERSIST_NAME(const PTB_PERSIS
   __shared__ ParticleStage stages[WARPS][2];
   __shared__ __align__(8) unsigned long long bars[WARPS][3];
   __shared__ __align__(128) unsigned char rows[kRows ? WARPS : 1][kRows ? 32 * kRowBytes : 16];
-  // The timed walk keeps the per-lane L1 fetch in the binned kernel: with the cooperative one it ran 19 % slower (DESIGN
-  // section 4.1, item 6).
+  // The timed walk keeps the per-lane L1 fetch in the binned kernel: with the cooperative one it ran 19 % slower, and
+  // still 12 % slower once that fetch was issued without branches (DESIGN section 4.1, item 6).
   constexpr bool kCoop = FETCH == kFetchCoopL1 && !TM;
   __shared__ __align__(16) unsigned char coop_rows[kCoop ? WARPS : 1][kCoop ? kCoopWarpBytes : 16];
   constexpr bool kEdge = FETCH == kFetchEdge;
